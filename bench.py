@@ -46,6 +46,7 @@ def parse_args():
     ap.add_argument("--large-bodies", type=int, default=1_000_000, help="body count of the large pile in the configs block (the scene size BASELINE.json's north_star targets); 0 = skip it")
     ap.add_argument("--no-sharded", action="store_true", help="N > 1: skip the one-graph-over-N-GPUs block")
     ap.add_argument("--sharded-bodies", type=int, default=1_000_000, help="N > 1: body count of the pile whose single constraint graph is split over the N GPUs")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write what the last timed step computed (body pose / velocity / world inertia, accumulated impulses) to DIR/<name>.npy")
     return ap.parse_args()
 
 
@@ -71,7 +72,7 @@ def build_sim(args, seed):
 
 class ClockSampler:
     """SM clock + throttle (clocks event) reasons sampled DURING the timed region: NVML every 5 ms from a thread (nvidia_ml_py), falling back to
-    `nvidia-smi -lms 100` (B200_PROFILING.md recipe) when NVML is unavailable."""
+    `nvidia-smi -lms 100` when NVML is unavailable."""
 
     FIELDS = "clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
 
@@ -157,20 +158,7 @@ class ClockSampler:
                 "source": "nvml" if self.nvml is not None else "nvidia-smi"}
 
 
-def load_traffic(bodies, kernel):
-    """DRAM bytes per launch of the dominant kernel from the committed `ncu --set full` capture of this workload (profiles/), or None."""
-    path = os.path.join(ROOT, "profiles", "dram_traffic.json")
-    try:
-        with open(path) as f:
-            for row in json.load(f)["captures"]:
-                if row["bodies"] == bodies and row["kernel"] == kernel:
-                    return row
-    except Exception:
-        pass
-    return None
-
-
-AUTO_MODE = {"shape_pile": "graph", "ragdolls": "graph", "fallback_stress": "graph"}  # updated from measurements (profiles/r02_summary.md)
+AUTO_MODE = {"shape_pile": "graph", "ragdolls": "graph", "fallback_stress": "graph"}  # the execution mode --mode auto runs per scene
 
 
 def resolve_mode(args):
@@ -283,8 +271,35 @@ def load_peaks():
     path = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(path):
         with open(path) as f:
-            return json.load(f).get("hbm_gbs", 6650.0), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+            return json.load(f).get("hbm_gbs", 3350.0), "measured (MEASURED_PEAKS.json)"
+    return 3350.0, "H100 SXM data sheet (HBM3, 3.35 TB/s)"
+
+
+BODY_OUTPUTS = {"body_pose": np.r_[0:7], "body_velocity": np.r_[8:11, 12:15], "body_world_inertia": np.r_[24:31]}  # floats of a BodyDynamics record
+DUMP_BYTES_PER_ARRAY = 15 << 20  # four arrays: less than 64 MB in all
+
+
+def dump_outputs(ts, sim, directory):
+    """Writes what a caller of the timed path receives after its last step: the body records (pose, velocity, world inertia) and the accumulated
+    impulses of every live constraint lane, in (batch, type batch, constraint, row) order, as float32 .npy files. An array larger than
+    DUMP_BYTES_PER_ARRAY keeps the rows np.sort(np.random.default_rng(0).choice(rows, size=keep, replace=False)), the same for every run with the
+    same arguments. The host copies the other legs of the bench upload from are restored afterwards, so dumping does not change what they measure."""
+    tbs = sim.type_batches()
+    saved_bodies, saved_impulses = sim.bodies.copy(), [tb.accumulated_impulses.copy() for tb in tbs]
+    ts.download_bodies()
+    ts.download_impulses()
+    outputs = {name: sim.bodies[:, cols].copy() for name, cols in BODY_OUTPUTS.items()}
+    live = [tb.accumulated_impulses.transpose(0, 2, 1)[tb.body_references[:, 0, :] >= 0].ravel() for tb in tbs]
+    outputs["accumulated_impulses"] = np.concatenate(live) if live else np.zeros(0, dtype=np.float32)
+    sim.bodies[:] = saved_bodies
+    for tb, saved in zip(tbs, saved_impulses):
+        tb.accumulated_impulses[:] = saved
+    os.makedirs(directory, exist_ok=True)
+    for name, a in outputs.items():
+        if a.nbytes > DUMP_BYTES_PER_ARRAY:
+            keep = DUMP_BYTES_PER_ARRAY // (a.nbytes // a.shape[0])
+            a = a[np.sort(np.random.default_rng(0).choice(a.shape[0], size=keep, replace=False))]
+        np.save(os.path.join(directory, name + ".npy"), np.ascontiguousarray(a, dtype=np.float32))
 
 
 def usable_cpu_count():
@@ -374,7 +389,7 @@ def main():
     ts.describe()
     ts.synchronize()
 
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")  # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")  # > 50 MB L2 of an H100
 
     def barrier():
         torch.cuda.synchronize()
@@ -400,6 +415,8 @@ def main():
     barrier()
     clocks = sampler.stop()
     t = ts.timings()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(ts, sim, args.dump_outputs)
     ci_per_step = int(t.constraint_iterations)
     launches_per_step = int(t.kernel_launches)
     alg_bytes_per_step = int(t.algorithmic_bytes)
@@ -582,14 +599,6 @@ def main():
         roof_extra = {"share_of_step": share, "achieved_serialised_launches": prof["solve"]["algorithmic_bytes"] / (prof["solve"]["ms"] * 1e-3) / 1e9,
                       "whole_step_achieved": alg_bytes_per_step / (total_ms / args.steps * 1e-3) / 1e9}
         achieved = roof_bytes / (roof_ms * 1e-3) / 1e9
-        traffic_row = load_traffic(args.bodies, "constraint_stage_kernel<Solve>") if args.scene == "shape_pile" else None
-        traffic = None
-        if traffic_row:
-            traffic = traffic_row["dram_bytes_per_launch"]
-            roof_extra["traffic_source"] = traffic_row["source"]
-            roof_extra["traffic_launch"] = traffic_row["launch"]
-            roof_extra["traffic_launch_algorithmic_bytes"] = traffic_row["algorithmic_bytes_per_launch"]
-            roof_extra["mean_algorithmic_bytes_per_launch"] = roof_bytes / launches
         line = {
             "metric": "constraint-iterations/sec (solver+integrator)", "value": value, "unit": "constraint-iterations/s", "n_gpus": world, "steps": args.steps, "warmup": max(args.warmup, 3),
             "ms_per_step": total_ms_max / args.steps, "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f32", "data": "synthetic",
@@ -599,7 +608,7 @@ def main():
                     "topology": "unchanged between steps (bodies + prestep + impulses re-uploaded, results downloaded)"},
             "gpu_launches": launches_per_step * args.steps,
             "clocks": clocks,
-            "roofline": {"bound": "hbm", "kernel": roof_kernel, "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "traffic": traffic,
+            "roofline": {"bound": "hbm", "kernel": roof_kernel, "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
                          "peak_source": peak_source, "algorithmic_bytes_per_step": alg_bytes_per_step, **roof_extra},
             "stage_profile_ms": {k: round(v["ms"], 4) for k, v in (prof or {}).items()},
         }

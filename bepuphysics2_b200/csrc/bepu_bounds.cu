@@ -1,4 +1,4 @@
-// PredictBoundingBoxes kernel (sm_100a), compiled -fmad=false with IEEE sqrt: the results are bit-identical to a non-contracting CPU evaluation of
+// PredictBoundingBoxes kernel (sm_90a), compiled -fmad=false with IEEE sqrt: the results are bit-identical to a non-contracting CPU evaluation of
 // the reference's expressions (tests/test_bounds.py). One thread per body, fully coalesced: reads the 32-B pose / velocity / local inertia records
 // the solver keeps resident (96 B), the 32-B shape record and the 8-B activity; writes 32 B of bounds + margin and the activity. HBM-bound
 // (168 B per body); the bounding boxes of every body are independent, so there is nothing to order.

@@ -1,4 +1,4 @@
-// Device-side batch colouring kernels (sm_100a). See bepu_coloring.h.
+// Device-side batch colouring kernels (sm_90a). See bepu_coloring.h.
 //
 // Why this reproduces sequential first fit exactly: Solver.Add gives constraint c the first batch that holds none of the constraints added before c
 // which share a dynamic body with c. Here c is assigned in the round in which it holds the lowest key on every one of its dynamic bodies, i.e. when
@@ -100,7 +100,7 @@ __global__ void color_assign_kernel(ColoringBuffers cb, int round) {
 
 inline unsigned grid_for(size_t n) {
     const size_t blocks = (n + 255) / 256;
-    return (unsigned)(blocks < 1 ? 1 : (blocks > 148 * 8 ? 148 * 8 : blocks));  // grid-stride: at most 8 CTAs per SM of a B200
+    return (unsigned)(blocks < 1 ? 1 : (blocks > 132 * 8 ? 132 * 8 : blocks));  // grid-stride: at most 8 CTAs per SM of an H100 SXM (132 SMs)
 }
 
 }  // namespace

@@ -1,4 +1,4 @@
-// Contact constraint functions for the sm_100a solver kernels: convex manifolds with 1-4 contacts and nonconvex
+// Contact constraint functions for the sm_90a solver kernels: convex manifolds with 1-4 contacts and nonconvex
 // manifolds with 2-4 contacts, one- and two-body (type ids 0-10, 15-17).
 // Reference behaviour: BepuPhysics/Constraints/Contact/{PenetrationLimit,PenetrationLimitOneBody,TangentFriction,
 // TangentFrictionOneBody,TwistFriction,TwistFrictionOneBody,ContactConvexTypes,ContactNonconvexCommon}.cs.
@@ -252,7 +252,7 @@ template <int N> struct ConvexTwoBody {
         if constexpr (N == 1) centerA = offs[0]; else centerA = friction_center<N>(offs, depths);
         V3 centerB = centerA - offsetB;
         tangent_apply(tangent_jacobians(x, z, centerA, centerB), iA, iB, V2{ldacc(a, 0), ldacc(a, 1)}, vA, vB);
-        // the per-contact rows as a real loop (smaller instruction footprint: -4 % per step on B200) -- rows re-read by index, same operations in the same order
+        // the per-contact rows as a real loop (smaller instruction footprint) -- rows re-read by index, same operations in the same order
 #pragma unroll 1
         for (int i = 0; i < N; ++i) {
             V3 offset = ldrow3(p, 4 * i);

@@ -1,4 +1,4 @@
-// Device-side fp32 math for the sm_100a constraint kernels. One thread = one constraint lane, so everything here is
+// Device-side fp32 math for the sm_90a constraint kernels. One thread = one constraint lane, so everything here is
 // plain scalar code on small register-resident aggregates.
 //
 // Expression shapes follow the reference's wide math (file:line cited per function) so that the strict build

@@ -1,4 +1,4 @@
-// Joint / motor / servo / limit constraint functions for the sm_100a solver kernels (one thread = one constraint).
+// Joint / motor / servo / limit constraint functions for the sm_90a solver kernels (one thread = one constraint).
 // Every type exposes: kBodies, kPrestepRows, kImpulseRows, kIncremental=false, kNeedsPose=true and
 //   warm_start(const BodyState* b, const float* p, const float* a, Velocity* v)
 //   solve(const BodyState* b, float dt, float inverseDt, const float* p, float* a, Velocity* v)

@@ -1,4 +1,4 @@
-// The remaining joint / motor / servo / limit constraint functions of the reference's default type set (DefaultTypes.cs) for the sm_100a
+// The remaining joint / motor / servo / limit constraint functions of the reference's default type set (DefaultTypes.cs) for the sm_90a
 // solver kernels (one thread = one constraint). Same call shape as bepu_joints.cuh:
 //   warm_start(const BodyState* b, const float* p, const float* a, Velocity* v)
 //   solve(const BodyState* b, float dt, float inverseDt, const float* p, float* a, Velocity* v)

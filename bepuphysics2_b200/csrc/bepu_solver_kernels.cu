@@ -17,7 +17,7 @@ void launch_stage_solve_sharded(const WorkRecord* records, const int32_t* ref_ro
 #ifndef BEPU_DEEP_MINB
 #define BEPU_DEEP_MINB 12
 #endif
-constexpr int kDeepBatchBundles = 2400;  // more bundles than the uncapped build keeps resident at once (148 SMs x 16 warps)
+constexpr int kDeepBatchBundles = 2150;  // more bundles than the uncapped build keeps resident at once (132 SMs x 16 warps on an H100 SXM)
 template <int STAGE, int MINB>
 static void launch_stage_variant(const WorkRecord* records, const int32_t* ref_rows, int work_count, const BodyBuffers& B, const FrameParams* fp, int launch_flags, cudaStream_t s) {
     static std::atomic<bool> carveout_set[64] = {};  // function attributes are per device: a process may hold contexts on several

@@ -1,4 +1,4 @@
-// Solver stage kernels (sm_100a): WarmStart (with embedded pose/velocity integration), Solve, IncrementallyUpdateForSubstep,
+// Solver stage kernels (sm_90a): WarmStart (with embedded pose/velocity integration), Solve, IncrementallyUpdateForSubstep,
 // the kinematic prepasses and the final pose pass. Included once per numerics flavour (BEPU_NS = bepu_fast with FMA
 // contraction, bepu_strict with -fmad=false).
 //
@@ -16,22 +16,32 @@ namespace BEPU_NS {
 
 using namespace bepucuda;
 
-// ---- body records: one 32-byte record = one DRAM sector = ONE 256-bit load/store (LDG.E.256 / STG.E.256, new on sm_100) ----------------
+// ---- body records: one 32-byte record = one DRAM sector = two back-to-back 128-bit loads/stores (LDG.E.128 / STG.E.128; sm_90 has no wider access)
 struct F8 { float a, b, c, d, e, f, g, h; };
-// Body records: one 256-bit access per 32-B record, marked evict-last in L2 (and never allocated in L1: other warps of the launch sequence write
+// Body records: both halves of a 32-B record are marked evict-last in L2 (and never allocated in L1: other warps of the launch sequence write
 // them) so that the body arrays stay L2-resident while the constraint rows stream past them (those are fetched evict-first, see the bulk copies).
-#define BEPU_BODY_LD "ld.global.L1::no_allocate.L2::evict_last.v8.f32"
-#define BEPU_BODY_ST "st.global.L1::no_allocate.L2::evict_last.v8.f32"
+// Both halves are issued from one asm statement so that they leave as one pair and fill the same sector. sm_90 takes the evict-last priority
+// as an L2 cache policy operand (the bare .L2::evict_last qualifier exists only on the 256-bit accesses of later architectures); the policy asm
+// is not volatile so that the compiler can hoist it and share it between accesses.
+#define BEPU_BODY_LD "ld.global.L1::no_allocate.L2::cache_hint.v4.f32"
+#define BEPU_BODY_ST "st.global.L1::no_allocate.L2::cache_hint.v4.f32"
+BEPU_DI uint64_t l2_evict_last_policy() {
+    uint64_t policy;
+    asm("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(policy));
+    return policy;
+}
 BEPU_DI F8 ld256(const float4* p) {
     F8 r;
-    asm volatile(BEPU_BODY_LD " {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
+    asm volatile(BEPU_BODY_LD " {%0,%1,%2,%3}, [%8], %9;\n\t" BEPU_BODY_LD " {%4,%5,%6,%7}, [%8+16], %9;"
                  : "=f"(r.a), "=f"(r.b), "=f"(r.c), "=f"(r.d), "=f"(r.e), "=f"(r.f), "=f"(r.g), "=f"(r.h)
-                 : "l"(p)
+                 : "l"(p), "l"(l2_evict_last_policy())
                  : "memory");
     return r;
 }
 BEPU_DI void st256(float4* p, float a, float b, float c, float d, float e, float f, float g, float h) {
-    asm volatile(BEPU_BODY_ST " [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(p), "f"(a), "f"(b), "f"(c), "f"(d), "f"(e), "f"(f), "f"(g), "f"(h) : "memory");
+    asm volatile(BEPU_BODY_ST " [%0], {%1,%2,%3,%4}, %9;\n\t" BEPU_BODY_ST " [%0+16], {%5,%6,%7,%8}, %9;" ::"l"(p), "f"(a), "f"(b), "f"(c), "f"(d), "f"(e), "f"(f), "f"(g), "f"(h),
+                 "l"(l2_evict_last_policy())
+                 : "memory");
 }
 BEPU_DI void load_velocity(const float4* vel, uint32_t i, Velocity& v) {
     const F8 r = ld256(vel + 2 * (size_t)i);

@@ -1,5 +1,5 @@
 /*
- * libbepucuda — C ABI of the B200-native constraint solver + integrator for bepuphysics2.
+ * libbepucuda — C ABI of the H100-native constraint solver + integrator for bepuphysics2.
  *
  * This is the drop-in boundary. The reference has no FFI at this seam (SURVEY.md §8b): the
  * solver is a C# class constructed inside Simulation.Create. The entry points below are what
@@ -46,7 +46,7 @@ enum bepucuda_execution_mode {
     BEPUCUDA_EXEC_GRAPH = 0,      /* one kernel per (batch, stage) chained by programmatic dependent launch, whole frame captured in a CUDA graph */
     BEPUCUDA_EXEC_STREAM = 2      /* the same launches issued directly on the stream, no graph (profiling with ncu; the exchange-callback sharding) */
     /* 1 and 3 were a persistent cooperative kernel (grid barrier per stage) and a dataflow kernel (per-body version dependencies); both measured
-     * slower than the graph on every benchmark configuration (profiles/r02_summary.md) and were removed: bepucuda_create rejects them. */
+     * slower than the graph on every benchmark configuration and were removed: bepucuda_create rejects them. */
 };
 
 typedef struct bepucuda_config {

@@ -61,8 +61,8 @@ def test_sequential_fallback_batch_bit_exact(libs):
 
 
 def test_fast_build_within_tolerance(libs):
-    """FMA-contracted + approximate div/sqrt build on contacts: relative RMS error <= 1e-5 and max abs error <= 1e-4 on velocities, poses and
-    accumulated impulses after one frame of 8 substeps x 2 iterations (measured: ~4e-7 / 2e-6)."""
+    """FMA-contracted + approximate sqrt build on contacts: relative RMS error <= 1e-5 and max abs error <= 1e-4 on velocities, poses and
+    accumulated impulses after one frame of 8 substeps x 2 iterations."""
     _parity(scenes.shape_pile(3000, seed=5), exact=False, rel_rms=1e-5, max_abs=1e-4, substeps=8, velocity_iterations=2)
 
 
@@ -119,7 +119,7 @@ def test_ragdolls_substepped_servo_variant_bit_exact(libs):
 
 
 def test_ragdolls_stream_mode_fast_within_tolerance(libs):
-    """Fast build on joints: relative RMS error <= 1e-3, max abs error <= 2e-2 after one frame (measured ~3e-5 / 1e-3; the twist/servo angle
+    """Fast build on joints: relative RMS error <= 1e-3, max abs error <= 2e-2 after one frame (the twist/servo angle
     measurements go through acos near 1, which amplifies rounding: see tests/tools/fast_error_stats.py)."""
     _parity(scenes.ragdolls(60, seed=5), exact=False, mode=EXEC_STREAM, rel_rms=1e-3, max_abs=2e-2, substeps=1, velocity_iterations=4)
 
@@ -171,7 +171,7 @@ def test_joint_zoo_with_fallback_batch_and_momentum_conserving_integration(libs)
 
 
 def test_joint_zoo_fast_build_within_tolerance(libs):
-    """Fast (FMA, approximate div/sqrt) build on the full zoo after one frame: relative RMS error <= 1e-3, max abs error <= 5e-2."""
+    """Fast (FMA, approximate sqrt) build on the full zoo after one frame: relative RMS error <= 1e-3, max abs error <= 5e-2."""
     _parity(scenes.joint_zoo(1500, 120, seed=6), exact=False, rel_rms=1e-3, max_abs=5e-2, substeps=2, velocity_iterations=2)
 
 
@@ -386,13 +386,13 @@ def _fast_drift(scene, frames, **kw):
 
 
 def test_fast_build_benchmark_scale_multi_frame_drift_bound(libs):
-    """The BENCHMARKED build (FMA contraction, approximate div/sqrt) at the benchmark's own size, 8 frames of 8 x 2 with per-frame refresh. A
-    contracting evaluation of a chaotic system separates from the non-contracting one; profiles/r01_summary.md section 6 measured the growth
+    """The BENCHMARKED build (FMA contraction, approximate sqrt) at the benchmark's own size, 8 frames of 8 x 2 with per-frame refresh. A
+    contracting evaluation of a chaotic system separates from the non-contracting one; tests/tools/drift_curve.py measures the growth
     with a CPU proxy (frame 8, 3000-body pile: position 1.1e-8, linear 3.4e-7, angular 6.4e-7 relative RMS). Bound asserted here: 100x that."""
     d = _fast_drift(scenes.shape_pile(100_000, seed=5), 8, substeps=8, velocity_iterations=2)
     assert d["position"][0] <= 1e-6 and d["orientation"][0] <= 1e-5
     assert d["linear"][0] <= 5e-5 and d["angular"][0] <= 1e-4
-    assert d["impulses"][0] <= 2e-2  # measured 2.4e-3: many contact impulses sit at the clamp, where a last-bit difference switches them on or off
+    assert d["impulses"][0] <= 2e-2  # 2.4e-3 on an H100: many contact impulses sit at the clamp, where a last-bit difference switches them on or off
 
 
 def test_fast_build_ragdoll_tube_multi_frame_drift_bound(libs):

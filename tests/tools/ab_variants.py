@@ -1,9 +1,9 @@
 """A/B of the staged kernel experiments (DESIGN.md §9) against the shipped library.
 
-    python tests/tools/ab_variants.py build [name ...]     # in the build container: libbepucuda_<name>.so per variant (about 5 min each)
-    python tests/tools/ab_variants.py run [name ...]       # on a B200: parity subset + bench per variant that has been built, one table
+    python tests/tools/ab_variants.py build [name ...]     # libbepucuda_<name>.so per variant (no GPU needed)
+    python tests/tools/ab_variants.py run [name ...]       # on an H100: parity subset + bench per variant that has been built, one table
 
-The built variant libraries travel to the GPU box with the snapshot (56 MB each): build only what a session will measure and delete them afterwards
+Variant libraries are large (about 33 MB each): build only what a session will measure and delete them afterwards
 (`python tests/tools/ab_variants.py clean`). A variant that fails the parity subset is reported as such and not benchmarked."""
 import json
 import os
@@ -13,7 +13,7 @@ import sys
 ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 PKG = os.path.join(ROOT, "bepuphysics2_b200")
 VARIANTS = {
-    # name: extra -D flags. Measured and rejected so far (profiles/r02_summary.md): deep16 = -DBEPU_DEEP_MINB=16 (64 registers for deep batches: slower).
+    # name: extra -D flags, e.g. deep16 = -DBEPU_DEEP_MINB=16 (64 registers for deep batches).
 }
 PARITY = "box_stack or shape_pile or fallback or randomised or unconstrained or registered_host or deterministic"
 

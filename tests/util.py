@@ -52,7 +52,7 @@ def run_gpu(sim, dt, frames=1, strict=True, mode=0, download_prestep=True):
 def compare(a, b, exact=True, rel_rms=1e-3, max_abs=5e-2):
     """Asserts two snapshots agree: bodies (meaningful floats), accumulated impulses and prestep on valid lanes.
     exact: bit-for-bit (the strict -fmad=false build against the non-contracting oracle).
-    otherwise (FMA-contracted, approximate div/sqrt build): per quantity, relative RMS error <= rel_rms and max abs error <= max_abs."""
+    otherwise (FMA-contracted, approximate sqrt build): per quantity, relative RMS error <= rel_rms and max abs error <= max_abs."""
     def check(x, y, what):
         if exact:
             same = np.array_equal(x, y) or np.array_equal(x.view(np.uint32), y.view(np.uint32))
