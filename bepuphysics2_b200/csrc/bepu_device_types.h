@@ -63,7 +63,6 @@ struct FrameParams {
     int32_t integrate_velocity_for_kinematics;
     uint32_t exchange_base;    // peer sharding: number of cross-GPU exchange points executed before this solve (the flag barrier counts them)
     uint32_t shard_solve_index;  // peer sharding: solves since the arrival targets were last published (the arrival counters keep counting)
-    int32_t tune[4];           // development knobs (env BEPUCUDA_TUNE=a,b,c,d; 0 = built-in default), never set in production
 };
 
 enum Stage : int32_t {
@@ -92,14 +91,6 @@ struct alignas(32) WorkRecord {
     int32_t live_lanes;
 };
 
-// Stage program entry (built by bepucuda_end_constraints, walked by the host when it issues or captures a frame).
-struct StageOp {
-    int32_t stage;
-    int32_t work_begin;   // into the work item array (constraint stages) / unused
-    int32_t work_count;   // warps of work (constraint stages), bodies (final pose), kinematics (kinematic stages)
-    int32_t pad;
-};
-
 // Peer sharding (bepucuda_shard_*): where the other ranks' body arrays and flag blocks are mapped in this process.
 constexpr int kMaxShardRanks = 8;
 struct ShardPeers {
@@ -113,7 +104,7 @@ struct ShardPeers {
 // WorkRecord::live_lanes, sorted to the front of the batch) first wait until every peer's boundary bundles of all earlier exchange points have
 // arrived, and announce their own arrival to every peer (one fire-and-forget red.add over NVLink) once their peer stores are out. Interior bundles
 // neither wait nor announce, so the NVLink round trip hides behind them. A rank's flag block (u64 slots):
-//   [0, 8)  barrier flags, slot w written by rank w (shard_exchange_kernel)      [8, 12) development accumulators
+//   [0, 8)  barrier flags, slot w written by rank w (shard_barrier_kernel)
 //   [16, 24) arrival counters, slot w incremented by rank w's boundary bundles
 //   [32 + w * kShardMaxExchanges ...) rank w's arrival targets: slot e = its boundary bundles through exchange point e of one solve, cumulative;
 //                                     the last slot holds the per-solve total
@@ -126,8 +117,6 @@ constexpr int kShardTargetSlot = 32;
 constexpr int kShardMaxExchanges = 4096;
 constexpr size_t kShardFlagBlockWords = kShardTargetSlot + (size_t)kMaxShardRanks * kShardMaxExchanges;
 constexpr int32_t kRecordBoundaryBit = 1 << 30;
-// One entry per (body written by this rank in a batch, destination rank): packed as body | rank << 28 | owner << 31.
-constexpr uint32_t kPushOwnerBit = 1u << 31;
 
 struct TypeInfo {
     int32_t bodies, prestep_rows, impulse_rows, incremental;

@@ -290,59 +290,26 @@ void launch_gather_body_motion(void* raw, int body_count, const BodyBuffers& B, 
     gather_body_motion_kernel<<<blocks_for((size_t)body_count * 4, 256), 256, 0, s>>>((float4*)raw, body_count, B);
 }
 // ---- peer sharding ------------------------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void copy_record(float4* dst, const float4* src, size_t body) {
-    const float4 a = src[2 * body], b = src[2 * body + 1];
-    dst[2 * body] = a;
-    dst[2 * body + 1] = b;
-}
-// Launched with programmatic stream serialization like the stage kernels: it may start while the stage before it is still running, waits for that
-// stage to complete, and only then lets the NEXT stage's grid start its prologue (work record, body references, row prefetch), which overlaps
-// with the pushes and the barrier below.
+// Rank barrier. Launched with programmatic stream serialization like the stage kernels: it may start while the stage before it is still running,
+// waits for that stage to complete, and only then lets the NEXT stage's grid start its prologue (work record, body references, row prefetch),
+// which overlaps with the barrier below.
 __global__ void __launch_bounds__(256, 1)
-shard_exchange_kernel(const uint32_t* __restrict__ pushes, int push_count, int what, BodyBuffers B, ShardPeers peers, const FrameParams* __restrict__ fpp, uint32_t exchange_index,
-                      int32_t* error_flag) {
+shard_barrier_kernel(ShardPeers peers, const FrameParams* __restrict__ fpp, uint32_t exchange_index, int32_t* error_flag) {
     asm volatile("griddepcontrol.wait;" ::: "memory");
     asm volatile("griddepcontrol.launch_dependents;");
-    unsigned long long t0 = 0, t1 = 0, t2 = 0;
-    const bool timing = fpp->tune[3] != 0 && threadIdx.x == (peers.rank == 0 ? 1 : 0);  // development knob: phase times of the thread that talks to one peer
-    if (timing) asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t0));
-    for (int i = threadIdx.x; i < push_count; i += blockDim.x) {
-        const uint32_t e = pushes[i];
-        const size_t body = e & 0x0FFFFFFFu;
-        const int dst = (int)((e >> 28) & 7u);
-        copy_record(peers.velocity[dst], B.velocity, body);
-        if ((e & kPushOwnerBit) && what > 1) {
-            copy_record(peers.inertia_world[dst], B.inertia_world, body);
-            if (what == 3) copy_record(peers.pose[dst], B.pose, body);
-        }
-    }
-    __threadfence_system();  // every thread's peer stores before the signal below
-    __syncthreads();
-    if (timing) asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t1));
     const unsigned long long seq = (unsigned long long)fpp->exchange_base + exchange_index + 1ull;
     const int p = threadIdx.x;
     if (p < peers.rank_count && p != peers.rank) {
         asm volatile("st.release.sys.global.u64 [%0], %1;" ::"l"(peers.flags[p] + peers.rank), "l"(seq) : "memory");
-        if (timing) asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t2));
         unsigned long long seen;
         unsigned int spins = 0;
         do {
             asm volatile("ld.acquire.sys.global.u64 %0, [%1];" : "=l"(seen) : "l"(peers.flags[peers.rank] + p) : "memory");
         } while (seen < seq && ++spins < 200000000u);
         if (seen < seq) atomicExch(error_flag, 5);  // a peer never arrived: results are void
-        if (timing) {
-            unsigned long long t3;
-            asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t3));
-            unsigned long long* acc = peers.flags[peers.rank] + kMaxShardRanks;  // four accumulators behind the flag slots: push, signal, wait (ns), count
-            acc[0] += t1 - t0;
-            acc[1] += t2 - t1;
-            acc[2] += t3 - t2;
-            acc[3] += 1;
-        }
     }
 }
-void launch_shard_exchange(const uint32_t* pushes, int push_count, int what, const BodyBuffers& B, const ShardPeers& peers, const FrameParams* fp, uint32_t exchange_index,
-                           int32_t* error_flag, cudaStream_t s) {
+void launch_shard_barrier(const ShardPeers& peers, const FrameParams* fp, uint32_t exchange_index, int32_t* error_flag, cudaStream_t s) {
     cudaLaunchConfig_t cfg{};
     cfg.gridDim = dim3(1);
     cfg.blockDim = dim3(256);
@@ -352,7 +319,7 @@ void launch_shard_exchange(const uint32_t* pushes, int push_count, int what, con
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
     cfg.numAttrs = 1;
-    cudaLaunchKernelEx(&cfg, shard_exchange_kernel, pushes, push_count, what, B, peers, fp, exchange_index, error_flag);
+    cudaLaunchKernelEx(&cfg, shard_barrier_kernel, peers, fp, exchange_index, error_flag);
 }
 __global__ void fill_peer_masks_kernel(const int32_t* __restrict__ refs, uint32_t* __restrict__ peer_masks, size_t count, const uint8_t* __restrict__ body_masks, int rank) {
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -409,101 +376,6 @@ void launch_ownership_rest(const DeviceTypeBatch* tbs, const WorkItem* work, int
     }
     if (body_count > 0) check_invariant_kernel<<<blocks_for(body_count, 256), 256, 0, s>>>(body_count, sync_refcount, sync_mask, error_flag);
     if (kinematic_count > 0) mark_kinematics_kernel<<<blocks_for(kinematic_count, 128), 128, 0, s>>>(kinematics, kinematic_count, body_count, constrained, error_flag);
-}
-
-// ---- sharded batches: exchange of the body records one rank wrote in a stage (see bepucuda_set_boundary_bodies) --------------------------------
-// staging = three planes of 8 words per body: velocity | world inertia | pose. A written record carries 1 in a padding word (velocity word 3,
-// inertia / pose word 7); everything else is zero, so an integer sum over ranks reproduces the one writer's bits.
-__global__ void collect_stage_kernel(const DeviceTypeBatch* __restrict__ tbs, const WorkItem* __restrict__ work, int work_count, const int32_t* __restrict__ bodies_per_type,
-                                     int stage, BodyBuffers B, int32_t* staging) {
-    const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-    if (warp >= work_count) return;
-    const WorkItem w = work[warp];
-    const DeviceTypeBatch tb = tbs[w.type_batch];
-    const int nb = bodies_per_type[tb.type_id];
-    const size_t n = (size_t)B.count;
-    for (int s = 0; s < nb; ++s) {
-        const int32_t enc = tb.refs[((size_t)w.bundle * nb + s) * 32 + lane];
-        if (enc < 0 || (enc & kRefKinematicBit)) continue;
-        const size_t idx = (size_t)(enc & kRefIndexMask);
-        int4* out = reinterpret_cast<int4*>(staging);
-        const int4* vel = reinterpret_cast<const int4*>(B.velocity) + 2 * idx;
-        int4 lo = vel[0], hi = vel[1];
-        lo.w = 1;
-        hi.w = 0;
-        out[2 * idx] = lo;
-        out[2 * idx + 1] = hi;
-        if (stage != kStageSolve && ((uint32_t)enc & kRefIntegrateBit)) {
-            const int4* in = reinterpret_cast<const int4*>(B.inertia_world) + 2 * idx;
-            lo = in[0];
-            hi = in[1];
-            hi.w = 1;
-            out[2 * (n + idx)] = lo;
-            out[2 * (n + idx) + 1] = hi;
-            if (stage == kStageWarmStart) {
-                const int4* po = reinterpret_cast<const int4*>(B.pose) + 2 * idx;
-                lo = po[0];
-                hi = po[1];
-                hi.w = 1;
-                out[2 * (2 * n + idx)] = lo;
-                out[2 * (2 * n + idx) + 1] = hi;
-            }
-        }
-    }
-}
-__global__ void apply_stage_kernel(const int32_t* __restrict__ staging, int planes, BodyBuffers B) {
-    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    const size_t n = (size_t)B.count;
-    if (i >= n) return;
-    const int4* in = reinterpret_cast<const int4*>(staging);
-    int4 lo = in[2 * i], hi = in[2 * i + 1];
-    if (lo.w != 0) {
-        lo.w = 0;
-        int4* vel = reinterpret_cast<int4*>(B.velocity) + 2 * i;
-        vel[0] = lo;
-        vel[1] = hi;
-    }
-    if (planes >= 2) {
-        lo = in[2 * (n + i)];
-        hi = in[2 * (n + i) + 1];
-        if (hi.w != 0) {
-            hi.w = 0;
-            int4* iw = reinterpret_cast<int4*>(B.inertia_world) + 2 * i;
-            iw[0] = lo;
-            iw[1] = hi;
-        }
-    }
-    if (planes >= 3) {
-        lo = in[2 * (2 * n + i)];
-        hi = in[2 * (2 * n + i) + 1];
-        if (hi.w != 0) {
-            hi.w = 0;
-            int4* po = reinterpret_cast<int4*>(B.pose) + 2 * i;
-            po[0] = lo;
-            po[1] = hi;
-        }
-    }
-}
-__global__ void widen_u8_kernel(const uint8_t* __restrict__ in, int32_t* out, size_t n) {
-    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) out[i] = in[i] ? 1 : 0;
-}
-__global__ void narrow_i32_kernel(const int32_t* __restrict__ in, uint8_t* out, size_t n) {
-    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) out[i] = in[i] != 0 ? 1 : 0;
-}
-void launch_collect_stage(const DeviceTypeBatch* tbs, const WorkItem* work, int work_count, const int32_t* bodies_per_type, int stage, const BodyBuffers& B, int32_t* staging,
-                          cudaStream_t s) {
-    if (work_count > 0) collect_stage_kernel<<<blocks_for((size_t)work_count * 32, 128), 128, 0, s>>>(tbs, work, work_count, bodies_per_type, stage, B, staging);
-}
-void launch_apply_stage(const int32_t* staging, int planes, const BodyBuffers& B, cudaStream_t s) {
-    if (B.count > 0) apply_stage_kernel<<<blocks_for((size_t)B.count, 256), 256, 0, s>>>(staging, planes, B);
-}
-void launch_widen_u8(const uint8_t* in, int32_t* out, size_t n, cudaStream_t s) {
-    if (n) widen_u8_kernel<<<blocks_for(n, 256), 256, 0, s>>>(in, out, n);
-}
-void launch_narrow_i32(const int32_t* in, uint8_t* out, size_t n, cudaStream_t s) {
-    if (n) narrow_i32_kernel<<<blocks_for(n, 256), 256, 0, s>>>(in, out, n);
 }
 
 }  // namespace bepucuda

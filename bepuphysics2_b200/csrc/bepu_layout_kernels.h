@@ -41,20 +41,11 @@ void launch_ownership_pass1(const DeviceTypeBatch* tbs, const WorkItem* work, in
 void launch_ownership_rest(const DeviceTypeBatch* tbs, const WorkItem* work, int work_count, const int32_t* bodies_per_type, int body_count, const int32_t* first_batch,
                            const int32_t* sync_refcount, const unsigned long long* sync_mask, uint8_t* constrained, const int32_t* kinematics, int kinematic_count,
                            int32_t* error_flag, const TransposeDesc* descs, int W, int32_t* source_bundle_flags, cudaStream_t s);
-// Sharded batches (bepucuda_set_boundary_bodies): pack the body records a stage wrote / write back every valid record / mask conversions.
-void launch_collect_stage(const DeviceTypeBatch* tbs, const WorkItem* work, int work_count, const int32_t* bodies_per_type, int stage, const BodyBuffers& B, int32_t* staging,
-                          cudaStream_t s);
-void launch_apply_stage(const int32_t* staging, int planes, const BodyBuffers& B, cudaStream_t s);
-void launch_widen_u8(const uint8_t* in, int32_t* out, size_t n, cudaStream_t s);
-void launch_narrow_i32(const int32_t* in, uint8_t* out, size_t n, cudaStream_t s);
+// Peer sharding, rank barrier: one CTA signals every peer and waits for every peer's signal of the same exchange point (flag barrier in peer
+// memory). Sets *error_flag to 5 when a peer does not arrive before the timeout.
+void launch_shard_barrier(const ShardPeers& peers, const FrameParams* fp, uint32_t exchange_index, int32_t* error_flag, cudaStream_t s);
 
-// Peer sharding: one CTA copies the records this rank's stage wrote for shared bodies into the destination ranks' arrays, then signals every peer
-// and waits for every peer's signal of the same exchange point (flag barrier in peer memory). what: 1 = velocity only (Solve),
-// 3 = + pose and world inertia of integrating entries (WarmStart), 2 = + world inertia only (first substep: poses are not integrated).
-void launch_shard_exchange(const uint32_t* pushes, int push_count, int what, const BodyBuffers& B, const ShardPeers& peers, const FrameParams* fp, uint32_t exchange_index,
-                           int32_t* error_flag, cudaStream_t s);
-
-// Peer sharding, fused pushes: peer_masks[i] = ranks other than `rank` that reference the dynamic body of device reference refs[i] (0 for empty and
+// Peer sharding: peer_masks[i] = ranks other than `rank` that reference the dynamic body of device reference refs[i] (0 for empty and
 // kinematic slots); body_masks[b] has bit r set when rank r references body b.
 void launch_fill_peer_masks(const int32_t* refs, uint32_t* peer_masks, size_t count, const uint8_t* body_masks, int rank, cudaStream_t s);
 // flags[i] = 1 when any lane of work record i has a non-empty destination mask (a "boundary" bundle, see ShardStage).

@@ -393,7 +393,7 @@ BEPU_DI void constraint_stage_body(const WorkRecord* __restrict__ records, const
     if constexpr (kSharded) {
         boundary = active && (rec.live_lanes & kRecordBoundaryBit) != 0;
         // records other ranks pushed in the previous exchange point are read below: all of them must have arrived
-        if (boundary && shard->exchange_index > 0 && !(fp.tune[0] & 1)) shard_wait(*peers, lane, fp.shard_solve_index, shard->exchange_index - 1u, shard->error_flag);
+        if (boundary && shard->exchange_index > 0) shard_wait(*peers, lane, fp.shard_solve_index, shard->exchange_index - 1u, shard->error_flag);
     }
     if (!active) return;
     if constexpr (kStaged) {
@@ -405,9 +405,9 @@ BEPU_DI void constraint_stage_body(const WorkRecord* __restrict__ records, const
         }
         __syncwarp();
         run_bundle_rows<STAGE, kSharded>(rec, lane, StagedRows{slab_addr + lane * 4, bar, 0u}, StagedAcc{slab_addr + prestep_bytes + lane * 4, rec.impulses + lane}, enc0, enc1, B, fp,
-                                         peers, boundary && !(fp.tune[0] & 4) ? peer_delta : 0);
+                                         peers, boundary ? peer_delta : 0);
         if constexpr (kSharded) {
-            if (boundary && !(fp.tune[0] & 2)) {  // (tune[0]: development knob for A/B timing -- 1 no waits, 2 no announcements, 4 no peer stores; results are void)
+            if (boundary) {
                 __syncwarp();                  // every lane's peer stores are ordered before ...
                 shard_announce(*peers, lane);  // ... the release that counts the warp as arrived
             }

@@ -2,10 +2,7 @@
 // C ABI declared in include/bepucuda.h. No CPU fallback lives here: without a usable CUDA device bepucuda_create fails.
 #include <algorithm>
 #include <cmath>
-#include <cstdio>
-#include <cstdlib>
 #include <cstring>
-#include <map>
 #include <string>
 #include <vector>
 
@@ -137,11 +134,20 @@ struct SourceTypeBatch {
     bool resident_impulses = false, redistribute = false;
 };
 
+// Stage program entry (built by build_program, walked by the host when it issues or captures a frame).
+struct StageOp {
+    int32_t stage;
+    int32_t work_begin;   // into the work item array (constraint stages) / unused
+    int32_t work_count;   // warps of work (constraint stages), bodies (final pose), kinematics (kinematic stages)
+    int32_t exchange;     // peer sharding: kRankBarrier, the device batch of a sharded WarmStart / Solve stage, or kNoExchange
+};
+// Rank barriers and sharded stages are the exchange points of a solve, numbered in program order (FrameParams::exchange_base, ShardStage).
+constexpr int32_t kNoExchange = -1, kRankBarrier = -2;
+
 }  // namespace bepucuda
 
 struct bepucuda_ctx {
     bepucuda_config cfg{};
-    int32_t tune[4] = {0, 0, 0, 0};
     int device = 0;
     cudaStream_t stream = nullptr;
     cudaEvent_t ev_solve_begin = nullptr, ev_solve_end = nullptr, ev_up_begin = nullptr, ev_up_end = nullptr, ev_down_begin = nullptr, ev_down_end = nullptr;
@@ -166,30 +172,24 @@ struct bepucuda_ctx {
     bool constraints_open = false, constraints_ready = false, data_dirty = false, descs_dirty = false;
     std::vector<SourceTypeBatch> sources;
     ChunkArena raw_arena, pinned_arena;
-    DeviceBuffer record_table, ref_rows, source_bundle_flags, refs32, prestep32, impulses32, tb_table, tdesc_table, work_table, map_table, bodies_per_type, kinematics_dev, program_dev, frame_params_dev, error_dev;
+    DeviceBuffer record_table, ref_rows, source_bundle_flags, refs32, prestep32, impulses32, tb_table, tdesc_table, work_table, map_table, bodies_per_type, kinematics_dev, frame_params_dev, error_dev;
     std::vector<DeviceTypeBatch> tbs;
     std::vector<TransposeDesc> tdescs;
     std::vector<WorkItem> work;                 // grouped by device batch, then the incremental list
     std::vector<int32_t> bundle_live;           // live constraints per work item (parallel to `work`)
     std::vector<WorkRecord> records;            // what the solver kernels read (parallel to `work`)
     std::vector<std::pair<int, int>> batch_work; // per device batch: (begin, count) into work
-    bool exchange_failed = false;
-    bepucuda_exchange_fn exchange = nullptr;    // sharded batches (bepucuda_set_boundary_bodies): all-reduce callback, its user pointer, staging planes
-    void* exchange_user = nullptr;
-    DeviceBuffer exchange_staging;
-    // peer sharding (bepucuda_shard_*): one constraint graph over several GPUs with NVLink peer stores and a flag barrier per stage
+    // peer sharding (bepucuda_shard_*): one constraint graph over several GPUs with NVLink peer stores from the stage kernels
     bool peer_mode = false;
     ShardPeers peers{};
-    DeviceBuffer shard_flags, pushes_dev, peer32, body_masks_dev, boundary_flags_dev;
+    DeviceBuffer shard_flags, peer32, body_masks_dev, boundary_flags_dev;
     uint32_t shard_solve_index = 0;                                 // solves since the arrival targets were last published
     std::vector<int> boundary_count;                                // per device batch: bundles that touch a body another rank references
-    std::vector<uint8_t> body_masks;                                // bepucuda_shard_set_body_masks: fused pushes from the stage kernels
+    std::vector<uint8_t> body_masks;                                // bepucuda_shard_set_body_masks: per body, the ranks that reference it
     size_t refs_words = 0;
     std::vector<void*> opened_ipc;
     std::vector<int32_t> global_first_batch;
     std::vector<uint8_t> global_constrained;
-    std::map<int, std::vector<uint32_t>> pushes_by_batch;          // host batch index -> packed (body | rank << 28 | owner << 31)
-    std::vector<std::pair<size_t, int>> push_range;                // per device batch: (offset, count) into pushes_dev
     uint32_t exchange_counter = 0;                                  // exchange points executed so far (flag barrier sequence)
     uint32_t exchanges_per_solve = 0;
     int inc_work_begin = 0, inc_work_count = 0;
@@ -321,42 +321,30 @@ void issue_stage_sequence(bepucuda_ctx* ctx, cudaStream_t s, int64_t* launches) 
     // batch's prestep rows (the incremental contact update does) nor its impulses (a stage of the same batch does: single-batch scenes).
     const StageOp* previous = nullptr;  // last launched op
     uint32_t exchange_index = 0;
-    const bool fused_pushes = ctx->peer_mode && !ctx->body_masks.empty();
     for (const StageOp& op : ctx->program) {
-        if (ctx->peer_mode && op.pad == -1) {
-            // all ranks meet (nothing to push): before the first stage of a solve; around the incremental contact update, which reads the velocities
-            // of shared bodies -- after every peer's last Solve stage has completed, before any peer's WarmStart stage stores into this rank's
-            // arrays; and before the final pose pass
-            launch_shard_exchange(nullptr, 0, 1, ctx->B, ctx->peers, fp, exchange_index++, ctx->error_dev.as<int32_t>(), s);
+        if (op.exchange == kRankBarrier) {
+            // all ranks meet: before the first stage of a solve; around the incremental contact update, which reads the velocities of shared
+            // bodies -- after every peer's last Solve stage has completed, before any peer's WarmStart stage stores into this rank's arrays; and
+            // before the final pose pass
+            launch_shard_barrier(ctx->peers, fp, exchange_index++, ctx->error_dev.as<int32_t>(), s);
             ++n;
             continue;
         }
-        if (ctx->peer_mode && op.pad >= 2 && op.stage <= kStageSolve) {
-            // peer sharding: the stage on this rank's constraints of the batch, then records written for shared bodies go to the ranks that
-            // reference them and all ranks meet at the flag barrier
+        if (op.exchange != kNoExchange) {
+            // sharded stage: it stores the records it writes for shared bodies into the ranks that reference them, and its boundary bundles wait
+            // for and announce arrivals themselves (ShardStage). A batch without constraints on this rank still counts as an exchange point:
+            // nothing arrives from this rank there, and its arrival targets say so.
             if (op.work_count > 0) {
-                // row prefetch in the prologue: the exchange kernel between two stages writes no rows, so the rule of the single-GPU sequence applies
+                // row prefetch in the prologue: a rank barrier between two stages writes no rows, so the rule of the single-GPU sequence applies
                 bool prefetch = previous != nullptr && previous->stage != kStageIncremental && !(previous->stage <= kStageSolve && previous->work_begin == op.work_begin && previous->work_count > 0);
                 const int launch_flags = (pdl ? kLaunchPdl : 0) | (prefetch ? kLaunchPrefetchRows : 0);
-                if (fused_pushes) {
-                    // the stage pushes, signals and (in its boundary bundles) waits itself: no exchange kernel
-                    const ShardStage shard{exchange_index, ctx->error_dev.as<int32_t>()};
-                    ctx->launchers->constraint_stage_sharded(op.stage, records + op.work_begin, ref_rows + (size_t)op.work_begin * 64, op.work_count, ctx->B, fp, launch_flags, ctx->peers,
-                                                             (long long)(ctx->peer32.as<int32_t>() - ctx->refs32.as<int32_t>()), shard, s);
-                    ++exchange_index;
-                    ++n;
-                    previous = &op;
-                    continue;
-                }
-                ctx->launchers->constraint_stage(op.stage, records + op.work_begin, ref_rows + (size_t)op.work_begin * 64, op.work_count, ctx->B, fp, launch_flags, s);
+                const ShardStage shard{exchange_index, ctx->error_dev.as<int32_t>()};
+                ctx->launchers->constraint_stage_sharded(op.stage, records + op.work_begin, ref_rows + (size_t)op.work_begin * 64, op.work_count, ctx->B, fp, launch_flags, ctx->peers,
+                                                         (long long)(ctx->peer32.as<int32_t>() - ctx->refs32.as<int32_t>()), shard, s);
                 ++n;
+                previous = &op;
             }
-            if (fused_pushes) { ++exchange_index; continue; }  // no constraint of this batch here: nothing arrives from this rank, its targets say so
-            const auto& range = ctx->push_range[op.pad - 2];
-            launch_shard_exchange(ctx->pushes_dev.as<uint32_t>() + range.first, range.second, op.stage == kStageSolve ? 1 : (op.stage == kStageWarmStart ? 3 : 2), ctx->B, ctx->peers, fp,
-                                  exchange_index++, ctx->error_dev.as<int32_t>(), s);
-            ++n;
-            if (op.work_count > 0) previous = &op;
+            ++exchange_index;
             continue;
         }
         switch (op.stage) {
@@ -364,23 +352,6 @@ void issue_stage_sequence(bepucuda_ctx* ctx, cudaStream_t s, int64_t* launches) 
                 if (op.work_count > 0) {
                     bool prefetch = op.stage != kStageIncremental && previous != nullptr && previous->stage != kStageIncremental;
                     if (prefetch && previous->stage <= kStageSolve && previous->work_begin == op.work_begin) prefetch = false;
-                    if (ctx->exchange) {
-                        // sharded batches: plain launches, then all ranks learn what this rank's constraints wrote in this stage
-                        ctx->launchers->constraint_stage(op.stage, records + op.work_begin, ref_rows + (size_t)op.work_begin * 64, op.work_count, ctx->B, fp, 0, s);
-                        ++n;
-                        if (op.stage != kStageIncremental) {
-                            const int planes = op.stage == kStageSolve ? 1 : (op.stage == kStageWarmStart ? 3 : 2);
-                            const size_t words = (size_t)ctx->body_count * 8 * planes;
-                            cudaMemsetAsync(ctx->exchange_staging.ptr, 0, words * 4, s);
-                            launch_collect_stage(ctx->tb_table.as<DeviceTypeBatch>(), ctx->work_table.as<WorkItem>() + op.work_begin, op.work_count, ctx->bodies_per_type.as<int32_t>(), op.stage,
-                                                 ctx->B, ctx->exchange_staging.as<int32_t>(), s);
-                            if (ctx->exchange(ctx->exchange_user, ctx->exchange_staging.ptr, (int64_t)words, 0, (void*)s) != 0) ctx->exchange_failed = true;
-                            launch_apply_stage(ctx->exchange_staging.as<int32_t>(), planes, ctx->B, s);
-                            n += 2;
-                        }
-                        previous = &op;
-                        break;
-                    }
                     ctx->launchers->constraint_stage(op.stage, records + op.work_begin, ref_rows + (size_t)op.work_begin * 64, op.work_count, ctx->B, fp, (pdl ? kLaunchPdl : 0) | (prefetch ? kLaunchPrefetchRows : 0), s);
                     previous = &op;
                     ++n;
@@ -403,43 +374,44 @@ void build_program(bepucuda_ctx* ctx) {
     ctx->program.clear();
     const int substeps = (int)ctx->iterations.size();
     const int kin = (int)ctx->kinematics.size();
+    const StageOp rank_barrier{kStageKinematic, 0, 0, kRankBarrier};
     for (int s = 0; s < substeps; ++s) {
         if (s > 0) {
-            // peer sharding: what peers pushed in the last Solve stages must have arrived before the contact update reads velocities (rank barrier)
-            if (ctx->peer_mode) ctx->program.push_back({kStageKinematic, 0, 0, -1});
-            if (ctx->inc_work_count > 0) ctx->program.push_back({kStageIncremental, ctx->inc_work_begin, ctx->inc_work_count, 0});
-            if (kin > 0) ctx->program.push_back({kStageKinematic, 0, kin, 0});
+            // peer sharding: what peers pushed in the last Solve stages must have arrived before the contact update reads velocities
+            if (ctx->peer_mode) ctx->program.push_back(rank_barrier);
+            if (ctx->inc_work_count > 0) ctx->program.push_back({kStageIncremental, ctx->inc_work_begin, ctx->inc_work_count, kNoExchange});
+            if (kin > 0) ctx->program.push_back({kStageKinematic, 0, kin, kNoExchange});
         } else if (ctx->integ.integrate_velocity_for_kinematics && kin > 0) {
-            ctx->program.push_back({kStageKinematicFirst, 0, kin, 0});
+            ctx->program.push_back({kStageKinematicFirst, 0, kin, kNoExchange});
         }
-        if (ctx->peer_mode) ctx->program.push_back({kStageKinematic, 0, 0, -1});  // rank barrier (see issue_stage_sequence)
-        // pad carries the device batch index + 2 in peer mode (every rank runs the exchange of every batch, also of one it has no constraint in)
+        if (ctx->peer_mode) ctx->program.push_back(rank_barrier);  // see issue_stage_sequence
+        // in peer mode every rank runs the exchange point of every batch, also of one it has no constraint in
         for (size_t b = 0; b < ctx->batch_work.size(); ++b) {
             auto& bw = ctx->batch_work[b];
-            if (bw.second > 0 || (ctx->peer_mode && (int)b < ctx->sync_batch_count)) ctx->program.push_back({s == 0 ? kStageWarmStartFirst : kStageWarmStart, bw.first, bw.second, ctx->peer_mode ? (int)b + 2 : 0});
+            if (bw.second > 0 || (ctx->peer_mode && (int)b < ctx->sync_batch_count)) ctx->program.push_back({s == 0 ? kStageWarmStartFirst : kStageWarmStart, bw.first, bw.second, ctx->peer_mode ? (int)b : kNoExchange});
         }
         for (int it = 0; it < ctx->iterations[s]; ++it)
             for (size_t b = 0; b < ctx->batch_work.size(); ++b) {
                 auto& bw = ctx->batch_work[b];
-                if (bw.second > 0 || (ctx->peer_mode && (int)b < ctx->sync_batch_count)) ctx->program.push_back({kStageSolve, bw.first, bw.second, ctx->peer_mode ? (int)b + 2 : 0});
+                if (bw.second > 0 || (ctx->peer_mode && (int)b < ctx->sync_batch_count)) ctx->program.push_back({kStageSolve, bw.first, bw.second, ctx->peer_mode ? (int)b : kNoExchange});
             }
     }
-    if (ctx->peer_mode) ctx->program.push_back({kStageKinematic, 0, 0, -1});  // ... and before the final pose pass reads them
-    ctx->program.push_back({kStageFinalPose, 0, ctx->body_count, 0});
+    if (ctx->peer_mode) ctx->program.push_back(rank_barrier);  // ... and before the final pose pass reads them
+    ctx->program.push_back({kStageFinalPose, 0, ctx->body_count, kNoExchange});
 }
 
 int upload_program(bepucuda_ctx* ctx) {
     build_program(ctx);
-    if (ctx->peer_mode && !ctx->body_masks.empty() && ctx->boundary_count.size() == ctx->batch_work.size()) {
-        // fused pushes: publish, to every peer, how many boundary bundles of this rank arrive through each exchange point of one solve (ShardStage),
-        // and restart the arrival counters other ranks increment here. Every rank does this for the same program, between solves.
+    if (ctx->peer_mode) {
+        // publish, to every peer, how many boundary bundles of this rank arrive through each exchange point of one solve (ShardStage), and restart
+        // the arrival counters other ranks increment here. Every rank does this for the same program, between solves.
         std::vector<unsigned long long> targets((size_t)kShardMaxExchanges, 0ull);
         unsigned long long arrived = 0;
         size_t e = 0;
         for (const StageOp& op : ctx->program) {
-            if (op.pad != -1 && !(op.pad >= 2 && op.stage <= kStageSolve)) continue;
+            if (op.exchange == kNoExchange) continue;
             if (e + 1 >= (size_t)kShardMaxExchanges) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, "peer sharding: more than 4095 exchange points per solve");
-            if (op.pad >= 2 && op.work_count > 0) arrived += (unsigned long long)ctx->boundary_count[(size_t)(op.pad - 2)];
+            if (op.exchange >= 0 && op.work_count > 0) arrived += (unsigned long long)ctx->boundary_count[(size_t)op.exchange];
             targets[e++] = arrived;
         }
         targets[(size_t)kShardMaxExchanges - 1] = arrived;
@@ -450,9 +422,7 @@ int upload_program(bepucuda_ctx* ctx) {
         CK(cudaMemset((unsigned long long*)ctx->shard_flags.ptr + kShardCounterSlot, 0, kMaxShardRanks * 8));
         ctx->shard_solve_index = 0;
     }
-    CK(ctx->program_dev.reserve(ctx->program.size() * sizeof(StageOp)));
-    CK(cudaMemcpyAsync(ctx->program_dev.ptr, ctx->program.data(), ctx->program.size() * sizeof(StageOp), cudaMemcpyHostToDevice, ctx->stream));
-    // The copy source is a std::vector: make sure the DMA read it before anyone mutates it.
+    // work issued under the previous program completes before that program and its graph are replaced
     CK(cudaStreamSynchronize(ctx->stream));
     invalidate_graph(ctx);
     // stage statistics
@@ -482,7 +452,6 @@ void compute_frame_params(bepucuda_ctx* ctx, float dt, FrameParams* fp) {
     fp->final_steps = d.allow_substeps_for_unconstrained ? substeps : 1;
     fp->angular_mode = d.angular_integration_mode;
     fp->integrate_velocity_for_kinematics = d.integrate_velocity_for_kinematics;
-    for (int i = 0; i < 4; ++i) fp->tune[i] = ctx->tune[i];
 }
 
 // Brings the device AOSOA-32 rows up to date with what the host queued since the last solve (bepucuda_update_type_batch / bepucuda_update_contacts):
@@ -543,7 +512,6 @@ int32_t bepucuda_create(const bepucuda_config* cfg, bepucuda_ctx** out) {
     if (cfg->execution_mode != BEPUCUDA_EXEC_GRAPH && cfg->execution_mode != BEPUCUDA_EXEC_STREAM) return BEPUCUDA_ERR_INVALID_ARGUMENT;  // 1 and 3 are retired modes
     bepucuda_ctx* ctx = new bepucuda_ctx();
     ctx->cfg = *cfg;
-    if (const char* tune = getenv("BEPUCUDA_TUNE")) sscanf(tune, "%d,%d,%d,%d", &ctx->tune[0], &ctx->tune[1], &ctx->tune[2], &ctx->tune[3]);
     ctx->device = cfg->device_ordinal;
     ctx->launchers = cfg->strict_fp ? get_launchers_bepu_strict() : get_launchers_bepu_fast();
     ctx->pinned_arena.pinned_host = true;
@@ -574,9 +542,9 @@ int32_t bepucuda_destroy(bepucuda_ctx* ctx) {
     if (ctx->stream) cudaStreamSynchronize(ctx->stream);
     invalidate_graph(ctx);
     for (void* p : ctx->opened_ipc) cudaIpcCloseMemHandle(p);
-    DeviceBuffer* bufs[] = {&ctx->shard_flags, &ctx->pushes_dev, &ctx->peer32, &ctx->body_masks_dev, &ctx->boundary_flags_dev, &ctx->raw_bodies, &ctx->pose, &ctx->velocity, &ctx->inertia_local, &ctx->inertia_world, &ctx->constrained, &ctx->first_batch, &ctx->sync_refcount,
+    DeviceBuffer* bufs[] = {&ctx->shard_flags, &ctx->peer32, &ctx->body_masks_dev, &ctx->boundary_flags_dev, &ctx->raw_bodies, &ctx->pose, &ctx->velocity, &ctx->inertia_local, &ctx->inertia_world, &ctx->constrained, &ctx->first_batch, &ctx->sync_refcount,
                             &ctx->sync_mask, &ctx->chunk_table, &ctx->record_table, &ctx->ref_rows, &ctx->body_shapes, &ctx->body_activities, &ctx->body_bounds, &ctx->color_refs, &ctx->color_priorities, &ctx->color_body_min, &ctx->color_body_mask, &ctx->color_out, &ctx->color_lists, &ctx->color_counts, &ctx->source_bundle_flags, &ctx->refs32, &ctx->prestep32, &ctx->impulses32, &ctx->tb_table, &ctx->tdesc_table, &ctx->work_table, &ctx->map_table,
-                            &ctx->bodies_per_type, &ctx->kinematics_dev, &ctx->program_dev, &ctx->frame_params_dev, &ctx->error_dev, &ctx->exchange_staging};
+                            &ctx->bodies_per_type, &ctx->kinematics_dev, &ctx->frame_params_dev, &ctx->error_dev};
     for (auto b : bufs) b->release();
     ctx->raw_arena.release();
     ctx->pinned_arena.release();
@@ -747,6 +715,8 @@ int32_t bepucuda_set_constrained_kinematics(bepucuda_ctx* ctx, const int32_t* bo
 int32_t bepucuda_end_constraints(bepucuda_ctx* ctx) {
     if (!ctx) return BEPUCUDA_ERR_INVALID_ARGUMENT;
     if (!ctx->constraints_open) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, "end_constraints without begin_constraints");
+    if (ctx->peer_mode && (int)ctx->body_masks.size() != ctx->body_count)
+        return fail(ctx, BEPUCUDA_ERR_BAD_STATE, "end_constraints: peer sharding needs bepucuda_shard_set_body_masks for the current body count");
     CK(cudaSetDevice(ctx->device));
     const int W = ctx->W;
     std::stable_sort(ctx->sources.begin(), ctx->sources.end(), [](const SourceTypeBatch& a, const SourceTypeBatch& b) {
@@ -793,16 +763,10 @@ int32_t bepucuda_end_constraints(bepucuda_ctx* ctx) {
             constraint_count += s.count;
         }
         if (ctx->peer_mode) {
-            // every rank runs the exchange of every batch, also of batches it has no constraint in
+            // every rank runs the exchange point of every batch, also of batches it has no constraint in
             while ((int)batch_tbs.size() < std::min(ctx->batch_count, ctx->fallback_threshold)) batch_tbs.emplace_back();
             for (const SourceTypeBatch& src : ctx->sources)
                 if (src.batch_index >= ctx->fallback_threshold) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, "end_constraints: the sequential fallback batch is not supported across ranks");
-        }
-        if (ctx->exchange && !ctx->peer_mode) {
-            // sharded batches through the exchange callback: levels computed from one rank's constraints differ between ranks, so would the number of
-            // collectives per step (a hang), and level indices are not comparable across ranks
-            for (const SourceTypeBatch& src : ctx->sources)
-                if (src.batch_index >= ctx->fallback_threshold) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, "end_constraints: the sequential fallback batch is not supported with an exchange callback");
         }
         (void)current_batch;
         ctx->sync_batch_count = (int)batch_tbs.size();
@@ -1001,40 +965,14 @@ int32_t bepucuda_end_constraints(bepucuda_ctx* ctx) {
         if ((int)ctx->global_first_batch.size() != ctx->body_count) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, "end_constraints: bepucuda_shard_set_global was not called for this body count");
         CK(cudaMemcpyAsync(ctx->first_batch.ptr, ctx->global_first_batch.data(), (size_t)ctx->body_count * 4, cudaMemcpyHostToDevice, ctx->stream));
     }
-    if (ctx->exchange && !ctx->peer_mode && nb > 0) {
-        // sharded batches: the integration owner of a body is the lowest batch referencing it on ANY rank
-        if (ctx->exchange(ctx->exchange_user, ctx->first_batch.ptr, (int64_t)ctx->body_count, 1, (void*)ctx->stream) != 0)
-            return fail(ctx, BEPUCUDA_ERR_CUDA, "end_constraints: the exchange callback failed (first-batch minimum)");
-    }
     launch_ownership_rest(ctx->tb_table.as<DeviceTypeBatch>(), ctx->work_table.as<WorkItem>(), ctx->all_work_count, ctx->bodies_per_type.as<int32_t>(), ctx->body_count,
                           ctx->first_batch.as<int32_t>(), ctx->sync_refcount.as<int32_t>(), (const unsigned long long*)ctx->sync_mask.ptr, ctx->constrained.as<uint8_t>(),
                           ctx->kinematics_dev.as<int32_t>(), (int)ctx->kinematics.size(), ctx->error_dev.as<int32_t>(), ctx->tdesc_table.as<TransposeDesc>(), W,
                           ctx->source_bundle_flags.as<int32_t>(), ctx->stream);
-    if (ctx->peer_mode && nb > 0) {
-        CK(cudaMemcpyAsync(ctx->constrained.ptr, ctx->global_constrained.data(), (size_t)ctx->body_count, cudaMemcpyHostToDevice, ctx->stream));
-        // the (body, destination rank) lists of every batch, back to back
-        std::vector<uint32_t> all;
-        ctx->push_range.assign(ctx->sync_batch_count, {0, 0});
-        for (int b = 0; b < ctx->sync_batch_count; ++b) {
-            auto it = ctx->pushes_by_batch.find(b);
-            if (it == ctx->pushes_by_batch.end()) continue;
-            ctx->push_range[b] = {all.size(), (int)it->second.size()};
-            all.insert(all.end(), it->second.begin(), it->second.end());
-        }
-        CK(ctx->pushes_dev.reserve(all.size() * 4 + 16));
-        if (!all.empty()) CK(cudaMemcpy(ctx->pushes_dev.ptr, all.data(), all.size() * 4, cudaMemcpyHostToDevice));
-    }
-    if (ctx->exchange && !ctx->peer_mode && nb > 0) {
+    if (ctx->peer_mode) {
         // ... and a body is "constrained" (final pose pass) if any rank constrains it
-        CK(ctx->exchange_staging.reserve((size_t)nb * 24 * 4));
-        launch_widen_u8(ctx->constrained.as<uint8_t>(), ctx->exchange_staging.as<int32_t>(), (size_t)ctx->body_count, ctx->stream);
-        if (ctx->exchange(ctx->exchange_user, ctx->exchange_staging.ptr, (int64_t)ctx->body_count, 0, (void*)ctx->stream) != 0)
-            return fail(ctx, BEPUCUDA_ERR_CUDA, "end_constraints: the exchange callback failed (constrained mask)");
-        launch_narrow_i32(ctx->exchange_staging.as<int32_t>(), ctx->constrained.as<uint8_t>(), (size_t)ctx->body_count, ctx->stream);
-    }
-    if (ctx->peer_mode && !ctx->body_masks.empty()) {
-        // fused pushes: per body reference, the other ranks that need what this rank's constraint writes
-        if ((int)ctx->body_masks.size() != ctx->body_count) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, "end_constraints: bepucuda_shard_set_body_masks was called for another body count");
+        CK(cudaMemcpyAsync(ctx->constrained.ptr, ctx->global_constrained.data(), (size_t)ctx->body_count, cudaMemcpyHostToDevice, ctx->stream));
+        // per body reference, the other ranks that need what this rank's constraint writes
         CK(ctx->peer32.reserve(ctx->refs_words * 4 + 1024));
         CK(ctx->body_masks_dev.reserve((size_t)ctx->body_count + 16));
         CK(cudaMemcpyAsync(ctx->body_masks_dev.ptr, ctx->body_masks.data(), (size_t)ctx->body_count, cudaMemcpyHostToDevice, ctx->stream));
@@ -1230,23 +1168,14 @@ int32_t bepucuda_solve(bepucuda_ctx* ctx, float dt) {
     ctx->frame_params_host->shard_solve_index = ctx->shard_solve_index;
     CK(cudaMemcpyAsync(ctx->frame_params_dev.ptr, ctx->frame_params_host, sizeof(FrameParams), cudaMemcpyHostToDevice, ctx->stream));
 
-    if (ctx->peer_mode && ctx->cfg.execution_mode != BEPUCUDA_EXEC_GRAPH && ctx->cfg.execution_mode != BEPUCUDA_EXEC_STREAM)
-        return fail(ctx, BEPUCUDA_ERR_BAD_STATE, "solve: peer sharding needs BEPUCUDA_EXEC_GRAPH or BEPUCUDA_EXEC_STREAM");
-    if (ctx->exchange && !ctx->peer_mode) {
-        if (ctx->cfg.execution_mode != BEPUCUDA_EXEC_STREAM) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, "solve: sharded batches need BEPUCUDA_EXEC_STREAM");
-        if (ctx->integ.angular_integration_mode != 0) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, "solve: sharded batches support AngularIntegrationMode.Nonconserving only");
-        ctx->exchange_failed = false;
-    }
     CK(cudaEventRecord(ctx->ev_solve_begin, ctx->stream));
     int64_t launches = 0;
     if (ctx->cfg.execution_mode == BEPUCUDA_EXEC_GRAPH) {
         if (!ctx->graph_valid) {
-            ctx->exchange_failed = false;
             CK(cudaStreamBeginCapture(ctx->stream, cudaStreamCaptureModeThreadLocal));
             int64_t n = 0;
             issue_stage_sequence(ctx, ctx->stream, &n);
             cudaError_t e = cudaStreamEndCapture(ctx->stream, &ctx->graph);
-            if (e == cudaSuccess && ctx->exchange_failed) e = cudaErrorUnknown;
             if (e == cudaSuccess) e = cudaGraphInstantiate(&ctx->graph_exec, ctx->graph, 0);
             if (e != cudaSuccess) return cuda_fail(ctx, e, "graph capture");
             ctx->graph_valid = true;
@@ -1260,7 +1189,6 @@ int32_t bepucuda_solve(bepucuda_ctx* ctx, float dt) {
     if (ctx->cfg.execution_mode == BEPUCUDA_EXEC_STREAM) {
         issue_stage_sequence(ctx, ctx->stream, &launches);
         CK(cudaGetLastError());
-        if (ctx->exchange_failed) return fail(ctx, BEPUCUDA_ERR_CUDA, "solve: the exchange callback failed");
     }
     CK(cudaEventRecord(ctx->ev_solve_end, ctx->stream));
     if (ctx->peer_mode) { ctx->exchange_counter += ctx->exchanges_per_solve; ++ctx->shard_solve_index; }  // the flag barrier and the arrival counters keep counting across solves
@@ -1285,12 +1213,6 @@ int32_t bepucuda_solve(bepucuda_ctx* ctx, float dt) {
 }
 
 static int check_device_error_flag(bepucuda_ctx* ctx) {
-    if (ctx->peer_mode && ctx->tune[3]) {
-        unsigned long long acc[4] = {};
-        cudaMemcpy(acc, (unsigned long long*)ctx->shard_flags.ptr + kMaxShardRanks, sizeof(acc), cudaMemcpyDeviceToHost);
-        if (acc[3]) fprintf(stderr, "[bepucuda shard rank %d] exchange phases, mean over %llu: push+fence %.2f us, signal %.2f us, wait %.2f us\n", ctx->peers.rank, acc[3],
-                            acc[0] / 1e3 / acc[3], acc[1] / 1e3 / acc[3], acc[2] / 1e3 / acc[3]);
-    }
     if (ctx->peer_mode) {
         int32_t e = 0;
         CK(cudaMemcpyAsync(&e, ctx->error_dev.ptr, 4, cudaMemcpyDeviceToHost, ctx->stream));
@@ -1385,7 +1307,6 @@ int32_t bepucuda_event_elapsed_ms(bepucuda_ctx* ctx, int32_t a, int32_t b, float
 }
 
 int32_t bepucuda_profile_stages(bepucuda_ctx* ctx, float dt, bepucuda_stage_profile* out) {
-    if (ctx && ctx->exchange) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, "profile_stages: not available with sharded batches");
     if (!ctx || !out || !(dt > 0)) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "profile_stages: bad arguments");
     if (!ctx->constraints_ready) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, "profile_stages before end_constraints");
     CK(cudaSetDevice(ctx->device));
@@ -1642,35 +1563,9 @@ int32_t bepucuda_shard_set_global(bepucuda_ctx* ctx, const int32_t* first_batch,
 }
 
 int32_t bepucuda_shard_set_body_masks(bepucuda_ctx* ctx, const uint8_t* rank_masks) {
-    if (!ctx) return BEPUCUDA_ERR_INVALID_ARGUMENT;
-    if (rank_masks) ctx->body_masks.assign(rank_masks, rank_masks + ctx->body_count);
-    else ctx->body_masks.clear();
+    if (!ctx || !rank_masks) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "shard_set_body_masks: bad arguments");
+    ctx->body_masks.assign(rank_masks, rank_masks + ctx->body_count);
     if (ctx->constraints_ready) ctx->constraints_ready = false;
-    return BEPUCUDA_OK;
-}
-
-int32_t bepucuda_shard_set_pushes(bepucuda_ctx* ctx, int32_t batch_index, int32_t count, const int32_t* bodies, const int32_t* ranks, const int32_t* owner_flags) {
-    if (!ctx || batch_index < 0 || count < 0 || (count > 0 && (!bodies || !ranks || !owner_flags))) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "shard_set_pushes: bad arguments");
-    std::vector<uint32_t>& list = ctx->pushes_by_batch[batch_index];
-    list.resize((size_t)count);
-    for (int i = 0; i < count; ++i) {
-        if (bodies[i] < 0 || bodies[i] >= ctx->body_count || ranks[i] < 0 || ranks[i] >= kMaxShardRanks) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "shard_set_pushes: body or rank out of range");
-        list[i] = (uint32_t)bodies[i] | ((uint32_t)ranks[i] << 28) | (owner_flags[i] ? kPushOwnerBit : 0u);
-    }
-    if (ctx->constraints_ready) ctx->constraints_ready = false;
-    return BEPUCUDA_OK;
-}
-
-int32_t bepucuda_set_boundary_bodies(bepucuda_ctx* ctx, const int32_t* body_indices, int32_t count, bepucuda_exchange_fn exchange, void* user) {
-    if (!ctx || count < 0) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "set_boundary_bodies: bad arguments");
-    (void)body_indices;  // every body is treated as possibly shared (see the header)
-    if (ctx->constraints_open) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, "set_boundary_bodies inside begin/end_constraints");
-    if (exchange && ctx->cfg.execution_mode != BEPUCUDA_EXEC_STREAM)
-        return fail(ctx, BEPUCUDA_ERR_BAD_STATE, "set_boundary_bodies: sharded batches need a context created with BEPUCUDA_EXEC_STREAM");
-    ctx->exchange = exchange;
-    ctx->exchange_user = user;
-    // ownership and the constrained mask depend on it: the constraint description has to be (re)built
-    if (ctx->constraints_ready && !ctx->sources.empty()) ctx->constraints_ready = false;
     return BEPUCUDA_OK;
 }
 

@@ -93,10 +93,10 @@ C_ABI_SYMBOLS = [
     "bepucuda_create", "bepucuda_destroy", "bepucuda_last_error", "bepucuda_type_info", "bepucuda_host_register", "bepucuda_host_unregister",
     "bepucuda_set_solve_description", "bepucuda_set_integrator", "bepucuda_upload_bodies", "bepucuda_begin_constraints", "bepucuda_upload_type_batch",
     "bepucuda_set_constrained_kinematics", "bepucuda_end_constraints", "bepucuda_update_type_batch", "bepucuda_solve", "bepucuda_synchronize",
-    "bepucuda_download_bodies", "bepucuda_download_impulses", "bepucuda_download_prestep", "bepucuda_get_timings", "bepucuda_set_boundary_bodies",
+    "bepucuda_download_bodies", "bepucuda_download_impulses", "bepucuda_download_prestep", "bepucuda_get_timings",
     "bepucuda_event_record", "bepucuda_event_elapsed_ms", "bepucuda_profile_stages",
     "bepucuda_set_contact_features", "bepucuda_update_contacts", "bepucuda_upload_body_motion", "bepucuda_download_body_motion",
-    "bepucuda_shard_export", "bepucuda_shard_import", "bepucuda_shard_set_global", "bepucuda_shard_set_pushes", "bepucuda_shard_set_body_masks", "bepucuda_shard_import_contexts",
+    "bepucuda_shard_export", "bepucuda_shard_import", "bepucuda_shard_set_global", "bepucuda_shard_set_body_masks", "bepucuda_shard_import_contexts",
     "bepucuda_color_constraints", "bepucuda_color_hash", "bepucuda_set_body_shapes", "bepucuda_predict_bounding_boxes",
 ]
 
@@ -107,8 +107,6 @@ BODY_SHAPE_DTYPE = np.dtype([("type", "<i4"), ("a", "<f4"), ("b", "<f4"), ("c", 
 BODY_ACTIVITY_DTYPE = np.dtype([("sleep_threshold", "<f4"), ("minimum_timesteps_under_threshold", "u1"), ("timesteps_under_threshold_count", "u1"), ("sleep_candidate", "u1"),
                                 ("reserved", "u1")])
 SHAPE_SPHERE, SHAPE_CAPSULE, SHAPE_BOX, SHAPE_CYLINDER = 0, 1, 2, 4  # Sphere.Id, Capsule.Id, Box.Id, Cylinder.Id of the reference
-
-EXCHANGE_FN = C.CFUNCTYPE(C.c_int32, C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_void_p)
 
 
 def load_libraries():
@@ -137,7 +135,6 @@ def load_libraries():
     cuda.bepucuda_type_info.argtypes = [i32, C.POINTER(i32), C.POINTER(i32), C.POINTER(i32)]
     cuda.bepucuda_get_timings.argtypes = [vp, C.POINTER(Timings)]
     cuda.bepucuda_solve.argtypes = [vp, f32]
-    cuda.bepucuda_set_boundary_bodies.argtypes = [vp, vp, i32, EXCHANGE_FN, vp]
     cuda.bepucuda_synchronize.argtypes = [vp]
     cuda.bepucuda_set_solve_description.argtypes = [vp, i32, C.POINTER(i32), i32]
     cuda.bepucuda_set_integrator.argtypes = [vp, C.POINTER(IntegratorDesc)]
@@ -405,27 +402,6 @@ class CudaTimestepper:
         """Page-locks the simulation's buffers (a C# host would register its BufferPool blocks once)."""
         self._check(self._host.bepuhost_cuda_register_buffers(self.sim._sim, self._ctx))
         self._registered = True
-
-    def set_exchange(self, callback):
-        """Sharded batches (bepucuda_set_boundary_bodies): `callback(device_pointer, word_count, op, cuda_stream) -> int` must combine `word_count` int32
-        words at `device_pointer` across all ranks in place (op 0 = sum, 1 = min) as stream-ordered work on `cuda_stream`. None switches it off.
-        Call before describe()."""
-        if callback is None:
-            self._exchange_cb = None
-            self._check(self._cuda.bepucuda_set_boundary_bodies(self._ctx, None, 0, None, None))
-            return
-
-        def trampoline(user, words, count, op, stream):
-            try:
-                return int(callback(words, count, op, stream) or 0)
-            except Exception:  # never unwind through the C frame
-                import traceback
-
-                traceback.print_exc()
-                return -1
-
-        self._exchange_cb = EXCHANGE_FN(trampoline)  # keep the thunk alive
-        self._check(self._cuda.bepucuda_set_boundary_bodies(self._ctx, None, 0, self._exchange_cb, None))
 
     def describe(self):
         """Uploads bodies + every type batch and rebuilds device topology (call after any add/remove)."""

@@ -77,40 +77,17 @@ def partition(simulation, rank_count):
     return shards, first_batch, constrained, masks
 
 
-def pushes_for_rank(shard, rank, rank_count, first_batch, masks):
-    """Per batch: (body, destination rank, owner flag) for every body this rank's constraints of the batch write and another rank references."""
-    out = {}
-    for tb in shard:
-        idx, dyn = tb["idx"], tb["dynamic"]
-        bodies = idx[dyn]
-        if bodies.size == 0:
-            continue
-        m = masks[bodies] & ~np.uint8(1 << rank)
-        for q in range(rank_count):
-            if q == rank:
-                continue
-            sel = (m >> q) & 1 == 1
-            if not sel.any():
-                continue
-            b = bodies[sel].astype(np.int32)
-            entry = out.setdefault(tb["batch_index"], [[], [], []])
-            entry[0].append(b)
-            entry[1].append(np.full(b.size, q, dtype=np.int32))
-            entry[2].append((first_batch[b] == tb["batch_index"]).astype(np.int32))
-    return {k: tuple(np.concatenate(x) for x in v) for k, v in out.items()}
-
-
 class ShardedSolver:
     """One rank of a sharded solve, straight on the C ABI. `exchange_handles(bytes) -> [bytes per rank]` moves the IPC handles between the ranks
     (torch.distributed.all_gather_object in the tools; a direct call when several contexts live in one process)."""
 
-    def __init__(self, simulation, rank, rank_count, device, strict_fp=False, execution_mode=native.EXEC_GRAPH, fused_pushes=True):
+    def __init__(self, simulation, rank, rank_count, device, strict_fp=False, execution_mode=native.EXEC_GRAPH):
         self._cuda, _ = native.load_libraries()
         for name, args in (("bepucuda_shard_export", [C.c_void_p, C.POINTER(IpcHandles)]), ("bepucuda_shard_import", [C.c_void_p, C.c_int32, C.c_int32, C.POINTER(IpcHandles)]),
-                           ("bepucuda_shard_set_global", [C.c_void_p, C.c_void_p, C.c_void_p]), ("bepucuda_shard_set_pushes", [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
+                           ("bepucuda_shard_set_global", [C.c_void_p, C.c_void_p, C.c_void_p]),
                            ("bepucuda_shard_set_body_masks", [C.c_void_p, C.c_void_p]), ("bepucuda_shard_import_contexts", [C.c_void_p, C.c_int32, C.c_int32, C.POINTER(C.c_void_p)])):
             getattr(self._cuda, name).argtypes = args
-        self.sim, self.rank, self.rank_count, self.fused_pushes = simulation, rank, rank_count, fused_pushes
+        self.sim, self.rank, self.rank_count = simulation, rank, rank_count
         cfg = native.Config()
         cfg.device_ordinal, cfg.strict_fp, cfg.execution_mode = device, int(bool(strict_fp)), execution_mode
         ctx = C.c_void_p()
@@ -154,11 +131,7 @@ class ShardedSolver:
         for tb in self.shard:
             self._check(self._cuda.bepucuda_upload_type_batch(self._ctx, tb["batch_index"], tb["type_batch_index"], tb["type_id"], tb["count"], tb["refs"].ctypes.data,
                                                               tb["prestep"].ctypes.data, tb["impulses"].ctypes.data))
-        if self.fused_pushes:
-            self._check(self._cuda.bepucuda_shard_set_body_masks(self._ctx, self.masks.ctypes.data))
-        else:
-            for batch, (b, q, o) in pushes_for_rank(self.shard, self.rank, self.rank_count, self.first_batch, self.masks).items():
-                self._check(self._cuda.bepucuda_shard_set_pushes(self._ctx, batch, b.size, b.ctypes.data, q.ctypes.data, o.ctypes.data))
+        self._check(self._cuda.bepucuda_shard_set_body_masks(self._ctx, self.masks.ctypes.data))
         kin = np.ascontiguousarray(sim.constrained_kinematics, dtype=np.int32)
         self._check(self._cuda.bepucuda_set_constrained_kinematics(self._ctx, kin.ctypes.data if kin.size else None, int(kin.size)))
         self._check(self._cuda.bepucuda_end_constraints(self._ctx))
@@ -178,6 +151,8 @@ class ShardedSolver:
         """Bodies (valid for the bodies this rank references) and this rank's impulses / prestep back into its shard arrays."""
         self._check(self._cuda.bepucuda_download_bodies(self._ctx, self.bodies.ctypes.data, self.sim.body_count))
         self._check(self._cuda.bepucuda_download_impulses(self._ctx))
+        for tb in self.shard:
+            self._check(self._cuda.bepucuda_download_prestep(self._ctx, tb["batch_index"], tb["type_batch_index"], tb["prestep"].ctypes.data))
         return self.bodies
 
     def referenced_bodies(self):

@@ -44,7 +44,7 @@ typedef struct bepucuda_ctx bepucuda_ctx;
  * on the device. */
 enum bepucuda_execution_mode {
     BEPUCUDA_EXEC_GRAPH = 0,      /* one kernel per (batch, stage) chained by programmatic dependent launch, whole frame captured in a CUDA graph */
-    BEPUCUDA_EXEC_STREAM = 2      /* the same launches issued directly on the stream, no graph (profiling with ncu; the exchange-callback sharding) */
+    BEPUCUDA_EXEC_STREAM = 2      /* the same launches issued directly on the stream, no graph (profiling with ncu) */
     /* 1 and 3 were a persistent cooperative kernel (grid barrier per stage) and a dataflow kernel (per-body version dependencies); both measured
      * slower than the graph on every benchmark configuration and were removed: bepucuda_create rejects them. */
 };
@@ -248,45 +248,26 @@ int32_t bepucuda_color_constraints(bepucuda_ctx* ctx, int32_t constraint_count, 
 /* The hash behind BEPUCUDA_COLOR_HASHED_ORDER: h = i * 0x9E3779B1; h ^= h >> 15; h *= 0x85EBCA77; h ^= h >> 13; h *= 0xC2B2AE3D; h ^= h >> 16 (uint32). */
 uint32_t bepucuda_color_hash(uint32_t constraint_index);
 
-/* Multi-GPU, one constraint graph over several contexts (SURVEY.md §8e; replaces the reference's multithreaded batch dispatch,
- * Solver_Solve.cs:L458-654, where workers split the constraints of a batch). Every participating context ("rank": one per GPU, normally one per
- * process) is given the WHOLE body set and the same batch layout, but only its share of the constraints (lanes of other ranks are empty, body
- * reference -1). Within a batch no dynamic body is referenced twice, so exactly one rank writes a given body in a given (batch, stage); after every
- * WarmStart / Solve stage the library packs the records this rank wrote (velocity; pose and world inertia too when the lane integrated) into a
- * zero-initialised staging buffer with a "valid" word, calls `exchange` to all-reduce it, and writes every valid record back, which keeps all
- * ranks' body arrays bit-identical to a single-context solve. At bepucuda_end_constraints the per-body integration owner (lowest batch referencing
- * the body) and the constrained-body mask are combined the same way.
- *   exchange(user, device_words, count, op, cuda_stream): combine `count` int32 words at `device_words` element-wise across all ranks, in place, as
- *   stream-ordered work on `cuda_stream` (e.g. ncclAllReduce with ncclInt32 and ncclSum for op 0 / ncclMin for op 1); return 0, or non-zero to fail
- *   the call that invoked it. With op 0 at most one rank contributes a non-zero word, so an integer sum transports bit patterns exactly.
- * Requirements: BEPUCUDA_EXEC_STREAM, AngularIntegrationMode.Nonconserving; call before bepucuda_begin_constraints. `body_indices` / `count` name the
- * bodies other ranks may also reference; NULL / 0 means "all of them" (the only form implemented: the list is accepted and ignored).
- * Passing exchange = NULL returns the context to single-rank operation. */
-typedef int32_t (*bepucuda_exchange_fn)(void* user, void* device_words, int64_t count, int32_t op, void* cuda_stream);
-int32_t bepucuda_set_boundary_bodies(bepucuda_ctx* ctx, const int32_t* body_indices, int32_t count,
-                                     bepucuda_exchange_fn exchange, void* user);
-
-/* Multi-GPU, ONE constraint graph over several GPUs with direct NVLink peer stores (SURVEY.md §8e; the fast successor of the callback path above).
- * Bodies are partitioned into owner slabs by the host; every rank (one context per GPU, normally one process per GPU) uploads ALL bodies (only
- * its own slab and the halo it references are kept current) and ONLY ITS OWN constraints, compacted, under their original batch indices. After
- * every WarmStart / Solve stage a rank copies the records its stage wrote for bodies other ranks also reference straight into those ranks' body
- * arrays (peer memory opened from CUDA IPC handles) and all ranks meet at a flag barrier in peer memory: no host round trip, no collective library.
- * Within a batch no dynamic body is referenced twice, so exactly one rank writes a given body in a given stage, and every rank's copy of a body
- * it references is bit-identical to the single-GPU solve at every stage.
+/* Multi-GPU, ONE constraint graph over several GPUs with direct NVLink peer stores (SURVEY.md §8e; replaces the reference's multithreaded batch
+ * dispatch, Solver_Solve.cs:L458-654, where workers split the constraints of a batch). Bodies are partitioned into owner slabs by the host; every
+ * rank (one context per GPU, normally one process per GPU) uploads ALL bodies (only its own slab and the halo it references are kept current) and
+ * ONLY ITS OWN constraints, compacted, under their original batch indices, so every rank has the same batch layout. A WarmStart / Solve stage
+ * stores each record it writes for a body other ranks also reference straight into those ranks' body arrays (peer memory opened from CUDA IPC
+ * handles), from the registers of the lane that computed it, and announces the arrival in their flag blocks; bundles that read such a body in a
+ * later stage first wait for those arrivals. Rank barriers in peer memory open every substep and precede the contact update and the final pose
+ * pass: no host round trip, no collective library. Within a batch no dynamic body is referenced twice, so exactly one rank writes a given body in
+ * a given stage, and every rank's copy of a body it references is bit-identical to the single-GPU solve at every stage.
  *   bepucuda_shard_export: IPC handles of this context's pose / velocity / world-inertia arrays and of its flag block (call after
  *     bepucuda_upload_bodies; the arrays must not be re-allocated afterwards, i.e. keep the body count).
  *   bepucuda_shard_import: this rank's index, the rank count (<= 8) and every rank's exported handles, in rank order.
  *   bepucuda_shard_set_global: per body, the lowest batch index that references it as a dynamic body on ANY rank (INT32_MAX if none) -- the owner of
  *     its integration, Solver_Solve.cs:L951-1044 -- and whether any rank constrains it (final pose pass, PoseIntegrator.cs:L537-693).
- *   bepucuda_shard_set_pushes: for one batch, the (body, destination rank) pairs of the bodies THIS rank's constraints of that batch write and the
- *     destination rank also references; owner_flags[i] != 0 when this batch integrates the body (pose and world inertia travel too in WarmStart).
- *     These lists are copied by the one-CTA exchange kernel that follows the stage.
- *   bepucuda_shard_set_body_masks (preferred, replaces the push lists): rank_masks[body] has bit r set when rank r references the body. The stage
- *     kernels then store a written record into the other referencing ranks' arrays themselves, from the registers of the lane that computed it,
- *     and the exchange kernel is only the flag barrier. NULL returns to the push lists.
- * Call order: upload_bodies, shard_export, (exchange handles), shard_import, shard_set_global, shard_set_body_masks | (begin_constraints ...
- * shard_set_pushes ...), end_constraints. Every rank must have finished uploading a frame's bodies before any rank's bepucuda_solve can complete
- * its first stage: the solve starts with a rank barrier, so issuing upload and solve on each rank in that order is enough. The sequential fallback batch is not supported across ranks (BEPUCUDA_ERR_BAD_STATE). BEPUCUDA_EXEC_GRAPH or _STREAM. */
+ *   bepucuda_shard_set_body_masks: rank_masks[body] has bit r set when rank r references the body (NULL: BEPUCUDA_ERR_INVALID_ARGUMENT).
+ * Call order: upload_bodies, shard_export, (exchange handles), shard_import, shard_set_global, shard_set_body_masks, begin/upload/end_constraints.
+ * In peer mode bepucuda_end_constraints returns BEPUCUDA_ERR_BAD_STATE when shard_set_body_masks was not called for the current body count, and when
+ * a constraint lies in the sequential fallback batch, which is not supported across ranks. Every rank must have finished uploading a frame's bodies
+ * before any rank's bepucuda_solve can complete its first stage: the solve starts with a rank barrier, so issuing upload and solve on each rank in
+ * that order is enough. BEPUCUDA_EXEC_GRAPH or _STREAM. */
 typedef struct bepucuda_ipc_handles {
     unsigned char bytes[4][64];
 } bepucuda_ipc_handles;
@@ -296,8 +277,6 @@ int32_t bepucuda_shard_import(bepucuda_ctx* ctx, int32_t rank, int32_t rank_coun
  * (peer access is enabled between different devices) instead of through IPC handles. all_ranks[rank] must be ctx itself. */
 int32_t bepucuda_shard_import_contexts(bepucuda_ctx* ctx, int32_t rank, int32_t rank_count, bepucuda_ctx* const* all_ranks);
 int32_t bepucuda_shard_set_global(bepucuda_ctx* ctx, const int32_t* first_batch_per_body, const uint8_t* constrained_per_body);
-int32_t bepucuda_shard_set_pushes(bepucuda_ctx* ctx, int32_t batch_index, int32_t count, const int32_t* body_indices, const int32_t* destination_ranks,
-                                  const int32_t* owner_flags);
 int32_t bepucuda_shard_set_body_masks(bepucuda_ctx* ctx, const uint8_t* rank_masks);
 
 #ifdef __cplusplus

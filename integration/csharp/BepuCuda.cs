@@ -33,9 +33,6 @@ namespace BepuCuda
         public fixed long AlgorithmicBytes[8];
     }
 
-    [UnmanagedFunctionPointer(CallingConvention.Cdecl)]
-    public unsafe delegate int ExchangeFn(void* user, void* deviceWords, long count, int op, void* cudaStream);
-
     public static unsafe class Native
     {
         const string Lib = "bepucuda";
@@ -69,7 +66,6 @@ namespace BepuCuda
         [DllImport(Lib)] public static extern int bepucuda_shard_export(IntPtr ctx, IpcHandles* handles);
         [DllImport(Lib)] public static extern int bepucuda_shard_import(IntPtr ctx, int rank, int rankCount, IpcHandles* allRanks);
         [DllImport(Lib)] public static extern int bepucuda_shard_set_global(IntPtr ctx, int* firstBatchPerBody, byte* constrainedPerBody);
-        [DllImport(Lib)] public static extern int bepucuda_shard_set_pushes(IntPtr ctx, int batchIndex, int count, int* bodyIndices, int* destinationRanks, int* ownerFlags);
         [DllImport(Lib)] public static extern int bepucuda_shard_set_body_masks(IntPtr ctx, byte* rankMasks);
         [DllImport(Lib)] public static extern int bepucuda_shard_import_contexts(IntPtr ctx, int rank, int rankCount, IntPtr* allRanks);
         /// <summary>PredictBoundingBoxes on the device: sleep candidacy + bounds and speculative margins of sphere / capsule / box / cylinder bodies from the resident body state.</summary>
@@ -78,6 +74,5 @@ namespace BepuCuda
         /// <summary>Device-side batch colouring: the batch Solver.Add's first-fit search would pick for every constraint of a list (order 0 = add order, 1 = hashed, 2 = priorities).</summary>
         [DllImport(Lib)] public static extern int bepucuda_color_constraints(IntPtr ctx, int constraintCount, int bodiesPerConstraint, int* encodedBodyReferences, int bodyCount, int fallbackBatchThreshold, int order, uint* priorities, int* batchIndicesOut, int* batchCountOut, int* roundsOut);
         [DllImport(Lib)] public static extern uint bepucuda_color_hash(uint constraintIndex);
-        [DllImport(Lib)] public static extern int bepucuda_set_boundary_bodies(IntPtr ctx, int* bodyIndices, int count, ExchangeFn exchange, void* user);
     }
 }

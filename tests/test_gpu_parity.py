@@ -209,97 +209,6 @@ def test_randomised_mixed_scenes_bit_exact(libs, seed):
             fallback_batch_threshold=int(rng.choice([6, 64])), substeps=substeps, velocity_iterations=iterations, integrator=integ, frames=2)
 
 
-def _shard_lanes(sim, rank, ranks, body_count):
-    """Keeps only this rank's share of the constraints: lanes whose first body lies outside the rank's body-index slab become empty (-1), exactly what a
-    host that splits every batch across devices would upload. Returns the per type batch lane masks it kept."""
-    kept = []
-    for tb in sim.type_batches():
-        refs = tb.body_references  # [bundles, bodies per constraint, W]
-        first = refs[:, 0, :]
-        owner = np.where(first >= 0, ((first & 0x3FFFFFFF).astype(np.int64) * ranks) // body_count, -1)
-        mine = owner == rank
-        refs[np.broadcast_to(~mine[:, None, :], refs.shape)] = -1
-        kept.append(mine)
-    return kept
-
-
-def test_sharded_batches_two_ranks_with_exchange_bit_exact(libs):
-    """One constraint graph over two contexts (bepucuda_set_boundary_bodies): each rank solves its share of every batch and the library exchanges the
-    written body records after every stage through the callback. Two ranks are emulated on one GPU (two contexts, two host threads, the all-reduce done
-    with torch between them); every rank must end with the single-context / oracle body state bit for bit, and the union of the ranks' impulses too."""
-    import threading
-
-    import torch
-
-    import bepuphysics2_b200 as bp
-
-    scene = scenes.merge(scenes.shape_pile(1200, seed=21), scenes.ragdolls(12, seed=22), scenes.joint_zoo(300, 20, seed=23))
-    kw = dict(substeps=3, velocity_iterations=2, fallback_batch_threshold=64)
-    ref_sim = util.make_sim(scene, **kw)
-    ref = util.run_oracle(ref_sim, DT, frames=2)
-    ranks, n = 2, scene["bodies"].shape[0]
-    sims = [util.make_sim(scene, **kw) for _ in range(ranks)]
-    kept = [_shard_lanes(sims[r], r, ranks, n) for r in range(ranks)]
-    assert all(k.any() for k in kept[0]) or True
-    barrier = threading.Barrier(ranks, timeout=60)
-    slots = [None] * ranks
-    errors = []
-
-    class Raw:
-        def __init__(self, ptr, count):
-            self.__cuda_array_interface__ = {"shape": (count,), "typestr": "<i4", "data": (ptr, False), "version": 3}
-
-    def make_callback(rank):
-        def callback(ptr, count, op, stream):
-            torch.cuda.synchronize()
-            slots[rank] = torch.as_tensor(Raw(ptr, count), device="cuda")
-            barrier.wait()
-            if rank == 0:
-                total = slots[0].clone()
-                for other in slots[1:]:
-                    total = total + other if op == 0 else torch.minimum(total, other)
-                for t in slots:
-                    t.copy_(total)
-                torch.cuda.synchronize()
-            barrier.wait()
-            return 0
-        return callback
-
-    def run(rank):
-        try:
-            ts = bp.CudaTimestepper(sims[rank], strict_fp=True, execution_mode=EXEC_STREAM)
-            ts.set_exchange(make_callback(rank))
-            ts.describe()
-            for f in range(2):
-                if f > 0:
-                    ts.refresh()
-                ts.solve(DT, download=True)
-                ts.download_prestep()
-            ts.close()
-        except Exception as e:  # noqa: BLE001
-            errors.append((rank, e))
-            barrier.abort()
-
-    threads = [threading.Thread(target=run, args=(r,)) for r in range(ranks)]
-    for t in threads:
-        t.start()
-    for t in threads:
-        t.join(timeout=180)
-    assert not errors, errors
-    for r in range(ranks):
-        snap = util.snapshot(sims[r])
-        for label, cols in (("poses", np.r_[0:7]), ("linear velocities", np.r_[8:11]), ("angular velocities", np.r_[12:15])):
-            assert np.array_equal(ref["bodies"][:, cols].view(np.uint32), snap["bodies"][:, cols].view(np.uint32)), "rank %d %s differ from the single-context result" % (r, label)
-        for tb_ref, tb_got, mine in zip(ref["type_batches"], snap["type_batches"], kept[r]):
-            m = np.broadcast_to(mine[:, None, :], tb_ref["impulses"].shape)
-            assert np.array_equal(np.where(m, tb_ref["impulses"], 0).view(np.uint32), np.where(m, tb_got["impulses"], 0).view(np.uint32)), "rank %d impulses of %s" % (r, tb_ref["key"],)
-            mp = np.broadcast_to(mine[:, None, :], tb_ref["prestep"].shape)
-            assert np.array_equal(np.where(mp, tb_ref["prestep"], 0).view(np.uint32), np.where(mp, tb_got["prestep"], 0).view(np.uint32)), "rank %d prestep of %s" % (r, tb_ref["key"],)
-    # every constraint is solved by exactly one rank
-    for masks in zip(*kept):
-        assert (np.sum(masks, axis=0) <= 1).all()
-
-
 @pytest.mark.parametrize("mode", [EXEC_GRAPH, EXEC_STREAM])
 def test_fast_build_is_run_to_run_deterministic(libs, mode):
     """The reference's own determinism harness (Demos/SpecializedTests/DeterminismTest.cs) repeats a simulation and demands bitwise identical

@@ -7,11 +7,12 @@ import sys
 import numpy as np
 import pytest
 
-from bepuphysics2_b200 import scenes, sharding
+from bepuphysics2_b200 import native, scenes, sharding
 from tests import util
 
 DT = 1.0 / 60.0
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+EXECUTION_MODES = {"graph": native.EXEC_GRAPH, "stream": native.EXEC_STREAM}
 
 
 def _global_rows(sim):
@@ -63,19 +64,6 @@ def test_partition_covers_every_constraint_once_and_masks_name_the_referencing_r
         assert writers.max() <= 1
 
 
-def test_push_lists_name_exactly_the_shared_bodies_a_rank_writes():
-    sim = util.make_sim(scenes.shape_pile(2000, seed=4))
-    shards, first_batch, constrained, masks = sharding.partition(sim, 2)
-    for rank in range(2):
-        pushes = sharding.pushes_for_rank(shards[rank], rank, 2, first_batch, masks)
-        for batch, (bodies, dst, owner) in pushes.items():
-            assert (dst == 1 - rank).all()
-            assert (masks[bodies] == 3).all()
-            assert np.array_equal(owner != 0, first_batch[bodies] == batch)
-            written = np.concatenate([tb["idx"][tb["dynamic"]] for tb in shards[rank] if tb["batch_index"] == batch])
-            assert np.array_equal(np.sort(bodies), np.sort(written[masks[written] == 3]))
-
-
 _GLOO_SCRIPT = r"""
 import hashlib, sys
 import numpy as np
@@ -108,13 +96,13 @@ def test_two_gloo_ranks_derive_the_same_global_tables(tmp_path):
     assert r.returncode == 0 and "OK" in r.stdout, r.stdout[-3000:]
 
 
-def _one_process_ranks(sim_scene, rank_count, frames, fused, libs, **kw):
+def _one_process_ranks(sim_scene, rank_count, frames, mode, libs, **kw):
     """`rank_count` contexts on device 0, wired to one another with bepucuda_shard_import_contexts; every rank's referenced bodies and its own
-    impulses against the oracle run on the whole graph."""
+    impulses and prestep rows (contact depths written by the incremental update) against the oracle run on the whole graph."""
     from oracle import binding as ob
 
     sim = util.make_sim(sim_scene, **kw)
-    solvers = [sharding.ShardedSolver(sim, r, rank_count, 0, strict_fp=True, fused_pushes=fused) for r in range(rank_count)]
+    solvers = [sharding.ShardedSolver(sim, r, rank_count, 0, strict_fp=True, execution_mode=EXECUTION_MODES[mode]) for r in range(rank_count)]
     try:
         for s in solvers:
             s.export_handles()
@@ -126,19 +114,20 @@ def _one_process_ranks(sim_scene, rank_count, frames, fused, libs, **kw):
             s.synchronize()
         for _ in range(frames):
             ob.solve(sim, DT)
-            for s in solvers:  # asynchronous launches: the ranks' graphs run side by side on the device and meet at their exchange points
+            for s in solvers:  # asynchronous launches: the ranks' frames run side by side on the device and meet at their exchange points
                 s.solve(DT)
         by_key = {(tb.batch_index, tb.type_batch_index): tb for tb in sim.type_batches()}
         for s in solvers:
             got = s.download()
             mine = s.referenced_bodies()
             assert mine.size > 0
-            assert np.array_equal(sim.bodies[mine][:, util.MOTION].view(np.uint32), got[mine][:, util.MOTION].view(np.uint32)), "rank %d bodies" % s.rank
+            assert np.array_equal(sim.bodies[mine][:, util.MOTION].view(np.uint32), got[mine][:, util.MOTION].view(np.uint32)), "rank %d bodies (%s)" % (s.rank, mode)
             for tb in s.shard:
                 g = by_key[(tb["batch_index"], tb["type_batch_index"])]
-                ref = g.accumulated_impulses.transpose(0, 2, 1).reshape(-1, g.accumulated_impulses.shape[1])[tb["source"]]
-                have = tb["impulses"].transpose(0, 2, 1).reshape(-1, tb["impulses"].shape[1])[:tb["count"]]
-                assert np.array_equal(ref.view(np.uint32), have.view(np.uint32)), "rank %d impulses of batch %d" % (s.rank, tb["batch_index"])
+                for what, ref_rows in (("impulses", g.accumulated_impulses), ("prestep", g.prestep)):
+                    ref = ref_rows.transpose(0, 2, 1).reshape(-1, ref_rows.shape[1])[tb["source"]]
+                    have = tb[what].transpose(0, 2, 1).reshape(-1, tb[what].shape[1])[:tb["count"]]
+                    assert np.array_equal(ref.view(np.uint32), have.view(np.uint32)), "rank %d %s of batch %d (%s)" % (s.rank, what, tb["batch_index"], mode)
         shared = int(((solvers[0].masks & (solvers[0].masks - 1)) != 0).sum())
         assert shared > 0
     finally:
@@ -147,17 +136,55 @@ def _one_process_ranks(sim_scene, rank_count, frames, fused, libs, **kw):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("rank_count,fused", [(2, True), (3, True), (2, False)])
-def test_one_graph_over_several_ranks_bit_exact(libs, rank_count, fused):
-    _one_process_ranks(scenes.shape_pile(2500, seed=6), rank_count, frames=3, fused=fused, libs=libs, substeps=4, velocity_iterations=2)
+@pytest.mark.parametrize("rank_count,mode", [(2, "graph"), (3, "graph"), (2, "stream")])
+def test_one_graph_over_several_ranks_bit_exact(libs, rank_count, mode):
+    _one_process_ranks(scenes.shape_pile(2500, seed=6), rank_count, frames=3, mode=mode, libs=libs, substeps=4, velocity_iterations=2)
 
 
 @pytest.mark.gpu
 def test_one_graph_over_two_ranks_ragdolls_bit_exact(libs):
-    _one_process_ranks(scenes.ragdolls(60, seed=2), 2, frames=2, fused=True, libs=libs, substeps=2, velocity_iterations=2)
+    _one_process_ranks(scenes.ragdolls(60, seed=2), 2, frames=2, mode="graph", libs=libs, substeps=2, velocity_iterations=2)
 
 
 @pytest.mark.gpu
 def test_one_graph_over_two_ranks_joint_zoo_bit_exact(libs):
     """Three- and four-body constraints, kinematic bodies, every joint type: the pushes of body slots 2 and 3 and the kinematic stages."""
-    _one_process_ranks(scenes.joint_zoo(1200, per_type=60, seed=8), 2, frames=2, fused=True, libs=libs, substeps=3, velocity_iterations=2)
+    _one_process_ranks(scenes.joint_zoo(1200, per_type=60, seed=8), 2, frames=2, mode="graph", libs=libs, substeps=3, velocity_iterations=2)
+
+
+@pytest.mark.gpu
+def test_one_graph_over_two_ranks_mixed_scene_bit_exact(libs):
+    """Contacts, ragdolls and a joint zoo in one graph, several substeps, in both execution modes: the incremental contact update between substeps
+    reads velocities that other ranks stored, and each rank's contact depths must still match the oracle bit for bit."""
+    scene = scenes.merge(scenes.shape_pile(1200, seed=21), scenes.ragdolls(12, seed=22), scenes.joint_zoo(300, 20, seed=23))
+    for mode in ("graph", "stream"):
+        _one_process_ranks(scene, 2, frames=2, mode=mode, libs=libs, substeps=3, velocity_iterations=2)
+
+
+@pytest.mark.gpu
+def test_peer_mode_needs_body_masks(libs):
+    """NULL masks are an argument error, and a rank whose masks are missing cannot build its stage program: end_constraints reports it before any
+    device work. Both are plain argument / state errors (no solve, so no rank barrier runs); describing with masks afterwards succeeds."""
+    sim = util.make_sim(scenes.shape_pile(400, seed=4), substeps=2, velocity_iterations=1)
+    solvers = [sharding.ShardedSolver(sim, r, 2, 0, strict_fp=True) for r in range(2)]
+    try:
+        for s in solvers:
+            s.export_handles()
+        for s in solvers:
+            s.import_contexts(solvers)
+        s, cuda = solvers[0], solvers[0]._cuda
+        with pytest.raises(native.BepuCudaError) as e:
+            s._check(cuda.bepucuda_shard_set_body_masks(s._ctx, None))
+        assert e.value.code == -1  # BEPUCUDA_ERR_INVALID_ARGUMENT
+        s._check(cuda.bepucuda_shard_set_global(s._ctx, s.first_batch.ctypes.data, s.constrained.ctypes.data))
+        s._check(cuda.bepucuda_begin_constraints(s._ctx, sim.bundle_width, sim.batch_count))
+        for tb in s.shard:
+            s._check(cuda.bepucuda_upload_type_batch(s._ctx, tb["batch_index"], tb["type_batch_index"], tb["type_id"], tb["count"], tb["refs"].ctypes.data,
+                                                     tb["prestep"].ctypes.data, tb["impulses"].ctypes.data))
+        with pytest.raises(native.BepuCudaError) as e:
+            s._check(cuda.bepucuda_end_constraints(s._ctx))
+        assert e.value.code == -6 and "shard_set_body_masks" in str(e.value)  # BEPUCUDA_ERR_BAD_STATE
+        s.describe()
+    finally:
+        for s in solvers:
+            s.close()

@@ -28,7 +28,6 @@ ap.add_argument("--frames", type=int, default=3)
 ap.add_argument("--steps", type=int, default=20)
 ap.add_argument("--check", action="store_true")
 ap.add_argument("--stream", action="store_true")
-ap.add_argument("--push-lists", action="store_true", help="copy shared records in the exchange kernel (push lists) instead of from the stage kernels' lanes")
 args = ap.parse_args()
 
 rank, world, local = int(os.environ.get("RANK", 0)), int(os.environ.get("WORLD_SIZE", 1)), int(os.environ.get("LOCAL_RANK", 0))
@@ -41,8 +40,7 @@ DT = 1.0 / 60.0
 scene = scenes.shape_pile(args.bodies, seed=5)
 sim = bp.Simulation(bundle_width=8, substeps=args.substeps, velocity_iterations=args.iterations)
 scenes.build(scene, sim)
-solver = sharding.ShardedSolver(sim, rank, world, local, strict_fp=args.check, execution_mode=bp.native.EXEC_STREAM if args.stream else bp.native.EXEC_GRAPH,
-                                fused_pushes=not args.push_lists)
+solver = sharding.ShardedSolver(sim, rank, world, local, strict_fp=args.check, execution_mode=bp.native.EXEC_STREAM if args.stream else bp.native.EXEC_GRAPH)
 mine = solver.export_handles()
 gathered = [None] * world
 dist.all_gather_object(gathered, mine)
