@@ -7,115 +7,69 @@
 
 namespace BEPU_NS {
 
-void launch_stage_warm_start_first(const WorkRecord* records, const int32_t* ref_rows, int work_count, const BodyBuffers& B, const FrameParams* fp, int launch_flags, cudaStream_t s);
-void launch_stage_warm_start(const WorkRecord* records, const int32_t* ref_rows, int work_count, const BodyBuffers& B, const FrameParams* fp, int launch_flags, cudaStream_t s);
-void launch_stage_solve(const WorkRecord* records, const int32_t* ref_rows, int work_count, const BodyBuffers& B, const FrameParams* fp, int launch_flags, cudaStream_t s);
-void launch_stage_warm_start_first_sharded(const WorkRecord* records, const int32_t* ref_rows, int work_count, const BodyBuffers& B, const FrameParams* fp, int launch_flags, const ShardPeers& peers, long long peer_delta, const ShardStage& shard, cudaStream_t s);
-void launch_stage_warm_start_sharded(const WorkRecord* records, const int32_t* ref_rows, int work_count, const BodyBuffers& B, const FrameParams* fp, int launch_flags, const ShardPeers& peers, long long peer_delta, const ShardStage& shard, cudaStream_t s);
-void launch_stage_solve_sharded(const WorkRecord* records, const int32_t* ref_rows, int work_count, const BodyBuffers& B, const FrameParams* fp, int launch_flags, const ShardPeers& peers, long long peer_delta, const ShardStage& shard, cudaStream_t s);
+using StageLauncher = void(const WorkRecord* records, const int32_t* ref_rows, int work_count, const BodyBuffers& B, const FrameParams* fp, int launch_flags,
+                           const ShardLaunch* shard, cudaStream_t s);
+StageLauncher launch_stage_warm_start_first, launch_stage_warm_start, launch_stage_solve;  // units 0, 1, 2
 
 #ifndef BEPU_DEEP_MINB
 #define BEPU_DEEP_MINB 12
 #endif
 constexpr int kDeepBatchBundles = 2150;  // more bundles than the uncapped build keeps resident at once (132 SMs x 16 warps on an H100 SXM)
-template <int STAGE, int MINB>
-static void launch_stage_variant(const WorkRecord* records, const int32_t* ref_rows, int work_count, const BodyBuffers& B, const FrameParams* fp, int launch_flags, cudaStream_t s) {
+// Launches one stage kernel instantiation (plain or sharded), one warp per bundle.
+template <auto Kernel, class... Args>
+static void launch_stage_kernel(int work_count, int launch_flags, cudaStream_t s, Args... args) {
     static std::atomic<bool> carveout_set[64] = {};  // function attributes are per device: a process may hold contexts on several
     int device = 0;
     cudaGetDevice(&device);
     if (!carveout_set[device & 63]) {  // the staged stages keep one 6 KB slab per resident warp in shared memory
-        cudaFuncSetAttribute(constraint_stage_kernel<STAGE, MINB>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+        cudaFuncSetAttribute(Kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
         carveout_set[device & 63] = true;
     }
     const unsigned blocks = (unsigned)(((size_t)work_count * 32 + kStageBlockThreads - 1) / kStageBlockThreads);
     cudaLaunchConfig_t cfg{};
     cfg.gridDim = dim3(blocks);
     cfg.blockDim = dim3(kStageBlockThreads);
-    cfg.dynamicSmemBytes = 0;
     cfg.stream = s;
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
     cfg.numAttrs = (launch_flags & bepucuda::kLaunchPdl) ? 1 : 0;
-    cudaLaunchKernelEx(&cfg, constraint_stage_kernel<STAGE, MINB>, records, ref_rows, work_count, B, fp, (launch_flags & bepucuda::kLaunchPrefetchRows) ? kStagePrefetchRows : 0);
+    cudaLaunchKernelEx(&cfg, Kernel, args...);
 }
 template <int STAGE, int MINB>
-static void launch_stage_variant_sharded(const WorkRecord* records, const int32_t* ref_rows, int work_count, const BodyBuffers& B, const FrameParams* fp, int launch_flags, const ShardPeers& peers, long long peer_delta,
-                                         const ShardStage& shard, cudaStream_t s) {
-    static std::atomic<bool> carveout_set[64] = {};
-    int device = 0;
-    cudaGetDevice(&device);
-    if (!carveout_set[device & 63]) {
-        cudaFuncSetAttribute(constraint_stage_kernel_sharded<STAGE, MINB>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-        carveout_set[device & 63] = true;
+static void launch_stage_variant(const WorkRecord* records, const int32_t* ref_rows, int work_count, const BodyBuffers& B, const FrameParams* fp, int launch_flags, const ShardLaunch* shard,
+                                 cudaStream_t s) {
+    const int flags = (launch_flags & bepucuda::kLaunchPrefetchRows) ? kStagePrefetchRows : 0;
+    if (!shard) launch_stage_kernel<constraint_stage_kernel<STAGE, MINB>>(work_count, launch_flags, s, records, ref_rows, work_count, B, fp, flags);
+    else if constexpr (STAGE != kStageIncremental)  // the incremental contact update is never sharded
+        launch_stage_kernel<constraint_stage_kernel_sharded<STAGE, MINB>>(work_count, launch_flags, s, records, ref_rows, work_count, B, fp, flags, shard->peers, shard->peer_delta, shard->stage);
+}
+template <int STAGE>
+static void launch_stage_t(const WorkRecord* records, const int32_t* ref_rows, int work_count, const BodyBuffers& B, const FrameParams* fp, int launch_flags, const ShardLaunch* shard, cudaStream_t s) {
+    if constexpr (STAGE != kStageIncremental) {
+        if (work_count >= kDeepBatchBundles) return launch_stage_variant<STAGE, BEPU_DEEP_MINB>(records, ref_rows, work_count, B, fp, launch_flags, shard, s);
     }
-    const unsigned blocks = (unsigned)(((size_t)work_count * 32 + kStageBlockThreads - 1) / kStageBlockThreads);
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(blocks);
-    cfg.blockDim = dim3(kStageBlockThreads);
-    cfg.stream = s;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = (launch_flags & bepucuda::kLaunchPdl) ? 1 : 0;
-    cudaLaunchKernelEx(&cfg, constraint_stage_kernel_sharded<STAGE, MINB>, records, ref_rows, work_count, B, fp, (launch_flags & bepucuda::kLaunchPrefetchRows) ? kStagePrefetchRows : 0, peers,
-                       peer_delta, shard);
-}
-template <int STAGE>
-static void launch_stage_sharded_t(const WorkRecord* records, const int32_t* ref_rows, int work_count, const BodyBuffers& B, const FrameParams* fp, int launch_flags, const ShardPeers& peers, long long peer_delta,
-                                   const ShardStage& shard, cudaStream_t s) {
-    if (work_count >= kDeepBatchBundles) launch_stage_variant_sharded<STAGE, BEPU_DEEP_MINB>(records, ref_rows, work_count, B, fp, launch_flags, peers, peer_delta, shard, s);
-    else launch_stage_variant_sharded<STAGE, 1>(records, ref_rows, work_count, B, fp, launch_flags, peers, peer_delta, shard, s);
-}
-template <int STAGE>
-static void launch_stage_t(const WorkRecord* records, const int32_t* ref_rows, int work_count, const BodyBuffers& B, const FrameParams* fp, int launch_flags, cudaStream_t s) {
-    if (STAGE != kStageIncremental && work_count >= kDeepBatchBundles) launch_stage_variant<STAGE, BEPU_DEEP_MINB>(records, ref_rows, work_count, B, fp, launch_flags, s);
-    else launch_stage_variant<STAGE, 1>(records, ref_rows, work_count, B, fp, launch_flags, s);
+    launch_stage_variant<STAGE, 1>(records, ref_rows, work_count, B, fp, launch_flags, shard, s);
 }
 
 #if BEPU_UNIT == 0
-void launch_stage_warm_start_first(const WorkRecord* records, const int32_t* ref_rows, int work_count, const BodyBuffers& B, const FrameParams* fp, int launch_flags, cudaStream_t s) {
-    launch_stage_t<kStageWarmStartFirst>(records, ref_rows, work_count, B, fp, launch_flags, s);
-}
-void launch_stage_warm_start_first_sharded(const WorkRecord* records, const int32_t* ref_rows, int work_count, const BodyBuffers& B, const FrameParams* fp, int launch_flags, const ShardPeers& peers, long long peer_delta, const ShardStage& shard, cudaStream_t s) {
-    launch_stage_sharded_t<kStageWarmStartFirst>(records, ref_rows, work_count, B, fp, launch_flags, peers, peer_delta, shard, s);
+void launch_stage_warm_start_first(const WorkRecord* records, const int32_t* ref_rows, int work_count, const BodyBuffers& B, const FrameParams* fp, int launch_flags, const ShardLaunch* shard, cudaStream_t s) {
+    launch_stage_t<kStageWarmStartFirst>(records, ref_rows, work_count, B, fp, launch_flags, shard, s);
 }
 #elif BEPU_UNIT == 1
-void launch_stage_warm_start(const WorkRecord* records, const int32_t* ref_rows, int work_count, const BodyBuffers& B, const FrameParams* fp, int launch_flags, cudaStream_t s) {
-    launch_stage_t<kStageWarmStart>(records, ref_rows, work_count, B, fp, launch_flags, s);
-}
-void launch_stage_warm_start_sharded(const WorkRecord* records, const int32_t* ref_rows, int work_count, const BodyBuffers& B, const FrameParams* fp, int launch_flags, const ShardPeers& peers, long long peer_delta, const ShardStage& shard, cudaStream_t s) {
-    launch_stage_sharded_t<kStageWarmStart>(records, ref_rows, work_count, B, fp, launch_flags, peers, peer_delta, shard, s);
+void launch_stage_warm_start(const WorkRecord* records, const int32_t* ref_rows, int work_count, const BodyBuffers& B, const FrameParams* fp, int launch_flags, const ShardLaunch* shard, cudaStream_t s) {
+    launch_stage_t<kStageWarmStart>(records, ref_rows, work_count, B, fp, launch_flags, shard, s);
 }
 #elif BEPU_UNIT == 2
-void launch_stage_solve(const WorkRecord* records, const int32_t* ref_rows, int work_count, const BodyBuffers& B, const FrameParams* fp, int launch_flags, cudaStream_t s) {
-    launch_stage_t<kStageSolve>(records, ref_rows, work_count, B, fp, launch_flags, s);
-}
-void launch_stage_solve_sharded(const WorkRecord* records, const int32_t* ref_rows, int work_count, const BodyBuffers& B, const FrameParams* fp, int launch_flags, const ShardPeers& peers, long long peer_delta, const ShardStage& shard, cudaStream_t s) {
-    launch_stage_sharded_t<kStageSolve>(records, ref_rows, work_count, B, fp, launch_flags, peers, peer_delta, shard, s);
+void launch_stage_solve(const WorkRecord* records, const int32_t* ref_rows, int work_count, const BodyBuffers& B, const FrameParams* fp, int launch_flags, const ShardLaunch* shard, cudaStream_t s) {
+    launch_stage_t<kStageSolve>(records, ref_rows, work_count, B, fp, launch_flags, shard, s);
 }
 #elif BEPU_UNIT == 3
-static void launch_constraint_stage(int stage, const WorkRecord* records, const int32_t* ref_rows, int work_count, const BodyBuffers& B, const FrameParams* fp, int launch_flags, cudaStream_t s) {
-    if (work_count <= 0) return;
-    switch (stage) {
-        case kStageWarmStartFirst: launch_stage_warm_start_first(records, ref_rows, work_count, B, fp, launch_flags, s); break;
-        case kStageWarmStart: launch_stage_warm_start(records, ref_rows, work_count, B, fp, launch_flags, s); break;
-        case kStageSolve: launch_stage_solve(records, ref_rows, work_count, B, fp, launch_flags, s); break;
-        case kStageIncremental: launch_stage_t<kStageIncremental>(records, ref_rows, work_count, B, fp, launch_flags, s); break;
-        default: break;
-    }
-}
-static void launch_constraint_stage_sharded(int stage, const WorkRecord* records, const int32_t* ref_rows, int work_count, const BodyBuffers& B, const FrameParams* fp, int launch_flags, const ShardPeers& peers,
-                                            long long peer_delta, const ShardStage& shard, cudaStream_t s) {
-    if (work_count <= 0) return;
-    switch (stage) {
-        case kStageWarmStartFirst: launch_stage_warm_start_first_sharded(records, ref_rows, work_count, B, fp, launch_flags, peers, peer_delta, shard, s); break;
-        case kStageWarmStart: launch_stage_warm_start_sharded(records, ref_rows, work_count, B, fp, launch_flags, peers, peer_delta, shard, s); break;
-        case kStageSolve: launch_stage_solve_sharded(records, ref_rows, work_count, B, fp, launch_flags, peers, peer_delta, shard, s); break;
-        default: break;
-    }
+static void launch_constraint_stage(int stage, const WorkRecord* records, const int32_t* ref_rows, int work_count, const BodyBuffers& B, const FrameParams* fp, int launch_flags,
+                                    const ShardLaunch* shard, cudaStream_t s) {
+    static StageLauncher* const kStages[] = {&launch_stage_warm_start_first, &launch_stage_warm_start, &launch_stage_solve, &launch_stage_t<kStageIncremental>};
+    if (work_count > 0 && stage >= kStageWarmStartFirst && stage <= kStageIncremental) kStages[stage](records, ref_rows, work_count, B, fp, launch_flags, shard, s);
 }
 static void launch_kinematic_stage(int stage, const int32_t* kinematics, int count, const BodyBuffers& B, const FrameParams* fp, cudaStream_t s) {
     if (count <= 0) return;
@@ -127,7 +81,7 @@ static void launch_final_pose(const BodyBuffers& B, const FrameParams* fp, cudaS
     if (B.count <= 0) return;
     final_pose_kernel<<<(unsigned)((B.count + 255) / 256), 256, 0, s>>>(B, fp);
 }
-static const bepucuda::SolverLaunchers kLaunchers = {&launch_constraint_stage, &launch_kinematic_stage, &launch_final_pose, &launch_constraint_stage_sharded};
+static const bepucuda::SolverLaunchers kLaunchers = {&launch_constraint_stage, &launch_kinematic_stage, &launch_final_pose};
 #else
 #error "BEPU_UNIT must be 0..3"
 #endif

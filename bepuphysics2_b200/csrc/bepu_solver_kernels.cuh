@@ -429,6 +429,7 @@ constraint_stage_kernel_sharded(const WorkRecord* __restrict__ records, const in
     constraint_stage_body<STAGE, true>(records, ref_rows, work_count, B, fpp, flags, &peers, peer_delta, &shard);
 }
 
+#if BEPU_UNIT == 3  // the per-body passes are launched from unit 3 only
 // IntegrateKinematicVelocities / IntegrateKinematicPosesAndVelocities (PoseIntegrator.cs:L451-487, L493-535)
 template <int STAGE> BEPU_DI void run_kinematic(int i, const int32_t* kinematics, const BodyBuffers& B, const FrameParams& fp) {
     const uint32_t idx = (uint32_t)kinematics[i];
@@ -498,5 +499,6 @@ static __global__ void final_pose_kernel(BodyBuffers B, const FrameParams* __res
     const FrameParams fp = *fpp;
     run_final_pose(i, B, fp);
 }
+#endif
 
 }  // namespace BEPU_NS

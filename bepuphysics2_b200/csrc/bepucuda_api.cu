@@ -191,7 +191,7 @@ struct bepucuda_ctx {
     std::vector<int32_t> global_first_batch;
     std::vector<uint8_t> global_constrained;
     uint32_t exchange_counter = 0;                                  // exchange points executed so far (flag barrier sequence)
-    uint32_t exchanges_per_solve = 0;
+    uint32_t exchanges_per_solve = 0;                               // exchange points of the stage program (upload_program)
     int inc_work_begin = 0, inc_work_count = 0;
     int all_work_count = 0;                     // work[0 .. all_work_count) covers every bundle once
     int sync_batch_count = 0, fallback_levels = 0;
@@ -308,65 +308,66 @@ void invalidate_graph(bepucuda_ctx* ctx) {
     ctx->graph_valid = false;
 }
 
-// Issues the whole stage sequence of one frame as individual launches on `s` (used directly in STREAM mode and under
-// capture in GRAPH mode). Order: Solver_Solve.cs:L1419-1479, then PoseIntegrator.IntegrateAfterSubstepping.
-void issue_stage_sequence(bepucuda_ctx* ctx, cudaStream_t s, int64_t* launches) {
+// Row prefetch in the PDL prologue (see constraint_stage_kernel): allowed when the stage launched immediately before `op` neither rewrites op's
+// prestep rows (the incremental contact update does) nor its impulses (a stage of the same batch does: single-batch scenes). A rank barrier in
+// between writes no rows, so `previous` skips rank barriers.
+bool rows_prefetchable(const StageOp* previous, const StageOp& op) {
+    return op.stage != kStageIncremental && previous != nullptr && previous->stage != kStageIncremental &&
+           !(previous->stage <= kStageSolve && previous->work_begin == op.work_begin);
+}
+
+// Profiling sink of issue_stage_sequence: the launch of program op i sets launched[i] and is bracketed by events[2i] and events[2i + 1].
+struct StageEvents {
+    const std::vector<cudaEvent_t>& events;
+    std::vector<int>& launched;
+};
+
+// Issues the whole stage sequence of one frame as individual launches on `s` (used directly in STREAM mode and under capture in GRAPH mode).
+// Order: Solver_Solve.cs:L1419-1479, then PoseIntegrator.IntegrateAfterSubstepping. With `profile`, stages are launched without programmatic
+// dependent launch and without row prefetch, so that each event pair times one kernel alone.
+void issue_stage_sequence(bepucuda_ctx* ctx, cudaStream_t s, int64_t* launches, const StageEvents* profile = nullptr) {
     const WorkRecord* records = ctx->record_table.as<WorkRecord>();
     const int32_t* ref_rows = ctx->ref_rows.as<int32_t>();
     const FrameParams* fp = ctx->frame_params_dev.as<FrameParams>();
     const int32_t* kin = ctx->kinematics_dev.as<int32_t>();
+    ShardLaunch shard{ctx->peers, (long long)(ctx->peer32.as<int32_t>() - ctx->refs32.as<int32_t>()), {0, ctx->error_dev.as<int32_t>()}};
     int64_t n = 0;
-    const bool pdl = ctx->cfg.reserved[1] == 0;
-    // Row prefetch in the PDL prologue (see constraint_stage_kernel): allowed when the kernel launched immediately before neither rewrites this
-    // batch's prestep rows (the incremental contact update does) nor its impulses (a stage of the same batch does: single-batch scenes).
-    const StageOp* previous = nullptr;  // last launched op
+    const StageOp* previous = nullptr;  // last launched stage
     uint32_t exchange_index = 0;
-    for (const StageOp& op : ctx->program) {
-        if (op.exchange == kRankBarrier) {
-            // all ranks meet: before the first stage of a solve; around the incremental contact update, which reads the velocities of shared
-            // bodies -- after every peer's last Solve stage has completed, before any peer's WarmStart stage stores into this rank's arrays; and
-            // before the final pose pass
-            launch_shard_barrier(ctx->peers, fp, exchange_index++, ctx->error_dev.as<int32_t>(), s);
-            ++n;
-            continue;
-        }
-        if (op.exchange != kNoExchange) {
-            // sharded stage: it stores the records it writes for shared bodies into the ranks that reference them, and its boundary bundles wait
-            // for and announce arrivals themselves (ShardStage). A batch without constraints on this rank still counts as an exchange point:
-            // nothing arrives from this rank there, and its arrival targets say so.
-            if (op.work_count > 0) {
-                // row prefetch in the prologue: a rank barrier between two stages writes no rows, so the rule of the single-GPU sequence applies
-                bool prefetch = previous != nullptr && previous->stage != kStageIncremental && !(previous->stage <= kStageSolve && previous->work_begin == op.work_begin && previous->work_count > 0);
-                const int launch_flags = (pdl ? kLaunchPdl : 0) | (prefetch ? kLaunchPrefetchRows : 0);
-                const ShardStage shard{exchange_index, ctx->error_dev.as<int32_t>()};
-                ctx->launchers->constraint_stage_sharded(op.stage, records + op.work_begin, ref_rows + (size_t)op.work_begin * 64, op.work_count, ctx->B, fp, launch_flags, ctx->peers,
-                                                         (long long)(ctx->peer32.as<int32_t>() - ctx->refs32.as<int32_t>()), shard, s);
-                ++n;
-                previous = &op;
+    for (size_t i = 0; i < ctx->program.size(); ++i) {
+        const StageOp& op = ctx->program[i];
+        const bool barrier = op.exchange == kRankBarrier;
+        // A sharded stage without constraints on this rank launches nothing but still counts as an exchange point: nothing arrives from this
+        // rank there, and its arrival targets say so.
+        if (barrier || (op.stage == kStageFinalPose ? ctx->B.count > 0 : op.work_count > 0)) {
+            if (profile) cudaEventRecord(profile->events[2 * i], s);
+            if (barrier) {
+                // all ranks meet: before the first stage of a solve; around the incremental contact update, which reads the velocities of shared
+                // bodies -- after every peer's last Solve stage has completed, before any peer's WarmStart stage stores into this rank's arrays; and
+                // before the final pose pass
+                launch_shard_barrier(ctx->peers, fp, exchange_index, ctx->error_dev.as<int32_t>(), s);
+            } else if (op.stage <= kStageIncremental) {
+                // a sharded stage stores the records it writes for shared bodies into the ranks that reference them, and its boundary bundles wait
+                // for and announce arrivals themselves (ShardStage)
+                shard.stage.exchange_index = exchange_index;
+                const int flags = profile ? 0 : kLaunchPdl | (rows_prefetchable(previous, op) ? kLaunchPrefetchRows : 0);
+                ctx->launchers->constraint_stage(op.stage, records + op.work_begin, ref_rows + (size_t)op.work_begin * 64, op.work_count, ctx->B, fp, flags,
+                                                 op.exchange == kNoExchange ? nullptr : &shard, s);
+            } else if (op.stage <= kStageKinematic) {
+                ctx->launchers->kinematic_stage(op.stage, kin, op.work_count, ctx->B, fp, s);
+            } else {
+                ctx->launchers->final_pose(ctx->B, fp, s);
             }
-            ++exchange_index;
-            continue;
+            if (profile) {
+                cudaEventRecord(profile->events[2 * i + 1], s);
+                profile->launched[i] = 1;
+            }
+            if (!barrier) previous = &op;
+            ++n;
         }
-        switch (op.stage) {
-            case kStageWarmStartFirst: case kStageWarmStart: case kStageSolve: case kStageIncremental:
-                if (op.work_count > 0) {
-                    bool prefetch = op.stage != kStageIncremental && previous != nullptr && previous->stage != kStageIncremental;
-                    if (prefetch && previous->stage <= kStageSolve && previous->work_begin == op.work_begin) prefetch = false;
-                    ctx->launchers->constraint_stage(op.stage, records + op.work_begin, ref_rows + (size_t)op.work_begin * 64, op.work_count, ctx->B, fp, (pdl ? kLaunchPdl : 0) | (prefetch ? kLaunchPrefetchRows : 0), s);
-                    previous = &op;
-                    ++n;
-                }
-                break;
-            case kStageKinematicFirst: case kStageKinematic:
-                if (op.work_count > 0) { ctx->launchers->kinematic_stage(op.stage, kin, op.work_count, ctx->B, fp, s); previous = &op; ++n; }
-                break;
-            case kStageFinalPose:
-                if (ctx->B.count > 0) { ctx->launchers->final_pose(ctx->B, fp, s); previous = &op; ++n; }
-                break;
-        }
+        if (op.exchange != kNoExchange) ++exchange_index;
     }
     if (launches) *launches = n;
-    ctx->exchanges_per_solve = exchange_index;
 }
 
 // Builds the flat stage program for the current topology + solve description.
@@ -415,6 +416,7 @@ int upload_program(bepucuda_ctx* ctx) {
             targets[e++] = arrived;
         }
         targets[(size_t)kShardMaxExchanges - 1] = arrived;
+        ctx->exchanges_per_solve = (uint32_t)e;
         CK(cudaStreamSynchronize(ctx->stream));
         for (int q = 0; q < ctx->peers.rank_count; ++q)
             if (q != ctx->peers.rank)
@@ -487,6 +489,27 @@ int refresh_device_rows(bepucuda_ctx* ctx) {
     }
     CK(cudaGetLastError());
     ctx->data_dirty = false;
+    return BEPUCUDA_OK;
+}
+
+// What a frame of length dt needs on the device before its first stage: the refreshed rows, the end of the upload window (bepucuda_timings
+// upload_ms / h2d_bytes) and the frame parameters.
+int prepare_frame(bepucuda_ctx* ctx, float dt) {
+    { int rc = refresh_device_rows(ctx); if (rc != BEPUCUDA_OK) return rc; }
+    if (ctx->up_open) {
+        cudaEventRecord(ctx->ev_up_end, ctx->stream);
+        ctx->up_open = false;
+        ctx->have_up = true;
+    }
+    ctx->timings.h2d_bytes = ctx->h2d_accum;
+    ctx->h2d_accum = 0;
+    // frame parameters (previous solve's copy has completed by stream order only after its graph, a stage profile's before it returned; wait for
+    // it before reusing the pinned struct)
+    CK(cudaEventSynchronize(ctx->ev_solve_end));
+    compute_frame_params(ctx, dt, ctx->frame_params_host);
+    ctx->frame_params_host->exchange_base = ctx->exchange_counter;
+    ctx->frame_params_host->shard_solve_index = ctx->shard_solve_index;
+    CK(cudaMemcpyAsync(ctx->frame_params_dev.ptr, ctx->frame_params_host, sizeof(FrameParams), cudaMemcpyHostToDevice, ctx->stream));
     return BEPUCUDA_OK;
 }
 
@@ -1153,21 +1176,7 @@ int32_t bepucuda_solve(bepucuda_ctx* ctx, float dt) {
         if (rc == BEPUCUDA_OK) rc = bepucuda_end_constraints(ctx);
         if (rc != BEPUCUDA_OK) return rc;
     }
-    { int rc = refresh_device_rows(ctx); if (rc != BEPUCUDA_OK) return rc; }
-    if (ctx->up_open) {
-        cudaEventRecord(ctx->ev_up_end, ctx->stream);
-        ctx->up_open = false;
-        ctx->have_up = true;
-    }
-    ctx->timings.h2d_bytes = ctx->h2d_accum;
-    ctx->h2d_accum = 0;
-    // frame parameters (previous frame's copy has completed by stream order only after its graph; wait for it before reusing the pinned struct)
-    CK(cudaEventSynchronize(ctx->ev_solve_end));
-    compute_frame_params(ctx, dt, ctx->frame_params_host);
-    ctx->frame_params_host->exchange_base = ctx->exchange_counter;
-    ctx->frame_params_host->shard_solve_index = ctx->shard_solve_index;
-    CK(cudaMemcpyAsync(ctx->frame_params_dev.ptr, ctx->frame_params_host, sizeof(FrameParams), cudaMemcpyHostToDevice, ctx->stream));
-
+    { int rc = prepare_frame(ctx, dt); if (rc != BEPUCUDA_OK) return rc; }
     CK(cudaEventRecord(ctx->ev_solve_begin, ctx->stream));
     int64_t launches = 0;
     if (ctx->cfg.execution_mode == BEPUCUDA_EXEC_GRAPH) {
@@ -1309,34 +1318,19 @@ int32_t bepucuda_event_elapsed_ms(bepucuda_ctx* ctx, int32_t a, int32_t b, float
 int32_t bepucuda_profile_stages(bepucuda_ctx* ctx, float dt, bepucuda_stage_profile* out) {
     if (!ctx || !out || !(dt > 0)) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "profile_stages: bad arguments");
     if (!ctx->constraints_ready) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, "profile_stages before end_constraints");
+    if (ctx->peer_mode) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, "profile_stages in peer mode: one rank alone cannot meet its peers at the rank barriers");
     CK(cudaSetDevice(ctx->device));
     std::memset(out, 0, sizeof(*out));
-    { int rc = refresh_device_rows(ctx); if (rc != BEPUCUDA_OK) return rc; }
-    CK(cudaStreamSynchronize(ctx->stream));
-    compute_frame_params(ctx, dt, ctx->frame_params_host);
-    CK(cudaMemcpyAsync(ctx->frame_params_dev.ptr, ctx->frame_params_host, sizeof(FrameParams), cudaMemcpyHostToDevice, ctx->stream));
     const size_t need = ctx->program.size() * 2;
     while (ctx->profile_events.size() < need) {
         cudaEvent_t ev;
         CK(cudaEventCreate(&ev));
         ctx->profile_events.push_back(ev);
     }
-    const WorkRecord* records = ctx->record_table.as<WorkRecord>();
-    const int32_t* ref_rows = ctx->ref_rows.as<int32_t>();
-    const FrameParams* fp = ctx->frame_params_dev.as<FrameParams>();
-    const int32_t* kin = ctx->kinematics_dev.as<int32_t>();
+    { int rc = prepare_frame(ctx, dt); if (rc != BEPUCUDA_OK) return rc; }
     std::vector<int> launched(ctx->program.size(), 0);
-    for (size_t i = 0; i < ctx->program.size(); ++i) {
-        const StageOp& op = ctx->program[i];
-        const bool has_work = op.stage == kStageFinalPose ? ctx->B.count > 0 : op.work_count > 0;
-        if (!has_work) continue;
-        CK(cudaEventRecord(ctx->profile_events[2 * i], ctx->stream));
-        if (op.stage <= kStageIncremental) ctx->launchers->constraint_stage(op.stage, records + op.work_begin, ref_rows + (size_t)op.work_begin * 64, op.work_count, ctx->B, fp, 0, ctx->stream);
-        else if (op.stage <= kStageKinematic) ctx->launchers->kinematic_stage(op.stage, kin, op.work_count, ctx->B, fp, ctx->stream);
-        else ctx->launchers->final_pose(ctx->B, fp, ctx->stream);
-        CK(cudaEventRecord(ctx->profile_events[2 * i + 1], ctx->stream));
-        launched[i] = 1;
-    }
+    const StageEvents sink{ctx->profile_events, launched};
+    issue_stage_sequence(ctx, ctx->stream, nullptr, &sink);
     CK(cudaStreamSynchronize(ctx->stream));
     CK(cudaGetLastError());
     for (size_t i = 0; i < ctx->program.size(); ++i) {

@@ -341,12 +341,11 @@ class Simulation:
 class CudaTimestepper:
     """The Solve slot of DefaultTimestepper.Timestep (DefaultTimestepper.cs:L28-43) on the GPU, through the C ABI only."""
 
-    def __init__(self, simulation, device=0, strict_fp=False, execution_mode=EXEC_GRAPH, disable_pdl=False):
+    def __init__(self, simulation, device=0, strict_fp=False, execution_mode=EXEC_GRAPH):
         self._cuda, self._host = load_libraries()
         self.sim = simulation
         cfg = Config()
         cfg.device_ordinal, cfg.strict_fp, cfg.execution_mode = device, int(bool(strict_fp)), execution_mode
-        cfg.reserved[1] = int(bool(disable_pdl))
         ctx = C.c_void_p()
         rc = self._cuda.bepucuda_create(C.byref(cfg), C.byref(ctx))
         if rc != 0:

@@ -55,7 +55,7 @@ typedef struct bepucuda_config {
      * (RyuJIT does not contract Vector<float> expressions; SURVEY.md §7-5). 0 = FMA contraction on (fast). */
     int32_t strict_fp;
     int32_t execution_mode;   /* enum bepucuda_execution_mode */
-    int32_t reserved[5];      /* reserved[0]: unused; reserved[1]: 1 disables programmatic dependent launch between stage kernels */
+    int32_t reserved[5];      /* reserved: ignored by bepucuda_create */
 } bepucuda_config;
 
 /* Declarative stand-in for the user's IPoseIntegratorCallbacks struct (BepuPhysics/PoseIntegrator.cs:L42-94).
@@ -182,9 +182,12 @@ int32_t bepucuda_get_timings(bepucuda_ctx* ctx, bepucuda_timings* out);
 int32_t bepucuda_event_record(bepucuda_ctx* ctx, int32_t slot);
 int32_t bepucuda_event_elapsed_ms(bepucuda_ctx* ctx, int32_t slot_begin, int32_t slot_end, float* ms);
 
-/* Per-stage-kind device time of ONE frame, measured with a CUDA event pair around every stage launch (plain stream launches, no graph).
+/* Per-stage-kind device time of ONE frame, measured with a CUDA event pair around every stage launch (plain stream launches, no graph, no
+ * programmatic dependent launch between stages).
  * Index by stage kind: 0 WarmStart(first substep), 1 WarmStart, 2 Solve, 3 IncrementallyUpdateForSubstep, 4/5 kinematic prepasses, 6 final pose pass.
- * algorithmic_bytes follows SURVEY.md §8d. Advances the simulation exactly like bepucuda_solve(ctx, dt). */
+ * algorithmic_bytes follows SURVEY.md §8d. Advances the simulation exactly like bepucuda_solve(ctx, dt), with the same kernel launches. A peer-mode
+ * context (bepucuda_shard_import*) returns BEPUCUDA_ERR_BAD_STATE before any device work: one rank alone cannot meet its peers at the rank
+ * barriers. */
 typedef struct bepucuda_stage_profile {
     float ms[8];
     int64_t launches[8];

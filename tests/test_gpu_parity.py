@@ -170,6 +170,35 @@ def test_joint_zoo_with_fallback_batch_and_momentum_conserving_integration(libs)
     assert got["timings"]["fallback_level_count"] > 0
 
 
+def test_profile_stages_advances_like_solve(libs):
+    """bepucuda_profile_stages runs one frame with an event pair around every launch and must advance the simulation exactly like bepucuda_solve:
+    bodies, impulses and contact depths bit for bit against the oracle, and as many launches as a graph solve of the same description. The scene
+    runs every stage kind: contacts (incremental update), joints in the sequential fallback batch, constrained kinematics with
+    IntegrateVelocityForKinematics (both kinematic prepasses), several substeps."""
+    import bepuphysics2_b200 as bp
+
+    integ = util.bp.IntegratorDesc.default()
+    integ.integrate_velocity_for_kinematics = 1
+    scene = scenes.merge(scenes.joint_zoo(250, 60, seed=9), scenes.shape_pile(300, seed=2))
+    kw = dict(fallback_batch_threshold=4, substeps=3, velocity_iterations=2, integrator=integ)
+    ref = util.run_oracle(util.make_sim(scene, **kw), DT)
+    sim = util.make_sim(scene, **kw)
+    ts = bp.CudaTimestepper(sim, strict_fp=True)
+    try:
+        ts.describe()
+        profile = ts.profile_stages(DT)
+        ts.download_bodies()
+        ts.download_impulses()
+        ts.download_prestep()
+    finally:
+        ts.close()
+    util.compare(ref, util.snapshot(sim), exact=True)
+    assert all(profile.launches[stage] > 0 for stage in range(7))
+    graph = util.run_gpu(util.make_sim(scene, **kw), DT, strict=True, mode=EXEC_GRAPH)
+    assert graph["timings"]["fallback_level_count"] > 0
+    assert sum(profile.launches) == graph["timings"]["kernel_launches"]
+
+
 def test_joint_zoo_fast_build_within_tolerance(libs):
     """Fast (FMA, approximate sqrt) build on the full zoo after one frame: relative RMS error <= 1e-3, max abs error <= 5e-2."""
     _parity(scenes.joint_zoo(1500, 120, seed=6), exact=False, rel_rms=1e-3, max_abs=5e-2, substeps=2, velocity_iterations=2)

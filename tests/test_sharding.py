@@ -1,5 +1,6 @@
 """One constraint graph over several GPUs (SURVEY.md §8e): the host partitioner (CPU: invariants, and a world-size-2 gloo run showing both ranks derive
 the same global tables from the same scene) and, on the GPU, several ranks as contexts of one process on one device against the oracle, bit for bit."""
+import ctypes
 import os
 import subprocess
 import sys
@@ -185,6 +186,31 @@ def test_peer_mode_needs_body_masks(libs):
             s._check(cuda.bepucuda_end_constraints(s._ctx))
         assert e.value.code == -6 and "shard_set_body_masks" in str(e.value)  # BEPUCUDA_ERR_BAD_STATE
         s.describe()
+    finally:
+        for s in solvers:
+            s.close()
+
+
+@pytest.mark.gpu
+def test_profile_stages_is_refused_in_peer_mode(libs):
+    """A stage profile is a frame of one rank alone, which cannot meet its peers at the rank barriers: a described peer-mode context refuses it
+    before any device work, so its bodies stay as uploaded."""
+    sim = util.make_sim(scenes.shape_pile(400, seed=4), substeps=2, velocity_iterations=1)
+    solvers = [sharding.ShardedSolver(sim, r, 2, 0, strict_fp=True) for r in range(2)]
+    try:
+        for s in solvers:
+            s.export_handles()
+        for s in solvers:
+            s.import_contexts(solvers)
+        for s in solvers:
+            s.describe()
+        s = solvers[0]
+        profile = native.StageProfile()
+        assert s._cuda.bepucuda_profile_stages(s._ctx, DT, ctypes.byref(profile)) == -6  # BEPUCUDA_ERR_BAD_STATE
+        assert sum(profile.launches) == 0
+        mine = s.referenced_bodies()
+        got = s.download()
+        assert np.array_equal(sim.bodies[mine][:, util.MOTION].view(np.uint32), got[mine][:, util.MOTION].view(np.uint32))
     finally:
         for s in solvers:
             s.close()

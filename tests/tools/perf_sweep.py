@@ -32,12 +32,12 @@ print(scene["description"], flush=True)
 flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")
 
 
-def run(mode, do_flush=True, strict=False, pdl=True):
+def run(mode, do_flush=True, strict=False):
     sim = bp.Simulation(substeps=args.substeps, velocity_iterations=args.iterations)
     t0 = time.time()
     scenes.build(scene, sim)
     build_s = time.time() - t0
-    ts = bp.CudaTimestepper(sim, strict_fp=strict, execution_mode=mode, disable_pdl=not pdl)
+    ts = bp.CudaTimestepper(sim, strict_fp=strict, execution_mode=mode)
     t0 = time.time()
     ts.describe()
     ts.synchronize()
@@ -53,19 +53,14 @@ def run(mode, do_flush=True, strict=False, pdl=True):
             ms.append(t.solve_ms)
     ci = t.constraint_iterations
     name = {EXEC_GRAPH: "graph", EXEC_STREAM: "stream"}[mode]
-    print("%-10s flush=%d strict=%d pdl=%d : %.3f ms/step (min %.3f)  %.2f G CI/s  batches=%d stages=%d alg=%.1f GB/s  [build %.1fs describe %.2fs]" % (
-        name, do_flush, strict, pdl, np.mean(ms), np.min(ms), ci / np.mean(ms) / 1e6, t.device_batch_count, t.stage_count, t.algorithmic_bytes / np.mean(ms) / 1e6, build_s, describe_s), flush=True)
+    print("%-10s flush=%d strict=%d : %.3f ms/step (min %.3f)  %.2f G CI/s  batches=%d stages=%d alg=%.1f GB/s  [build %.1fs describe %.2fs]" % (
+        name, do_flush, strict, np.mean(ms), np.min(ms), ci / np.mean(ms) / 1e6, t.device_batch_count, t.stage_count, t.algorithmic_bytes / np.mean(ms) / 1e6, build_s, describe_s), flush=True)
     ts.close()
 
 
-if os.environ.get("SWEEP", "full") == "graph":
-    run(EXEC_GRAPH)
-    run(EXEC_GRAPH, pdl=False)
-else:
-    run(EXEC_GRAPH)
-    run(EXEC_GRAPH, pdl=False)
+run(EXEC_GRAPH)
+if os.environ.get("SWEEP", "full") != "graph":
     run(EXEC_STREAM)
-    run(EXEC_STREAM, pdl=False)
     run(EXEC_GRAPH, strict=True)
 
 if args.cpu:

@@ -18,7 +18,7 @@ args = ap.parse_args()
 scene = scenes.shape_pile(args.bodies, seed=5) if args.scene == "shape_pile" else scenes.ragdolls(args.bodies // 16, seed=5)
 sim = bp.Simulation(substeps=args.substeps, velocity_iterations=args.iterations)
 scenes.build(scene, sim)
-ts = bp.CudaTimestepper(sim, execution_mode=EXEC_STREAM, disable_pdl=True)
+ts = bp.CudaTimestepper(sim, execution_mode=EXEC_STREAM)
 ts.describe()
 for _ in range(args.frames):
     ts.solve_device_only(1 / 60)
