@@ -4,6 +4,7 @@
 // (168 B per body); the bounding boxes of every body are independent, so there is nothing to order.
 #define BEPU_NS bepu_bounds_math
 #include "bepu_bounds_math.cuh"
+#include "bepu_integration.cuh"
 #include "bepu_bounds.h"
 
 namespace bepucuda {
@@ -30,6 +31,17 @@ __global__ void predict_bounding_boxes_kernel(BodyBuffers B, const BodyShape* __
     if (integrate) {
         velocity.lin = (velocity.lin + V3{p.gravity_dt[0], p.gravity_dt[1], p.gravity_dt[2]}) * p.linear_damping_dt;
         velocity.ang = velocity.ang * p.angular_damping_dt;
+        if (p.integrate_extensions) {
+            V3 linearAcceleration{0.0f, 0.0f, 0.0f}, angularAcceleration{0.0f, 0.0f, 0.0f};
+            if (p.integrate_extensions & kIntegrateAccelerations) {
+                const float4 a0 = p.accelerations[2 * (size_t)i], a1 = p.accelerations[2 * (size_t)i + 1];
+                linearAcceleration = {a0.x, a0.y, a0.z};
+                angularAcceleration = {a1.x, a1.y, a1.z};
+            }
+            integrate_velocity_extensions(velocity, (p.integrate_extensions & kIntegrateAccelerations) != 0, linearAcceleration, angularAcceleration, p.dt,
+                                          (p.integrate_extensions & kIntegratePointGravity) != 0, position,
+                                          V3{p.attractor_center[0], p.attractor_center[1], p.attractor_center[2]}, p.attractor_dt);
+        }
     }
     // UpdateSleepCandidacy (PoseIntegrator.cs:L286-304)
     BodyActivityRecord activity = activities[i];

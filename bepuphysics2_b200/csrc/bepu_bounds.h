@@ -28,6 +28,11 @@ struct PredictParams {
     float gravity_dt[3];           // PrepareForIntegration(dt) of the declarative callback (Demos/DemoCallbacks.cs:L79-86), with the FULL frame dt
     float linear_damping_dt, angular_damping_dt;
     int32_t integrate_velocity_for_kinematics;
+    // bepucuda_set_body_accelerations / bepucuda_set_point_gravity, as in FrameParams (with the frame dt)
+    const float4* accelerations;
+    uint32_t integrate_extensions;
+    float attractor_center[3];
+    float attractor_dt;
 };
 // bounds: 8 floats per body {min.xyz, speculative margin, max.xyz, 1 if bounds were produced else 0}
 void launch_predict_bounding_boxes(const BodyBuffers& B, const BodyShape* shapes, BodyActivityRecord* activities, float4* bounds, const PredictParams& params, cudaStream_t s);

@@ -63,7 +63,15 @@ struct FrameParams {
     int32_t integrate_velocity_for_kinematics;
     uint32_t exchange_base;    // peer sharding: number of cross-GPU exchange points executed before this solve (the flag barrier counts them)
     uint32_t shard_solve_index;  // peer sharding: solves since the arrival targets were last published (the arrival counters keep counting)
+    // bepucuda_set_body_accelerations / bepucuda_set_point_gravity: the optional velocity terms after the declarative callback
+    uint32_t accelerations[2];     // device address of the per-body array {a.xyz 0 | alpha.xyz 0} (active-set index) as two words, which keeps the
+                                   // struct 4-byte aligned like every field the stage kernels copy; read only with kIntegrateAccelerations
+    uint32_t integrate_extensions;  // kIntegrateAccelerations | kIntegratePointGravity; 0 = the declarative callback alone
+    float attractor_center[3];
+    float attractor_dt;            // PrepareForIntegration(substep dt) of the point gravity: dt * strength
+    float final_attractor_dt;      // the same with final_dt
 };
+constexpr uint32_t kIntegrateAccelerations = 1u, kIntegratePointGravity = 2u;
 
 enum Stage : int32_t {
     kStageWarmStartFirst = 0,  // substep 0: integrate velocity only (DisallowPoseIntegration)

@@ -20,6 +20,23 @@ BEPU_DI void callback_integrate_velocity(Velocity& v, float gx, float gy, float 
     v.lin = (v.lin + V3{gx, gy, gz}) * linearDampingDt;
     v.ang = v.ang * angularDampingDt;
 }
+// The two optional terms of bepucuda_set_body_accelerations / bepucuda_set_point_gravity, applied after callback_integrate_velocity wherever its
+// result is kept. Per-body accelerations (PerBodyGravityDemo.cs:L57-88): v += a * dt, not damped. Point gravity (PlanetDemo.cs:L36-47), in its
+// operation order: offset = position - center, v.lin -= (attractorDt * offset) * (1 / max(1, |offset|^3)), with attractorDt = dt * strength from
+// PrepareForIntegration; Vector3Wide / Vector<float> multiplies by the reciprocal (Vector3Wide.cs:L357-363).
+BEPU_DI void integrate_velocity_extensions(Velocity& v, bool accelerations, V3 linearAcceleration, V3 angularAcceleration, float dt, bool pointGravity, V3 position,
+                                           V3 center, float attractorDt) {
+    if (accelerations) {
+        v.lin = v.lin + linearAcceleration * dt;
+        v.ang = v.ang + angularAcceleration * dt;
+    }
+    if (pointGravity) {
+        const V3 offset = position - center;
+        const float distance = length(offset);
+        const float inverse = 1.0f / fmaxf(1.0f, distance * distance * distance);
+        v.lin = v.lin - (offset * attractorDt) * inverse;
+    }
+}
 BEPU_DI void fallback_if_inertia_incompatible(V3 previous, V3& w) {  // L180-190
     const float inf = __int_as_float(0x7f800000);
     bool useNew = fabsf(w.x) < inf && fabsf(w.y) < inf && fabsf(w.z) < inf;

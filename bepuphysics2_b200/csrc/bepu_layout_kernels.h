@@ -56,7 +56,7 @@ void launch_boundary_flags(const WorkRecord* records, int count, const int32_t* 
 void launch_pack_ref_rows(const WorkRecord* records, int count, int32_t* rows, cudaStream_t s);
 
 // Numerics flavours (bepu_solver_kernels.cu, compiled twice).
-constexpr int kLaunchPdl = 1, kLaunchPrefetchRows = 2;
+constexpr int kLaunchPdl = 1, kLaunchPrefetchRows = 2, kLaunchIntegratorExtensions = 4;
 // Peer-sharded stage (bepucuda_shard_*): every written body record also goes to the ranks named by the per-(lane, slot) destination masks at
 // refs + peer_delta (launch_fill_peer_masks).
 struct ShardLaunch {
@@ -68,12 +68,14 @@ struct SolverLaunchers {
     // Launches one constraint stage (kStageWarmStartFirst / kStageWarmStart / kStageSolve / kStageIncremental) over `work_count` bundles.
     // launch_flags: kLaunchPdl = launch with programmatic stream serialization (the kernel overlaps its prologue with the previous stage);
     // kLaunchPrefetchRows = the kernel launched just before this one writes neither this batch's prestep nor its impulses, so the prologue may fetch them.
+    // kLaunchIntegratorExtensions = per-body accelerations or point gravity are set: the WarmStart stages run the instantiation that applies them.
     // ref_rows: the packed reference rows of records[0 .. work_count) (launch_pack_ref_rows).
     // shard: nullptr on a single GPU; a WarmStartFirst / WarmStart / Solve stage of a peer-sharded solve otherwise.
     void (*constraint_stage)(int stage, const WorkRecord* records, const int32_t* ref_rows, int work_count, const BodyBuffers& B, const FrameParams* fp, int launch_flags,
                              const ShardLaunch* shard, cudaStream_t s);
-    void (*kinematic_stage)(int stage, const int32_t* kinematics, int count, const BodyBuffers& B, const FrameParams* fp, cudaStream_t s);
-    void (*final_pose)(const BodyBuffers& B, const FrameParams* fp, cudaStream_t s);
+    // launch_flags: kLaunchIntegratorExtensions or 0 (the other bits do not apply to the per-body passes)
+    void (*kinematic_stage)(int stage, const int32_t* kinematics, int count, const BodyBuffers& B, const FrameParams* fp, int launch_flags, cudaStream_t s);
+    void (*final_pose)(const BodyBuffers& B, const FrameParams* fp, int launch_flags, cudaStream_t s);
 };
 const SolverLaunchers* get_launchers_bepu_fast();
 const SolverLaunchers* get_launchers_bepu_strict();

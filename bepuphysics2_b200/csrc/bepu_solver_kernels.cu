@@ -37,13 +37,23 @@ static void launch_stage_kernel(int work_count, int launch_flags, cudaStream_t s
     cfg.numAttrs = (launch_flags & bepucuda::kLaunchPdl) ? 1 : 0;
     cudaLaunchKernelEx(&cfg, Kernel, args...);
 }
+template <int STAGE, int MINB, bool kExt>
+static void launch_stage_instance(const WorkRecord* records, const int32_t* ref_rows, int work_count, const BodyBuffers& B, const FrameParams* fp, int launch_flags, const ShardLaunch* shard,
+                                  cudaStream_t s) {
+    const int flags = (launch_flags & bepucuda::kLaunchPrefetchRows) ? kStagePrefetchRows : 0;
+    if (!shard) launch_stage_kernel<constraint_stage_kernel<STAGE, MINB, kExt>>(work_count, launch_flags, s, records, ref_rows, work_count, B, fp, flags);
+    else if constexpr (STAGE != kStageIncremental)  // the incremental contact update is never sharded
+        launch_stage_kernel<constraint_stage_kernel_sharded<STAGE, MINB, kExt>>(work_count, launch_flags, s, records, ref_rows, work_count, B, fp, flags, shard->peers, shard->peer_delta,
+                                                                               shard->stage);
+}
+// The WarmStart stages integrate: contexts with per-body accelerations or point gravity run their own instantiation (kLaunchIntegratorExtensions).
 template <int STAGE, int MINB>
 static void launch_stage_variant(const WorkRecord* records, const int32_t* ref_rows, int work_count, const BodyBuffers& B, const FrameParams* fp, int launch_flags, const ShardLaunch* shard,
                                  cudaStream_t s) {
-    const int flags = (launch_flags & bepucuda::kLaunchPrefetchRows) ? kStagePrefetchRows : 0;
-    if (!shard) launch_stage_kernel<constraint_stage_kernel<STAGE, MINB>>(work_count, launch_flags, s, records, ref_rows, work_count, B, fp, flags);
-    else if constexpr (STAGE != kStageIncremental)  // the incremental contact update is never sharded
-        launch_stage_kernel<constraint_stage_kernel_sharded<STAGE, MINB>>(work_count, launch_flags, s, records, ref_rows, work_count, B, fp, flags, shard->peers, shard->peer_delta, shard->stage);
+    if constexpr (STAGE == kStageWarmStartFirst || STAGE == kStageWarmStart) {
+        if (launch_flags & bepucuda::kLaunchIntegratorExtensions) return launch_stage_instance<STAGE, MINB, true>(records, ref_rows, work_count, B, fp, launch_flags, shard, s);
+    }
+    launch_stage_instance<STAGE, MINB, false>(records, ref_rows, work_count, B, fp, launch_flags, shard, s);
 }
 template <int STAGE>
 static void launch_stage_t(const WorkRecord* records, const int32_t* ref_rows, int work_count, const BodyBuffers& B, const FrameParams* fp, int launch_flags, const ShardLaunch* shard, cudaStream_t s) {
@@ -71,15 +81,22 @@ static void launch_constraint_stage(int stage, const WorkRecord* records, const 
     static StageLauncher* const kStages[] = {&launch_stage_warm_start_first, &launch_stage_warm_start, &launch_stage_solve, &launch_stage_t<kStageIncremental>};
     if (work_count > 0 && stage >= kStageWarmStartFirst && stage <= kStageIncremental) kStages[stage](records, ref_rows, work_count, B, fp, launch_flags, shard, s);
 }
-static void launch_kinematic_stage(int stage, const int32_t* kinematics, int count, const BodyBuffers& B, const FrameParams* fp, cudaStream_t s) {
-    if (count <= 0) return;
+// The per-body passes, like the WarmStart stages, have an instantiation of their own for per-body accelerations or point gravity.
+template <bool kExt> static void launch_kinematic_instance(int stage, const int32_t* kinematics, int count, const BodyBuffers& B, const FrameParams* fp, cudaStream_t s) {
     const unsigned blocks = (unsigned)((count + 127) / 128);
-    if (stage == kStageKinematicFirst) kinematic_stage_kernel<kStageKinematicFirst><<<blocks, 128, 0, s>>>(kinematics, count, B, fp);
-    else kinematic_stage_kernel<kStageKinematic><<<blocks, 128, 0, s>>>(kinematics, count, B, fp);
+    if (stage == kStageKinematicFirst) kinematic_stage_kernel<kStageKinematicFirst, kExt><<<blocks, 128, 0, s>>>(kinematics, count, B, fp);
+    else kinematic_stage_kernel<kStageKinematic, kExt><<<blocks, 128, 0, s>>>(kinematics, count, B, fp);
 }
-static void launch_final_pose(const BodyBuffers& B, const FrameParams* fp, cudaStream_t s) {
+static void launch_kinematic_stage(int stage, const int32_t* kinematics, int count, const BodyBuffers& B, const FrameParams* fp, int launch_flags, cudaStream_t s) {
+    if (count <= 0) return;
+    if (launch_flags & bepucuda::kLaunchIntegratorExtensions) launch_kinematic_instance<true>(stage, kinematics, count, B, fp, s);
+    else launch_kinematic_instance<false>(stage, kinematics, count, B, fp, s);
+}
+static void launch_final_pose(const BodyBuffers& B, const FrameParams* fp, int launch_flags, cudaStream_t s) {
     if (B.count <= 0) return;
-    final_pose_kernel<<<(unsigned)((B.count + 255) / 256), 256, 0, s>>>(B, fp);
+    const unsigned blocks = (unsigned)((B.count + 255) / 256);
+    if (launch_flags & bepucuda::kLaunchIntegratorExtensions) final_pose_kernel<true><<<blocks, 256, 0, s>>>(B, fp);
+    else final_pose_kernel<false><<<blocks, 256, 0, s>>>(B, fp);
 }
 static const bepucuda::SolverLaunchers kLaunchers = {&launch_constraint_stage, &launch_kinematic_stage, &launch_final_pose};
 #else

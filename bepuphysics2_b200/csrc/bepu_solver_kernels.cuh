@@ -62,10 +62,33 @@ BEPU_DI void load_pose(const float4* pose, uint32_t i, V3& pos, Q4& q) {
 }
 BEPU_DI void store_pose(float4* pose, uint32_t i, V3 pos, Q4 q) { st256(pose + 2 * (size_t)i, q.x, q.y, q.z, q.w, pos.x, pos.y, pos.z, 0.0f); }
 
+// Per-body accelerations and point gravity (FrameParams::integrate_extensions != 0) at one integrating lane, after the declarative callback. Out of
+// line, like the momentum-conserving angular modes, and reached only from the kExt instantiations of the WarmStart stages and the per-body
+// passes. dt / attractorDt are those of the site's PrepareForIntegration; position is the pose the reference hands the callback there.
+static __device__ __noinline__ Velocity integrate_velocity_extensions_at(uint32_t flags, const float4* accelerations, uint32_t idx, V3 lin, V3 ang, float dt, V3 position, V3 center,
+                                                                         float attractorDt) {
+    Velocity v{lin, ang};
+    V3 linearAcceleration{0.0f, 0.0f, 0.0f}, angularAcceleration{0.0f, 0.0f, 0.0f};
+    if (flags & kIntegrateAccelerations) {
+        const F8 a = ld256(accelerations + 2 * (size_t)idx);
+        linearAcceleration = {a.a, a.b, a.c};
+        angularAcceleration = {a.e, a.f, a.g};
+    }
+    integrate_velocity_extensions(v, (flags & kIntegrateAccelerations) != 0, linearAcceleration, angularAcceleration, dt, (flags & kIntegratePointGravity) != 0, position, center,
+                                  attractorDt);
+    return v;
+}
+BEPU_DI void apply_velocity_extensions(const FrameParams& fp, uint32_t idx, V3 position, float dt, float attractorDt, Velocity& v) {
+    const float4* accelerations = reinterpret_cast<const float4*>((unsigned long long)fp.accelerations[0] | ((unsigned long long)fp.accelerations[1] << 32));
+    v = integrate_velocity_extensions_at(fp.integrate_extensions, accelerations, idx, v.lin, v.ang, dt, position, V3{fp.attractor_center[0], fp.attractor_center[1], fp.attractor_center[2]},
+                                         attractorDt);
+}
+
 // GatherAndIntegrate for one body slot of one lane (TypeProcessor.cs:L1298-1397), after the velocity has been loaded. The lane integrates iff the
 // device body reference carries kRefIntegrateBit; all other lanes read the world inertia their owner constraint stored earlier in this substep,
-// which is bit-identical to what the reference's bundle-wide recompute would give them.
-template <int STAGE, bool NeedsPose>
+// which is bit-identical to what the reference's bundle-wide recompute would give them. kExt: the stage kernel instantiation for contexts with
+// per-body accelerations or point gravity (the launcher picks it), so that the default path carries none of it.
+template <int STAGE, bool NeedsPose, bool kExt>
 BEPU_DI void warm_start_body(uint32_t enc, const BodyBuffers& B, const FrameParams& fp, BodyState& b, Velocity& v) {
     const uint32_t idx = enc & kRefIndexMask;
     if (enc & kRefIntegrateBit) {
@@ -93,6 +116,8 @@ BEPU_DI void warm_start_body(uint32_t enc, const BodyBuffers& B, const FramePara
             }
         }
         callback_integrate_velocity(v, fp.gravity_dt[0], fp.gravity_dt[1], fp.gravity_dt[2], fp.linear_damping_dt, fp.angular_damping_dt);
+        // the callback sees the current pose in the first substep and the freshly integrated one after (TypeProcessor.cs:L1244, L1276)
+        if constexpr (kExt) apply_velocity_extensions(fp, idx, b.pos, fp.dt, fp.attractor_dt, v);
         store_inertia(B.inertia_world, idx, b.inertia);
     } else {
         load_inertia(B.inertia_world, idx, b.inertia);
@@ -111,10 +136,10 @@ BEPU_DI void warm_start_body(uint32_t enc, const BodyBuffers& B, const FramePara
         }
     }
 }
-template <int STAGE, bool NeedsPose>
+template <int STAGE, bool NeedsPose, bool kExt>
 BEPU_DI void gather_for_warm_start(uint32_t enc, const BodyBuffers& B, const FrameParams& fp, BodyState& b, Velocity& v) {
     load_velocity(B.velocity, enc & kRefIndexMask, v);
-    warm_start_body<STAGE, NeedsPose>(enc, B, fp, b, v);
+    warm_start_body<STAGE, NeedsPose, kExt>(enc, B, fp, b, v);
 }
 
 // ---- uniform call shapes over contact and joint types ------------------------------------------------------------------
@@ -154,7 +179,7 @@ BEPU_DI void push_record(float4* const* arrays, uint32_t mask, uint32_t idx, flo
         dst[1] = make_float4(e, f, g, h);
     }
 }
-template <class T, int STAGE, bool kSharded, class PR, class AR>
+template <class T, int STAGE, bool kSharded, bool kExt, class PR, class AR>
 BEPU_DI void run_lane(const int32_t* refs, PR p, AR a, float* p_rw, uint32_t enc0, uint32_t enc1, const BodyBuffers& B, const FrameParams& fp, const ShardPeers* peers = nullptr,
                       long long peer_delta = 0) {
     constexpr int NB = T::kBodies;
@@ -196,7 +221,7 @@ BEPU_DI void run_lane(const int32_t* refs, PR p, AR a, float* p_rw, uint32_t enc
             }
     } else {
 #pragma unroll
-        for (int s = 0; s < NB; ++s) gather_for_warm_start<STAGE, T::kNeedsPose>(enc[s], B, fp, b[s], v[s]);
+        for (int s = 0; s < NB; ++s) gather_for_warm_start<STAGE, T::kNeedsPose, kExt>(enc[s], B, fp, b[s], v[s]);
         rows_ready(p);
         call_warm_start<T>(b, p, a, v);
 #pragma unroll
@@ -220,7 +245,7 @@ BEPU_DI void run_lane(const int32_t* refs, PR p, AR a, float* p_rw, uint32_t enc
 }
 template <class T, int STAGE, class PR, class AR>
 BEPU_DI void run_lane(const int32_t* refs, PR p, AR a, float* p_rw, uint32_t enc0, uint32_t enc1, const BodyBuffers& B, const FrameParams& fp) {
-    run_lane<T, STAGE, false>(refs, p, a, p_rw, enc0, enc1, B, fp);
+    run_lane<T, STAGE, false, false>(refs, p, a, p_rw, enc0, enc1, B, fp);
 }
 
 // Work records and body references are loaded with `asm volatile` so that the loads are ISSUED where the source places them (a whole pipeline
@@ -248,14 +273,14 @@ BEPU_DI WorkRecord load_record(const WorkRecord* r) {
     X(8, NonconvexOneBody<2>) X(9, NonconvexOneBody<3>) X(10, NonconvexOneBody<4>)                                                \
     X(15, NonconvexTwoBody<2>) X(16, NonconvexTwoBody<3>) X(17, NonconvexTwoBody<4>)
 
-template <int STAGE, bool kSharded, class PR, class AR>
+template <int STAGE, bool kSharded, bool kExt, class PR, class AR>
 BEPU_DI void run_bundle_rows(const WorkRecord& rec, int lane, PR p, AR a, uint32_t enc0, uint32_t enc1, const BodyBuffers& B, const FrameParams& fp, const ShardPeers* peers = nullptr,
                              long long peer_delta = 0) {
     const int32_t* refs = rec.refs + lane;
     float* p_rw = rec.prestep + lane;
     switch (rec.type_id) {
 #define BEPU_CASE(ID, T) \
-    case ID: run_lane<T, STAGE, kSharded>(refs, p, a, p_rw, enc0, enc1, B, fp, peers, peer_delta); break;
+    case ID: run_lane<T, STAGE, kSharded, kExt>(refs, p, a, p_rw, enc0, enc1, B, fp, peers, peer_delta); break;
         BEPU_CONTACT_TYPES(BEPU_CASE)
         BEPU_JOINT_TYPES(BEPU_CASE)
         BEPU_JOINT_TYPES_MORE(BEPU_CASE)
@@ -265,7 +290,7 @@ BEPU_DI void run_bundle_rows(const WorkRecord& rec, int lane, PR p, AR a, uint32
 }
 template <int STAGE, class PR, class AR>
 BEPU_DI void run_bundle_rows(const WorkRecord& rec, int lane, PR p, AR a, uint32_t enc0, uint32_t enc1, const BodyBuffers& B, const FrameParams& fp) {
-    run_bundle_rows<STAGE, false>(rec, lane, p, a, enc0, enc1, B, fp);
+    run_bundle_rows<STAGE, false, false>(rec, lane, p, a, enc0, enc1, B, fp);
 }
 // Rows straight from HBM (the incremental stage).
 template <int STAGE>
@@ -349,7 +374,7 @@ BEPU_DI void shard_wait(const ShardPeers& peers, int lane, uint32_t solve_index,
     }
     __syncwarp();
 }
-template <int STAGE, bool kSharded>
+template <int STAGE, bool kSharded, bool kExt>
 BEPU_DI void constraint_stage_body(const WorkRecord* __restrict__ records, const int32_t* __restrict__ ref_rows, int work_count, const BodyBuffers& B, const FrameParams* __restrict__ fpp, int flags, const ShardPeers* peers,
                                    long long peer_delta, const ShardStage* shard = nullptr) {
     constexpr bool kStaged = STAGE != kStageIncremental;
@@ -404,7 +429,7 @@ BEPU_DI void constraint_stage_body(const WorkRecord* __restrict__ records, const
             bulk_copy_g2s(slab_addr + prestep_bytes, rec.impulses, impulse_bytes, bar, policy);
         }
         __syncwarp();
-        run_bundle_rows<STAGE, kSharded>(rec, lane, StagedRows{slab_addr + lane * 4, bar, 0u}, StagedAcc{slab_addr + prestep_bytes + lane * 4, rec.impulses + lane}, enc0, enc1, B, fp,
+        run_bundle_rows<STAGE, kSharded, kExt>(rec, lane, StagedRows{slab_addr + lane * 4, bar, 0u}, StagedAcc{slab_addr + prestep_bytes + lane * 4, rec.impulses + lane}, enc0, enc1, B, fp,
                                          peers, boundary ? peer_delta : 0);
         if constexpr (kSharded) {
             if (boundary) {
@@ -417,27 +442,27 @@ BEPU_DI void constraint_stage_body(const WorkRecord* __restrict__ records, const
     }
 }
 
-template <int STAGE, int MINB>
+template <int STAGE, int MINB, bool kExt>
 __global__ void __launch_bounds__(kStageBlockThreads, MINB) constraint_stage_kernel(const WorkRecord* __restrict__ records, const int32_t* __restrict__ ref_rows, int work_count, BodyBuffers B, const FrameParams* __restrict__ fpp, int flags) {
-    constraint_stage_body<STAGE, false>(records, ref_rows, work_count, B, fpp, flags, nullptr, 0);
+    constraint_stage_body<STAGE, false, kExt>(records, ref_rows, work_count, B, fpp, flags, nullptr, 0);
 }
 // Peer-sharded variant (bepucuda_shard_*): the lane that writes a body another rank references stores the record into that rank's arrays too.
-template <int STAGE, int MINB>
+template <int STAGE, int MINB, bool kExt>
 __global__ void __launch_bounds__(kStageBlockThreads, MINB)
 constraint_stage_kernel_sharded(const WorkRecord* __restrict__ records, const int32_t* __restrict__ ref_rows, int work_count, BodyBuffers B, const FrameParams* __restrict__ fpp, int flags, const __grid_constant__ ShardPeers peers,
                                 long long peer_delta, const __grid_constant__ ShardStage shard) {
-    constraint_stage_body<STAGE, true>(records, ref_rows, work_count, B, fpp, flags, &peers, peer_delta, &shard);
+    constraint_stage_body<STAGE, true, kExt>(records, ref_rows, work_count, B, fpp, flags, &peers, peer_delta, &shard);
 }
 
 #if BEPU_UNIT == 3  // the per-body passes are launched from unit 3 only
 // IntegrateKinematicVelocities / IntegrateKinematicPosesAndVelocities (PoseIntegrator.cs:L451-487, L493-535)
-template <int STAGE> BEPU_DI void run_kinematic(int i, const int32_t* kinematics, const BodyBuffers& B, const FrameParams& fp) {
+template <int STAGE, bool kExt> BEPU_DI void run_kinematic(int i, const int32_t* kinematics, const BodyBuffers& B, const FrameParams& fp) {
     const uint32_t idx = (uint32_t)kinematics[i];
     Velocity v;
     load_velocity(B.velocity, idx, v);
+    V3 pos{0.0f, 0.0f, 0.0f};
+    Q4 q;
     if (STAGE == kStageKinematic) {
-        V3 pos;
-        Q4 q;
         load_pose(B.pose, idx, pos, q);
         pos = pos + v.lin * fp.dt;
         q = integrate_orientation(q, v.ang, fp.dt * 0.5f);
@@ -445,19 +470,24 @@ template <int STAGE> BEPU_DI void run_kinematic(int i, const int32_t* kinematics
     }
     if (fp.integrate_velocity_for_kinematics) {
         callback_integrate_velocity(v, fp.gravity_dt[0], fp.gravity_dt[1], fp.gravity_dt[2], fp.linear_damping_dt, fp.angular_damping_dt);
+        if constexpr (kExt) {
+            // the callback sees the gathered pose in the first substep (PoseIntegrator.cs:L480) and the integrated one after (L529)
+            if (STAGE == kStageKinematicFirst && (fp.integrate_extensions & kIntegratePointGravity)) load_pose(B.pose, idx, pos, q);
+            apply_velocity_extensions(fp, idx, pos, fp.dt, fp.attractor_dt, v);
+        }
         store_velocity(B.velocity, idx, v);
     }
 }
-template <int STAGE>
+template <int STAGE, bool kExt>
 __global__ void kinematic_stage_kernel(const int32_t* __restrict__ kinematics, int count, BodyBuffers B, const FrameParams* __restrict__ fpp) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= count) return;
     const FrameParams fp = *fpp;
-    run_kinematic<STAGE>(i, kinematics, B, fp);
+    run_kinematic<STAGE, kExt>(i, kinematics, B, fp);
 }
 
 // IntegrateBundlesAfterSubstepping (PoseIntegrator.cs:L537-693), per body.
-BEPU_DI void run_final_pose(int i, const BodyBuffers& B, const FrameParams& fp) {
+template <bool kExt> BEPU_DI void run_final_pose(int i, const BodyBuffers& B, const FrameParams& fp) {
     V3 pos;
     Q4 q;
     Velocity v;
@@ -476,8 +506,10 @@ BEPU_DI void run_final_pose(int i, const BodyBuffers& B, const FrameParams& fp) 
     const bool integrateVelocity = fp.integrate_velocity_for_kinematics || !kinematic;
     const float dt = fp.final_dt, halfDt = fp.final_dt * 0.5f;
     for (int step = 0; step < fp.final_steps; ++step) {
-        if (integrateVelocity)
+        if (integrateVelocity) {
             callback_integrate_velocity(v, fp.final_gravity_dt[0], fp.final_gravity_dt[1], fp.final_gravity_dt[2], fp.final_linear_damping_dt, fp.final_angular_damping_dt);
+            if constexpr (kExt) apply_velocity_extensions(fp, i, pos, dt, fp.final_attractor_dt, v);  // the position before this step's update
+        }
         pos = pos + v.lin * dt;
         if (fp.angular_mode == 1) {
             Q4 previousOrientation = q;
@@ -493,11 +525,11 @@ BEPU_DI void run_final_pose(int i, const BodyBuffers& B, const FrameParams& fp) 
     store_pose(B.pose, i, pos, q);
     if (integrateVelocity) store_velocity(B.velocity, i, v);
 }
-static __global__ void final_pose_kernel(BodyBuffers B, const FrameParams* __restrict__ fpp) {
+template <bool kExt> static __global__ void final_pose_kernel(BodyBuffers B, const FrameParams* __restrict__ fpp) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= B.count) return;
     const FrameParams fp = *fpp;
-    run_final_pose(i, B, fp);
+    run_final_pose<kExt>(i, B, fp);
 }
 #endif
 

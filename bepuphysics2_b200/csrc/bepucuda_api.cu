@@ -160,6 +160,16 @@ struct bepucuda_ctx {
     int fallback_threshold = 64;
     bepucuda_integrator_desc integ{};
     bool integ_set = false;
+    // bepucuda_set_body_accelerations: device copy, the body count it was set for (-1: not set), and the pinned staging of the last upload
+    DeviceBuffer accelerations;
+    int accelerations_count = -1;
+    void* accelerations_stage = nullptr;
+    size_t accelerations_stage_bytes = 0;
+    cudaEvent_t accelerations_staged = nullptr;
+    // bepucuda_set_point_gravity
+    bool point_gravity = false;
+    float attractor_center[3] = {0.0f, 0.0f, 0.0f};
+    float attractor_strength = 0.0f;
 
     // bodies
     int body_count = 0;
@@ -308,6 +318,10 @@ void invalidate_graph(bepucuda_ctx* ctx) {
     ctx->graph_valid = false;
 }
 
+// Per-body accelerations or point gravity set: the WarmStart stages and the per-body passes launch the instantiations that apply them, so switching either on or
+// off changes the launch sequence (a captured graph is rebuilt); their values are frame parameters.
+bool integrator_extensions(const bepucuda_ctx* ctx) { return ctx->accelerations_count >= 0 || ctx->point_gravity; }
+
 // Row prefetch in the PDL prologue (see constraint_stage_kernel): allowed when the stage launched immediately before `op` neither rewrites op's
 // prestep rows (the incremental contact update does) nor its impulses (a stage of the same batch does: single-batch scenes). A rank barrier in
 // between writes no rows, so `previous` skips rank barriers.
@@ -334,6 +348,7 @@ void issue_stage_sequence(bepucuda_ctx* ctx, cudaStream_t s, int64_t* launches, 
     int64_t n = 0;
     const StageOp* previous = nullptr;  // last launched stage
     uint32_t exchange_index = 0;
+    const int extensions = integrator_extensions(ctx) ? kLaunchIntegratorExtensions : 0;
     for (size_t i = 0; i < ctx->program.size(); ++i) {
         const StageOp& op = ctx->program[i];
         const bool barrier = op.exchange == kRankBarrier;
@@ -350,13 +365,13 @@ void issue_stage_sequence(bepucuda_ctx* ctx, cudaStream_t s, int64_t* launches, 
                 // a sharded stage stores the records it writes for shared bodies into the ranks that reference them, and its boundary bundles wait
                 // for and announce arrivals themselves (ShardStage)
                 shard.stage.exchange_index = exchange_index;
-                const int flags = profile ? 0 : kLaunchPdl | (rows_prefetchable(previous, op) ? kLaunchPrefetchRows : 0);
+                const int flags = (profile ? 0 : kLaunchPdl | (rows_prefetchable(previous, op) ? kLaunchPrefetchRows : 0)) | extensions;
                 ctx->launchers->constraint_stage(op.stage, records + op.work_begin, ref_rows + (size_t)op.work_begin * 64, op.work_count, ctx->B, fp, flags,
                                                  op.exchange == kNoExchange ? nullptr : &shard, s);
             } else if (op.stage <= kStageKinematic) {
-                ctx->launchers->kinematic_stage(op.stage, kin, op.work_count, ctx->B, fp, s);
+                ctx->launchers->kinematic_stage(op.stage, kin, op.work_count, ctx->B, fp, extensions, s);
             } else {
-                ctx->launchers->final_pose(ctx->B, fp, s);
+                ctx->launchers->final_pose(ctx->B, fp, extensions, s);
             }
             if (profile) {
                 cudaEventRecord(profile->events[2 * i + 1], s);
@@ -454,6 +469,23 @@ void compute_frame_params(bepucuda_ctx* ctx, float dt, FrameParams* fp) {
     fp->final_steps = d.allow_substeps_for_unconstrained ? substeps : 1;
     fp->angular_mode = d.angular_integration_mode;
     fp->integrate_velocity_for_kinematics = d.integrate_velocity_for_kinematics;
+    // optional velocity terms (bepucuda_set_body_accelerations / bepucuda_set_point_gravity); PrepareForIntegration: gravityDt = dt * Gravity
+    // (PlanetDemo.cs:L36-40)
+    const unsigned long long accelerations = ctx->accelerations_count >= 0 ? (unsigned long long)ctx->accelerations.ptr : 0ull;
+    fp->accelerations[0] = (uint32_t)accelerations;
+    fp->accelerations[1] = (uint32_t)(accelerations >> 32);
+    fp->integrate_extensions = (ctx->accelerations_count >= 0 ? kIntegrateAccelerations : 0u) | (ctx->point_gravity ? kIntegratePointGravity : 0u);
+    for (int i = 0; i < 3; ++i) fp->attractor_center[i] = ctx->attractor_center[i];
+    fp->attractor_dt = substepDt * ctx->attractor_strength;
+    fp->final_attractor_dt = finalDt * ctx->attractor_strength;
+}
+
+// Accelerations set for another body count than the current one index the wrong bodies: solve, profile_stages and predict_bounding_boxes refuse
+// to run before any device work.
+int check_accelerations(bepucuda_ctx* ctx, const char* what) {
+    if (ctx->accelerations_count >= 0 && ctx->accelerations_count != ctx->body_count)
+        return fail(ctx, BEPUCUDA_ERR_BAD_STATE, std::string(what) + ": the body count changed after bepucuda_set_body_accelerations; set them again (or clear them with NULL)");
+    return BEPUCUDA_OK;
 }
 
 // Brings the device AOSOA-32 rows up to date with what the host queued since the last solve (bepucuda_update_type_batch / bepucuda_update_contacts):
@@ -567,8 +599,10 @@ int32_t bepucuda_destroy(bepucuda_ctx* ctx) {
     for (void* p : ctx->opened_ipc) cudaIpcCloseMemHandle(p);
     DeviceBuffer* bufs[] = {&ctx->shard_flags, &ctx->peer32, &ctx->body_masks_dev, &ctx->boundary_flags_dev, &ctx->raw_bodies, &ctx->pose, &ctx->velocity, &ctx->inertia_local, &ctx->inertia_world, &ctx->constrained, &ctx->first_batch, &ctx->sync_refcount,
                             &ctx->sync_mask, &ctx->chunk_table, &ctx->record_table, &ctx->ref_rows, &ctx->body_shapes, &ctx->body_activities, &ctx->body_bounds, &ctx->color_refs, &ctx->color_priorities, &ctx->color_body_min, &ctx->color_body_mask, &ctx->color_out, &ctx->color_lists, &ctx->color_counts, &ctx->source_bundle_flags, &ctx->refs32, &ctx->prestep32, &ctx->impulses32, &ctx->tb_table, &ctx->tdesc_table, &ctx->work_table, &ctx->map_table,
-                            &ctx->bodies_per_type, &ctx->kinematics_dev, &ctx->frame_params_dev, &ctx->error_dev};
+                            &ctx->bodies_per_type, &ctx->kinematics_dev, &ctx->frame_params_dev, &ctx->error_dev, &ctx->accelerations};
     for (auto b : bufs) b->release();
+    if (ctx->accelerations_stage) cudaFreeHost(ctx->accelerations_stage);
+    if (ctx->accelerations_staged) cudaEventDestroy(ctx->accelerations_staged);
     ctx->raw_arena.release();
     ctx->pinned_arena.release();
     if (ctx->frame_params_host) cudaFreeHost(ctx->frame_params_host);
@@ -635,6 +669,49 @@ int32_t bepucuda_set_integrator(bepucuda_ctx* ctx, const bepucuda_integrator_des
         CK(cudaSetDevice(ctx->device));
         return upload_program(ctx);
     }
+    return BEPUCUDA_OK;
+}
+
+int32_t bepucuda_set_body_accelerations(bepucuda_ctx* ctx, const float* accelerations, int32_t body_count) {
+    if (!ctx) return BEPUCUDA_ERR_INVALID_ARGUMENT;
+    if (!accelerations) {
+        const bool was = integrator_extensions(ctx);
+        ctx->accelerations_count = -1;
+        if (was != integrator_extensions(ctx)) invalidate_graph(ctx);
+        return BEPUCUDA_OK;
+    }
+    if (body_count != ctx->body_count) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "set_body_accelerations: the body count must match the last upload_bodies");
+    CK(cudaSetDevice(ctx->device));
+    open_upload_window(ctx);
+    const size_t bytes = (size_t)body_count * 32;
+    CK(ctx->accelerations.reserve(std::max(bytes, (size_t)32)));
+    if (bytes > 0) {
+        // through a pinned staging copy, so that the caller's buffer is free when the call returns without waiting for the device
+        if (!ctx->accelerations_staged) CK(cudaEventCreateWithFlags(&ctx->accelerations_staged, cudaEventDisableTiming));
+        CK(cudaEventSynchronize(ctx->accelerations_staged));  // the previous upload has left the staging buffer
+        if (ctx->accelerations_stage_bytes < bytes) {
+            if (ctx->accelerations_stage) cudaFreeHost(ctx->accelerations_stage);
+            ctx->accelerations_stage = nullptr;
+            ctx->accelerations_stage_bytes = 0;
+            CK(cudaMallocHost(&ctx->accelerations_stage, bytes));
+            ctx->accelerations_stage_bytes = bytes;
+        }
+        std::memcpy(ctx->accelerations_stage, accelerations, bytes);
+        CK(cudaMemcpyAsync(ctx->accelerations.ptr, ctx->accelerations_stage, bytes, cudaMemcpyHostToDevice, ctx->stream));
+        CK(cudaEventRecord(ctx->accelerations_staged, ctx->stream));
+        ctx->h2d_accum += (int64_t)bytes;
+    }
+    if (!integrator_extensions(ctx)) invalidate_graph(ctx);
+    ctx->accelerations_count = body_count;
+    return BEPUCUDA_OK;
+}
+
+int32_t bepucuda_set_point_gravity(bepucuda_ctx* ctx, int32_t enabled, const float* center, float strength) {
+    if (!ctx || (enabled && !center)) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "set_point_gravity: bad arguments");
+    if (ctx->point_gravity != (enabled != 0) && ctx->accelerations_count < 0) invalidate_graph(ctx);
+    ctx->point_gravity = enabled != 0;
+    for (int i = 0; i < 3; ++i) ctx->attractor_center[i] = enabled ? center[i] : 0.0f;
+    ctx->attractor_strength = enabled ? strength : 0.0f;
     return BEPUCUDA_OK;
 }
 
@@ -1167,6 +1244,7 @@ int32_t bepucuda_download_body_motion(bepucuda_ctx* ctx, void* out, int32_t body
 
 int32_t bepucuda_solve(bepucuda_ctx* ctx, float dt) {
     if (!ctx || !(dt > 0)) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "solve: bad arguments");
+    { int rc = check_accelerations(ctx, "solve"); if (rc != BEPUCUDA_OK) return rc; }
     CK(cudaSetDevice(ctx->device));
     if (!ctx->constraints_ready) {
         // No constraints were ever described (or the description was invalidated): only legal when nothing was uploaded.
@@ -1216,6 +1294,7 @@ int32_t bepucuda_solve(bepucuda_ctx* ctx, float dt) {
         }
     }
     bytes += (int64_t)ctx->body_count * 108;
+    if (ctx->accelerations_count >= 0) bytes += (int64_t)ctx->body_count * substeps * 32;  // one acceleration record per integrating lane: one per body and substep
     ctx->timings.constraint_iterations = ci;
     ctx->timings.algorithmic_bytes = bytes;
     return BEPUCUDA_OK;
@@ -1319,6 +1398,7 @@ int32_t bepucuda_profile_stages(bepucuda_ctx* ctx, float dt, bepucuda_stage_prof
     if (!ctx || !out || !(dt > 0)) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "profile_stages: bad arguments");
     if (!ctx->constraints_ready) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, "profile_stages before end_constraints");
     if (ctx->peer_mode) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, "profile_stages in peer mode: one rank alone cannot meet its peers at the rank barriers");
+    { int rc = check_accelerations(ctx, "profile_stages"); if (rc != BEPUCUDA_OK) return rc; }
     CK(cudaSetDevice(ctx->device));
     std::memset(out, 0, sizeof(*out));
     const size_t need = ctx->program.size() * 2;
@@ -1374,6 +1454,7 @@ int32_t bepucuda_set_body_shapes(bepucuda_ctx* ctx, const bepucuda_body_shape* s
 int32_t bepucuda_predict_bounding_boxes(bepucuda_ctx* ctx, float dt, bepucuda_body_activity* activities, float* bounds_out) {
     if (!ctx || !(dt > 0) || !activities || !bounds_out) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "predict_bounding_boxes: bad arguments");
     if (ctx->shape_count != ctx->body_count) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, "predict_bounding_boxes: bepucuda_set_body_shapes was not called for the current body count");
+    { int rc = check_accelerations(ctx, "predict_bounding_boxes"); if (rc != BEPUCUDA_OK) return rc; }
     const int n = ctx->body_count;
     if (n == 0) return BEPUCUDA_OK;
     CK(cudaSetDevice(ctx->device));
@@ -1388,6 +1469,10 @@ int32_t bepucuda_predict_bounding_boxes(bepucuda_ctx* ctx, float dt, bepucuda_bo
     p.linear_damping_dt = powf(clamp01(1 - ctx->integ.linear_damping), dt);
     p.angular_damping_dt = powf(clamp01(1 - ctx->integ.angular_damping), dt);
     p.integrate_velocity_for_kinematics = ctx->integ.integrate_velocity_for_kinematics;
+    p.accelerations = ctx->accelerations_count >= 0 ? ctx->accelerations.as<float4>() : nullptr;
+    p.integrate_extensions = (ctx->accelerations_count >= 0 ? kIntegrateAccelerations : 0u) | (ctx->point_gravity ? kIntegratePointGravity : 0u);
+    for (int i = 0; i < 3; ++i) p.attractor_center[i] = ctx->attractor_center[i];
+    p.attractor_dt = dt * ctx->attractor_strength;
     launch_predict_bounding_boxes(ctx->B, ctx->body_shapes.as<BodyShape>(), ctx->body_activities.as<BodyActivityRecord>(), ctx->body_bounds.as<float4>(), p, ctx->stream);
     CK(cudaGetLastError());
     CK(cudaMemcpyAsync(activities, ctx->body_activities.ptr, (size_t)n * sizeof(BodyActivityRecord), cudaMemcpyDeviceToHost, ctx->stream));

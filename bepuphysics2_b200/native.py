@@ -98,6 +98,7 @@ C_ABI_SYMBOLS = [
     "bepucuda_set_contact_features", "bepucuda_update_contacts", "bepucuda_upload_body_motion", "bepucuda_download_body_motion",
     "bepucuda_shard_export", "bepucuda_shard_import", "bepucuda_shard_set_global", "bepucuda_shard_set_body_masks", "bepucuda_shard_import_contexts",
     "bepucuda_color_constraints", "bepucuda_color_hash", "bepucuda_set_body_shapes", "bepucuda_predict_bounding_boxes",
+    "bepucuda_set_body_accelerations", "bepucuda_set_point_gravity",
 ]
 
 
@@ -161,6 +162,8 @@ def load_libraries():
     cuda.bepucuda_set_body_shapes.argtypes = [vp, vp, i32]
     cuda.bepucuda_predict_bounding_boxes.argtypes = [vp, f32, vp, vp]
     cuda.bepucuda_color_hash.restype = C.c_uint32
+    cuda.bepucuda_set_body_accelerations.argtypes = [vp, vp, i32]
+    cuda.bepucuda_set_point_gravity.argtypes = [vp, i32, vp, f32]
 
     host.bepuhost_create.restype = vp
     host.bepuhost_create.argtypes = [i32, i32]
@@ -388,6 +391,23 @@ class CudaTimestepper:
         """bepucuda_set_body_shapes: one BODY_SHAPE_DTYPE record per body (static between frames unless a shape changes)."""
         shapes = np.ascontiguousarray(shapes, dtype=BODY_SHAPE_DTYPE)
         self._check(self._cuda.bepucuda_set_body_shapes(self._ctx, shapes.ctypes.data, shapes.shape[0]))
+
+    def set_body_accelerations(self, accelerations):
+        """bepucuda_set_body_accelerations: accelerations[n, 8] = {ax, ay, az, 0, alpha_x, alpha_y, alpha_z, 0} per active-set body index, added
+        as a * dt after the declarative callback (PerBodyGravityDemo); None clears them. n must be the uploaded body count."""
+        if accelerations is None:
+            self._check(self._cuda.bepucuda_set_body_accelerations(self._ctx, None, 0))
+            return
+        a = np.ascontiguousarray(accelerations, dtype=np.float32).reshape(-1, 8)
+        self._check(self._cuda.bepucuda_set_body_accelerations(self._ctx, a.ctypes.data, a.shape[0]))
+
+    def set_point_gravity(self, center, strength):
+        """bepucuda_set_point_gravity: gravity towards `center` (PlanetDemo); center None switches it off."""
+        if center is None:
+            self._check(self._cuda.bepucuda_set_point_gravity(self._ctx, 0, None, 0.0))
+            return
+        c = np.ascontiguousarray(center, dtype=np.float32).reshape(3)
+        self._check(self._cuda.bepucuda_set_point_gravity(self._ctx, 1, c.ctypes.data, float(strength)))
 
     def predict_bounding_boxes(self, dt, activities):
         """bepucuda_predict_bounding_boxes on the body state resident on the device. `activities` (BODY_ACTIVITY_DTYPE) is updated in place.

@@ -113,6 +113,27 @@ int32_t bepucuda_set_solve_description(bepucuda_ctx* ctx, int32_t substep_count,
 /* Replaces: the TIntegrationCallbacks type argument of Solver<T>/PoseIntegrator<T>. */
 int32_t bepucuda_set_integrator(bepucuda_ctx* ctx, const bepucuda_integrator_desc* desc);
 
+/* Two optional terms after the declarative callback, for IntegrateVelocity bodies the descriptor cannot express. Each is applied wherever the
+ * reference calls IntegrateVelocity and keeps its result: the integrating lane of WarmStart (TypeProcessor.cs:L1204-1283), the kinematic prepasses
+ * when integrate_velocity_for_kinematics (PoseIntegrator.cs:L451-535), the final pass of unconstrained bodies (L632-645, L707-712) and
+ * bepucuda_predict_bounding_boxes (L339-341, L428). With dt and position what the reference passes the callback at that site (the dt of its
+ * PrepareForIntegration; the pose after this substep's pose integration in WarmStart of substeps > 0 and in the kinematic pose prepass):
+ *   v.linear  += a_linear[i] * dt;  v.angular += a_angular[i] * dt                     (not damped)
+ *   offset = position - center;  d = |offset|;  v.linear -= (attractorDt * offset) * (1 / max(1, d * d * d)),  attractorDt = dt * strength
+ * Neither term set: exactly the declarative callback, with no extra arithmetic.
+ *
+ * bepucuda_set_body_accelerations: per-body accelerations, as Demos/Demos/PerBodyGravityDemo.cs:L20-89 applies them (there: a_linear = (0, g_i, 0)).
+ * 8 floats per body {ax, ay, az, 0, alpha_x, alpha_y, alpha_z, 0} indexed by active-set body index, the record shape of a velocity. Copied to
+ * the device (counted in h2d_bytes / upload_ms); the caller's buffer is free when the call returns. NULL clears them. body_count must equal the
+ * one of the last bepucuda_upload_bodies (else BEPUCUDA_ERR_INVALID_ARGUMENT); if the body count changes afterwards, bepucuda_solve,
+ * bepucuda_profile_stages and bepucuda_predict_bounding_boxes return BEPUCUDA_ERR_BAD_STATE before any device work until they are set again or
+ * cleared. A peer-sharded rank is given the whole array, like its bodies.
+ * bepucuda_set_point_gravity: gravity towards a point, Demos/Demos/PlanetDemo.cs:L20-48 (center = PlanetCenter, strength = Gravity). A frame
+ * parameter like the integrator's gravity: changing it does not rebuild the captured graph. enabled = 0 switches it off (center may be NULL).
+ * Arbitrary callback code and per-body damping are not covered. */
+int32_t bepucuda_set_body_accelerations(bepucuda_ctx* ctx, const float* accelerations, int32_t body_count);
+int32_t bepucuda_set_point_gravity(bepucuda_ctx* ctx, int32_t enabled, const float* center, float strength);
+
 /* Replaces: reads of Bodies.ActiveSet.DynamicsState (BepuPhysics/BodySet.cs:L33). `body_dynamics` is the raw
  * Buffer<BodyDynamics>.Memory: body_count records of 128 B (BepuPhysics/BodyProperties.cs:L11-46,L318-338). */
 int32_t bepucuda_upload_bodies(bepucuda_ctx* ctx, const void* body_dynamics, int32_t body_count);

@@ -44,6 +44,9 @@ namespace BepuCuda
         [DllImport(Lib)] public static extern int bepucuda_host_unregister(IntPtr ctx, void* ptr);
         [DllImport(Lib)] public static extern int bepucuda_set_solve_description(IntPtr ctx, int substepCount, int* velocityIterationsPerSubstep, int fallbackBatchThreshold);
         [DllImport(Lib)] public static extern int bepucuda_set_integrator(IntPtr ctx, IntegratorDesc* desc);
+        /// <summary>Optional terms after the declarative callback: per-body accelerations (PerBodyGravityDemo) and gravity towards a point (PlanetDemo).</summary>
+        [DllImport(Lib)] public static extern int bepucuda_set_body_accelerations(IntPtr ctx, float* accelerations, int bodyCount);
+        [DllImport(Lib)] public static extern int bepucuda_set_point_gravity(IntPtr ctx, int enabled, float* center, float strength);
         [DllImport(Lib)] public static extern int bepucuda_upload_bodies(IntPtr ctx, void* bodyDynamics, int bodyCount);
         [DllImport(Lib)] public static extern int bepucuda_begin_constraints(IntPtr ctx, int sourceBundleWidth, int batchCount);
         [DllImport(Lib)] public static extern int bepucuda_upload_type_batch(IntPtr ctx, int batchIndex, int typeBatchIndex, int typeId, int constraintCount, void* bodyReferences, void* prestep, void* accumulatedImpulses);

@@ -22,6 +22,27 @@ public unsafe class CudaTimestepper<TCallbacks> : ITimestepper, IDisposable wher
     IntPtr ctx;
     IntegratorDesc integrator;
     ulong uploadedTopology;   // signature of the constraint graph the device currently holds (0 = none)
+    float[] bodyAccelerations;  // SetBodyAccelerations: 8 floats per active-set body index, uploaded after the bodies every frame (null = none)
+
+    /// <summary>Per-body accelerations added as a * dt after the declarative callback (PerBodyGravityDemo's IntegrateVelocity): 8 floats per
+    /// active-set body index {ax, ay, az, 0, alpha_x, alpha_y, alpha_z, 0}. The application keeps the array in step with the active set (its length is
+    /// checked against the body count every frame); null switches them off.</summary>
+    public void SetBodyAccelerations(float[] accelerations) => bodyAccelerations = accelerations;
+
+    /// <summary>Gravity towards a point after the declarative callback (PlanetDemo's IntegrateVelocity: center = PlanetCenter, strength = Gravity);
+    /// null switches it off.</summary>
+    public void SetPointGravity(Vector3? center, float strength)
+    {
+        if (center is Vector3 c)
+        {
+            var xyz = stackalloc float[3] { c.X, c.Y, c.Z };
+            Check(Native.bepucuda_set_point_gravity(ctx, 1, xyz, strength));
+        }
+        else
+        {
+            Check(Native.bepucuda_set_point_gravity(ctx, 0, null, 0));
+        }
+    }
 
     public CudaTimestepper(in TCallbacks callbacks, Vector3 gravity, float linearDamping = 0.03f, float angularDamping = 0.03f, int device = 0, bool strict = false)
     {
@@ -72,6 +93,8 @@ public unsafe class CudaTimestepper<TCallbacks> : ITimestepper, IDisposable wher
         Check(Native.bepucuda_set_solve_description(ctx, solver.SubstepCount, iterations, solver.FallbackBatchThreshold));
         fixed (IntegratorDesc* d = &integrator) Check(Native.bepucuda_set_integrator(ctx, d));
         Check(Native.bepucuda_upload_bodies(ctx, bodies.DynamicsState.Memory, bodies.Count));                       // BodySet.cs:L33
+        if (bodyAccelerations == null) Check(Native.bepucuda_set_body_accelerations(ctx, null, 0));
+        else fixed (float* a = bodyAccelerations) Check(Native.bepucuda_set_body_accelerations(ctx, a, bodyAccelerations.Length / 8));
 
         // Frames whose constraint graph did not change (same type batches, same body references, same kinematics) only refresh what the
         // narrow phase rewrote: the device keeps its batch analysis and the captured CUDA graph (INTEGRATION.md, performance notes).
