@@ -184,24 +184,65 @@ template <> inline i8 make_mask<f8>(const bool* m) {
 }
 
 // ---- integration: PoseIntegrator.cs:L99-261, Demos/DemoCallbacks.cs:L79-105 ----------------------------------------
+// The optional terms, integrate_velocity_extensions of csrc/bepu_integration.cuh (PerBodyGravityDemo.cs:L57-88: v += a * dt, not damped;
+// PlanetDemo.cs:L44-46 in its operation order, with Vector3Wide.Length and Vector3Wide / Vector<float> = multiply by the reciprocal,
+// Vector3Wide.cs:L357-363, L573-576).
+template <class F>
+static inline void apply_velocity_terms(Velocity<F>& v, bool accelerations, const V3<F>& linearAcceleration, const V3<F>& angularAcceleration, float dt, bool pointGravity,
+                                        const V3<F>& position, const V3<F>& center, float attractorDt) {
+    if (accelerations) {
+        v.lin = add(v.lin, scale(linearAcceleration, bc<F>(dt)));
+        v.ang = add(v.ang, scale(angularAcceleration, bc<F>(dt)));
+    }
+    if (pointGravity) {
+        V3<F> offset = sub(position, center);
+        F distance = length(offset);
+        F inverse = bc<F>(1.0f) / vmax(bc<F>(1.0f), distance * distance * distance);
+        v.lin = sub(v.lin, scale(scale(offset, bc<F>(attractorDt)), inverse));
+    }
+}
+
 struct Callbacks {
     float gravity[3];
     float linear_damping, angular_damping;
     int angular_mode;
     bool allow_substeps_unconstrained, integrate_kinematic_velocity;
+    oracle_integrator_terms terms{};  // zeroed: no terms
     // PrepareForIntegration products
     float gravity_dt[3];
     float linear_damping_dt, angular_damping_dt;
-    void prepare(float dt) {  // DemoCallbacks.cs:L79-86
+    float dt, attractor_dt;
+    void prepare(float dt) {  // DemoCallbacks.cs:L79-86, PlanetDemo.cs:L36-40
         auto clamp01 = [](float v) { return v < 0.f ? 0.f : (v > 1.f ? 1.f : v); };
         linear_damping_dt = powf(clamp01(1 - linear_damping), dt);
         angular_damping_dt = powf(clamp01(1 - angular_damping), dt);
         for (int i = 0; i < 3; ++i) gravity_dt[i] = gravity[i] * dt;
+        this->dt = dt;
+        attractor_dt = dt * terms.strength;
     }
     template <class F> void integrate_velocity(Velocity<F>& v) const {  // DemoCallbacks.cs:L99-102
         V3<F> g{bc<F>(gravity_dt[0]), bc<F>(gravity_dt[1]), bc<F>(gravity_dt[2])};
         v.lin = scale(add(v.lin, g), bc<F>(linear_damping_dt));
         v.ang = scale(v.ang, bc<F>(angular_damping_dt));
+    }
+    // The declarative callback, then the terms of the lanes' bodies at the position the reference hands the callback. refs: the encoded body
+    // references of the lanes (negative = empty lane).
+    template <class F> void integrate_velocity(Velocity<F>& v, const V3<F>& position, const int32_t* refs) const {
+        integrate_velocity(v);
+        if (terms.accelerations || terms.point_gravity) integrate_velocity_terms(v, position, refs);
+    }
+    template <class F> void integrate_velocity_terms(Velocity<F>& v, const V3<F>& position, const int32_t* refs) const {
+        constexpr int PW = LaneTraits<F>::Width;
+        V3<F> al{bc<F>(0.0f), bc<F>(0.0f), bc<F>(0.0f)}, aa = al;
+        if (terms.accelerations)
+            for (int l = 0; l < PW; ++l) {
+                if (refs[l] < 0) continue;
+                const float* a = terms.accelerations + (size_t)(refs[l] & kBodyReferenceMask) * 8;
+                set_lane(al.x, l, a[0]); set_lane(al.y, l, a[1]); set_lane(al.z, l, a[2]);
+                set_lane(aa.x, l, a[4]); set_lane(aa.y, l, a[5]); set_lane(aa.z, l, a[6]);
+            }
+        const float* c = terms.center;
+        apply_velocity_terms<F>(v, terms.accelerations != nullptr, al, aa, dt, terms.point_gravity != 0, position, V3<F>{bc<F>(c[0]), bc<F>(c[1]), bc<F>(c[2])}, attractor_dt);
     }
 };
 
@@ -287,9 +328,10 @@ static inline void integrate_angular_gyroscopic(const Q4<F>& orientation, const 
     fallback_if_inertia_incompatible(previous, w);
 }
 
-// TypeProcessor.cs:L1204-1248 IntegratePoseAndVelocity
+// TypeProcessor.cs:L1204-1248 IntegratePoseAndVelocity; the callback sees the integrated pose (L1244). refs: the lanes' body references.
 template <class F>
-static inline void integrate_pose_and_velocity(const Callbacks& cb, const Inertia<F>& local, float dt, const MaskOf<F>& mask, V3<F>& pos, Q4<F>& q, Velocity<F>& v, Inertia<F>& world) {
+static inline void integrate_pose_and_velocity(const Callbacks& cb, const Inertia<F>& local, float dt, const MaskOf<F>& mask, V3<F>& pos, Q4<F>& q, Velocity<F>& v, Inertia<F>& world,
+                                               const int32_t* refs) {
     F dtWide = bc<F>(dt);
     V3<F> newPosition = add(pos, scale(v.lin, dtWide));
     pos = sel3<F>(mask, newPosition, pos);
@@ -312,13 +354,14 @@ static inline void integrate_pose_and_velocity(const Callbacks& cb, const Inerti
         q = sel4<F>(mask, newOrientation, q);
         world.t = rotate_inverse_inertia(local.t, q);
     }
-    cb.integrate_velocity(v);
+    cb.integrate_velocity(v, pos, refs);
     v.lin = sel3<F>(mask, v.lin, previousVelocity.lin);
     v.ang = sel3<F>(mask, v.ang, previousVelocity.ang);
 }
-// TypeProcessor.cs:L1251-1283 IntegrateVelocity
+// TypeProcessor.cs:L1251-1283 IntegrateVelocity; the callback sees the current pose (L1276).
 template <class F>
-static inline void integrate_velocity_only(const Callbacks& cb, const Inertia<F>& local, float dt, const MaskOf<F>& mask, bool conditional, const Q4<F>& q, Velocity<F>& v, Inertia<F>& world) {
+static inline void integrate_velocity_only(const Callbacks& cb, const Inertia<F>& local, float dt, const MaskOf<F>& mask, bool conditional, const V3<F>& pos, const Q4<F>& q,
+                                           Velocity<F>& v, Inertia<F>& world, const int32_t* refs) {
     world.inv_mass = local.inv_mass;
     world.t = rotate_inverse_inertia(local.t, q);
     if (cb.angular_mode == 1) {
@@ -329,11 +372,11 @@ static inline void integrate_velocity_only(const Callbacks& cb, const Inertia<F>
     }
     if (conditional) {
         Velocity<F> previousVelocity = v;
-        cb.integrate_velocity(v);
+        cb.integrate_velocity(v, pos, refs);
         v.lin = sel3<F>(mask, v.lin, previousVelocity.lin);
         v.ang = sel3<F>(mask, v.ang, previousVelocity.ang);
     } else {
-        cb.integrate_velocity(v);
+        cb.integrate_velocity(v, pos, refs);
     }
 }
 
@@ -490,11 +533,11 @@ static void warm_start_bundle(Solver& s, const TypeOps<F>& ops, oracle_type_batc
             body[slot].pos = g.pos;
             body[slot].q = g.q;
             if (allowPose) {
-                integrate_pose_and_velocity<F>(s.cb, g.inertia, dt, mask, body[slot].pos, body[slot].q, vel[slot], body[slot].inertia);
+                integrate_pose_and_velocity<F>(s.cb, g.inertia, dt, mask, body[slot].pos, body[slot].q, vel[slot], body[slot].inertia, refs);
                 scatter_pose<F>(sc.bodies, refs, m, body[slot].pos, body[slot].q);
                 scatter_world_inertia<F>(sc.bodies, refs, m, body[slot].inertia);
             } else {
-                integrate_velocity_only<F>(s.cb, g.inertia, dt, mask, batchIndex != 0, body[slot].q, vel[slot], body[slot].inertia);
+                integrate_velocity_only<F>(s.cb, g.inertia, dt, mask, batchIndex != 0, body[slot].pos, body[slot].q, vel[slot], body[slot].inertia, refs);
                 scatter_world_inertia<F>(sc.bodies, refs, m, body[slot].inertia);
             }
         }
@@ -541,7 +584,7 @@ template <class F> static void incremental_bundle(Solver& s, const TypeOps<F>& o
     }
 }
 
-// ---- kinematic prepasses: PoseIntegrator.cs:L451-487, L493-535 -----------------------------------------------------
+// ---- kinematic prepasses: PoseIntegrator.cs:L451-487 (the gathered pose, L480), L493-535 (the integrated pose, L529) ------------------------
 static void integrate_kinematic_velocities(Solver& s) {
     oracle_scene& sc = *s.sc;
     for (int i = 0; i < sc.constrained_kinematic_count; ++i) {
@@ -549,7 +592,7 @@ static void integrate_kinematic_velocities(Solver& s) {
         BodyIn<float> b;
         Velocity<float> v;
         gather_state<float>(sc.bodies, &idx, false, b, v);
-        s.cb.integrate_velocity(v);
+        s.cb.integrate_velocity(v, b.pos, &idx);
         scatter_velocities<float>(sc.bodies, &idx, v);
     }
 }
@@ -565,13 +608,13 @@ static void integrate_kinematic_poses_and_velocities(Solver& s, float dt) {
         bool m = true;
         scatter_pose<float>(sc.bodies, &idx, &m, b.pos, b.q);
         if (s.cb.integrate_kinematic_velocity) {
-            s.cb.integrate_velocity(v);
+            s.cb.integrate_velocity(v, b.pos, &idx);
             scatter_velocities<float>(sc.bodies, &idx, v);
         }
     }
 }
 
-// ---- final pass: PoseIntegrator.cs:L537-693 IntegrateBundlesAfterSubstepping ---------------------------------------
+// ---- final pass: PoseIntegrator.cs:L537-693 IntegrateBundlesAfterSubstepping; the callback sees the position before each step's update ------
 static void integrate_after_substepping(Solver& s, float dt, int substepCount) {
     oracle_scene& sc = *s.sc;
     float substepDt = dt / substepCount;
@@ -599,7 +642,7 @@ static void integrate_after_substepping(Solver& s, float dt, int substepCount) {
         bool integrateVelocity = s.cb.integrate_kinematic_velocity || !kinematic;
         int steps = s.cb.allow_substeps_unconstrained ? substepCount : 1;
         for (int step = 0; step < steps; ++step) {
-            if (integrateVelocity) s.cb.integrate_velocity(v);
+            if (integrateVelocity) s.cb.integrate_velocity(v, b.pos, &idx);
             b.pos = add(b.pos, scale(v.lin, effectiveDt));
             if (s.cb.angular_mode == 1) {
                 Q4<float> previousOrientation = b.q;
@@ -796,7 +839,7 @@ extern "C" int32_t oracle_eval_lane(int32_t type_id, int32_t stage, const float*
     return 0;
 }
 
-// The integration arithmetic, one call per function (same operand layout as device_on_host_eval_integration in tests/device_on_host).
+// The integration arithmetic, one call per function (same ops and operand layout as device_on_host_eval_integration in tests/device_on_host).
 extern "C" int32_t oracle_eval_integration(int32_t op, const float* in, float* out) {
     auto sym = [&](int i) { return Sym3<float>{in[i], in[i + 1], in[i + 2], in[i + 3], in[i + 4], in[i + 5]}; };
     if (op == 0) {
@@ -819,6 +862,11 @@ extern "C" int32_t oracle_eval_integration(int32_t op, const float* in, float* o
         cb.linear_damping_dt = in[9]; cb.angular_damping_dt = in[10];
         Velocity<float> v{{in[0], in[1], in[2]}, {in[3], in[4], in[5]}};
         cb.integrate_velocity(v);
+        out[0] = v.lin.x; out[1] = v.lin.y; out[2] = v.lin.z; out[3] = v.ang.x; out[4] = v.ang.y; out[5] = v.ang.z;
+    } else if (op == 5) {
+        Velocity<float> v{{in[0], in[1], in[2]}, {in[3], in[4], in[5]}};
+        apply_velocity_terms<float>(v, in[20] != 0.0f, V3<float>{in[6], in[7], in[8]}, V3<float>{in[9], in[10], in[11]}, in[12], in[21] != 0.0f,
+                                    V3<float>{in[13], in[14], in[15]}, V3<float>{in[16], in[17], in[18]}, in[19]);
         out[0] = v.lin.x; out[1] = v.lin.y; out[2] = v.lin.z; out[3] = v.ang.x; out[4] = v.ang.y; out[5] = v.ang.z;
     } else {
         return -1;
@@ -924,13 +972,17 @@ extern "C" int32_t oracle_first_fit_batches(int32_t constraint_count, int32_t bo
 // Cylinder.cs:L222-235, BoundingBoxHelpers.GetAngularBoundsExpansion / GetBoundsExpansion (BoundingBoxHelpers.cs:L12-58).
 struct oracle_body_shape { int32_t type; float a, b, c, minimum_speculative_margin, maximum_speculative_margin; int32_t allow_expansion_beyond_speculative_margin, reserved; };
 struct oracle_body_activity { float sleep_threshold; uint8_t minimum_timesteps_under_threshold, timesteps_under_threshold_count, sleep_candidate, reserved; };
+// terms: the optional velocity terms, or NULL (the default) for none.
 extern "C" int32_t oracle_predict_bounding_boxes(int32_t body_count, const float* bodies, const oracle_body_shape* shapes, oracle_body_activity* activities, float dt,
-                                                 const float* gravity, float linear_damping, float angular_damping, int32_t integrate_velocity_for_kinematics, float* bounds_out) {
-    auto clamp01 = [](float v) { return v < 0.f ? 0.f : (v > 1.f ? 1.f : v); };
-    // Callbacks.PrepareForIntegration(dt), Demos/DemoCallbacks.cs:L79-86
-    const float linearDampingDt = powf(clamp01(1 - linear_damping), dt), angularDampingDt = powf(clamp01(1 - angular_damping), dt);
-    const V3<float> gravityDt = {gravity[0] * dt, gravity[1] * dt, gravity[2] * dt};
-    for (int i = 0; i < body_count; ++i) {
+                                                 const float* gravity, float linear_damping, float angular_damping, int32_t integrate_velocity_for_kinematics,
+                                                 float* bounds_out, const oracle_integrator_terms* terms = nullptr) {
+    Callbacks cb{};
+    std::copy(gravity, gravity + 3, cb.gravity);
+    cb.linear_damping = linear_damping;
+    cb.angular_damping = angular_damping;
+    if (terms) cb.terms = *terms;
+    cb.prepare(dt);  // PoseIntegrator.cs:L428: PrepareForIntegration with the frame dt
+    for (int32_t i = 0; i < body_count; ++i) {
         const float* b = bodies + (size_t)i * 32;
         const Q4<float> orientation = {b[0], b[1], b[2], b[3]};
         const V3<float> position = {b[4], b[5], b[6]};
@@ -939,9 +991,11 @@ extern "C" int32_t oracle_predict_bounding_boxes(int32_t body_count, const float
         for (int k = 16; k < 23; ++k) { uint32_t bits; std::memcpy(&bits, b + k, 4); kinematic = kinematic && bits == 0u; }
         const bool integrate = integrate_velocity_for_kinematics != 0 || !kinematic;
         const float sleepEnergy = length_squared(linear) + length_squared(angular);
-        if (integrate) {  // DemoPoseIntegratorCallbacks.IntegrateVelocity, Demos/DemoCallbacks.cs:L99-104; the result is not stored (PoseIntegrator.cs:L339)
-            linear = scale(add(linear, gravityDt), linearDampingDt);
-            angular = scale(angular, angularDampingDt);
+        if (integrate) {  // IntegrateVelocity at the current pose (PoseIntegrator.cs:L339-341); the result is not stored
+            Velocity<float> v{linear, angular};
+            cb.integrate_velocity(v, position, &i);
+            linear = v.lin;
+            angular = v.ang;
         }
         oracle_body_activity& activity = activities[i];
         if (sleepEnergy > activity.sleep_threshold) {
@@ -1033,6 +1087,7 @@ extern "C" int32_t oracle_solve(oracle_scene* sc, float dt) {
     s.cb.angular_mode = sc->angular_integration_mode;
     s.cb.allow_substeps_unconstrained = sc->allow_substeps_for_unconstrained != 0;
     s.cb.integrate_kinematic_velocity = sc->integrate_velocity_for_kinematics != 0;
+    s.cb.terms = sc->terms;
     // Simulation.Solve: Simulation.cs:L278-290
     prepare_integration_responsibilities(s);
     if (sc->simd)

@@ -23,6 +23,15 @@ typedef struct oracle_batch {
     oracle_type_batch* type_batches;
 } oracle_batch;
 
+/* Optional velocity terms applied after the declarative callback wherever its result is kept (bepucuda_set_body_accelerations /
+ * bepucuda_set_point_gravity in include/bepucuda.h). All zero: no terms. */
+typedef struct oracle_integrator_terms {
+    const float* accelerations;   /* body_count x 8 floats {a.xyz 0 | alpha.xyz 0} (PerBodyGravityDemo), or NULL */
+    int32_t point_gravity;        /* nonzero: PlanetDemo's attractor at center with strength */
+    float center[3];
+    float strength;
+} oracle_integrator_terms;
+
 typedef struct oracle_scene {
     float* bodies;                /* body_count x 32 floats (BepuPhysics/BodyProperties.cs:L11-46,L318-338) */
     int32_t body_count;
@@ -42,6 +51,7 @@ typedef struct oracle_scene {
     int32_t constrained_kinematic_count;
     int32_t threads;              /* OpenMP threads for synchronized batches (fallback batch is always sequential) */
     int32_t simd;                 /* 0: scalar-per-lane evaluation; 1: 8-wide vector evaluation (requires bundle_width == 8) */
+    oracle_integrator_terms terms;
 } oracle_scene;
 
 /* PrepareConstraintIntegrationResponsibilities + Solver.Solve + PoseIntegrator.IntegrateAfterSubstepping. 0 on success. */

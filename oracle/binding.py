@@ -18,6 +18,10 @@ class OracleBatch(C.Structure):
     _fields_ = [("type_batch_count", C.c_int32), ("type_batches", C.POINTER(OracleTypeBatch))]
 
 
+class OracleIntegratorTerms(C.Structure):
+    _fields_ = [("accelerations", C.c_void_p), ("point_gravity", C.c_int32), ("center", C.c_float * 3), ("strength", C.c_float)]
+
+
 class OracleScene(C.Structure):
     _fields_ = [
         ("bodies", C.c_void_p), ("body_count", C.c_int32), ("batch_count", C.c_int32), ("batches", C.POINTER(OracleBatch)), ("bundle_width", C.c_int32),
@@ -25,7 +29,24 @@ class OracleScene(C.Structure):
         ("gravity", C.c_float * 3), ("linear_damping", C.c_float), ("angular_damping", C.c_float), ("angular_integration_mode", C.c_int32),
         ("allow_substeps_for_unconstrained", C.c_int32), ("integrate_velocity_for_kinematics", C.c_int32),
         ("constrained_kinematics", C.c_void_p), ("constrained_kinematic_count", C.c_int32), ("threads", C.c_int32), ("simd", C.c_int32),
+        ("terms", OracleIntegratorTerms),
     ]
+
+
+def _terms(body_count, accelerations, center, strength):
+    """The optional velocity terms: per-body accelerations (body_count x 8 floats {a.xyz 0 | alpha.xyz 0}) and point gravity toward `center`
+    with `strength` (None: off). Returns the struct and the array it points into, which the caller keeps alive."""
+    t = OracleIntegratorTerms()
+    acc = None
+    if accelerations is not None:
+        acc = np.ascontiguousarray(accelerations, dtype=np.float32).reshape(-1, 8)
+        assert acc.shape[0] == body_count
+        t.accelerations = acc.ctypes.data if acc.size else None
+    if center is not None:
+        t.point_gravity = 1
+        t.center[:] = [float(c) for c in center]
+        t.strength = strength
+    return t, acc
 
 
 def build(force=False):
@@ -62,8 +83,9 @@ def max_threads():
     return load().oracle_max_threads()
 
 
-def solve(simulation, dt, threads=1, simd=False):
-    """Runs the oracle's Simulation.Solve restatement in place on `simulation`'s buffers (bodies, prestep depths, accumulated impulses)."""
+def solve(simulation, dt, threads=1, simd=False, accelerations=None, center=None, strength=0.0):
+    """Runs the oracle's Simulation.Solve restatement in place on `simulation`'s buffers (bodies, prestep depths, accumulated impulses), with the
+    optional velocity terms of bepucuda_set_body_accelerations / bepucuda_set_point_gravity (see _terms)."""
     lib = load()
     tbs = simulation.type_batches()
     batch_count = simulation.batch_count
@@ -106,6 +128,7 @@ def solve(simulation, dt, threads=1, simd=False):
     sc.constrained_kinematic_count = int(kin.size)
     sc.threads = threads
     sc.simd = 1 if simd else 0
+    sc.terms, acc = _terms(simulation.body_count, accelerations, center, strength)  # acc stays alive until oracle_solve returns
     rc = lib.oracle_solve(C.byref(sc), dt)
     if rc != 0:
         raise RuntimeError("oracle_solve failed: %d" % rc)
@@ -137,9 +160,10 @@ def first_fit_batches(refs, body_count, fallback_threshold=64, order=0, prioriti
     return out, count
 
 
-def predict_bounding_boxes(bodies, shapes, activities, dt, integrator):
+def predict_bounding_boxes(bodies, shapes, activities, dt, integrator, accelerations=None, center=None, strength=0.0):
     """PoseIntegrator.PredictBoundingBoxes restated (PoseIntegrator.cs:L307-370): bodies[n, 32], shapes / activities as the record arrays of
-    bepuphysics2_b200.native (activities updated in place). Returns bounds[n, 8] = {min.xyz, speculative margin, max.xyz, valid}."""
+    bepuphysics2_b200.native (activities updated in place), velocity terms as for solve. Returns bounds[n, 8] = {min.xyz, speculative margin,
+    max.xyz, valid}."""
     lib = load()
     bodies = np.ascontiguousarray(bodies, dtype=np.float32).reshape(-1, 32)
     n = bodies.shape[0]
@@ -147,8 +171,10 @@ def predict_bounding_boxes(bodies, shapes, activities, dt, integrator):
     shapes = np.ascontiguousarray(shapes)
     bounds = np.zeros((max(n, 1), 8), dtype=np.float32)
     gravity = (C.c_float * 3)(*integrator.gravity)
-    lib.oracle_predict_bounding_boxes.argtypes = [C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_float, C.c_void_p, C.c_float, C.c_float, C.c_int32, C.c_void_p]
+    terms, acc = _terms(n, accelerations, center, strength)
+    lib.oracle_predict_bounding_boxes.argtypes = [C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_float, C.c_void_p, C.c_float, C.c_float, C.c_int32, C.c_void_p,
+                                                  C.POINTER(OracleIntegratorTerms)]
     rc = lib.oracle_predict_bounding_boxes(n, bodies.ctypes.data, shapes.ctypes.data, activities.ctypes.data, dt, gravity, integrator.linear_damping, integrator.angular_damping,
-                                           int(integrator.integrate_velocity_for_kinematics), bounds.ctypes.data)
+                                           int(integrator.integrate_velocity_for_kinematics), bounds.ctypes.data, C.byref(terms))
     assert rc == 0
     return bounds[:n]

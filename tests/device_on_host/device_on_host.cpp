@@ -97,7 +97,8 @@ extern "C" int32_t device_on_host_type_info(int32_t type_id, int32_t* bodies, in
 // The integration arithmetic of csrc/bepu_integration.cuh. op 0: integrate_orientation(q[0..3], w[4..6], halfDt[7]) -> q; 1: rotate_inverse_inertia(
 // local[0..5], q[6..9]) -> 6 floats; 2: integrate_angular_conserve_momentum(previous q[0..3], local[4..9], world[10..15], w[16..18]) -> w;
 // 3: integrate_angular_gyroscopic(q[0..3], local[4..9], w[10..12], dt[13]) -> w; 4: callback_integrate_velocity(v[0..5], gravity dt[6..8],
-// linear damping dt[9], angular damping dt[10]) -> v.
+// linear damping dt[9], angular damping dt[10]) -> v; 5: integrate_velocity_extensions(v[0..5], linear acceleration[6..8], angular acceleration[9..11],
+// dt[12], position[13..15], center[16..18], attractorDt[19], accelerations on[20] != 0, point gravity on[21] != 0) -> v.
 extern "C" int32_t device_on_host_eval_integration(int32_t op, const float* in, float* out) {
     auto sym = [&](int i) { return Sym3{in[i], in[i + 1], in[i + 2], in[i + 3], in[i + 4], in[i + 5]}; };
     if (op == 0) {
@@ -117,6 +118,11 @@ extern "C" int32_t device_on_host_eval_integration(int32_t op, const float* in, 
     } else if (op == 4) {
         Velocity v{{in[0], in[1], in[2]}, {in[3], in[4], in[5]}};
         callback_integrate_velocity(v, in[6], in[7], in[8], in[9], in[10]);
+        out[0] = v.lin.x; out[1] = v.lin.y; out[2] = v.lin.z; out[3] = v.ang.x; out[4] = v.ang.y; out[5] = v.ang.z;
+    } else if (op == 5) {
+        Velocity v{{in[0], in[1], in[2]}, {in[3], in[4], in[5]}};
+        integrate_velocity_extensions(v, in[20] != 0.0f, V3{in[6], in[7], in[8]}, V3{in[9], in[10], in[11]}, in[12], in[21] != 0.0f, V3{in[13], in[14], in[15]},
+                                      V3{in[16], in[17], in[18]}, in[19]);
         out[0] = v.lin.x; out[1] = v.lin.y; out[2] = v.lin.z; out[3] = v.ang.x; out[4] = v.ang.y; out[5] = v.ang.z;
     } else {
         return -1;

@@ -111,7 +111,8 @@ def test_device_constraint_source_matches_the_oracle_bit_for_bit(libs, device_on
 
 def test_device_integration_source_matches_the_oracle_bit_for_bit(libs, device_on_host):
     """csrc/bepu_integration.cuh (orientation integration through the custom sin / cos, inertia rotation, both momentum-conserving angular
-    updates, the velocity callback) against the oracle's restatement of PoseIntegrator.cs:L146-253, function by function."""
+    updates, the velocity callback, the optional per-body acceleration and point-gravity terms) against the oracle's restatement of
+    PoseIntegrator.cs:L146-253, DemoCallbacks.cs, PerBodyGravityDemo.cs and PlanetDemo.cs, function by function."""
     dev, orc = device_on_host
     rng = np.random.default_rng(11)
 
@@ -144,6 +145,21 @@ def test_device_integration_source_matches_the_oracle_bit_for_bit(libs, device_o
             assert orc.oracle_eval_integration(op, _ptr(operands), _ptr(b)) == 0
             assert np.isfinite(b).all()
             assert np.array_equal(a.view(np.uint32), b.view(np.uint32)), "integration op %d, trial %d: %s vs %s" % (op, trial, a, b)
+
+    # op 5, the optional terms: neither, point gravity alone and both; positions and center close together (|offset| <= 1 clamps) and far apart
+    rng = np.random.default_rng(17)
+    for trial in range(4000):
+        operands = np.zeros(22, dtype=np.float32)
+        operands[0:12] = rng.normal(0, 5, size=12)
+        operands[12] = rng.uniform(1e-3, 0.05)
+        operands[13:19] = rng.normal(0, 3 if trial % 2 else 50, size=6)
+        operands[19] = rng.uniform(-100, 100)
+        operands[20], operands[21] = (trial >> 1) & 1, 1 if trial % 4 != 1 else 0
+        a, b = np.zeros(6, dtype=np.float32), np.zeros(6, dtype=np.float32)
+        assert dev.device_on_host_eval_integration(5, _ptr(operands), _ptr(a)) == 0
+        assert orc.oracle_eval_integration(5, _ptr(operands), _ptr(b)) == 0
+        assert np.isfinite(b).all()
+        assert np.array_equal(a.view(np.uint32), b.view(np.uint32)), "integration op 5, trial %d: %s -> %s vs %s" % (trial, operands, a, b)
 
 
 def test_bounds_source_reproduces_the_reference_vectors_bit_for_bit(device_on_host):

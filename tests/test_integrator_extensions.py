@@ -1,15 +1,10 @@
 """Per-body accelerations and point gravity after the declarative velocity callback (bepucuda_set_body_accelerations /
-bepucuda_set_point_gravity; PerBodyGravityDemo.cs and PlanetDemo.cs of the reference). The oracle of the terms is
-tests/integrator_extensions/oracle_integrator_extensions.cpp: the oracle's translation unit with the driver functions that call IntegrateVelocity
-restated. CPU: that oracle against closed forms, its scalar against its 8-wide evaluation, per-body gravity against uniform gravity, no terms
-against oracle_solve, and the CUDA arithmetic compiled for the host against it. GPU: the strict build against it bit for bit at every
-integration site, the fast build within tolerance, and the error rules."""
-import atexit
+bepucuda_set_point_gravity; PerBodyGravityDemo.cs and PlanetDemo.cs of the reference). The terms are part of the oracle (ob.solve and
+ob.predict_bounding_boxes take them as keywords). CPU: the oracle with the terms against closed forms, its scalar against its 8-wide
+evaluation, per-body gravity against uniform gravity (its threaded path is in tests/test_oracle.py, the CUDA arithmetic compiled for the host
+in tests/test_device_source_on_host.py). GPU: the strict build against the oracle bit for bit at every integration site, the fast build within
+tolerance, and the error rules."""
 import ctypes as C
-import os
-import shutil
-import subprocess
-import tempfile
 
 import numpy as np
 import pytest
@@ -20,95 +15,6 @@ from tests import util
 
 DT = 1.0 / 60.0
 f32 = np.float32
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-HERE = os.path.join(ROOT, "tests", "integrator_extensions")
-_LIBS = {}
-
-
-class Terms(C.Structure):
-    """bepu_oracle::ext::Terms of oracle_integrator_extensions.cpp."""
-    _fields_ = [("accelerations", C.c_void_p), ("point_gravity", C.c_int32), ("center", C.c_float * 3), ("strength", C.c_float)]
-
-
-def _compile(name, source, flags):
-    """Both test libraries are compiled once per process into a temporary directory: the tree itself may be read-only."""
-    if name not in _LIBS:
-        if "dir" not in _LIBS:
-            _LIBS["dir"] = tempfile.mkdtemp(prefix="bepu_integrator_extensions_")
-            atexit.register(shutil.rmtree, _LIBS["dir"], True)
-        lib = os.path.join(_LIBS["dir"], name)
-        subprocess.check_call(["/usr/bin/g++", "-O2", "-std=c++17", "-fPIC", "-shared", "-ffp-contract=off", "-fno-fast-math", "-march=x86-64-v3", "-Wall",
-                               "-Wno-unused-function", "-Wno-psabi"] + flags + ["-o", lib, os.path.join(HERE, source)])
-        _LIBS[name] = C.CDLL(lib)
-    return _LIBS[name]
-
-
-def _oracle_ext():
-    lib = _compile("liboracle_integrator_extensions.so", "oracle_integrator_extensions.cpp", ["-fopenmp", "-I", os.path.join(ROOT, "oracle")])
-    lib.oracle_ext_solve.argtypes = [C.POINTER(ob.OracleScene), C.POINTER(Terms), C.c_float]
-    lib.oracle_ext_predict_bounding_boxes.argtypes = [C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_float, C.c_void_p, C.c_float, C.c_float, C.c_int32,
-                                                      C.POINTER(Terms), C.c_void_p]
-    lib.oracle_ext_eval.argtypes = [C.c_void_p, C.c_void_p]
-    return lib
-
-
-def _terms(accelerations, center, strength):
-    t = Terms()
-    acc = None if accelerations is None else np.ascontiguousarray(accelerations, dtype=np.float32).reshape(-1, 8)
-    t.accelerations = acc.ctypes.data if acc is not None and acc.size else None
-    t.point_gravity = 0 if center is None else 1
-    if center is not None:
-        for i in range(3):
-            t.center[i] = float(np.float32(center[i]))
-        t.strength = float(np.float32(strength))
-    return t, acc
-
-
-def solve_ex(simulation, dt, accelerations=None, center=None, strength=0.0, simd=False):
-    """ob.solve on `simulation`'s buffers in place, with the terms (oracle_ext_solve; one worker)."""
-    terms, acc = _terms(accelerations, center, strength)
-    assert acc is None or acc.shape[0] == simulation.body_count
-    per_batch = [[] for _ in range(simulation.batch_count)]
-    for tb in simulation.type_batches():
-        per_batch[tb.batch_index].append(tb)
-    keep = []
-    batches = (ob.OracleBatch * max(simulation.batch_count, 1))()
-    for b, tbs in enumerate(per_batch):
-        arr = (ob.OracleTypeBatch * max(len(tbs), 1))()
-        for i, tb in enumerate(tbs):
-            arr[i].type_id, arr[i].constraint_count = tb.type_id, tb.constraint_count
-            arr[i].body_references, arr[i].prestep, arr[i].accumulated_impulses = tb.body_references.ctypes.data, tb.prestep.ctypes.data, tb.accumulated_impulses.ctypes.data
-        keep.append(arr)
-        batches[b].type_batch_count, batches[b].type_batches = len(tbs), arr
-    sc = ob.OracleScene()
-    sc.bodies = simulation.bodies.ctypes.data if simulation.body_count else None
-    sc.body_count, sc.batch_count, sc.batches, sc.bundle_width = simulation.body_count, simulation.batch_count, batches, simulation.bundle_width
-    its = (C.c_int32 * len(simulation.velocity_iterations))(*simulation.velocity_iterations)
-    sc.substep_count, sc.velocity_iterations, sc.fallback_batch_threshold = len(simulation.velocity_iterations), its, simulation.fallback_batch_threshold
-    d = simulation.integrator
-    for i in range(3):
-        sc.gravity[i] = d.gravity[i]
-    sc.linear_damping, sc.angular_damping, sc.angular_integration_mode = d.linear_damping, d.angular_damping, d.angular_integration_mode
-    sc.allow_substeps_for_unconstrained, sc.integrate_velocity_for_kinematics = d.allow_substeps_for_unconstrained, d.integrate_velocity_for_kinematics
-    kin = np.ascontiguousarray(simulation.constrained_kinematics, dtype=np.int32)
-    sc.constrained_kinematics, sc.constrained_kinematic_count = (kin.ctypes.data if kin.size else None), int(kin.size)
-    sc.threads, sc.simd = 1, 1 if simd else 0
-    rc = _oracle_ext().oracle_ext_solve(C.byref(sc), C.byref(terms), dt)
-    assert rc == 0, "oracle_ext_solve failed: %d" % rc
-
-
-def predict_bounding_boxes_ex(bodies, shapes, activities, dt, integrator, accelerations=None, center=None, strength=0.0):
-    """ob.predict_bounding_boxes with the terms (oracle_ext_predict_bounding_boxes); activities updated in place."""
-    bodies = np.ascontiguousarray(bodies, dtype=np.float32).reshape(-1, 32)
-    n = bodies.shape[0]
-    shapes = np.ascontiguousarray(shapes)
-    terms, acc = _terms(accelerations, center, strength)
-    bounds = np.zeros((max(n, 1), 8), dtype=np.float32)
-    gravity = (C.c_float * 3)(*integrator.gravity)
-    rc = _oracle_ext().oracle_ext_predict_bounding_boxes(n, bodies.ctypes.data, shapes.ctypes.data, activities.ctypes.data, dt, gravity, integrator.linear_damping,
-                                                         integrator.angular_damping, int(integrator.integrate_velocity_for_kinematics), C.byref(terms), bounds.ctypes.data)
-    assert rc == 0
-    return bounds[:n]
 
 
 def _integrator(gravity=(0.0, -10.0, 0.0), damping=0.03, angular_mode=0, allow_substeps=0, kinematics=0):
@@ -148,7 +54,7 @@ def test_unconstrained_body_takes_a_times_dt(libs, allow_substeps):
     v = sim.bodies[0, 8:11].copy()
     w = sim.bodies[0, 12:15].copy()
     p = sim.bodies[0, 4:7].copy()
-    solve_ex(sim, DT, accelerations=a)
+    ob.solve(sim, DT, accelerations=a)
     dt = f32(DT) / f32(substeps) if allow_substeps else f32(DT)
     for _ in range(substeps if allow_substeps else 1):
         v = (v + np.array([0, g * dt, 0], dtype=f32)) * f32(1.0)
@@ -165,7 +71,7 @@ def test_point_gravity_one_step(libs):
     center, strength = np.array([0.5, -20.0, 3.0], dtype=f32), f32(1000.0)
     sim = util.make_sim(_one_body((4, 7, -2), (0.0, 0.0, 0.0), (0.0, 0.0, 0.0)), integrator=_integrator(gravity=(0, 0, 0), damping=0.0))
     pos = sim.bodies[0, 4:7].copy()
-    solve_ex(sim, DT, center=center, strength=strength)
+    ob.solve(sim, DT, center=center, strength=strength)
     offset = pos - center
     d = np.sqrt(offset[0] * offset[0] + offset[1] * offset[1] + offset[2] * offset[2])
     inverse = f32(1.0) / max(f32(1.0), d * d * d)
@@ -185,8 +91,8 @@ def test_scalar_and_eight_wide_oracle_agree_with_both_terms(libs, angular_mode):
     a, b = (util.make_sim(scene, substeps=3, velocity_iterations=2, integrator=integ) for _ in range(2))
     acc = _accelerations(a.body_count, 5)
     for _ in range(2):
-        solve_ex(a, DT, accelerations=acc, center=(0, -30, 0), strength=500.0)
-        solve_ex(b, DT, accelerations=acc, center=(0, -30, 0), strength=500.0, simd=True)
+        ob.solve(a, DT, accelerations=acc, center=(0, -30, 0), strength=500.0)
+        ob.solve(b, DT, simd=True, accelerations=acc, center=(0, -30, 0), strength=500.0)
     util.compare(util.snapshot(a), util.snapshot(b), exact=True)
 
 
@@ -202,37 +108,18 @@ def test_per_body_acceleration_equal_to_gravity_matches_uniform_gravity(libs):
     acc[:, 1] = -10.0
     for _ in range(2):
         ob.solve(uniform, DT)
-        solve_ex(per_body, DT, accelerations=acc)
+        ob.solve(per_body, DT, accelerations=acc)
     cols = util.MEANINGFUL
     assert (uniform.bodies[:, cols] == per_body.bodies[:, cols]).all()
 
 
 def test_no_extension_is_oracle_solve_bit_for_bit(libs):
+    """Zero accelerations and point gravity of strength 0 run the terms at every integration site and must change nothing."""
     scene = _mixed_scene()
     a, b = (util.make_sim(scene, substeps=2, velocity_iterations=2, integrator=_integrator(kinematics=1)) for _ in range(2))
     ob.solve(a, DT)
-    solve_ex(b, DT)
+    ob.solve(b, DT, accelerations=np.zeros((b.body_count, 8), dtype=np.float32), center=(0, -30, 0), strength=0.0)
     util.compare(util.snapshot(a), util.snapshot(b), exact=True)
-
-
-def test_extension_source_on_host_matches_the_oracle_bit_for_bit():
-    """integrate_velocity_extensions of csrc/bepu_integration.cuh compiled for the host against the oracle's statement, on random operands."""
-    dev = _compile("libdevice_integrator_extensions_on_host.so", "device_integrator_extensions_on_host.cpp",
-                   ["-I", os.path.join(ROOT, "tests", "device_on_host", "stubs"), "-I", os.path.join(ROOT, "bepuphysics2_b200", "csrc")])
-    dev.device_integrator_extensions_on_host_eval.argtypes = [C.c_void_p, C.c_void_p]
-    orc = _oracle_ext()
-    rng = np.random.default_rng(17)
-    for k in range(4000):
-        x = np.zeros(22, dtype=np.float32)
-        x[0:12] = rng.normal(0, 5, size=12)
-        x[12] = rng.uniform(1e-3, 0.05)
-        x[13:19] = rng.normal(0, 3 if k % 2 else 50, size=6)
-        x[19] = rng.uniform(-100, 100)
-        x[20], x[21] = (k >> 1) & 1, 1 if k % 4 != 1 else 0
-        a, b = np.zeros(6, dtype=np.float32), np.zeros(6, dtype=np.float32)
-        assert dev.device_integrator_extensions_on_host_eval(x.ctypes.data, a.ctypes.data) == 0
-        assert orc.oracle_ext_eval(x.ctypes.data, b.ctypes.data) == 0
-        assert np.array_equal(a.view(np.uint32), b.view(np.uint32)), (k, x, a, b)
 
 
 # ---- GPU -------------------------------------------------------------------------------------------------------------------------------------------
@@ -244,7 +131,7 @@ def _gpu_parity(scene, frames=2, mode=native.EXEC_GRAPH, exact=True, resident=Fa
     a, b = util.make_sim(scene, **kw), util.make_sim(scene, **kw)
     acc = _accelerations(a.body_count, 11)
     for _ in range(frames):
-        solve_ex(a, DT, accelerations=acc, center=CENTER, strength=STRENGTH)
+        ob.solve(a, DT, accelerations=acc, center=CENTER, strength=STRENGTH)
     ts = native.CudaTimestepper(b, strict_fp=exact, execution_mode=mode)
     try:
         ts.describe()
@@ -314,7 +201,7 @@ def test_predict_bounding_boxes_with_both_terms(libs):
     activities["sleep_threshold"], activities["minimum_timesteps_under_threshold"] = 0.01, 4
     acc = _accelerations(n, 4, scale=50.0)
     ref_act = activities.copy()
-    ref = predict_bounding_boxes_ex(sim.bodies, shapes, ref_act, DT, sim.integrator, accelerations=acc, center=CENTER, strength=STRENGTH)
+    ref = ob.predict_bounding_boxes(sim.bodies, shapes, ref_act, DT, sim.integrator, accelerations=acc, center=CENTER, strength=STRENGTH)
     plain = ob.predict_bounding_boxes(sim.bodies, shapes, activities.copy(), DT, sim.integrator)
     assert not np.array_equal(ref, plain)
     ts = native.CudaTimestepper(sim, strict_fp=True)
@@ -335,7 +222,7 @@ def test_profile_stages_advances_like_solve(libs):
     scene = scenes.merge(scenes.box_stacks(6, 8), scenes.joint_zoo(400, 20, seed=6))
     a, b = (util.make_sim(scene, substeps=2, velocity_iterations=2, integrator=_integrator(kinematics=1)) for _ in range(2))
     acc = _accelerations(a.body_count, 12)
-    solve_ex(a, DT, accelerations=acc, center=CENTER, strength=STRENGTH)
+    ob.solve(a, DT, accelerations=acc, center=CENTER, strength=STRENGTH)
     ts = native.CudaTimestepper(b, strict_fp=True)
     try:
         ts.describe()
@@ -369,7 +256,7 @@ def test_two_shard_ranks_bit_exact(libs):
         for s in solvers:
             s.synchronize()
         for _ in range(2):
-            solve_ex(sim, DT, accelerations=acc, center=CENTER, strength=STRENGTH)
+            ob.solve(sim, DT, accelerations=acc, center=CENTER, strength=STRENGTH)
             for s in solvers:
                 s.solve(DT)
         for s in solvers:

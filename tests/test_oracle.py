@@ -42,12 +42,21 @@ def test_ragdolls_scalar_and_simd_are_bit_identical(libs):
     util.compare(a, b, exact=True)
 
 
-@pytest.mark.parametrize("name,threads", [("pile", 4), ("pile", 3), ("fallback", 3), ("ragdolls", 5)])
+@pytest.mark.parametrize("name,threads", [("pile", 4), ("pile", 3), ("fallback", 3), ("ragdolls", 5), ("mixed_with_terms", 4)])
 def test_thread_count_does_not_change_results(libs, name, threads):
-    """The worker loop (one share of every batch stage per worker, spin sync between stages, fallback batch on worker 0) against one thread."""
-    scene = {"pile": lambda: scenes.shape_pile(3000, seed=8), "fallback": lambda: scenes.fallback_stress(1500, hubs=2, seed=8), "ragdolls": lambda: scenes.ragdolls(40, seed=8)}[name]()
-    a = util.run_oracle(util.make_sim(scene, substeps=3, velocity_iterations=2), DT, frames=2, threads=1, simd=True)
-    b = util.run_oracle(util.make_sim(scene, substeps=3, velocity_iterations=2), DT, frames=2, threads=threads, simd=True)
+    """The worker loop (one share of every batch stage per worker, spin sync between stages, fallback batch on worker 0) against one thread.
+    mixed_with_terms: contacts, ragdolls and a joint zoo with kinematic velocity integration, per-body accelerations and point gravity."""
+    scene = {"pile": lambda: scenes.shape_pile(3000, seed=8), "fallback": lambda: scenes.fallback_stress(1500, hubs=2, seed=8), "ragdolls": lambda: scenes.ragdolls(40, seed=8),
+             "mixed_with_terms": lambda: scenes.merge(scenes.box_stacks(4, 6), scenes.ragdolls(6, seed=3), scenes.joint_zoo(400, 20, seed=4))}[name]()
+    integ, terms = None, {}
+    if name == "mixed_with_terms":
+        integ = bp.IntegratorDesc.default()
+        integ.integrate_velocity_for_kinematics = 1
+        accelerations = np.random.default_rng(5).uniform(-5, 5, size=(scene["bodies"].shape[0], 8)).astype(np.float32)
+        accelerations[:, 3] = accelerations[:, 7] = 0.0
+        terms = {"accelerations": accelerations, "center": (0, -30, 0), "strength": 500.0}
+    a = util.run_oracle(util.make_sim(scene, substeps=3, velocity_iterations=2, integrator=integ), DT, frames=2, threads=1, simd=True, **terms)
+    b = util.run_oracle(util.make_sim(scene, substeps=3, velocity_iterations=2, integrator=integ), DT, frames=2, threads=threads, simd=True, **terms)
     util.compare(a, b, exact=True)
 
 

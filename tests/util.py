@@ -25,9 +25,9 @@ def snapshot(sim):
     return out
 
 
-def run_oracle(sim, dt, frames=1, threads=1, simd=False):
+def run_oracle(sim, dt, frames=1, threads=1, simd=False, accelerations=None, center=None, strength=0.0):
     for _ in range(frames):
-        ob.solve(sim, dt, threads=threads, simd=simd)
+        ob.solve(sim, dt, threads=threads, simd=simd, accelerations=accelerations, center=center, strength=strength)
     return snapshot(sim)
 
 
