@@ -15,6 +15,17 @@ StageLauncher launch_stage_warm_start_first, launch_stage_warm_start, launch_sta
 #define BEPU_DEEP_MINB 12
 #endif
 constexpr int kDeepBatchBundles = 2150;  // more bundles than the uncapped build keeps resident at once (132 SMs x 16 warps on an H100 SXM)
+// Register budgets of the contact-only stage kernels (kLaunchContactsOnly, below kDeepBatchBundles). The next stage's CTAs can become resident (and
+// run their prologue) only in the slots this one leaves free, so the head batches of a 100 k-body pile (1100-1500 bundles, 8-11 warps per SM)
+// overlap where 16 warps did not. WarmStart: 10 two-warp CTAs = 20 warps per SM, at most 96 registers, no spills. Solve: 12 CTAs = 24 warps per
+// SM at 80 registers (no spills in the fast build); on an H100 it took the Solve stages of the pile 5 % below the 96-register budget, while the
+// WarmStart stages at 80 registers spill and were no faster.
+#ifndef BEPU_CONTACT_MINB
+#define BEPU_CONTACT_MINB 10
+#endif
+#ifndef BEPU_CONTACT_SOLVE_MINB
+#define BEPU_CONTACT_SOLVE_MINB 12
+#endif
 // Launches one stage kernel instantiation (plain or sharded), one warp per bundle.
 template <auto Kernel, class... Args>
 static void launch_stage_kernel(int work_count, int launch_flags, cudaStream_t s, Args... args) {
@@ -37,30 +48,32 @@ static void launch_stage_kernel(int work_count, int launch_flags, cudaStream_t s
     cfg.numAttrs = (launch_flags & bepucuda::kLaunchPdl) ? 1 : 0;
     cudaLaunchKernelEx(&cfg, Kernel, args...);
 }
-template <int STAGE, int MINB, bool kExt>
+template <int STAGE, int MINB, bool kExt, bool kContacts>
 static void launch_stage_instance(const WorkRecord* records, const int32_t* ref_rows, int work_count, const BodyBuffers& B, const FrameParams* fp, int launch_flags, const ShardLaunch* shard,
                                   cudaStream_t s) {
-    const int flags = (launch_flags & bepucuda::kLaunchPrefetchRows) ? kStagePrefetchRows : 0;
-    if (!shard) launch_stage_kernel<constraint_stage_kernel<STAGE, MINB, kExt>>(work_count, launch_flags, s, records, ref_rows, work_count, B, fp, flags);
-    else if constexpr (STAGE != kStageIncremental)  // the incremental contact update is never sharded
+    const int flags = ((launch_flags & bepucuda::kLaunchPrefetchRows) ? kStagePrefetchRows : 0) | ((launch_flags & bepucuda::kLaunchPrefetchBodies) ? kStagePrefetchBodies : 0);
+    if (!shard) launch_stage_kernel<constraint_stage_kernel<STAGE, MINB, kExt, kContacts>>(work_count, launch_flags, s, records, ref_rows, work_count, B, fp, flags);
+    else if constexpr (STAGE != kStageIncremental && !kContacts)  // the incremental contact update is never sharded; sharded stages run the full switch
         launch_stage_kernel<constraint_stage_kernel_sharded<STAGE, MINB, kExt>>(work_count, launch_flags, s, records, ref_rows, work_count, B, fp, flags, shard->peers, shard->peer_delta,
                                                                                shard->stage);
 }
 // The WarmStart stages integrate: contexts with per-body accelerations or point gravity run their own instantiation (kLaunchIntegratorExtensions).
-template <int STAGE, int MINB>
+template <int STAGE, int MINB, bool kContacts>
 static void launch_stage_variant(const WorkRecord* records, const int32_t* ref_rows, int work_count, const BodyBuffers& B, const FrameParams* fp, int launch_flags, const ShardLaunch* shard,
                                  cudaStream_t s) {
     if constexpr (STAGE == kStageWarmStartFirst || STAGE == kStageWarmStart) {
-        if (launch_flags & bepucuda::kLaunchIntegratorExtensions) return launch_stage_instance<STAGE, MINB, true>(records, ref_rows, work_count, B, fp, launch_flags, shard, s);
+        if (launch_flags & bepucuda::kLaunchIntegratorExtensions) return launch_stage_instance<STAGE, MINB, true, kContacts>(records, ref_rows, work_count, B, fp, launch_flags, shard, s);
     }
-    launch_stage_instance<STAGE, MINB, false>(records, ref_rows, work_count, B, fp, launch_flags, shard, s);
+    launch_stage_instance<STAGE, MINB, false, kContacts>(records, ref_rows, work_count, B, fp, launch_flags, shard, s);
 }
 template <int STAGE>
 static void launch_stage_t(const WorkRecord* records, const int32_t* ref_rows, int work_count, const BodyBuffers& B, const FrameParams* fp, int launch_flags, const ShardLaunch* shard, cudaStream_t s) {
     if constexpr (STAGE != kStageIncremental) {
-        if (work_count >= kDeepBatchBundles) return launch_stage_variant<STAGE, BEPU_DEEP_MINB>(records, ref_rows, work_count, B, fp, launch_flags, shard, s);
+        if (work_count >= kDeepBatchBundles) return launch_stage_variant<STAGE, BEPU_DEEP_MINB, false>(records, ref_rows, work_count, B, fp, launch_flags, shard, s);
+        if (!shard && (launch_flags & bepucuda::kLaunchContactsOnly))
+            return launch_stage_variant<STAGE, STAGE == kStageSolve ? BEPU_CONTACT_SOLVE_MINB : BEPU_CONTACT_MINB, true>(records, ref_rows, work_count, B, fp, launch_flags, shard, s);
     }
-    launch_stage_variant<STAGE, 1>(records, ref_rows, work_count, B, fp, launch_flags, shard, s);
+    launch_stage_variant<STAGE, 1, false>(records, ref_rows, work_count, B, fp, launch_flags, shard, s);
 }
 
 #if BEPU_UNIT == 0

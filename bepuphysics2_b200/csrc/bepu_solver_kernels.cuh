@@ -84,17 +84,32 @@ BEPU_DI void apply_velocity_extensions(const FrameParams& fp, uint32_t idx, V3 p
                                          attractorDt);
 }
 
+// Body records of body slots 0 and 1 that a plain stage kernel loaded before its grid-dependency wait (see constraint_stage_body); bit s of
+// `slots` is set when slot s was loaded. Solve: world inertia, and pose for kNeedsPose types. WarmStart: local inertia and pose of an integrating slot.
+struct EarlyBodies {
+    uint32_t slots;
+    Inertia inertia[2];
+    V3 pos[2];
+    Q4 q[2];
+};
+
 // GatherAndIntegrate for one body slot of one lane (TypeProcessor.cs:L1298-1397), after the velocity has been loaded. The lane integrates iff the
 // device body reference carries kRefIntegrateBit; all other lanes read the world inertia their owner constraint stored earlier in this substep,
 // which is bit-identical to what the reference's bundle-wide recompute would give them. kExt: the stage kernel instantiation for contexts with
 // per-body accelerations or point gravity (the launcher picks it), so that the default path carries none of it.
 template <int STAGE, bool NeedsPose, bool kExt>
-BEPU_DI void warm_start_body(uint32_t enc, const BodyBuffers& B, const FrameParams& fp, BodyState& b, Velocity& v) {
+BEPU_DI void warm_start_body(uint32_t enc, const BodyBuffers& B, const FrameParams& fp, bool early_slot, const EarlyBodies& early, int s, BodyState& b, Velocity& v) {
     const uint32_t idx = enc & kRefIndexMask;
     if (enc & kRefIntegrateBit) {
         Inertia local;
-        load_inertia(B.inertia_local, idx, local);
-        load_pose(B.pose, idx, b.pos, b.q);
+        if (early_slot) {
+            local = early.inertia[s];
+            b.pos = early.pos[s];
+            b.q = early.q[s];
+        } else {
+            load_inertia(B.inertia_local, idx, local);
+            load_pose(B.pose, idx, b.pos, b.q);
+        }
         b.inertia.inv_mass = local.inv_mass;
         if (STAGE == kStageWarmStart) {
             // IntegratePoseAndVelocity, TypeProcessor.cs:L1204-1248
@@ -137,9 +152,9 @@ BEPU_DI void warm_start_body(uint32_t enc, const BodyBuffers& B, const FramePara
     }
 }
 template <int STAGE, bool NeedsPose, bool kExt>
-BEPU_DI void gather_for_warm_start(uint32_t enc, const BodyBuffers& B, const FrameParams& fp, BodyState& b, Velocity& v) {
+BEPU_DI void gather_for_warm_start(uint32_t enc, const BodyBuffers& B, const FrameParams& fp, bool early_slot, const EarlyBodies& early, int s, BodyState& b, Velocity& v) {
     load_velocity(B.velocity, enc & kRefIndexMask, v);
-    warm_start_body<STAGE, NeedsPose, kExt>(enc, B, fp, b, v);
+    warm_start_body<STAGE, NeedsPose, kExt>(enc, B, fp, early_slot, early, s, b, v);
 }
 
 // ---- uniform call shapes over contact and joint types ------------------------------------------------------------------
@@ -180,8 +195,8 @@ BEPU_DI void push_record(float4* const* arrays, uint32_t mask, uint32_t idx, flo
     }
 }
 template <class T, int STAGE, bool kSharded, bool kExt, class PR, class AR>
-BEPU_DI void run_lane(const int32_t* refs, PR p, AR a, float* p_rw, uint32_t enc0, uint32_t enc1, const BodyBuffers& B, const FrameParams& fp, const ShardPeers* peers = nullptr,
-                      long long peer_delta = 0) {
+BEPU_DI void run_lane(const int32_t* refs, PR p, AR a, float* p_rw, uint32_t enc0, uint32_t enc1, const BodyBuffers& B, const FrameParams& fp, const EarlyBodies& early,
+                      const ShardPeers* peers = nullptr, long long peer_delta = 0) {
     constexpr int NB = T::kBodies;
     uint32_t enc[NB];
     enc[0] = enc0;
@@ -205,8 +220,13 @@ BEPU_DI void run_lane(const int32_t* refs, PR p, AR a, float* p_rw, uint32_t enc
         for (int s = 0; s < NB; ++s) {
             const uint32_t idx = enc[s] & kRefIndexMask;
             load_velocity(B.velocity, idx, v[s]);
-            load_inertia(B.inertia_world, idx, b[s].inertia);
-            if (T::kNeedsPose) load_pose(B.pose, idx, b[s].pos, b[s].q);
+            if (s < 2 && (early.slots >> s & 1u)) {
+                b[s].inertia = early.inertia[s & 1];
+                if (T::kNeedsPose) b[s].pos = early.pos[s & 1], b[s].q = early.q[s & 1];
+            } else {
+                load_inertia(B.inertia_world, idx, b[s].inertia);
+                if (T::kNeedsPose) load_pose(B.pose, idx, b[s].pos, b[s].q);
+            }
         }
         rows_ready(p);
         call_solve<T>(b, fp.dt, fp.inverse_dt, p, a, v);
@@ -221,7 +241,7 @@ BEPU_DI void run_lane(const int32_t* refs, PR p, AR a, float* p_rw, uint32_t enc
             }
     } else {
 #pragma unroll
-        for (int s = 0; s < NB; ++s) gather_for_warm_start<STAGE, T::kNeedsPose, kExt>(enc[s], B, fp, b[s], v[s]);
+        for (int s = 0; s < NB; ++s) gather_for_warm_start<STAGE, T::kNeedsPose, kExt>(enc[s], B, fp, s < 2 && (early.slots >> s & 1u), early, s & 1, b[s], v[s]);
         rows_ready(p);
         call_warm_start<T>(b, p, a, v);
 #pragma unroll
@@ -242,10 +262,6 @@ BEPU_DI void run_lane(const int32_t* refs, PR p, AR a, float* p_rw, uint32_t enc
                 }
             }
     }
-}
-template <class T, int STAGE, class PR, class AR>
-BEPU_DI void run_lane(const int32_t* refs, PR p, AR a, float* p_rw, uint32_t enc0, uint32_t enc1, const BodyBuffers& B, const FrameParams& fp) {
-    run_lane<T, STAGE, false, false>(refs, p, a, p_rw, enc0, enc1, B, fp);
 }
 
 // Work records and body references are loaded with `asm volatile` so that the loads are ISSUED where the source places them (a whole pipeline
@@ -273,29 +289,34 @@ BEPU_DI WorkRecord load_record(const WorkRecord* r) {
     X(8, NonconvexOneBody<2>) X(9, NonconvexOneBody<3>) X(10, NonconvexOneBody<4>)                                                \
     X(15, NonconvexTwoBody<2>) X(16, NonconvexTwoBody<3>) X(17, NonconvexTwoBody<4>)
 
-template <int STAGE, bool kSharded, bool kExt, class PR, class AR>
-BEPU_DI void run_bundle_rows(const WorkRecord& rec, int lane, PR p, AR a, uint32_t enc0, uint32_t enc1, const BodyBuffers& B, const FrameParams& fp, const ShardPeers* peers = nullptr,
-                             long long peer_delta = 0) {
+// kContacts: the switch covers the contact types only. The host launches that instantiation for device batches whose every bundle is a contact
+// (kLaunchContactsOnly); it is about half the code of the full switch and fits a smaller register budget (bepu_solver_kernels.cu).
+template <int STAGE, bool kSharded, bool kExt, bool kContacts, class PR, class AR>
+BEPU_DI void run_bundle_rows(const WorkRecord& rec, int lane, PR p, AR a, uint32_t enc0, uint32_t enc1, const BodyBuffers& B, const FrameParams& fp, const EarlyBodies& early,
+                             const ShardPeers* peers = nullptr, long long peer_delta = 0) {
     const int32_t* refs = rec.refs + lane;
     float* p_rw = rec.prestep + lane;
-    switch (rec.type_id) {
 #define BEPU_CASE(ID, T) \
-    case ID: run_lane<T, STAGE, kSharded, kExt>(refs, p, a, p_rw, enc0, enc1, B, fp, peers, peer_delta); break;
-        BEPU_CONTACT_TYPES(BEPU_CASE)
-        BEPU_JOINT_TYPES(BEPU_CASE)
-        BEPU_JOINT_TYPES_MORE(BEPU_CASE)
-#undef BEPU_CASE
-        default: break;
+    case ID: run_lane<T, STAGE, kSharded, kExt>(refs, p, a, p_rw, enc0, enc1, B, fp, early, peers, peer_delta); break;
+    if constexpr (kContacts) {
+        switch (rec.type_id) {
+            BEPU_CONTACT_TYPES(BEPU_CASE)
+            default: break;
+        }
+    } else {
+        switch (rec.type_id) {
+            BEPU_CONTACT_TYPES(BEPU_CASE)
+            BEPU_JOINT_TYPES(BEPU_CASE)
+            BEPU_JOINT_TYPES_MORE(BEPU_CASE)
+            default: break;
+        }
     }
-}
-template <int STAGE, class PR, class AR>
-BEPU_DI void run_bundle_rows(const WorkRecord& rec, int lane, PR p, AR a, uint32_t enc0, uint32_t enc1, const BodyBuffers& B, const FrameParams& fp) {
-    run_bundle_rows<STAGE, false, false>(rec, lane, p, a, enc0, enc1, B, fp);
+#undef BEPU_CASE
 }
 // Rows straight from HBM (the incremental stage).
 template <int STAGE>
 BEPU_DI void run_bundle(const WorkRecord& rec, int lane, uint32_t enc0, uint32_t enc1, const BodyBuffers& B, const FrameParams& fp) {
-    run_bundle_rows<STAGE>(rec, lane, GlobalRows{rec.prestep + lane}, GlobalAcc{rec.impulses + lane}, enc0, enc1, B, fp);
+    run_bundle_rows<STAGE, false, false, false>(rec, lane, GlobalRows{rec.prestep + lane}, GlobalAcc{rec.impulses + lane}, enc0, enc1, B, fp, EarlyBodies{});
 }
 // The reference arena is padded, so reading a second body-reference row is always in bounds (one-body types ignore it).
 template <int STAGE> BEPU_DI void run_bundle(const WorkRecord& rec, int lane, const BodyBuffers& B, const FrameParams& fp) {
@@ -304,11 +325,12 @@ template <int STAGE> BEPU_DI void run_bundle(const WorkRecord& rec, int lane, co
 }
 
 // ---- bulk staging of one bundle's prestep + accumulated impulse block into shared memory (cp.async.bulk + mbarrier) ----------------
-// Block sizes per type id (rows of 128 B); 0 for ids without a type.
-struct StageRowCounts { uint8_t prestep[64], impulses[64]; };
+// Block sizes per type id (rows of 128 B), and the body slots and pose use the pre-wait body loads need; 0 for ids without a type.
+struct StageRowCounts { uint8_t prestep[64], impulses[64], bodies[64], needs_pose[64]; };
 __host__ __device__ constexpr StageRowCounts make_stage_row_counts() {
     StageRowCounts c{};
-#define BEPU_ROWS(ID, T) c.prestep[ID] = (uint8_t)T::kPrestepRows; c.impulses[ID] = (uint8_t)T::kImpulseRows;
+#define BEPU_ROWS(ID, T) \
+    c.prestep[ID] = (uint8_t)T::kPrestepRows; c.impulses[ID] = (uint8_t)T::kImpulseRows; c.bodies[ID] = (uint8_t)T::kBodies; c.needs_pose[ID] = T::kNeedsPose ? 1 : 0;
     BEPU_CONTACT_TYPES(BEPU_ROWS)
     BEPU_JOINT_TYPES(BEPU_ROWS)
     BEPU_JOINT_TYPES_MORE(BEPU_ROWS)
@@ -354,7 +376,34 @@ constexpr int kStageBlockThreads = BEPU_STAGE_BLOCK_THREADS;
 // body references (immutable during a solve) always, and -- when the host says so (kStagePrefetchRows: the predecessor is neither the incremental
 // contact update, which rewrites depth rows, nor a stage of this same batch, which rewrites these impulses) -- the whole row block. That takes the
 // bulk copy's latency off the critical path; after the wait only the body gather, the math and the scatter remain.
-constexpr int kStagePrefetchRows = 1;
+//
+// The body records of slots 0 and 1 that the immediate predecessor cannot write are loaded in the prologue too (plain kernels, kStagePrefetchBodies:
+// the predecessor is a stage of this solve and not the WarmStart of this same batch), so that the post-wait gather is the velocities alone:
+//   - WarmStart, integrating slot: local inertia (never written during a solve) and pose (written only by this batch's own WarmStart, a substep ago);
+//   - Solve: world inertia (and pose for kNeedsPose types), written only by the WarmStart stages of batches up to this one.
+// Sharded kernels load every body record after the wait: a peer's stores are only known to have arrived after shard_wait.
+constexpr int kStagePrefetchRows = 1, kStagePrefetchBodies = 2;
+template <int STAGE, bool kContacts>
+BEPU_DI void load_early_bodies(int type_id, uint32_t enc0, uint32_t enc1, const BodyBuffers& B, EarlyBodies& e) {
+    if ((int32_t)enc0 == kRefEmpty) return;
+    const int bodies = kStageRowCounts.bodies[type_id];
+    const bool pose = !kContacts && kStageRowCounts.needs_pose[type_id];
+#pragma unroll
+    for (int s = 0; s < 2; ++s) {
+        const uint32_t enc = s == 0 ? enc0 : enc1;
+        const uint32_t idx = enc & kRefIndexMask;
+        if (s >= bodies) break;
+        if (STAGE == kStageSolve) {
+            load_inertia(B.inertia_world, idx, e.inertia[s]);
+            if (pose) load_pose(B.pose, idx, e.pos[s], e.q[s]);
+            e.slots |= 1u << s;
+        } else if (enc & kRefIntegrateBit) {
+            load_inertia(B.inertia_local, idx, e.inertia[s]);
+            load_pose(B.pose, idx, e.pos[s], e.q[s]);
+            e.slots |= 1u << s;
+        }
+    }
+}
 // Arrival counting of the sharded stages (ShardStage). Lanes 0..rank_count-1 of a boundary warp each talk to one peer.
 BEPU_DI void shard_announce(const ShardPeers& peers, int lane) {
     if (lane < peers.rank_count && lane != peers.rank)
@@ -374,7 +423,7 @@ BEPU_DI void shard_wait(const ShardPeers& peers, int lane, uint32_t solve_index,
     }
     __syncwarp();
 }
-template <int STAGE, bool kSharded, bool kExt>
+template <int STAGE, bool kSharded, bool kExt, bool kContacts, bool kEarlyBodies>
 BEPU_DI void constraint_stage_body(const WorkRecord* __restrict__ records, const int32_t* __restrict__ ref_rows, int work_count, const BodyBuffers& B, const FrameParams* __restrict__ fpp, int flags, const ShardPeers* peers,
                                    long long peer_delta, const ShardStage* shard = nullptr) {
     constexpr bool kStaged = STAGE != kStageIncremental;
@@ -392,6 +441,7 @@ BEPU_DI void constraint_stage_body(const WorkRecord* __restrict__ records, const
     const uint32_t bar = smem_u32(&bars[warp_in_block]);
     const bool early_rows = kStaged && (flags & kStagePrefetchRows);
     uint32_t prestep_bytes = 0, impulse_bytes = 0;
+    EarlyBodies early{};
     if (active) {
         rec = load_record(records + warp);
         if constexpr (kStaged) {
@@ -410,6 +460,9 @@ BEPU_DI void constraint_stage_body(const WorkRecord* __restrict__ records, const
         // the first two reference rows come from the packed copy next to the work list: their address does not depend on the record (no second round trip)
         enc0 = ldg_nc_u32(ref_rows + (size_t)warp * (2 * kLanes) + lane);
         enc1 = ldg_nc_u32(ref_rows + (size_t)warp * (2 * kLanes) + kLanes + lane);
+        if constexpr (kStaged && kEarlyBodies) {
+            if (flags & kStagePrefetchBodies) load_early_bodies<STAGE, kContacts>(rec.type_id, enc0, enc1, B, early);
+        }
     }
     const FrameParams fp = *fpp;
     asm volatile("griddepcontrol.wait;" ::: "memory");
@@ -429,8 +482,8 @@ BEPU_DI void constraint_stage_body(const WorkRecord* __restrict__ records, const
             bulk_copy_g2s(slab_addr + prestep_bytes, rec.impulses, impulse_bytes, bar, policy);
         }
         __syncwarp();
-        run_bundle_rows<STAGE, kSharded, kExt>(rec, lane, StagedRows{slab_addr + lane * 4, bar, 0u}, StagedAcc{slab_addr + prestep_bytes + lane * 4, rec.impulses + lane}, enc0, enc1, B, fp,
-                                         peers, boundary ? peer_delta : 0);
+        run_bundle_rows<STAGE, kSharded, kExt, kContacts>(rec, lane, StagedRows{slab_addr + lane * 4, bar, 0u}, StagedAcc{slab_addr + prestep_bytes + lane * 4, rec.impulses + lane}, enc0,
+                                                          enc1, B, fp, early, peers, boundary ? peer_delta : 0);
         if constexpr (kSharded) {
             if (boundary) {
                 __syncwarp();                  // every lane's peer stores are ordered before ...
@@ -442,16 +495,18 @@ BEPU_DI void constraint_stage_body(const WorkRecord* __restrict__ records, const
     }
 }
 
-template <int STAGE, int MINB, bool kExt>
+// The pre-wait body loads are compiled into the uncapped and the contact-only budgets. The deep budget (full switch at 80 registers) would spill
+// with them, and a batch several waves deep has only its first wave's CTAs in a prologue while the predecessor runs.
+template <int STAGE, int MINB, bool kExt, bool kContacts>
 __global__ void __launch_bounds__(kStageBlockThreads, MINB) constraint_stage_kernel(const WorkRecord* __restrict__ records, const int32_t* __restrict__ ref_rows, int work_count, BodyBuffers B, const FrameParams* __restrict__ fpp, int flags) {
-    constraint_stage_body<STAGE, false, kExt>(records, ref_rows, work_count, B, fpp, flags, nullptr, 0);
+    constraint_stage_body<STAGE, false, kExt, kContacts, MINB == 1 || kContacts>(records, ref_rows, work_count, B, fpp, flags, nullptr, 0);
 }
 // Peer-sharded variant (bepucuda_shard_*): the lane that writes a body another rank references stores the record into that rank's arrays too.
 template <int STAGE, int MINB, bool kExt>
 __global__ void __launch_bounds__(kStageBlockThreads, MINB)
 constraint_stage_kernel_sharded(const WorkRecord* __restrict__ records, const int32_t* __restrict__ ref_rows, int work_count, BodyBuffers B, const FrameParams* __restrict__ fpp, int flags, const __grid_constant__ ShardPeers peers,
                                 long long peer_delta, const __grid_constant__ ShardStage shard) {
-    constraint_stage_body<STAGE, true, kExt>(records, ref_rows, work_count, B, fpp, flags, &peers, peer_delta, &shard);
+    constraint_stage_body<STAGE, true, kExt, false, false>(records, ref_rows, work_count, B, fpp, flags, &peers, peer_delta, &shard);
 }
 
 #if BEPU_UNIT == 3  // the per-body passes are launched from unit 3 only

@@ -65,6 +65,11 @@ const TypeInfo* get_type_info(int type_id) {
     if (type_id < 0 || type_id >= 64 || !registry().present[type_id]) return nullptr;
     return &registry().types[type_id];
 }
+// The contact types (BEPU_CONTACT_TYPES of bepu_solver_kernels.cuh) are exactly the types with an incremental contact update.
+static bool is_contact_type(int type_id) {
+    const TypeInfo* t = get_type_info(type_id);
+    return t && t->incremental != 0;
+}
 
 // ---- small RAII helpers ------------------------------------------------------------------------------------------------------
 struct DeviceBuffer {
@@ -140,6 +145,7 @@ struct StageOp {
     int32_t work_begin;   // into the work item array (constraint stages) / unused
     int32_t work_count;   // warps of work (constraint stages), bodies (final pose), kinematics (kinematic stages)
     int32_t exchange;     // peer sharding: kRankBarrier, the device batch of a sharded WarmStart / Solve stage, or kNoExchange
+    int32_t contacts_only;  // WarmStart / Solve: every bundle of the batch is a contact (kLaunchContactsOnly)
 };
 // Rank barriers and sharded stages are the exchange points of a solve, numbered in program order (FrameParams::exchange_base, ShardStage).
 constexpr int32_t kNoExchange = -1, kRankBarrier = -2;
@@ -189,6 +195,7 @@ struct bepucuda_ctx {
     std::vector<int32_t> bundle_live;           // live constraints per work item (parallel to `work`)
     std::vector<WorkRecord> records;            // what the solver kernels read (parallel to `work`)
     std::vector<std::pair<int, int>> batch_work; // per device batch: (begin, count) into work
+    std::vector<int32_t> batch_contacts_only;    // per device batch: every work record is a contact type
     // peer sharding (bepucuda_shard_*): one constraint graph over several GPUs with NVLink peer stores from the stage kernels
     bool peer_mode = false;
     ShardPeers peers{};
@@ -329,6 +336,12 @@ bool rows_prefetchable(const StageOp* previous, const StageOp& op) {
     return op.stage != kStageIncremental && previous != nullptr && previous->stage != kStageIncremental &&
            !(previous->stage <= kStageSolve && previous->work_begin == op.work_begin);
 }
+// Body-record loads in the PDL prologue (see constraint_stage_body): allowed for a WarmStart / Solve stage when the stage launched immediately before
+// it belongs to this solve (what ran before the solve, such as a body upload, has no stage to order against) and is not the WarmStart of the same
+// batch, the only stage that writes the records these loads read: world inertia and pose of this batch's bodies, the pose of an integrating one.
+bool bodies_prefetchable(const StageOp* previous, const StageOp& op) {
+    return op.stage <= kStageSolve && previous != nullptr && !(previous->stage <= kStageWarmStart && previous->work_begin == op.work_begin);
+}
 
 // Profiling sink of issue_stage_sequence: the launch of program op i sets launched[i] and is bracketed by events[2i] and events[2i + 1].
 struct StageEvents {
@@ -365,7 +378,8 @@ void issue_stage_sequence(bepucuda_ctx* ctx, cudaStream_t s, int64_t* launches, 
                 // a sharded stage stores the records it writes for shared bodies into the ranks that reference them, and its boundary bundles wait
                 // for and announce arrivals themselves (ShardStage)
                 shard.stage.exchange_index = exchange_index;
-                const int flags = (profile ? 0 : kLaunchPdl | (rows_prefetchable(previous, op) ? kLaunchPrefetchRows : 0)) | extensions;
+                const int prefetch = (rows_prefetchable(previous, op) ? kLaunchPrefetchRows : 0) | (bodies_prefetchable(previous, op) ? kLaunchPrefetchBodies : 0);
+                const int flags = (profile ? 0 : kLaunchPdl | prefetch) | extensions | (op.contacts_only ? kLaunchContactsOnly : 0);
                 ctx->launchers->constraint_stage(op.stage, records + op.work_begin, ref_rows + (size_t)op.work_begin * 64, op.work_count, ctx->B, fp, flags,
                                                  op.exchange == kNoExchange ? nullptr : &shard, s);
             } else if (op.stage <= kStageKinematic) {
@@ -404,12 +418,14 @@ void build_program(bepucuda_ctx* ctx) {
         // in peer mode every rank runs the exchange point of every batch, also of one it has no constraint in
         for (size_t b = 0; b < ctx->batch_work.size(); ++b) {
             auto& bw = ctx->batch_work[b];
-            if (bw.second > 0 || (ctx->peer_mode && (int)b < ctx->sync_batch_count)) ctx->program.push_back({s == 0 ? kStageWarmStartFirst : kStageWarmStart, bw.first, bw.second, ctx->peer_mode ? (int)b : kNoExchange});
+            if (bw.second > 0 || (ctx->peer_mode && (int)b < ctx->sync_batch_count))
+                ctx->program.push_back({s == 0 ? kStageWarmStartFirst : kStageWarmStart, bw.first, bw.second, ctx->peer_mode ? (int)b : kNoExchange, ctx->batch_contacts_only[b]});
         }
         for (int it = 0; it < ctx->iterations[s]; ++it)
             for (size_t b = 0; b < ctx->batch_work.size(); ++b) {
                 auto& bw = ctx->batch_work[b];
-                if (bw.second > 0 || (ctx->peer_mode && (int)b < ctx->sync_batch_count)) ctx->program.push_back({kStageSolve, bw.first, bw.second, ctx->peer_mode ? (int)b : kNoExchange});
+                if (bw.second > 0 || (ctx->peer_mode && (int)b < ctx->sync_batch_count))
+                    ctx->program.push_back({kStageSolve, bw.first, bw.second, ctx->peer_mode ? (int)b : kNoExchange, ctx->batch_contacts_only[b]});
             }
     }
     if (ctx->peer_mode) ctx->program.push_back(rank_barrier);  // ... and before the final pose pass reads them
@@ -991,6 +1007,7 @@ int32_t bepucuda_end_constraints(bepucuda_ctx* ctx) {
     ctx->work.clear();
     ctx->bundle_live.clear();
     ctx->batch_work.clear();
+    ctx->batch_contacts_only.clear();
     auto live_in_bundle = [&](int tb, int k) {
         // identity-mapped type batches: lanes beyond the source count are padding; mapped (fallback level) ones: -1 entries are padding
         if (map_offset[tb] == SIZE_MAX) return std::max(0, std::min(32, ctx->tdescs[tb].src_count - k * 32));
@@ -1000,9 +1017,13 @@ int32_t bepucuda_end_constraints(bepucuda_ctx* ctx) {
     };
     for (auto& list : batch_tbs) {
         const int begin = (int)ctx->work.size();
-        for (int tb : list)
+        bool contacts_only = true;
+        for (int tb : list) {
+            contacts_only = contacts_only && is_contact_type(ctx->tbs[tb].type_id);
             for (int k = 0; k < ctx->tbs[tb].bundle_count; ++k) { ctx->work.push_back({tb, k}); ctx->bundle_live.push_back(live_in_bundle(tb, k)); }
+        }
         ctx->batch_work.push_back({begin, (int)ctx->work.size() - begin});
+        ctx->batch_contacts_only.push_back(contacts_only ? 1 : 0);
     }
     ctx->all_work_count = (int)ctx->work.size();
     ctx->inc_work_begin = (int)ctx->work.size();
