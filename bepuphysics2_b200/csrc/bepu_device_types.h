@@ -126,11 +126,4 @@ constexpr int kShardMaxExchanges = 4096;
 constexpr size_t kShardFlagBlockWords = kShardTargetSlot + (size_t)kMaxShardRanks * kShardMaxExchanges;
 constexpr int32_t kRecordBoundaryBit = 1 << 30;
 
-struct TypeInfo {
-    int32_t bodies, prestep_rows, impulse_rows, incremental;
-    int32_t solve_bytes, warm_start_bytes, incremental_bytes;  // SURVEY.md §8d algorithmic bytes per evaluation
-    const char* name;
-};
-const TypeInfo* get_type_info(int type_id);  // nullptr if unsupported
-
 }  // namespace bepucuda

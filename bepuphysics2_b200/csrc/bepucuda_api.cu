@@ -1,4 +1,4 @@
-// libbepucuda host side: context, device memory, uploads/downloads, topology analysis, stage program, CUDA graph.
+// libbepucuda host side: context, device memory, uploads/downloads, device tables of the topology plan (bepu_topology.h), stage launches, CUDA graph.
 // C ABI declared in include/bepucuda.h. No CPU fallback lives here: without a usable CUDA device bepucuda_create fails.
 #include <algorithm>
 #include <cmath>
@@ -10,66 +10,11 @@
 #include "bepu_layout_kernels.h"
 #include "bepu_coloring.h"
 #include "bepu_bounds.h"
+#include "bepu_topology.h"
 
 using namespace bepucuda;
 
 namespace bepucuda {
-
-// ---- type registry -------------------------------------------------------------------------------------------------------
-// bodies / prestep floats / impulse floats per BatchTypeId, and SURVEY.md §8d algorithmic bytes:
-//   solve       = 4 * (P + 2D + n + sum(R_i + W_i))        R/W from the type's Solve access filters
-//   warm start  = 4 * (P + D + n + sum(R'_i + W'_i))       (non-integrating lane, WarmStart filters)
-//   incremental = 4 * (P_read + contacts_written + n + 6n)
-// Filters (IBodyAccessFilter.cs:L38-126): pos 3, orientation 4, lin 3, ang 3, inertia tensor 6, mass 1.
-static TypeInfo make_contact(int bodies, int prestep, int impulses, int contacts, const char* name) {
-    TypeInfo t{};
-    t.bodies = bodies; t.prestep_rows = prestep; t.impulse_rows = impulses; t.incremental = 1; t.name = name;
-    const int body_rw = 13 + 6;  // AccessNoPose: velocity 6 + inertia 7 read, velocity 6 written
-    t.solve_bytes = 4 * (prestep + 2 * impulses + bodies + bodies * body_rw);
-    t.warm_start_bytes = 4 * (prestep + impulses + bodies + bodies * body_rw);
-    t.incremental_bytes = 4 * (prestep + contacts + bodies + 6 * bodies);
-    return t;
-}
-static TypeInfo make_joint(int bodies, int prestep, int impulses, int solve_r, int solve_w, int ws_r, int ws_w, const char* name) {
-    TypeInfo t{};
-    t.bodies = bodies; t.prestep_rows = prestep; t.impulse_rows = impulses; t.incremental = 0; t.name = name;
-    t.solve_bytes = 4 * (prestep + 2 * impulses + bodies + solve_r + solve_w);
-    t.warm_start_bytes = 4 * (prestep + impulses + bodies + ws_r + ws_w);
-    t.incremental_bytes = 0;
-    return t;
-}
-struct Registry {
-    TypeInfo types[64];
-    bool present[64];
-    Registry() {
-        std::memset(present, 0, sizeof(present));
-        auto add = [&](int id, TypeInfo t) { types[id] = t; present[id] = true; };
-        add(0, make_contact(1, 11, 4, 1, "Contact1OneBody")); add(1, make_contact(1, 15, 5, 2, "Contact2OneBody"));
-        add(2, make_contact(1, 19, 6, 3, "Contact3OneBody")); add(3, make_contact(1, 23, 7, 4, "Contact4OneBody"));
-        add(4, make_contact(2, 14, 4, 1, "Contact1")); add(5, make_contact(2, 18, 5, 2, "Contact2"));
-        add(6, make_contact(2, 22, 6, 3, "Contact3")); add(7, make_contact(2, 26, 7, 4, "Contact4"));
-        add(8, make_contact(1, 18, 6, 2, "Contact2NonconvexOneBody")); add(9, make_contact(1, 25, 9, 3, "Contact3NonconvexOneBody"));
-        add(10, make_contact(1, 32, 12, 4, "Contact4NonconvexOneBody"));
-        add(15, make_contact(2, 21, 6, 2, "Contact2Nonconvex")); add(16, make_contact(2, 28, 9, 3, "Contact3Nonconvex"));
-        add(17, make_contact(2, 35, 12, 4, "Contact4Nonconvex"));
-#define BEPU_REGISTER_JOINTS
-#include "bepu_joint_registry.inc"
-#undef BEPU_REGISTER_JOINTS
-    }
-};
-static const Registry& registry() {
-    static Registry r;
-    return r;
-}
-const TypeInfo* get_type_info(int type_id) {
-    if (type_id < 0 || type_id >= 64 || !registry().present[type_id]) return nullptr;
-    return &registry().types[type_id];
-}
-// The contact types (BEPU_CONTACT_TYPES of bepu_solver_kernels.cuh) are exactly the types with an incremental contact update.
-static bool is_contact_type(int type_id) {
-    const TypeInfo* t = get_type_info(type_id);
-    return t && t->incremental != 0;
-}
 
 // ---- small RAII helpers ------------------------------------------------------------------------------------------------------
 struct DeviceBuffer {
@@ -124,31 +69,18 @@ struct ChunkArena {
 
 struct SourceTypeBatch {
     int batch_index, type_batch_index, type_id, count;
-    int live = 0;          // constraints actually present (fallback type batches may contain holes)
     float* host_impulses;
     int32_t* raw_refs;     // device, reference AOSOA-W layout
     float* raw_prestep;
     float* raw_impulses;
     size_t refs_bytes, prestep_bytes, impulse_bytes;
     std::vector<int32_t> host_refs;  // retained only for fallback batches (levelisation)
-    std::vector<int> device_tbs;
     // device-side contact update (bepucuda_update_contacts): feature ids of the resident impulses / of the frame being uploaded
     int32_t* raw_features_old = nullptr;
     int32_t* raw_features_new = nullptr;
     size_t feature_bytes = 0;
     bool resident_impulses = false, redistribute = false;
 };
-
-// Stage program entry (built by build_program, walked by the host when it issues or captures a frame).
-struct StageOp {
-    int32_t stage;
-    int32_t work_begin;   // into the work item array (constraint stages) / unused
-    int32_t work_count;   // warps of work (constraint stages), bodies (final pose), kinematics (kinematic stages)
-    int32_t exchange;     // peer sharding: kRankBarrier, the device batch of a sharded WarmStart / Solve stage, or kNoExchange
-    int32_t contacts_only;  // WarmStart / Solve: every bundle of the batch is a contact (kLaunchContactsOnly)
-};
-// Rank barriers and sharded stages are the exchange points of a solve, numbered in program order (FrameParams::exchange_base, ShardStage).
-constexpr int32_t kNoExchange = -1, kRankBarrier = -2;
 
 }  // namespace bepucuda
 
@@ -189,13 +121,9 @@ struct bepucuda_ctx {
     std::vector<SourceTypeBatch> sources;
     ChunkArena raw_arena, pinned_arena;
     DeviceBuffer record_table, ref_rows, source_bundle_flags, refs32, prestep32, impulses32, tb_table, tdesc_table, work_table, map_table, bodies_per_type, kinematics_dev, frame_params_dev, error_dev;
-    std::vector<DeviceTypeBatch> tbs;
-    std::vector<TransposeDesc> tdescs;
-    std::vector<WorkItem> work;                 // grouped by device batch, then the incremental list
-    std::vector<int32_t> bundle_live;           // live constraints per work item (parallel to `work`)
-    std::vector<WorkRecord> records;            // what the solver kernels read (parallel to `work`)
-    std::vector<std::pair<int, int>> batch_work; // per device batch: (begin, count) into work
-    std::vector<int32_t> batch_contacts_only;    // per device batch: every work record is a contact type
+    TopologyPlan topo;                          // device batches and work list of the last successful end_constraints
+    std::vector<TransposeDesc> tdescs;          // per planned type batch
+    std::vector<WorkRecord> records;            // what the solver kernels read (parallel to topo.work)
     // peer sharding (bepucuda_shard_*): one constraint graph over several GPUs with NVLink peer stores from the stage kernels
     bool peer_mode = false;
     ShardPeers peers{};
@@ -203,17 +131,12 @@ struct bepucuda_ctx {
     uint32_t shard_solve_index = 0;                                 // solves since the arrival targets were last published
     std::vector<int> boundary_count;                                // per device batch: bundles that touch a body another rank references
     std::vector<uint8_t> body_masks;                                // bepucuda_shard_set_body_masks: per body, the ranks that reference it
-    size_t refs_words = 0;
     std::vector<void*> opened_ipc;
     std::vector<int32_t> global_first_batch;
     std::vector<uint8_t> global_constrained;
     uint32_t exchange_counter = 0;                                  // exchange points executed so far (flag barrier sequence)
-    uint32_t exchanges_per_solve = 0;                               // exchange points of the stage program (upload_program)
-    int inc_work_begin = 0, inc_work_count = 0;
-    int all_work_count = 0;                     // work[0 .. all_work_count) covers every bundle once
-    int sync_batch_count = 0, fallback_levels = 0;
     std::vector<int32_t> kinematics;
-    std::vector<StageOp> program;
+    StageProgram program;
     FrameParams* frame_params_host = nullptr;   // pinned
 
     cudaGraph_t graph = nullptr;
@@ -329,20 +252,6 @@ void invalidate_graph(bepucuda_ctx* ctx) {
 // off changes the launch sequence (a captured graph is rebuilt); their values are frame parameters.
 bool integrator_extensions(const bepucuda_ctx* ctx) { return ctx->accelerations_count >= 0 || ctx->point_gravity; }
 
-// Row prefetch in the PDL prologue (see constraint_stage_kernel): allowed when the stage launched immediately before `op` neither rewrites op's
-// prestep rows (the incremental contact update does) nor its impulses (a stage of the same batch does: single-batch scenes). A rank barrier in
-// between writes no rows, so `previous` skips rank barriers.
-bool rows_prefetchable(const StageOp* previous, const StageOp& op) {
-    return op.stage != kStageIncremental && previous != nullptr && previous->stage != kStageIncremental &&
-           !(previous->stage <= kStageSolve && previous->work_begin == op.work_begin);
-}
-// Body-record loads in the PDL prologue (see constraint_stage_body): allowed for a WarmStart / Solve stage when the stage launched immediately before
-// it belongs to this solve (what ran before the solve, such as a body upload, has no stage to order against) and is not the WarmStart of the same
-// batch, the only stage that writes the records these loads read: world inertia and pose of this batch's bodies, the pose of an integrating one.
-bool bodies_prefetchable(const StageOp* previous, const StageOp& op) {
-    return op.stage <= kStageSolve && previous != nullptr && !(previous->stage <= kStageWarmStart && previous->work_begin == op.work_begin);
-}
-
 // Profiling sink of issue_stage_sequence: the launch of program op i sets launched[i] and is bracketed by events[2i] and events[2i + 1].
 struct StageEvents {
     const std::vector<cudaEvent_t>& events;
@@ -350,8 +259,8 @@ struct StageEvents {
 };
 
 // Issues the whole stage sequence of one frame as individual launches on `s` (used directly in STREAM mode and under capture in GRAPH mode).
-// Order: Solver_Solve.cs:L1419-1479, then PoseIntegrator.IntegrateAfterSubstepping. With `profile`, stages are launched without programmatic
-// dependent launch and without row prefetch, so that each event pair times one kernel alone.
+// With `profile`, stages are launched without programmatic dependent launch and without prologue prefetch, so that each event pair times one
+// kernel alone.
 void issue_stage_sequence(bepucuda_ctx* ctx, cudaStream_t s, int64_t* launches, const StageEvents* profile = nullptr) {
     const WorkRecord* records = ctx->record_table.as<WorkRecord>();
     const int32_t* ref_rows = ctx->ref_rows.as<int32_t>();
@@ -359,11 +268,9 @@ void issue_stage_sequence(bepucuda_ctx* ctx, cudaStream_t s, int64_t* launches, 
     const int32_t* kin = ctx->kinematics_dev.as<int32_t>();
     ShardLaunch shard{ctx->peers, (long long)(ctx->peer32.as<int32_t>() - ctx->refs32.as<int32_t>()), {0, ctx->error_dev.as<int32_t>()}};
     int64_t n = 0;
-    const StageOp* previous = nullptr;  // last launched stage
-    uint32_t exchange_index = 0;
     const int extensions = integrator_extensions(ctx) ? kLaunchIntegratorExtensions : 0;
-    for (size_t i = 0; i < ctx->program.size(); ++i) {
-        const StageOp& op = ctx->program[i];
+    for (size_t i = 0; i < ctx->program.ops.size(); ++i) {
+        const StageOp& op = ctx->program.ops[i];
         const bool barrier = op.exchange == kRankBarrier;
         // A sharded stage without constraints on this rank launches nothing but still counts as an exchange point: nothing arrives from this
         // rank there, and its arrival targets say so.
@@ -371,15 +278,13 @@ void issue_stage_sequence(bepucuda_ctx* ctx, cudaStream_t s, int64_t* launches, 
             if (profile) cudaEventRecord(profile->events[2 * i], s);
             if (barrier) {
                 // all ranks meet: before the first stage of a solve; around the incremental contact update, which reads the velocities of shared
-                // bodies -- after every peer's last Solve stage has completed, before any peer's WarmStart stage stores into this rank's arrays; and
-                // before the final pose pass
-                launch_shard_barrier(ctx->peers, fp, exchange_index, ctx->error_dev.as<int32_t>(), s);
+                // bodies; and before the final pose pass
+                launch_shard_barrier(ctx->peers, fp, op.exchange_index, ctx->error_dev.as<int32_t>(), s);
             } else if (op.stage <= kStageIncremental) {
                 // a sharded stage stores the records it writes for shared bodies into the ranks that reference them, and its boundary bundles wait
                 // for and announce arrivals themselves (ShardStage)
-                shard.stage.exchange_index = exchange_index;
-                const int prefetch = (rows_prefetchable(previous, op) ? kLaunchPrefetchRows : 0) | (bodies_prefetchable(previous, op) ? kLaunchPrefetchBodies : 0);
-                const int flags = (profile ? 0 : kLaunchPdl | prefetch) | extensions | (op.contacts_only ? kLaunchContactsOnly : 0);
+                shard.stage.exchange_index = op.exchange_index;
+                const int flags = (profile ? op.launch_flags & kLaunchContactsOnly : kLaunchPdl | op.launch_flags) | extensions;
                 ctx->launchers->constraint_stage(op.stage, records + op.work_begin, ref_rows + (size_t)op.work_begin * 64, op.work_count, ctx->B, fp, flags,
                                                  op.exchange == kNoExchange ? nullptr : &shard, s);
             } else if (op.stage <= kStageKinematic) {
@@ -391,63 +296,22 @@ void issue_stage_sequence(bepucuda_ctx* ctx, cudaStream_t s, int64_t* launches, 
                 cudaEventRecord(profile->events[2 * i + 1], s);
                 profile->launched[i] = 1;
             }
-            if (!barrier) previous = &op;
             ++n;
         }
-        if (op.exchange != kNoExchange) ++exchange_index;
     }
     if (launches) *launches = n;
 }
 
-// Builds the flat stage program for the current topology + solve description.
-void build_program(bepucuda_ctx* ctx) {
-    ctx->program.clear();
-    const int substeps = (int)ctx->iterations.size();
-    const int kin = (int)ctx->kinematics.size();
-    const StageOp rank_barrier{kStageKinematic, 0, 0, kRankBarrier};
-    for (int s = 0; s < substeps; ++s) {
-        if (s > 0) {
-            // peer sharding: what peers pushed in the last Solve stages must have arrived before the contact update reads velocities
-            if (ctx->peer_mode) ctx->program.push_back(rank_barrier);
-            if (ctx->inc_work_count > 0) ctx->program.push_back({kStageIncremental, ctx->inc_work_begin, ctx->inc_work_count, kNoExchange});
-            if (kin > 0) ctx->program.push_back({kStageKinematic, 0, kin, kNoExchange});
-        } else if (ctx->integ.integrate_velocity_for_kinematics && kin > 0) {
-            ctx->program.push_back({kStageKinematicFirst, 0, kin, kNoExchange});
-        }
-        if (ctx->peer_mode) ctx->program.push_back(rank_barrier);  // see issue_stage_sequence
-        // in peer mode every rank runs the exchange point of every batch, also of one it has no constraint in
-        for (size_t b = 0; b < ctx->batch_work.size(); ++b) {
-            auto& bw = ctx->batch_work[b];
-            if (bw.second > 0 || (ctx->peer_mode && (int)b < ctx->sync_batch_count))
-                ctx->program.push_back({s == 0 ? kStageWarmStartFirst : kStageWarmStart, bw.first, bw.second, ctx->peer_mode ? (int)b : kNoExchange, ctx->batch_contacts_only[b]});
-        }
-        for (int it = 0; it < ctx->iterations[s]; ++it)
-            for (size_t b = 0; b < ctx->batch_work.size(); ++b) {
-                auto& bw = ctx->batch_work[b];
-                if (bw.second > 0 || (ctx->peer_mode && (int)b < ctx->sync_batch_count))
-                    ctx->program.push_back({kStageSolve, bw.first, bw.second, ctx->peer_mode ? (int)b : kNoExchange, ctx->batch_contacts_only[b]});
-            }
-    }
-    if (ctx->peer_mode) ctx->program.push_back(rank_barrier);  // ... and before the final pose pass reads them
-    ctx->program.push_back({kStageFinalPose, 0, ctx->body_count, kNoExchange});
-}
-
 int upload_program(bepucuda_ctx* ctx) {
-    build_program(ctx);
+    ctx->program = build_stage_program(ctx->topo, ctx->iterations, (int)ctx->kinematics.size(), ctx->integ.integrate_velocity_for_kinematics != 0, ctx->peer_mode,
+                                       ctx->body_count);
     if (ctx->peer_mode) {
         // publish, to every peer, how many boundary bundles of this rank arrive through each exchange point of one solve (ShardStage), and restart
         // the arrival counters other ranks increment here. Every rank does this for the same program, between solves.
-        std::vector<unsigned long long> targets((size_t)kShardMaxExchanges, 0ull);
-        unsigned long long arrived = 0;
-        size_t e = 0;
-        for (const StageOp& op : ctx->program) {
-            if (op.exchange == kNoExchange) continue;
-            if (e + 1 >= (size_t)kShardMaxExchanges) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, "peer sharding: more than 4095 exchange points per solve");
-            if (op.exchange >= 0 && op.work_count > 0) arrived += (unsigned long long)ctx->boundary_count[(size_t)op.exchange];
-            targets[e++] = arrived;
-        }
-        targets[(size_t)kShardMaxExchanges - 1] = arrived;
-        ctx->exchanges_per_solve = (uint32_t)e;
+        std::vector<unsigned long long> targets;
+        std::string error;
+        const int rc = exchange_targets(ctx->program, ctx->boundary_count, &targets, &error);
+        if (rc != BEPUCUDA_OK) return fail(ctx, rc, error);
         CK(cudaStreamSynchronize(ctx->stream));
         for (int q = 0; q < ctx->peers.rank_count; ++q)
             if (q != ctx->peers.rank)
@@ -458,10 +322,7 @@ int upload_program(bepucuda_ctx* ctx) {
     // work issued under the previous program completes before that program and its graph are replaced
     CK(cudaStreamSynchronize(ctx->stream));
     invalidate_graph(ctx);
-    // stage statistics
-    int64_t stages = 0;
-    for (auto& op : ctx->program) stages += (op.work_count > 0 || op.stage == kStageFinalPose) ? 1 : 0;
-    ctx->timings.stage_count = stages;
+    ctx->timings.stage_count = ctx->program.stage_count;
     return BEPUCUDA_OK;
 }
 
@@ -512,20 +373,20 @@ int refresh_device_rows(bepucuda_ctx* ctx) {
     { int rc = flush_chunks(ctx, ctx->pending_h2d); if (rc != BEPUCUDA_OK) return rc; }
     bool any_redistribute = false;
     if (ctx->descs_dirty) {
-        for (SourceTypeBatch& s : ctx->sources)
-            for (int tb : s.device_tbs) {
-                TransposeDesc& d = ctx->tdescs[tb];
-                d.flags = (s.resident_impulses ? kDescResidentImpulses : 0) | (s.redistribute ? kDescRedistribute : 0);
-                d.features_old = s.raw_features_old;
-                d.features_new = s.raw_features_new;
-                any_redistribute |= s.redistribute;
-            }
+        for (size_t tb = 0; tb < ctx->topo.tbs.size(); ++tb) {
+            const SourceTypeBatch& s = ctx->sources[(size_t)ctx->topo.tbs[tb].source];
+            TransposeDesc& d = ctx->tdescs[tb];
+            d.flags = (s.resident_impulses ? kDescResidentImpulses : 0) | (s.redistribute ? kDescRedistribute : 0);
+            d.features_old = s.raw_features_old;
+            d.features_new = s.raw_features_new;
+            any_redistribute |= s.redistribute;
+        }
         CK(cudaMemcpyAsync(ctx->tdesc_table.ptr, ctx->tdescs.data(), ctx->tdescs.size() * sizeof(TransposeDesc), cudaMemcpyHostToDevice, ctx->stream));
     }
-    launch_transpose_in_all(ctx->tb_table.as<DeviceTypeBatch>(), ctx->tdesc_table.as<TransposeDesc>(), ctx->work_table.as<WorkItem>(), ctx->all_work_count, ctx->W,
+    launch_transpose_in_all(ctx->tb_table.as<DeviceTypeBatch>(), ctx->tdesc_table.as<TransposeDesc>(), ctx->work_table.as<WorkItem>(), ctx->topo.all_work_count, ctx->W,
                             kTransposePrestep | kTransposeImpulses, ctx->stream);
     if (any_redistribute) {
-        launch_redistribute_impulses(ctx->tb_table.as<DeviceTypeBatch>(), ctx->tdesc_table.as<TransposeDesc>(), ctx->work_table.as<WorkItem>(), ctx->all_work_count, ctx->stream);
+        launch_redistribute_impulses(ctx->tb_table.as<DeviceTypeBatch>(), ctx->tdesc_table.as<TransposeDesc>(), ctx->work_table.as<WorkItem>(), ctx->topo.all_work_count, ctx->stream);
         for (SourceTypeBatch& s : ctx->sources)
             if (s.redistribute) {
                 std::swap(s.raw_features_old, s.raw_features_new);  // the resident impulses now belong to the new ids
@@ -835,237 +696,55 @@ int32_t bepucuda_end_constraints(bepucuda_ctx* ctx) {
         return fail(ctx, BEPUCUDA_ERR_BAD_STATE, "end_constraints: peer sharding needs bepucuda_shard_set_body_masks for the current body count");
     CK(cudaSetDevice(ctx->device));
     const int W = ctx->W;
-    std::stable_sort(ctx->sources.begin(), ctx->sources.end(), [](const SourceTypeBatch& a, const SourceTypeBatch& b) {
-        return a.batch_index != b.batch_index ? a.batch_index < b.batch_index : a.type_batch_index < b.type_batch_index;
-    });
-
-    std::vector<int32_t> source_bundle_base(ctx->sources.size());
-    int32_t total_source_bundles = 0;
-    for (size_t si = 0; si < ctx->sources.size(); ++si) {
-        source_bundle_base[si] = total_source_bundles;
-        total_source_bundles += (ctx->sources[si].count + W - 1) / W;
-    }
-
-    // ---- device batches: synchronized batches in order, then dependency levels of the sequential fallback batch ----
-    ctx->tbs.clear();
-    ctx->tdescs.clear();
-    std::vector<int32_t> maps;                       // concatenated slot->source maps for fallback-level type batches
-    std::vector<size_t> map_offset;                  // per device tb: offset into maps or SIZE_MAX
-    std::vector<std::vector<int>> batch_tbs;         // device batch -> device tb indices
-    int64_t constraint_count = 0;
-    ctx->sync_batch_count = 0;
-    ctx->fallback_levels = 0;
     {
-        int current_batch = -1;
-        for (size_t si = 0; si < ctx->sources.size(); ++si) {
-            SourceTypeBatch& s = ctx->sources[si];
-            s.device_tbs.clear();
-            if (s.batch_index >= ctx->fallback_threshold) continue;
-            // device batch index == host batch index (empty batches stay as empty slots): ranks of a sharded graph then agree on batch numbers
-            while ((int)batch_tbs.size() <= s.batch_index) batch_tbs.emplace_back();
-            current_batch = s.batch_index;
-            const TypeInfo* t = get_type_info(s.type_id);
-            DeviceTypeBatch d{};
-            d.type_id = s.type_id;
-            d.bundle_count = (s.count + 31) / 32;
-            d.device_batch = s.batch_index;
-            TransposeDesc td{s.raw_refs, s.raw_prestep, s.raw_impulses, nullptr, s.count, t->bodies, t->prestep_rows, t->impulse_rows, source_bundle_base[si], 0, nullptr, nullptr};
-            s.device_tbs.push_back((int)ctx->tbs.size());
-            batch_tbs[s.batch_index].push_back((int)ctx->tbs.size());
-            ctx->tbs.push_back(d);
-            ctx->tdescs.push_back(td);
-            map_offset.push_back(SIZE_MAX);
-            s.live = s.count;
-            constraint_count += s.count;
-        }
-        if (ctx->peer_mode) {
-            // every rank runs the exchange point of every batch, also of batches it has no constraint in
-            while ((int)batch_tbs.size() < std::min(ctx->batch_count, ctx->fallback_threshold)) batch_tbs.emplace_back();
-            for (const SourceTypeBatch& src : ctx->sources)
-                if (src.batch_index >= ctx->fallback_threshold) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, "end_constraints: the sequential fallback batch is not supported across ranks");
-        }
-        (void)current_batch;
-        ctx->sync_batch_count = (int)batch_tbs.size();
+        std::vector<SourceView> views;
+        for (const SourceTypeBatch& s : ctx->sources) views.push_back({s.batch_index, s.type_batch_index, s.type_id, s.count, s.host_refs.data()});
+        TopologyPlan plan;
+        std::string error;
+        const int rc = plan_topology(views, W, ctx->fallback_threshold, ctx->batch_count, ctx->body_count, ctx->peer_mode, &plan, &error);
+        if (rc != BEPUCUDA_OK) return fail(ctx, rc, error);
+        ctx->topo = std::move(plan);
     }
-    {
-        // Fallback levelisation. The reference executes fallback bundles one after another on a single thread
-        // (Solver_Solve.cs:L546-583); within a bundle no dynamic body repeats (TypeProcessor.cs:L338-359). A constraint's
-        // level is 1 + the highest level of any earlier-bundle constraint sharing a dynamic body with it: executing levels in
-        // order with a barrier in between preserves every read-after-write of the sequential loop, so results are identical.
-        std::vector<int32_t> last_level;  // per body: highest level assigned so far (0 = none)
-        struct Slot { int level; int source; int constraint; };
-        std::vector<Slot> slots;
-        bool any = false;
-        for (size_t si = 0; si < ctx->sources.size(); ++si) {
-            SourceTypeBatch& s = ctx->sources[si];
-            if (s.batch_index < ctx->fallback_threshold) continue;
-            if (!any) { last_level.assign((size_t)ctx->body_count, 0); any = true; }
-            s.live = 0;
-            const TypeInfo* t = get_type_info(s.type_id);
-            const int nb = t->bodies;
-            const int bundles = (s.count + W - 1) / W;
-            std::vector<int> lane_level(W);
-            for (int k = 0; k < bundles; ++k) {
-                // all lanes of a bundle read the state left by earlier bundles
-                for (int l = 0; l < W; ++l) {
-                    lane_level[l] = 0;
-                    const int c = k * W + l;
-                    if (c >= s.count) continue;
-                    const int32_t first = s.host_refs[((size_t)k * nb) * W + l];
-                    if (first < 0) continue;  // hole
-                    int lvl = 0;
-                    for (int b = 0; b < nb; ++b) {
-                        const int32_t enc = s.host_refs[((size_t)k * nb + b) * W + l];
-                        if (enc < 0 || ((uint32_t)enc & kRefKinematicBit)) continue;
-                        const uint32_t idx = (uint32_t)enc & kRefIndexMask;
-                        if ((int)idx >= ctx->body_count) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "end_constraints: body reference out of range");
-                        lvl = std::max(lvl, last_level[idx]);
-                    }
-                    lane_level[l] = lvl + 1;
-                }
-                for (int l = 0; l < W; ++l) {
-                    if (lane_level[l] == 0) continue;
-                    for (int b = 0; b < nb; ++b) {
-                        const int32_t enc = s.host_refs[((size_t)k * nb + b) * W + l];
-                        if (enc < 0 || ((uint32_t)enc & kRefKinematicBit)) continue;
-                        last_level[(uint32_t)enc & kRefIndexMask] = lane_level[l];
-                    }
-                    // TypeProcessor.cs:L338-359: a fallback bundle never holds a dynamic body twice (two lanes of one level would race on its record)
-                    for (int l2 = 0; l2 < l; ++l2) {
-                        if (lane_level[l2] == 0) continue;
-                        for (int b = 0; b < nb; ++b) {
-                            const int32_t e1 = s.host_refs[((size_t)k * nb + b) * W + l];
-                            if (e1 < 0 || ((uint32_t)e1 & kRefKinematicBit)) continue;
-                            for (int b2 = 0; b2 < nb; ++b2) {
-                                const int32_t e2 = s.host_refs[((size_t)k * nb + b2) * W + l2];
-                                if (e2 >= 0 && !((uint32_t)e2 & kRefKinematicBit) && (((uint32_t)e1 ^ (uint32_t)e2) & kRefIndexMask) == 0)
-                                    return fail(ctx, BEPUCUDA_ERR_BATCH_INVARIANT, "end_constraints: a fallback bundle references the same dynamic body more than once");
-                            }
-                        }
-                    }
-                    slots.push_back({lane_level[l], (int)si, k * W + l});
-                    ++s.live;
-                    ++constraint_count;
-                }
-            }
-        }
-        if (any) {
-            std::stable_sort(slots.begin(), slots.end(), [](const Slot& a, const Slot& b) { return a.level != b.level ? a.level < b.level : a.source < b.source; });
-            size_t i = 0;
-            while (i < slots.size()) {
-                const int level = slots[i].level;
-                batch_tbs.emplace_back();
-                ++ctx->fallback_levels;
-                while (i < slots.size() && slots[i].level == level) {
-                    const int source = slots[i].source;
-                    size_t j = i;
-                    while (j < slots.size() && slots[j].level == level && slots[j].source == source) ++j;
-                    SourceTypeBatch& s = ctx->sources[source];
-                    const TypeInfo* t = get_type_info(s.type_id);
-                    const int n = (int)(j - i);
-                    DeviceTypeBatch d{};
-                    d.type_id = s.type_id;
-                    d.bundle_count = (n + 31) / 32;
-                    d.device_batch = (int)batch_tbs.size() - 1;
-                    map_offset.push_back(maps.size());
-                    for (size_t q = i; q < j; ++q) maps.push_back(slots[q].constraint);
-                    for (int q = n; q < d.bundle_count * 32; ++q) maps.push_back(-1);
-                    TransposeDesc td{s.raw_refs, s.raw_prestep, s.raw_impulses, nullptr, s.count, t->bodies, t->prestep_rows, t->impulse_rows, source_bundle_base[source], 0, nullptr, nullptr};
-                    s.device_tbs.push_back((int)ctx->tbs.size());
-                    batch_tbs.back().push_back((int)ctx->tbs.size());
-                    ctx->tbs.push_back(d);
-                    ctx->tdescs.push_back(td);
-                    i = j;
-                }
-            }
-        }
-    }
+    const TopologyPlan& topo = ctx->topo;
 
-    // ---- device arenas for the AOSOA-32 image ----
-    size_t refs_floats = 0, prestep_floats = 0, impulse_floats = 0;
-    std::vector<size_t> ro(ctx->tbs.size()), po(ctx->tbs.size()), io(ctx->tbs.size());
-    for (size_t i = 0; i < ctx->tbs.size(); ++i) {
-        const TypeInfo* t = get_type_info(ctx->tbs[i].type_id);
-        ro[i] = refs_floats; po[i] = prestep_floats; io[i] = impulse_floats;
-        refs_floats += (size_t)ctx->tbs[i].bundle_count * t->bodies * 32;
-        prestep_floats += (size_t)ctx->tbs[i].bundle_count * t->prestep_rows * 32;
-        impulse_floats += (size_t)ctx->tbs[i].bundle_count * t->impulse_rows * 32;
+    // ---- device arenas for the AOSOA-32 image, type batches, transposition descriptors, work records ----
+    CK(ctx->refs32.reserve(topo.refs_words * 4 + 1024));  // slack: solver warps always read two body-reference rows
+    CK(ctx->prestep32.reserve(topo.prestep_words * 4 + 4));
+    CK(ctx->impulses32.reserve(topo.impulse_words * 4 + 4));
+    CK(ctx->map_table.reserve(topo.maps.size() * 4 + 4));
+    std::vector<DeviceTypeBatch> tbs(topo.tbs.size());
+    ctx->tdescs.resize(topo.tbs.size());
+    for (size_t i = 0; i < topo.tbs.size(); ++i) {
+        const PlannedTypeBatch& p = topo.tbs[i];
+        const SourceTypeBatch& s = ctx->sources[(size_t)p.source];
+        const TypeInfo* t = get_type_info(p.type_id);
+        tbs[i] = {p.type_id, p.bundle_count, p.device_batch, 0, ctx->refs32.as<int32_t>() + p.refs_offset, ctx->prestep32.as<float>() + p.prestep_offset,
+                  ctx->impulses32.as<float>() + p.impulse_offset};
+        ctx->tdescs[i] = {s.raw_refs, s.raw_prestep, s.raw_impulses, p.map_offset < 0 ? nullptr : ctx->map_table.as<int32_t>() + p.map_offset, s.count, t->bodies, t->prestep_rows,
+                          t->impulse_rows, topo.source_bundle_base[(size_t)p.source], 0, nullptr, nullptr};
     }
-    CK(ctx->refs32.reserve(refs_floats * 4 + 1024));  // slack: solver warps always read two body-reference rows
-    ctx->refs_words = refs_floats;
-    CK(ctx->prestep32.reserve(prestep_floats * 4 + 4));
-    CK(ctx->impulses32.reserve(impulse_floats * 4 + 4));
-    CK(ctx->map_table.reserve(maps.size() * 4 + 4));
-    for (size_t i = 0; i < ctx->tbs.size(); ++i) {
-        ctx->tbs[i].refs = ctx->refs32.as<int32_t>() + ro[i];
-        ctx->tbs[i].prestep = ctx->prestep32.as<float>() + po[i];
-        ctx->tbs[i].impulses = ctx->impulses32.as<float>() + io[i];
-        ctx->tdescs[i].map = map_offset[i] == SIZE_MAX ? nullptr : ctx->map_table.as<int32_t>() + map_offset[i];
-    }
-
-    // ---- work lists: per device batch (one warp per bundle), then the incremental-update list over all contact bundles ----
-    ctx->work.clear();
-    ctx->bundle_live.clear();
-    ctx->batch_work.clear();
-    ctx->batch_contacts_only.clear();
-    auto live_in_bundle = [&](int tb, int k) {
-        // identity-mapped type batches: lanes beyond the source count are padding; mapped (fallback level) ones: -1 entries are padding
-        if (map_offset[tb] == SIZE_MAX) return std::max(0, std::min(32, ctx->tdescs[tb].src_count - k * 32));
-        int n = 0;
-        for (int l = 0; l < 32; ++l) n += maps[map_offset[tb] + (size_t)k * 32 + l] >= 0;
-        return n;
-    };
-    for (auto& list : batch_tbs) {
-        const int begin = (int)ctx->work.size();
-        bool contacts_only = true;
-        for (int tb : list) {
-            contacts_only = contacts_only && is_contact_type(ctx->tbs[tb].type_id);
-            for (int k = 0; k < ctx->tbs[tb].bundle_count; ++k) { ctx->work.push_back({tb, k}); ctx->bundle_live.push_back(live_in_bundle(tb, k)); }
-        }
-        ctx->batch_work.push_back({begin, (int)ctx->work.size() - begin});
-        ctx->batch_contacts_only.push_back(contacts_only ? 1 : 0);
-    }
-    ctx->all_work_count = (int)ctx->work.size();
-    ctx->inc_work_begin = (int)ctx->work.size();
-    for (size_t tb = 0; tb < ctx->tbs.size(); ++tb)
-        if (get_type_info(ctx->tbs[tb].type_id)->incremental)
-            for (int k = 0; k < ctx->tbs[tb].bundle_count; ++k) { ctx->work.push_back({(int)tb, k}); ctx->bundle_live.push_back(live_in_bundle((int)tb, k)); }
-    ctx->inc_work_count = (int)ctx->work.size() - ctx->inc_work_begin;
-
-    ctx->records.resize(ctx->work.size());
-    for (size_t i = 0; i < ctx->work.size(); ++i) {
-        const WorkItem& w = ctx->work[i];
-        const DeviceTypeBatch& tb = ctx->tbs[w.type_batch];
-        const TypeInfo* t = get_type_info(tb.type_id);
-        WorkRecord r{};
-        r.refs = tb.refs + (size_t)w.bundle * t->bodies * 32;
-        r.prestep = tb.prestep + (size_t)w.bundle * t->prestep_rows * 32;
-        r.impulses = tb.impulses + (size_t)w.bundle * t->impulse_rows * 32;
-        r.type_id = tb.type_id;
-        r.live_lanes = ctx->bundle_live[i];
-        ctx->records[i] = r;
-    }
+    ctx->records = work_records(topo, ctx->refs32.as<int32_t>(), ctx->prestep32.as<float>(), ctx->impulses32.as<float>());
 
     // ---- upload tables ----
     int32_t bodies_per_type[64];
     for (int i = 0; i < 64; ++i) bodies_per_type[i] = get_type_info(i) ? get_type_info(i)->bodies : 0;
-    CK(ctx->tb_table.reserve(ctx->tbs.size() * sizeof(DeviceTypeBatch) + 16));
+    CK(ctx->tb_table.reserve(tbs.size() * sizeof(DeviceTypeBatch) + 16));
     CK(ctx->tdesc_table.reserve(ctx->tdescs.size() * sizeof(TransposeDesc) + 16));
-    CK(ctx->work_table.reserve(ctx->work.size() * sizeof(WorkItem) + 16));
+    CK(ctx->work_table.reserve(topo.work.size() * sizeof(WorkItem) + 16));
     CK(ctx->record_table.reserve(ctx->records.size() * sizeof(WorkRecord) + 64));
     CK(ctx->bodies_per_type.reserve(sizeof(bodies_per_type)));
     CK(ctx->kinematics_dev.reserve(ctx->kinematics.size() * 4 + 4));
-    if (!ctx->tbs.empty()) CK(cudaMemcpyAsync(ctx->tb_table.ptr, ctx->tbs.data(), ctx->tbs.size() * sizeof(DeviceTypeBatch), cudaMemcpyHostToDevice, ctx->stream));
+    if (!tbs.empty()) CK(cudaMemcpyAsync(ctx->tb_table.ptr, tbs.data(), tbs.size() * sizeof(DeviceTypeBatch), cudaMemcpyHostToDevice, ctx->stream));
     if (!ctx->tdescs.empty()) CK(cudaMemcpyAsync(ctx->tdesc_table.ptr, ctx->tdescs.data(), ctx->tdescs.size() * sizeof(TransposeDesc), cudaMemcpyHostToDevice, ctx->stream));
-    if (!ctx->work.empty()) CK(cudaMemcpyAsync(ctx->work_table.ptr, ctx->work.data(), ctx->work.size() * sizeof(WorkItem), cudaMemcpyHostToDevice, ctx->stream));
+    if (!topo.work.empty()) CK(cudaMemcpyAsync(ctx->work_table.ptr, topo.work.data(), topo.work.size() * sizeof(WorkItem), cudaMemcpyHostToDevice, ctx->stream));
     if (!ctx->records.empty()) CK(cudaMemcpyAsync(ctx->record_table.ptr, ctx->records.data(), ctx->records.size() * sizeof(WorkRecord), cudaMemcpyHostToDevice, ctx->stream));
-    if (!maps.empty()) CK(cudaMemcpyAsync(ctx->map_table.ptr, maps.data(), maps.size() * 4, cudaMemcpyHostToDevice, ctx->stream));
+    if (!topo.maps.empty()) CK(cudaMemcpyAsync(ctx->map_table.ptr, topo.maps.data(), topo.maps.size() * 4, cudaMemcpyHostToDevice, ctx->stream));
     CK(cudaMemcpyAsync(ctx->bodies_per_type.ptr, bodies_per_type, sizeof(bodies_per_type), cudaMemcpyHostToDevice, ctx->stream));
     if (!ctx->kinematics.empty()) CK(cudaMemcpyAsync(ctx->kinematics_dev.ptr, ctx->kinematics.data(), ctx->kinematics.size() * 4, cudaMemcpyHostToDevice, ctx->stream));
 
     // ---- transposition into AOSOA-32 + ownership analysis ----
     { int rc = flush_chunks(ctx, ctx->pending_h2d); if (rc != BEPUCUDA_OK) return rc; }
-    launch_transpose_in_all(ctx->tb_table.as<DeviceTypeBatch>(), ctx->tdesc_table.as<TransposeDesc>(), ctx->work_table.as<WorkItem>(), ctx->all_work_count, W,
+    launch_transpose_in_all(ctx->tb_table.as<DeviceTypeBatch>(), ctx->tdesc_table.as<TransposeDesc>(), ctx->work_table.as<WorkItem>(), topo.all_work_count, W,
                             kTransposeRefs | kTransposePrestep | kTransposeImpulses, ctx->stream);
     const size_t nb = (size_t)std::max(ctx->body_count, 1);
     CK(ctx->first_batch.reserve(nb * 4));
@@ -1076,9 +755,9 @@ int32_t bepucuda_end_constraints(bepucuda_ctx* ctx) {
     CK(cudaMemsetAsync(ctx->sync_mask.ptr, 0, nb * 8, ctx->stream));
     CK(cudaMemsetAsync(ctx->constrained.ptr, 0, nb, ctx->stream));
     CK(cudaMemsetAsync(ctx->error_dev.ptr, 0, 32, ctx->stream));
-    CK(ctx->source_bundle_flags.reserve((size_t)std::max(total_source_bundles, 1) * 16));
-    CK(cudaMemsetAsync(ctx->source_bundle_flags.ptr, 0, (size_t)std::max(total_source_bundles, 1) * 16, ctx->stream));
-    launch_ownership_pass1(ctx->tb_table.as<DeviceTypeBatch>(), ctx->work_table.as<WorkItem>(), ctx->all_work_count, ctx->bodies_per_type.as<int32_t>(), ctx->sync_batch_count,
+    CK(ctx->source_bundle_flags.reserve((size_t)std::max(topo.source_bundles, 1) * 16));
+    CK(cudaMemsetAsync(ctx->source_bundle_flags.ptr, 0, (size_t)std::max(topo.source_bundles, 1) * 16, ctx->stream));
+    launch_ownership_pass1(ctx->tb_table.as<DeviceTypeBatch>(), ctx->work_table.as<WorkItem>(), topo.all_work_count, ctx->bodies_per_type.as<int32_t>(), topo.sync_batch_count,
                            ctx->body_count, ctx->first_batch.as<int32_t>(), ctx->sync_refcount.as<int32_t>(), (unsigned long long*)ctx->sync_mask.ptr, ctx->error_dev.as<int32_t>(),
                            ctx->stream);
     if (ctx->peer_mode && nb > 0) {
@@ -1086,7 +765,7 @@ int32_t bepucuda_end_constraints(bepucuda_ctx* ctx) {
         if ((int)ctx->global_first_batch.size() != ctx->body_count) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, "end_constraints: bepucuda_shard_set_global was not called for this body count");
         CK(cudaMemcpyAsync(ctx->first_batch.ptr, ctx->global_first_batch.data(), (size_t)ctx->body_count * 4, cudaMemcpyHostToDevice, ctx->stream));
     }
-    launch_ownership_rest(ctx->tb_table.as<DeviceTypeBatch>(), ctx->work_table.as<WorkItem>(), ctx->all_work_count, ctx->bodies_per_type.as<int32_t>(), ctx->body_count,
+    launch_ownership_rest(ctx->tb_table.as<DeviceTypeBatch>(), ctx->work_table.as<WorkItem>(), topo.all_work_count, ctx->bodies_per_type.as<int32_t>(), ctx->body_count,
                           ctx->first_batch.as<int32_t>(), ctx->sync_refcount.as<int32_t>(), (const unsigned long long*)ctx->sync_mask.ptr, ctx->constrained.as<uint8_t>(),
                           ctx->kinematics_dev.as<int32_t>(), (int)ctx->kinematics.size(), ctx->error_dev.as<int32_t>(), ctx->tdesc_table.as<TransposeDesc>(), W,
                           ctx->source_bundle_flags.as<int32_t>(), ctx->stream);
@@ -1094,34 +773,20 @@ int32_t bepucuda_end_constraints(bepucuda_ctx* ctx) {
         // ... and a body is "constrained" (final pose pass) if any rank constrains it
         CK(cudaMemcpyAsync(ctx->constrained.ptr, ctx->global_constrained.data(), (size_t)ctx->body_count, cudaMemcpyHostToDevice, ctx->stream));
         // per body reference, the other ranks that need what this rank's constraint writes
-        CK(ctx->peer32.reserve(ctx->refs_words * 4 + 1024));
+        CK(ctx->peer32.reserve(topo.refs_words * 4 + 1024));
         CK(ctx->body_masks_dev.reserve((size_t)ctx->body_count + 16));
         CK(cudaMemcpyAsync(ctx->body_masks_dev.ptr, ctx->body_masks.data(), (size_t)ctx->body_count, cudaMemcpyHostToDevice, ctx->stream));
-        launch_fill_peer_masks(ctx->refs32.as<int32_t>(), ctx->peer32.as<uint32_t>(), ctx->refs_words, ctx->body_masks_dev.as<uint8_t>(), ctx->peers.rank, ctx->stream);
+        launch_fill_peer_masks(ctx->refs32.as<int32_t>(), ctx->peer32.as<uint32_t>(), topo.refs_words, ctx->body_masks_dev.as<uint8_t>(), ctx->peers.rank, ctx->stream);
         // boundary bundles (any lane writes a shared body) go to the front of their batch and carry kRecordBoundaryBit: they are scheduled first, and
         // the flag barrier of the stage involves only them (ShardStage)
-        const int n_rec = ctx->all_work_count;
+        const int n_rec = topo.all_work_count;
         CK(ctx->boundary_flags_dev.reserve((size_t)n_rec + 16));
         launch_boundary_flags(ctx->record_table.as<WorkRecord>(), n_rec, ctx->bodies_per_type.as<int32_t>(), (long long)(ctx->peer32.as<int32_t>() - ctx->refs32.as<int32_t>()),
                               ctx->boundary_flags_dev.as<uint8_t>(), ctx->stream);
         std::vector<uint8_t> is_boundary((size_t)n_rec);
         if (n_rec > 0) CK(cudaMemcpyAsync(is_boundary.data(), ctx->boundary_flags_dev.ptr, (size_t)n_rec, cudaMemcpyDeviceToHost, ctx->stream));
         CK(cudaStreamSynchronize(ctx->stream));
-        ctx->boundary_count.assign(ctx->batch_work.size(), 0);
-        std::vector<WorkRecord> sorted;
-        for (size_t b = 0; b < ctx->batch_work.size(); ++b) {
-            const int begin = ctx->batch_work[b].first, count = ctx->batch_work[b].second;
-            sorted.clear();
-            for (int pass = 0; pass < 2; ++pass)
-                for (int i = begin; i < begin + count; ++i)
-                    if ((is_boundary[(size_t)i] != 0) == (pass == 0)) {
-                        WorkRecord r = ctx->records[(size_t)i];
-                        r.live_lanes = (r.live_lanes & ~kRecordBoundaryBit) | (pass == 0 ? kRecordBoundaryBit : 0);
-                        sorted.push_back(r);
-                        ctx->boundary_count[b] += pass == 0;
-                    }
-            std::copy(sorted.begin(), sorted.end(), ctx->records.begin() + begin);
-        }
+        ctx->boundary_count = sort_boundary_first(topo, is_boundary.data(), ctx->records);
         if (n_rec > 0) CK(cudaMemcpyAsync(ctx->record_table.ptr, ctx->records.data(), (size_t)n_rec * sizeof(WorkRecord), cudaMemcpyHostToDevice, ctx->stream));
     }
     // the first two body-reference rows of every work record, packed in work-list order (they carry the ownership bits set above)
@@ -1134,9 +799,9 @@ int32_t bepucuda_end_constraints(bepucuda_ctx* ctx) {
     if (err == 1) return fail(ctx, BEPUCUDA_ERR_BATCH_INVARIANT, "end_constraints: a synchronized batch references the same dynamic body more than once");
     if (err == 2) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "end_constraints: body reference out of range");
 
-    ctx->timings.constraint_count = constraint_count;
-    ctx->timings.device_batch_count = (int)batch_tbs.size();
-    ctx->timings.fallback_level_count = ctx->fallback_levels;
+    ctx->timings.constraint_count = topo.constraint_count;
+    ctx->timings.device_batch_count = (int)topo.batches.size();
+    ctx->timings.fallback_level_count = topo.fallback_levels;
     ctx->constraints_open = false;
     ctx->constraints_ready = true;
     ctx->data_dirty = false;
@@ -1169,12 +834,6 @@ int32_t bepucuda_update_type_batch(bepucuda_ctx* ctx, int32_t batch_index, int32
     return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "update_type_batch: unknown type batch");
 }
 
-static int contact_count_of_type(int type_id) {
-    if (type_id >= 0 && type_id <= 7) return (type_id & 3) + 1;
-    if (type_id >= 8 && type_id <= 10) return type_id - 6;
-    if (type_id >= 15 && type_id <= 17) return type_id - 13;
-    return 0;
-}
 static SourceTypeBatch* find_source(bepucuda_ctx* ctx, int32_t batch_index, int32_t type_batch_index) {
     for (auto& s : ctx->sources)
         if (s.batch_index == batch_index && s.type_batch_index == type_batch_index) return &s;
@@ -1182,7 +841,7 @@ static SourceTypeBatch* find_source(bepucuda_ctx* ctx, int32_t batch_index, int3
 }
 static int ensure_feature_arrays(bepucuda_ctx* ctx, SourceTypeBatch& s) {
     if (s.raw_features_old) return BEPUCUDA_OK;
-    s.feature_bytes = (size_t)s.count * contact_count_of_type(s.type_id) * sizeof(int32_t);
+    s.feature_bytes = (size_t)s.count * get_type_info(s.type_id)->contacts * sizeof(int32_t);
     cudaError_t e = cudaSuccess;
     s.raw_features_old = (int32_t*)ctx->raw_arena.alloc(s.feature_bytes, &e);
     s.raw_features_new = (int32_t*)ctx->raw_arena.alloc(s.feature_bytes, &e);
@@ -1195,7 +854,7 @@ int32_t bepucuda_set_contact_features(bepucuda_ctx* ctx, int32_t batch_index, in
     if (!ctx->constraints_open && !ctx->constraints_ready) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, "set_contact_features before the type batch was uploaded");
     SourceTypeBatch* s = find_source(ctx, batch_index, type_batch_index);
     if (!s) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "set_contact_features: unknown type batch");
-    if (contact_count_of_type(s->type_id) == 0) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "set_contact_features: not a contact constraint type");
+    if (get_type_info(s->type_id)->contacts == 0) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "set_contact_features: not a contact constraint type");
     CK(cudaSetDevice(ctx->device));
     { int rc = ensure_feature_arrays(ctx, *s); if (rc != BEPUCUDA_OK) return rc; }
     return copy_in(ctx, s->raw_features_old, feature_ids, s->feature_bytes);
@@ -1299,25 +958,15 @@ int32_t bepucuda_solve(bepucuda_ctx* ctx, float dt) {
         CK(cudaGetLastError());
     }
     CK(cudaEventRecord(ctx->ev_solve_end, ctx->stream));
-    if (ctx->peer_mode) { ctx->exchange_counter += ctx->exchanges_per_solve; ++ctx->shard_solve_index; }  // the flag barrier and the arrival counters keep counting across solves
+    if (ctx->peer_mode) { ctx->exchange_counter += ctx->program.exchange_count; ++ctx->shard_solve_index; }  // the flag barrier and the arrival counters keep counting across solves
     ctx->have_solve = true;
     ctx->timings.kernel_launches = launches;
 
     // metric bookkeeping (SURVEY.md §8d)
-    int64_t ci = 0, bytes = 0;
-    const int substeps = (int)ctx->iterations.size();
-    for (const SourceTypeBatch& s : ctx->sources) {
-        const TypeInfo* t = get_type_info(s.type_id);
-        const int64_t n = s.live;
-        for (int sub = 0; sub < substeps; ++sub) {
-            ci += n * ctx->iterations[sub];
-            bytes += n * ((int64_t)t->warm_start_bytes + (int64_t)ctx->iterations[sub] * t->solve_bytes + (sub > 0 ? t->incremental_bytes : 0));
-        }
-    }
-    bytes += (int64_t)ctx->body_count * 108;
-    if (ctx->accelerations_count >= 0) bytes += (int64_t)ctx->body_count * substeps * 32;  // one acceleration record per integrating lane: one per body and substep
-    ctx->timings.constraint_iterations = ci;
-    ctx->timings.algorithmic_bytes = bytes;
+    ctx->timings.constraint_iterations = ctx->program.constraint_iterations;
+    ctx->timings.algorithmic_bytes = ctx->program.algorithmic_bytes;
+    // one acceleration record per integrating lane: one per body and substep
+    if (ctx->accelerations_count >= 0) ctx->timings.algorithmic_bytes += (int64_t)ctx->body_count * (int64_t)ctx->iterations.size() * 32;
     return BEPUCUDA_OK;
 }
 
@@ -1356,7 +1005,7 @@ int32_t bepucuda_download_impulses(bepucuda_ctx* ctx) {
     if (!ctx) return BEPUCUDA_ERR_INVALID_ARGUMENT;
     if (!ctx->constraints_ready) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, "download_impulses before end_constraints");
     CK(cudaSetDevice(ctx->device));
-    launch_transpose_out_all(ctx->tb_table.as<DeviceTypeBatch>(), ctx->tdesc_table.as<TransposeDesc>(), ctx->work_table.as<WorkItem>(), ctx->all_work_count, ctx->W,
+    launch_transpose_out_all(ctx->tb_table.as<DeviceTypeBatch>(), ctx->tdesc_table.as<TransposeDesc>(), ctx->work_table.as<WorkItem>(), ctx->topo.all_work_count, ctx->W,
                              kTransposeImpulses, ctx->stream);
     CK(cudaGetLastError());
     int64_t bytes = 0;
@@ -1378,7 +1027,7 @@ int32_t bepucuda_download_prestep(bepucuda_ctx* ctx, int32_t batch_index, int32_
     CK(cudaSetDevice(ctx->device));
     for (auto& s : ctx->sources)
         if (s.batch_index == batch_index && s.type_batch_index == type_batch_index) {
-            launch_transpose_out_all(ctx->tb_table.as<DeviceTypeBatch>(), ctx->tdesc_table.as<TransposeDesc>(), ctx->work_table.as<WorkItem>(), ctx->all_work_count, ctx->W,
+            launch_transpose_out_all(ctx->tb_table.as<DeviceTypeBatch>(), ctx->tdesc_table.as<TransposeDesc>(), ctx->work_table.as<WorkItem>(), ctx->topo.all_work_count, ctx->W,
                                      kTransposePrestep, ctx->stream);
             CK(cudaGetLastError());
             CK(cudaMemcpyAsync(prestep_out, s.raw_prestep, s.prestep_bytes, cudaMemcpyDeviceToHost, ctx->stream));
@@ -1422,40 +1071,26 @@ int32_t bepucuda_profile_stages(bepucuda_ctx* ctx, float dt, bepucuda_stage_prof
     { int rc = check_accelerations(ctx, "profile_stages"); if (rc != BEPUCUDA_OK) return rc; }
     CK(cudaSetDevice(ctx->device));
     std::memset(out, 0, sizeof(*out));
-    const size_t need = ctx->program.size() * 2;
+    const size_t need = ctx->program.ops.size() * 2;
     while (ctx->profile_events.size() < need) {
         cudaEvent_t ev;
         CK(cudaEventCreate(&ev));
         ctx->profile_events.push_back(ev);
     }
     { int rc = prepare_frame(ctx, dt); if (rc != BEPUCUDA_OK) return rc; }
-    std::vector<int> launched(ctx->program.size(), 0);
+    std::vector<int> launched(ctx->program.ops.size(), 0);
     const StageEvents sink{ctx->profile_events, launched};
     issue_stage_sequence(ctx, ctx->stream, nullptr, &sink);
     CK(cudaStreamSynchronize(ctx->stream));
     CK(cudaGetLastError());
-    for (size_t i = 0; i < ctx->program.size(); ++i) {
+    for (size_t i = 0; i < ctx->program.ops.size(); ++i) {
         if (!launched[i]) continue;
         float ms = 0;
         CK(cudaEventElapsedTime(&ms, ctx->profile_events[2 * i], ctx->profile_events[2 * i + 1]));
-        const StageOp& op = ctx->program[i];
+        const StageOp& op = ctx->program.ops[i];
         out->ms[op.stage] += ms;
         out->launches[op.stage] += 1;
-        int64_t bytes = 0;
-        if (op.stage <= kStageIncremental) {
-            // live constraints per work item are not tracked per bundle; use 32 lanes per bundle minus padding via the per-type-batch totals
-            for (int w = 0; w < op.work_count; ++w) {
-                const WorkItem& wi = ctx->work[op.work_begin + w];
-                const TypeInfo* t = get_type_info(ctx->tbs[wi.type_batch].type_id);
-                const int per = op.stage == kStageSolve ? t->solve_bytes : op.stage == kStageIncremental ? t->incremental_bytes : t->warm_start_bytes;
-                bytes += (int64_t)per * ctx->bundle_live[(size_t)op.work_begin + w];
-            }
-        } else if (op.stage == kStageFinalPose) {
-            bytes = (int64_t)ctx->body_count * 108;
-        } else {
-            bytes = (int64_t)op.work_count * 108;
-        }
-        out->algorithmic_bytes[op.stage] += bytes;
+        out->algorithmic_bytes[op.stage] += op.algorithmic_bytes;
     }
     return BEPUCUDA_OK;
 }

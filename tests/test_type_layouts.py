@@ -114,14 +114,14 @@ def test_contact_prestep_generators_write_rows_in_reference_order():
 
 def test_roofline_byte_model_uses_the_reference_access_filters():
     """The SURVEY.md §8d algorithmic bytes per evaluation behind `roofline.achieved` (csrc/bepu_joint_registry.inc, make_contact in
-    csrc/bepucuda_api.cu): per-body read / written float counts must be the sums over the access filters the reference declares for each type
+    csrc/bepu_topology.cpp): per-body read / written float counts must be the sums over the access filters the reference declares for each type
     (fixture: parsed from the processor declarations and IBodyAccessFilter.cs), and the resulting bytes must reproduce the worked examples of
     SURVEY.md §8d."""
     with open(os.path.join(ROOT, "tests", "golden", "type_layouts.json")) as f:
         filters = json.load(f)["access_filters"]
     csrc = os.path.join(ROOT, "bepuphysics2_b200", "csrc")
     inc = open(os.path.join(csrc, "bepu_joint_registry.inc")).read()
-    api = open(os.path.join(csrc, "bepucuda_api.cu")).read()
+    api = open(os.path.join(csrc, "bepu_topology.cpp")).read()
     solve_bytes, warm_start_bytes = {}, {}
     seen = set()
     for m in re.finditer(r"add\((\d+),\s*make_joint\((\d+),\s*(\d+),\s*(\d+),\s*(\d+),\s*(\d+),\s*(\d+),\s*(\d+),", inc):
