@@ -34,6 +34,7 @@ struct BodyBuffers {
     float4* inertia_local;
     float4* inertia_world;
     const uint8_t* constrained;  // 1 if the body is referenced by any constraint or is a constrained kinematic
+    const int32_t* first_batch;  // lowest device batch that references the body as a dynamic body (its integrating lane's), INT32_MAX if none
     int32_t count;
 };
 

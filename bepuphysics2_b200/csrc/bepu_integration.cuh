@@ -16,6 +16,13 @@ BEPU_DI Q4 integrate_orientation(Q4 start, V3 w, float halfDt) {  // PoseIntegra
     return speed > 1e-15f ? end : start;
 }
 BEPU_DI Sym3 rotate_inverse_inertia(Sym3 local, Q4 q) { return rotation_sandwich(matrix_from_quaternion(q), local); }  // L166-175
+// The pose half of IntegratePoseAndVelocity (TypeProcessor.cs:L1204-1248): position and orientation advance by the velocity over dt, and the
+// local inverse inertia is rotated into the new orientation. Shared by the WarmStart stages and the body part of the incremental contact update.
+BEPU_DI void integrate_pose_and_inertia(V3 lin, V3 ang, float dt, Sym3 local, V3& pos, Q4& q, Sym3& world) {
+    pos = pos + lin * dt;
+    q = integrate_orientation(q, ang, dt * 0.5f);
+    world = rotate_inverse_inertia(local, q);
+}
 BEPU_DI void callback_integrate_velocity(Velocity& v, float gx, float gy, float gz, float linearDampingDt, float angularDampingDt) {
     v.lin = (v.lin + V3{gx, gy, gz}) * linearDampingDt;
     v.ang = v.ang * angularDampingDt;

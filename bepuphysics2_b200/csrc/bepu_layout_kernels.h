@@ -56,7 +56,7 @@ void launch_boundary_flags(const WorkRecord* records, int count, const int32_t* 
 void launch_pack_ref_rows(const WorkRecord* records, int count, int32_t* rows, cudaStream_t s);
 
 // Numerics flavours (bepu_solver_kernels.cu, compiled twice).
-constexpr int kLaunchPdl = 1, kLaunchPrefetchRows = 2, kLaunchIntegratorExtensions = 4, kLaunchContactsOnly = 8, kLaunchPrefetchBodies = 16;
+constexpr int kLaunchPdl = 1, kLaunchPrefetchRows = 2, kLaunchIntegratorExtensions = 4, kLaunchContactsOnly = 8, kLaunchPrefetchBodies = 16, kLaunchBodiesIntegrated = 32;
 // Peer-sharded stage (bepucuda_shard_*): every written body record also goes to the ranks named by the per-(lane, slot) destination masks at
 // refs + peer_delta (launch_fill_peer_masks).
 struct ShardLaunch {
@@ -72,6 +72,8 @@ struct SolverLaunchers {
     // kLaunchContactsOnly = every bundle of the batch is a contact: the WarmStart / Solve stage runs the contact-only instantiation (not sharded).
     // kLaunchPrefetchBodies = the kernel launched just before this one is a stage of this solve and not the WarmStart of this batch, so the prologue
     // may load the body records it does not write (constraint_stage_body).
+    // kLaunchBodiesIntegrated (substeps > 0, FrameParams::angular_mode 0): the incremental contact update also integrates the pose and rotates the
+    // world inertia of every body a constraint lane integrates, one thread per body, and the WarmStart stages leave that part to it.
     // ref_rows: the packed reference rows of records[0 .. work_count) (launch_pack_ref_rows).
     // shard: nullptr on a single GPU; a WarmStartFirst / WarmStart / Solve stage of a peer-sharded solve otherwise.
     void (*constraint_stage)(int stage, const WorkRecord* records, const int32_t* ref_rows, int work_count, const BodyBuffers& B, const FrameParams* fp, int launch_flags,

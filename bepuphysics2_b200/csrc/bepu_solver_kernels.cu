@@ -26,9 +26,9 @@ constexpr int kDeepBatchBundles = 2150;  // more bundles than the uncapped build
 #ifndef BEPU_CONTACT_SOLVE_MINB
 #define BEPU_CONTACT_SOLVE_MINB 12
 #endif
-// Launches one stage kernel instantiation (plain or sharded), one warp per bundle.
+// Launches one stage kernel instantiation (plain or sharded), one warp per bundle, and `extra_blocks` CTAs after the bundles'.
 template <auto Kernel, class... Args>
-static void launch_stage_kernel(int work_count, int launch_flags, cudaStream_t s, Args... args) {
+static void launch_stage_kernel(int work_count, unsigned extra_blocks, int launch_flags, cudaStream_t s, Args... args) {
     static std::atomic<bool> carveout_set[64] = {};  // function attributes are per device: a process may hold contexts on several
     int device = 0;
     cudaGetDevice(&device);
@@ -36,7 +36,7 @@ static void launch_stage_kernel(int work_count, int launch_flags, cudaStream_t s
         cudaFuncSetAttribute(Kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
         carveout_set[device & 63] = true;
     }
-    const unsigned blocks = (unsigned)(((size_t)work_count * 32 + kStageBlockThreads - 1) / kStageBlockThreads);
+    const unsigned blocks = (unsigned)(((size_t)work_count * 32 + kStageBlockThreads - 1) / kStageBlockThreads) + extra_blocks;
     cudaLaunchConfig_t cfg{};
     cfg.gridDim = dim3(blocks);
     cfg.blockDim = dim3(kStageBlockThreads);
@@ -51,11 +51,15 @@ static void launch_stage_kernel(int work_count, int launch_flags, cudaStream_t s
 template <int STAGE, int MINB, bool kExt, bool kContacts>
 static void launch_stage_instance(const WorkRecord* records, const int32_t* ref_rows, int work_count, const BodyBuffers& B, const FrameParams* fp, int launch_flags, const ShardLaunch* shard,
                                   cudaStream_t s) {
-    const int flags = ((launch_flags & bepucuda::kLaunchPrefetchRows) ? kStagePrefetchRows : 0) | ((launch_flags & bepucuda::kLaunchPrefetchBodies) ? kStagePrefetchBodies : 0);
-    if (!shard) launch_stage_kernel<constraint_stage_kernel<STAGE, MINB, kExt, kContacts>>(work_count, launch_flags, s, records, ref_rows, work_count, B, fp, flags);
+    const bool bodies_integrated = (launch_flags & bepucuda::kLaunchBodiesIntegrated) != 0;
+    const int flags = ((launch_flags & bepucuda::kLaunchPrefetchRows) ? kStagePrefetchRows : 0) | ((launch_flags & bepucuda::kLaunchPrefetchBodies) ? kStagePrefetchBodies : 0) |
+                      (bodies_integrated ? kStageBodiesIntegrated : 0);
+    // the incremental contact update that integrates poses has one thread per body after its bundles (integrate_body_pose)
+    const unsigned body_blocks = STAGE == kStageIncremental && bodies_integrated ? (unsigned)((B.count + kStageBlockThreads - 1) / kStageBlockThreads) : 0u;
+    if (!shard) launch_stage_kernel<constraint_stage_kernel<STAGE, MINB, kExt, kContacts>>(work_count, body_blocks, launch_flags, s, records, ref_rows, work_count, B, fp, flags);
     else if constexpr (STAGE != kStageIncremental && !kContacts)  // the incremental contact update is never sharded; sharded stages run the full switch
-        launch_stage_kernel<constraint_stage_kernel_sharded<STAGE, MINB, kExt>>(work_count, launch_flags, s, records, ref_rows, work_count, B, fp, flags, shard->peers, shard->peer_delta,
-                                                                               shard->stage);
+        launch_stage_kernel<constraint_stage_kernel_sharded<STAGE, MINB, kExt>>(work_count, 0u, launch_flags, s, records, ref_rows, work_count, B, fp, flags, shard->peers,
+                                                                               shard->peer_delta, shard->stage);
 }
 // The WarmStart stages integrate: contexts with per-body accelerations or point gravity run their own instantiation (kLaunchIntegratorExtensions).
 template <int STAGE, int MINB, bool kContacts>

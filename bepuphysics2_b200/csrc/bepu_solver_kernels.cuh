@@ -85,7 +85,8 @@ BEPU_DI void apply_velocity_extensions(const FrameParams& fp, uint32_t idx, V3 p
 }
 
 // Body records of body slots 0 and 1 that a plain stage kernel loaded before its grid-dependency wait (see constraint_stage_body); bit s of
-// `slots` is set when slot s was loaded. Solve: world inertia, and pose for kNeedsPose types. WarmStart: local inertia and pose of an integrating slot.
+// `slots` is set when slot s was loaded. Solve: world inertia, and pose for kNeedsPose types. WarmStart: local inertia and pose of an integrating slot;
+// with kStageBodiesIntegrated, world inertia of every slot instead.
 struct EarlyBodies {
     uint32_t slots;
     Inertia inertia[2];
@@ -97,45 +98,55 @@ struct EarlyBodies {
 // device body reference carries kRefIntegrateBit; all other lanes read the world inertia their owner constraint stored earlier in this substep,
 // which is bit-identical to what the reference's bundle-wide recompute would give them. kExt: the stage kernel instantiation for contexts with
 // per-body accelerations or point gravity (the launcher picks it), so that the default path carries none of it.
+// integrated: a WarmStart stage whose pose half the incremental contact update of this substep has done (kStageBodiesIntegrated, angular mode 0,
+// integrate_body_pose): the integrating lane reads the pose and world inertia that update stored and integrates the velocity only. Never in the
+// kExt instantiations: the host does not pass the flag to contexts with per-body accelerations or point gravity, since the pose the point-gravity
+// term reads would take the contact-only kExt WarmStart kernel past its register budget.
 template <int STAGE, bool NeedsPose, bool kExt>
-BEPU_DI void warm_start_body(uint32_t enc, const BodyBuffers& B, const FrameParams& fp, bool early_slot, const EarlyBodies& early, int s, BodyState& b, Velocity& v) {
+BEPU_DI void warm_start_body(uint32_t enc, const BodyBuffers& B, const FrameParams& fp, bool integrated, bool early_slot, const EarlyBodies& early, int s, BodyState& b,
+                             Velocity& v) {
     const uint32_t idx = enc & kRefIndexMask;
     if (enc & kRefIntegrateBit) {
-        Inertia local;
-        if (early_slot) {
-            local = early.inertia[s];
-            b.pos = early.pos[s];
-            b.q = early.q[s];
+        if (STAGE == kStageWarmStart && !kExt && integrated) {
+            if (early_slot) b.inertia = early.inertia[s];
+            else load_inertia(B.inertia_world, idx, b.inertia);
+            if (NeedsPose) load_pose(B.pose, idx, b.pos, b.q);
         } else {
-            load_inertia(B.inertia_local, idx, local);
-            load_pose(B.pose, idx, b.pos, b.q);
-        }
-        b.inertia.inv_mass = local.inv_mass;
-        if (STAGE == kStageWarmStart) {
-            // IntegratePoseAndVelocity, TypeProcessor.cs:L1204-1248
-            b.pos = b.pos + v.lin * fp.dt;
-            Q4 previousOrientation = b.q;
-            b.q = integrate_orientation(b.q, v.ang, fp.dt * 0.5f);
-            b.inertia.t = rotate_inverse_inertia(local.t, b.q);
-            if (fp.angular_mode == 1) integrate_angular_conserve_momentum(previousOrientation, local.t, b.inertia.t, v.ang);
-            else if (fp.angular_mode == 2) integrate_angular_gyroscopic(b.q, local.t, v.ang, fp.dt);
-            store_pose(B.pose, idx, b.pos, b.q);
-        } else {
-            // IntegrateVelocity, TypeProcessor.cs:L1251-1283
-            b.inertia.t = rotate_inverse_inertia(local.t, b.q);
-            if (fp.angular_mode == 1) {
-                Q4 previousOrientation = integrate_orientation(b.q, v.ang, fp.dt * -0.5f);
-                integrate_angular_conserve_momentum(previousOrientation, local.t, b.inertia.t, v.ang);
-            } else if (fp.angular_mode == 2) {
-                integrate_angular_gyroscopic(b.q, local.t, v.ang, fp.dt);
+            Inertia local;
+            if (early_slot) {
+                local = early.inertia[s];
+                b.pos = early.pos[s];
+                b.q = early.q[s];
+            } else {
+                load_inertia(B.inertia_local, idx, local);
+                load_pose(B.pose, idx, b.pos, b.q);
             }
+            b.inertia.inv_mass = local.inv_mass;
+            if (STAGE == kStageWarmStart) {
+                // IntegratePoseAndVelocity, TypeProcessor.cs:L1204-1248
+                Q4 previousOrientation = b.q;
+                integrate_pose_and_inertia(v.lin, v.ang, fp.dt, local.t, b.pos, b.q, b.inertia.t);
+                if (fp.angular_mode == 1) integrate_angular_conserve_momentum(previousOrientation, local.t, b.inertia.t, v.ang);
+                else if (fp.angular_mode == 2) integrate_angular_gyroscopic(b.q, local.t, v.ang, fp.dt);
+                store_pose(B.pose, idx, b.pos, b.q);
+            } else {
+                // IntegrateVelocity, TypeProcessor.cs:L1251-1283
+                b.inertia.t = rotate_inverse_inertia(local.t, b.q);
+                if (fp.angular_mode == 1) {
+                    Q4 previousOrientation = integrate_orientation(b.q, v.ang, fp.dt * -0.5f);
+                    integrate_angular_conserve_momentum(previousOrientation, local.t, b.inertia.t, v.ang);
+                } else if (fp.angular_mode == 2) {
+                    integrate_angular_gyroscopic(b.q, local.t, v.ang, fp.dt);
+                }
+            }
+            store_inertia(B.inertia_world, idx, b.inertia);
         }
         callback_integrate_velocity(v, fp.gravity_dt[0], fp.gravity_dt[1], fp.gravity_dt[2], fp.linear_damping_dt, fp.angular_damping_dt);
         // the callback sees the current pose in the first substep and the freshly integrated one after (TypeProcessor.cs:L1244, L1276)
         if constexpr (kExt) apply_velocity_extensions(fp, idx, b.pos, fp.dt, fp.attractor_dt, v);
-        store_inertia(B.inertia_world, idx, b.inertia);
     } else {
-        load_inertia(B.inertia_world, idx, b.inertia);
+        if (STAGE == kStageWarmStart && !kExt && early_slot) b.inertia = early.inertia[s];  // only ever set for a non-integrating lane when integrated
+        else load_inertia(B.inertia_world, idx, b.inertia);
         if (NeedsPose) load_pose(B.pose, idx, b.pos, b.q);
         if (STAGE == kStageWarmStartFirst && fp.angular_mode != 0 && (enc & kRefBundleIntegratesBit) && !(enc & kRefKinematicBit)) {
             // Reference quirk, reproduced for identical results: in the first substep IntegrateVelocity runs the momentum-conserving angular
@@ -152,9 +163,10 @@ BEPU_DI void warm_start_body(uint32_t enc, const BodyBuffers& B, const FramePara
     }
 }
 template <int STAGE, bool NeedsPose, bool kExt>
-BEPU_DI void gather_for_warm_start(uint32_t enc, const BodyBuffers& B, const FrameParams& fp, bool early_slot, const EarlyBodies& early, int s, BodyState& b, Velocity& v) {
+BEPU_DI void gather_for_warm_start(uint32_t enc, const BodyBuffers& B, const FrameParams& fp, bool integrated, bool early_slot, const EarlyBodies& early, int s, BodyState& b,
+                                   Velocity& v) {
     load_velocity(B.velocity, enc & kRefIndexMask, v);
-    warm_start_body<STAGE, NeedsPose, kExt>(enc, B, fp, early_slot, early, s, b, v);
+    warm_start_body<STAGE, NeedsPose, kExt>(enc, B, fp, integrated, early_slot, early, s, b, v);
 }
 
 // ---- uniform call shapes over contact and joint types ------------------------------------------------------------------
@@ -195,8 +207,8 @@ BEPU_DI void push_record(float4* const* arrays, uint32_t mask, uint32_t idx, flo
     }
 }
 template <class T, int STAGE, bool kSharded, bool kExt, class PR, class AR>
-BEPU_DI void run_lane(const int32_t* refs, PR p, AR a, float* p_rw, uint32_t enc0, uint32_t enc1, const BodyBuffers& B, const FrameParams& fp, const EarlyBodies& early,
-                      const ShardPeers* peers = nullptr, long long peer_delta = 0) {
+BEPU_DI void run_lane(const int32_t* refs, PR p, AR a, float* p_rw, uint32_t enc0, uint32_t enc1, const BodyBuffers& B, const FrameParams& fp, bool integrated,
+                      const EarlyBodies& early, const ShardPeers* peers = nullptr, long long peer_delta = 0) {
     constexpr int NB = T::kBodies;
     uint32_t enc[NB];
     enc[0] = enc0;
@@ -241,7 +253,7 @@ BEPU_DI void run_lane(const int32_t* refs, PR p, AR a, float* p_rw, uint32_t enc
             }
     } else {
 #pragma unroll
-        for (int s = 0; s < NB; ++s) gather_for_warm_start<STAGE, T::kNeedsPose, kExt>(enc[s], B, fp, s < 2 && (early.slots >> s & 1u), early, s & 1, b[s], v[s]);
+        for (int s = 0; s < NB; ++s) gather_for_warm_start<STAGE, T::kNeedsPose, kExt>(enc[s], B, fp, integrated, s < 2 && (early.slots >> s & 1u), early, s & 1, b[s], v[s]);
         rows_ready(p);
         call_warm_start<T>(b, p, a, v);
 #pragma unroll
@@ -292,12 +304,12 @@ BEPU_DI WorkRecord load_record(const WorkRecord* r) {
 // kContacts: the switch covers the contact types only. The host launches that instantiation for device batches whose every bundle is a contact
 // (kLaunchContactsOnly); it is about half the code of the full switch and fits a smaller register budget (bepu_solver_kernels.cu).
 template <int STAGE, bool kSharded, bool kExt, bool kContacts, class PR, class AR>
-BEPU_DI void run_bundle_rows(const WorkRecord& rec, int lane, PR p, AR a, uint32_t enc0, uint32_t enc1, const BodyBuffers& B, const FrameParams& fp, const EarlyBodies& early,
-                             const ShardPeers* peers = nullptr, long long peer_delta = 0) {
+BEPU_DI void run_bundle_rows(const WorkRecord& rec, int lane, PR p, AR a, uint32_t enc0, uint32_t enc1, const BodyBuffers& B, const FrameParams& fp, bool integrated,
+                             const EarlyBodies& early, const ShardPeers* peers = nullptr, long long peer_delta = 0) {
     const int32_t* refs = rec.refs + lane;
     float* p_rw = rec.prestep + lane;
 #define BEPU_CASE(ID, T) \
-    case ID: run_lane<T, STAGE, kSharded, kExt>(refs, p, a, p_rw, enc0, enc1, B, fp, early, peers, peer_delta); break;
+    case ID: run_lane<T, STAGE, kSharded, kExt>(refs, p, a, p_rw, enc0, enc1, B, fp, integrated, early, peers, peer_delta); break;
     if constexpr (kContacts) {
         switch (rec.type_id) {
             BEPU_CONTACT_TYPES(BEPU_CASE)
@@ -316,7 +328,7 @@ BEPU_DI void run_bundle_rows(const WorkRecord& rec, int lane, PR p, AR a, uint32
 // Rows straight from HBM (the incremental stage).
 template <int STAGE>
 BEPU_DI void run_bundle(const WorkRecord& rec, int lane, uint32_t enc0, uint32_t enc1, const BodyBuffers& B, const FrameParams& fp) {
-    run_bundle_rows<STAGE, false, false, false>(rec, lane, GlobalRows{rec.prestep + lane}, GlobalAcc{rec.impulses + lane}, enc0, enc1, B, fp, EarlyBodies{});
+    run_bundle_rows<STAGE, false, false, false>(rec, lane, GlobalRows{rec.prestep + lane}, GlobalAcc{rec.impulses + lane}, enc0, enc1, B, fp, false, EarlyBodies{});
 }
 // The reference arena is padded, so reading a second body-reference row is always in bounds (one-body types ignore it).
 template <int STAGE> BEPU_DI void run_bundle(const WorkRecord& rec, int lane, const BodyBuffers& B, const FrameParams& fp) {
@@ -382,7 +394,12 @@ constexpr int kStageBlockThreads = BEPU_STAGE_BLOCK_THREADS;
 //   - WarmStart, integrating slot: local inertia (never written during a solve) and pose (written only by this batch's own WarmStart, a substep ago);
 //   - Solve: world inertia (and pose for kNeedsPose types), written only by the WarmStart stages of batches up to this one.
 // Sharded kernels load every body record after the wait: a peer's stores are only known to have arrived after shard_wait.
-constexpr int kStagePrefetchRows = 1, kStagePrefetchBodies = 2;
+// A WarmStart stage with kStageBodiesIntegrated (angular mode 0) writes no world inertia and no pose: the incremental contact update at the start
+// of the substep wrote them for every integrated body, and nothing else writes them before the substep's Solve stages. So such a stage loads the
+// world inertia of slots 0 and 1, for integrating and other lanes alike, before its wait, like a Solve stage, whenever its predecessor is not that
+// update (kStagePrefetchRows: behind a WarmStart stage of an earlier batch or the kinematic pass, which writes kinematic poses and velocities
+// only). Contact-only kernels only: no contact type reads a pose. Otherwise the flagged stage loads no body record before the wait.
+constexpr int kStagePrefetchRows = 1, kStagePrefetchBodies = 2, kStageBodiesIntegrated = 4;
 template <int STAGE, bool kContacts>
 BEPU_DI void load_early_bodies(int type_id, uint32_t enc0, uint32_t enc1, const BodyBuffers& B, EarlyBodies& e) {
     if ((int32_t)enc0 == kRefEmpty) return;
@@ -423,11 +440,43 @@ BEPU_DI void shard_wait(const ShardPeers& peers, int lane, uint32_t solve_index,
     }
     __syncwarp();
 }
+// Body part of the incremental contact update (kStageBodiesIntegrated, angular mode 0): thread i does the pose half of IntegratePoseAndVelocity
+// for body i if a constraint lane integrates it (first_batch set; kinematic bodies have none), so that the WarmStart stage of the body's first
+// batch only integrates its velocity. The velocity is loaded after the wait: the predecessor, the last stage of the previous substep, writes it.
+// Pose and local inertia are loaded before it: no stage that can precede an incremental update writes them (Solve writes velocities and
+// impulses, WarmStartFirst and, with this flag, WarmStart velocities and world inertia only; the kinematic pass of the previous substep, which
+// writes kinematic poses, is older than that predecessor).
+BEPU_DI void integrate_body_pose(int i, const BodyBuffers& B, const FrameParams* __restrict__ fpp) {
+    const FrameParams fp = *fpp;
+    const bool owned = i < B.count && fp.angular_mode == 0 && (int32_t)ldg_nc_u32(B.first_batch + i) != 0x7fffffff;
+    Inertia local;
+    V3 pos;
+    Q4 q;
+    if (owned) {
+        load_inertia(B.inertia_local, (uint32_t)i, local);
+        load_pose(B.pose, (uint32_t)i, pos, q);
+    }
+    asm volatile("griddepcontrol.wait;" ::: "memory");
+    asm volatile("griddepcontrol.launch_dependents;");
+    if (!owned) return;
+    Velocity v;
+    load_velocity(B.velocity, (uint32_t)i, v);
+    Inertia world;
+    world.inv_mass = local.inv_mass;
+    integrate_pose_and_inertia(v.lin, v.ang, fp.dt, local.t, pos, q, world.t);
+    store_pose(B.pose, (uint32_t)i, pos, q);
+    store_inertia(B.inertia_world, (uint32_t)i, world);
+}
 template <int STAGE, bool kSharded, bool kExt, bool kContacts, bool kEarlyBodies>
 BEPU_DI void constraint_stage_body(const WorkRecord* __restrict__ records, const int32_t* __restrict__ ref_rows, int work_count, const BodyBuffers& B, const FrameParams* __restrict__ fpp, int flags, const ShardPeers* peers,
                                    long long peer_delta, const ShardStage* shard = nullptr) {
     constexpr bool kStaged = STAGE != kStageIncremental;
     constexpr int kWarps = kStageBlockThreads / 32;
+    if constexpr (STAGE == kStageIncremental) {
+        // the CTAs past the bundles' (launch_stage_instance adds them with kStageBodiesIntegrated) hold one thread per body
+        const int bundle_blocks = (work_count + kWarps - 1) / kWarps;
+        if ((int)blockIdx.x >= bundle_blocks) return integrate_body_pose(((int)blockIdx.x - bundle_blocks) * kStageBlockThreads + (int)threadIdx.x, B, fpp);
+    }
     __shared__ __align__(128) float slab[kStaged ? kWarps * kStageSlabRows * kLanes : 1];
     __shared__ __align__(8) unsigned long long bars[kWarps];
     const int warp_in_block = threadIdx.x >> 5;
@@ -461,12 +510,17 @@ BEPU_DI void constraint_stage_body(const WorkRecord* __restrict__ records, const
         enc0 = ldg_nc_u32(ref_rows + (size_t)warp * (2 * kLanes) + lane);
         enc1 = ldg_nc_u32(ref_rows + (size_t)warp * (2 * kLanes) + kLanes + lane);
         if constexpr (kStaged && kEarlyBodies) {
-            if (flags & kStagePrefetchBodies) load_early_bodies<STAGE, kContacts>(rec.type_id, enc0, enc1, B, early);
+            if (flags & kStagePrefetchBodies) {
+                if (!(flags & kStageBodiesIntegrated)) load_early_bodies<STAGE, kContacts>(rec.type_id, enc0, enc1, B, early);
+                else if (STAGE == kStageWarmStart && kContacts && !kExt && (flags & kStagePrefetchRows) && fpp->angular_mode == 0)
+                    load_early_bodies<kStageSolve, kContacts>(rec.type_id, enc0, enc1, B, early);  // world inertia of every slot, as a Solve stage does
+            }
         }
     }
     const FrameParams fp = *fpp;
     asm volatile("griddepcontrol.wait;" ::: "memory");
     asm volatile("griddepcontrol.launch_dependents;");
+    const bool integrated = STAGE == kStageWarmStart && !kExt && (flags & kStageBodiesIntegrated) && fp.angular_mode == 0;
     bool boundary = false;
     if constexpr (kSharded) {
         boundary = active && (rec.live_lanes & kRecordBoundaryBit) != 0;
@@ -483,7 +537,7 @@ BEPU_DI void constraint_stage_body(const WorkRecord* __restrict__ records, const
         }
         __syncwarp();
         run_bundle_rows<STAGE, kSharded, kExt, kContacts>(rec, lane, StagedRows{slab_addr + lane * 4, bar, 0u}, StagedAcc{slab_addr + prestep_bytes + lane * 4, rec.impulses + lane}, enc0,
-                                                          enc1, B, fp, early, peers, boundary ? peer_delta : 0);
+                                                          enc1, B, fp, integrated, early, peers, boundary ? peer_delta : 0);
         if constexpr (kSharded) {
             if (boundary) {
                 __syncwarp();                  // every lane's peer stores are ordered before ...

@@ -259,15 +259,21 @@ StageProgram build_stage_program(const TopologyPlan& plan, const std::vector<int
         warm_start_bytes.push_back(work_bytes(bw.begin, bw.count, &TypeInfo::warm_start_bytes));
         solve_bytes.push_back(work_bytes(bw.begin, bw.count, &TypeInfo::solve_bytes));
     }
-    auto batch_stages = [&](int32_t stage) {
+    auto batch_stages = [&](int32_t stage, int32_t flags) {
         // in peer mode every rank runs the exchange point of every batch, also of one it has no constraint in
         for (size_t b = 0; b < plan.batches.size(); ++b) {
             const TopologyPlan::Batch& bw = plan.batches[b];
             if (bw.count > 0 || (peer_mode && (int)b < plan.sync_batch_count))
-                push(stage, bw.begin, bw.count, peer_mode ? (int32_t)b : kNoExchange, bw.contacts_only ? kLaunchContactsOnly : 0,
+                push(stage, bw.begin, bw.count, peer_mode ? (int32_t)b : kNoExchange, flags | (bw.contacts_only ? kLaunchContactsOnly : 0),
                      stage == kStageSolve ? solve_bytes[b] : warm_start_bytes[b]);
         }
     };
+    // In substeps > 0 the incremental contact update integrates the pose and world inertia of every body that a constraint lane integrates, and
+    // the WarmStart stages only integrate velocity. That update is exact there: a body's pose update depends on its pose, its local inertia and its
+    // velocity at the start of the substep, and nothing writes those between the start of the substep and the WarmStart of the body's first batch
+    // (the incremental update writes rows, the kinematic pass kinematic bodies, and earlier batches do not reference the body). Peer-sharded
+    // solves keep the integration in the owning lane, which also pushes the new records to the peers.
+    const int32_t bodies_integrated = plan.inc_count > 0 && !peer_mode ? kLaunchBodiesIntegrated : 0;
     const int64_t incremental_bytes = work_bytes(plan.inc_begin, plan.inc_count, &TypeInfo::incremental_bytes);
     const int64_t kinematic_bytes = (int64_t)kinematic_count * 108;  // per-body passes: 108 bytes per body
     const int substeps = (int)iterations.size();
@@ -275,7 +281,7 @@ StageProgram build_stage_program(const TopologyPlan& plan, const std::vector<int
         if (s > 0) {
             // peer sharding: what peers pushed in the last Solve stages must have arrived before the contact update reads velocities
             if (peer_mode) push(kStageKinematic, 0, 0, kRankBarrier, 0, 0);
-            if (plan.inc_count > 0) push(kStageIncremental, plan.inc_begin, plan.inc_count, kNoExchange, 0, incremental_bytes);
+            if (plan.inc_count > 0) push(kStageIncremental, plan.inc_begin, plan.inc_count, kNoExchange, bodies_integrated, incremental_bytes);
             if (kinematic_count > 0) push(kStageKinematic, 0, kinematic_count, kNoExchange, 0, kinematic_bytes);
         } else if (integrate_velocity_for_kinematics && kinematic_count > 0) {
             push(kStageKinematicFirst, 0, kinematic_count, kNoExchange, 0, kinematic_bytes);
@@ -283,8 +289,9 @@ StageProgram build_stage_program(const TopologyPlan& plan, const std::vector<int
         // all ranks meet before the first stage of a substep's WarmStart: after every peer's last Solve stage has completed, before any peer's
         // WarmStart stage stores into this rank's arrays
         if (peer_mode) push(kStageKinematic, 0, 0, kRankBarrier, 0, 0);
-        batch_stages(s == 0 ? kStageWarmStartFirst : kStageWarmStart);
-        for (int it = 0; it < iterations[(size_t)s]; ++it) batch_stages(kStageSolve);
+        if (s == 0) batch_stages(kStageWarmStartFirst, 0);
+        else batch_stages(kStageWarmStart, bodies_integrated);
+        for (int it = 0; it < iterations[(size_t)s]; ++it) batch_stages(kStageSolve, 0);
     }
     if (peer_mode) push(kStageKinematic, 0, 0, kRankBarrier, 0, 0);  // ... and before the final pose pass reads them
     push(kStageFinalPose, 0, body_count, kNoExchange, 0, (int64_t)body_count * 108);

@@ -68,7 +68,7 @@ struct StageOp {
     int32_t work_count;       // warps of work (constraint stages), bodies (final pose), kinematics (kinematic stages)
     int32_t exchange;         // peer sharding: kRankBarrier, the device batch of a sharded WarmStart / Solve stage, or kNoExchange
     uint32_t exchange_index;  // exchange points before this op in the solve (FrameParams::exchange_base, ShardStage)
-    int32_t launch_flags;     // kLaunchContactsOnly | kLaunchPrefetchRows | kLaunchPrefetchBodies
+    int32_t launch_flags;     // kLaunchContactsOnly | kLaunchPrefetchRows | kLaunchPrefetchBodies | kLaunchBodiesIntegrated
     int64_t algorithmic_bytes;  // SURVEY.md §8d bytes of the stage
 };
 constexpr int32_t kNoExchange = -1, kRankBarrier = -2;

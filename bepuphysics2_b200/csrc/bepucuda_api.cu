@@ -284,7 +284,9 @@ void issue_stage_sequence(bepucuda_ctx* ctx, cudaStream_t s, int64_t* launches, 
                 // a sharded stage stores the records it writes for shared bodies into the ranks that reference them, and its boundary bundles wait
                 // for and announce arrivals themselves (ShardStage)
                 shard.stage.exchange_index = op.exchange_index;
-                const int flags = (profile ? op.launch_flags & kLaunchContactsOnly : kLaunchPdl | op.launch_flags) | extensions;
+                // with per-body accelerations or point gravity the WarmStart stages keep the pose integration (warm_start_body)
+                const int op_flags = extensions ? op.launch_flags & ~kLaunchBodiesIntegrated : op.launch_flags;
+                const int flags = (profile ? op_flags & (kLaunchContactsOnly | kLaunchBodiesIntegrated) : kLaunchPdl | op_flags) | extensions;
                 ctx->launchers->constraint_stage(op.stage, records + op.work_begin, ref_rows + (size_t)op.work_begin * 64, op.work_count, ctx->B, fp, flags,
                                                  op.exchange == kNoExchange ? nullptr : &shard, s);
             } else if (op.stage <= kStageKinematic) {
@@ -618,9 +620,10 @@ int32_t bepucuda_upload_bodies(bepucuda_ctx* ctx, const void* body_dynamics, int
     B.inertia_local = ctx->inertia_local.as<float4>();
     B.inertia_world = ctx->inertia_world.as<float4>();
     B.constrained = ctx->constrained.as<uint8_t>();
+    B.first_batch = ctx->first_batch.as<int32_t>();
     B.count = body_count;
     if (B.pose != ctx->B.pose || B.velocity != ctx->B.velocity || B.inertia_local != ctx->B.inertia_local || B.inertia_world != ctx->B.inertia_world ||
-        B.constrained != ctx->B.constrained || B.count != ctx->B.count)
+        B.constrained != ctx->B.constrained || B.first_batch != ctx->B.first_batch || B.count != ctx->B.count)
         invalidate_graph(ctx);  // kernel arguments are baked into graph nodes
     ctx->B = B;
     if (body_count > 0) {
@@ -750,6 +753,7 @@ int32_t bepucuda_end_constraints(bepucuda_ctx* ctx) {
     CK(ctx->first_batch.reserve(nb * 4));
     CK(ctx->sync_refcount.reserve(nb * 4));
     CK(ctx->sync_mask.reserve(nb * 8));
+    ctx->B.first_batch = ctx->first_batch.as<int32_t>();  // the graph is re-captured below (upload_program)
     launch_fill_i32(ctx->first_batch.as<int32_t>(), nb, 0x7fffffff, ctx->stream);
     CK(cudaMemsetAsync(ctx->sync_refcount.ptr, 0, nb * 4, ctx->stream));
     CK(cudaMemsetAsync(ctx->sync_mask.ptr, 0, nb * 8, ctx->stream));
