@@ -84,6 +84,23 @@ enum Stage : int32_t {
     kStageFinalPose = 6,
 };
 
+// How one stage is launched, decided on the host by resolve_stage_launch (bepu_topology.h) and obeyed as is by the stage kernels.
+// Which instantiation of a constraint stage runs:
+enum StageKernel : int32_t {
+    kKernelFull = 0,      // the full type switch, uncapped
+    kKernelContacts = 1,  // the contact types only, at the contact-only register budget (never sharded)
+    kKernelDeep = 2,      // the full type switch at the deep register budget (batches of kDeepBatchBundles bundles or more)
+};
+// Launch flags:
+//   kLaunchPdl: programmatic stream serialization, the kernel runs its prologue while its predecessor finishes;
+//   kLaunchPrefetchRows: the prologue fetches the bundle's prestep and impulse rows;
+//   kLaunchIntegratorExtensions: per-body accelerations or point gravity; the WarmStart stages and the per-body passes run the kExt instantiation;
+//   kLaunchEarlyWorld: the prologue loads world inertia of body slots 0 and 1, and pose for kNeedsPose types (Solve, and flagged contact-only WarmStart);
+//   kLaunchEarlyOwned: the prologue loads local inertia and pose of the integrating slots among 0 and 1 (WarmStartFirst / WarmStart);
+//   kLaunchBodiesIntegrated: the incremental contact update of this substep integrates the pose and world inertia of every body a constraint lane
+//   integrates, one thread per body, and the WarmStart stages integrate velocity only.
+constexpr int32_t kLaunchPdl = 1, kLaunchPrefetchRows = 2, kLaunchIntegratorExtensions = 4, kLaunchEarlyWorld = 8, kLaunchEarlyOwned = 16, kLaunchBodiesIntegrated = 32;
+
 // One entry per warp of a stage launch: which bundle of which device type batch.
 struct WorkItem {
     int32_t type_batch;

@@ -56,7 +56,6 @@ void launch_boundary_flags(const WorkRecord* records, int count, const int32_t* 
 void launch_pack_ref_rows(const WorkRecord* records, int count, int32_t* rows, cudaStream_t s);
 
 // Numerics flavours (bepu_solver_kernels.cu, compiled twice).
-constexpr int kLaunchPdl = 1, kLaunchPrefetchRows = 2, kLaunchIntegratorExtensions = 4, kLaunchContactsOnly = 8, kLaunchPrefetchBodies = 16, kLaunchBodiesIntegrated = 32;
 // Peer-sharded stage (bepucuda_shard_*): every written body record also goes to the ranks named by the per-(lane, slot) destination masks at
 // refs + peer_delta (launch_fill_peer_masks).
 struct ShardLaunch {
@@ -65,20 +64,13 @@ struct ShardLaunch {
     ShardStage stage;
 };
 struct SolverLaunchers {
-    // Launches one constraint stage (kStageWarmStartFirst / kStageWarmStart / kStageSolve / kStageIncremental) over `work_count` bundles.
-    // launch_flags: kLaunchPdl = launch with programmatic stream serialization (the kernel overlaps its prologue with the previous stage);
-    // kLaunchPrefetchRows = the kernel launched just before this one writes neither this batch's prestep nor its impulses, so the prologue may fetch them.
-    // kLaunchIntegratorExtensions = per-body accelerations or point gravity are set: the WarmStart stages run the instantiation that applies them.
-    // kLaunchContactsOnly = every bundle of the batch is a contact: the WarmStart / Solve stage runs the contact-only instantiation (not sharded).
-    // kLaunchPrefetchBodies = the kernel launched just before this one is a stage of this solve and not the WarmStart of this batch, so the prologue
-    // may load the body records it does not write (constraint_stage_body).
-    // kLaunchBodiesIntegrated (substeps > 0, FrameParams::angular_mode 0): the incremental contact update also integrates the pose and rotates the
-    // world inertia of every body a constraint lane integrates, one thread per body, and the WarmStart stages leave that part to it.
+    // Launches one constraint stage (kStageWarmStartFirst / kStageWarmStart / kStageSolve / kStageIncremental) over `work_count` bundles, in the
+    // instantiation `kernel` (StageKernel) with the launch flags that resolve_stage_launch (bepu_topology.h) chose for it.
     // ref_rows: the packed reference rows of records[0 .. work_count) (launch_pack_ref_rows).
     // shard: nullptr on a single GPU; a WarmStartFirst / WarmStart / Solve stage of a peer-sharded solve otherwise.
-    void (*constraint_stage)(int stage, const WorkRecord* records, const int32_t* ref_rows, int work_count, const BodyBuffers& B, const FrameParams* fp, int launch_flags,
-                             const ShardLaunch* shard, cudaStream_t s);
-    // launch_flags: kLaunchIntegratorExtensions or 0 (the other bits do not apply to the per-body passes)
+    void (*constraint_stage)(int stage, int kernel, const WorkRecord* records, const int32_t* ref_rows, int work_count, const BodyBuffers& B, const FrameParams* fp,
+                             int launch_flags, const ShardLaunch* shard, cudaStream_t s);
+    // launch_flags: kLaunchIntegratorExtensions or 0
     void (*kinematic_stage)(int stage, const int32_t* kinematics, int count, const BodyBuffers& B, const FrameParams* fp, int launch_flags, cudaStream_t s);
     void (*final_pose)(const BodyBuffers& B, const FrameParams* fp, int launch_flags, cudaStream_t s);
 };

@@ -85,8 +85,8 @@ BEPU_DI void apply_velocity_extensions(const FrameParams& fp, uint32_t idx, V3 p
 }
 
 // Body records of body slots 0 and 1 that a plain stage kernel loaded before its grid-dependency wait (see constraint_stage_body); bit s of
-// `slots` is set when slot s was loaded. Solve: world inertia, and pose for kNeedsPose types. WarmStart: local inertia and pose of an integrating slot;
-// with kStageBodiesIntegrated, world inertia of every slot instead.
+// `slots` is set when slot s was loaded. kLaunchEarlyWorld: world inertia, and pose for kNeedsPose types. kLaunchEarlyOwned: local inertia and
+// pose of an integrating slot.
 struct EarlyBodies {
     uint32_t slots;
     Inertia inertia[2];
@@ -98,10 +98,9 @@ struct EarlyBodies {
 // device body reference carries kRefIntegrateBit; all other lanes read the world inertia their owner constraint stored earlier in this substep,
 // which is bit-identical to what the reference's bundle-wide recompute would give them. kExt: the stage kernel instantiation for contexts with
 // per-body accelerations or point gravity (the launcher picks it), so that the default path carries none of it.
-// integrated: a WarmStart stage whose pose half the incremental contact update of this substep has done (kStageBodiesIntegrated, angular mode 0,
+// integrated: a WarmStart stage whose pose half the incremental contact update of this substep has done (kLaunchBodiesIntegrated,
 // integrate_body_pose): the integrating lane reads the pose and world inertia that update stored and integrates the velocity only. Never in the
-// kExt instantiations: the host does not pass the flag to contexts with per-body accelerations or point gravity, since the pose the point-gravity
-// term reads would take the contact-only kExt WarmStart kernel past its register budget.
+// kExt instantiations (resolve_stage_launch).
 template <int STAGE, bool NeedsPose, bool kExt>
 BEPU_DI void warm_start_body(uint32_t enc, const BodyBuffers& B, const FrameParams& fp, bool integrated, bool early_slot, const EarlyBodies& early, int s, BodyState& b,
                              Velocity& v) {
@@ -301,8 +300,7 @@ BEPU_DI WorkRecord load_record(const WorkRecord* r) {
     X(8, NonconvexOneBody<2>) X(9, NonconvexOneBody<3>) X(10, NonconvexOneBody<4>)                                                \
     X(15, NonconvexTwoBody<2>) X(16, NonconvexTwoBody<3>) X(17, NonconvexTwoBody<4>)
 
-// kContacts: the switch covers the contact types only. The host launches that instantiation for device batches whose every bundle is a contact
-// (kLaunchContactsOnly); it is about half the code of the full switch and fits a smaller register budget (bepu_solver_kernels.cu).
+// kContacts: the switch covers the contact types only (kKernelContacts, for device batches whose every bundle is a contact); it is about half the code of the full switch and fits a smaller register budget (bepu_solver_kernels.cu).
 template <int STAGE, bool kSharded, bool kExt, bool kContacts, class PR, class AR>
 BEPU_DI void run_bundle_rows(const WorkRecord& rec, int lane, PR p, AR a, uint32_t enc0, uint32_t enc1, const BodyBuffers& B, const FrameParams& fp, bool integrated,
                              const EarlyBodies& early, const ShardPeers* peers = nullptr, long long peer_delta = 0) {
@@ -385,21 +383,9 @@ constexpr int kStageBlockThreads = BEPU_STAGE_BLOCK_THREADS;
 // Programmatic dependent launch, with the trigger placed AFTER this kernel's own wait: the next stage's grid can start once every CTA here has
 // passed `griddepcontrol.wait`, i.e. once the PREVIOUS stage has completed and flushed. So while a kernel runs its pre-wait prologue, everything
 // older than its immediate predecessor is final, and the prologue may read whatever that one predecessor does not write: the work record and
-// body references (immutable during a solve) always, and -- when the host says so (kStagePrefetchRows: the predecessor is neither the incremental
-// contact update, which rewrites depth rows, nor a stage of this same batch, which rewrites these impulses) -- the whole row block. That takes the
-// bulk copy's latency off the critical path; after the wait only the body gather, the math and the scatter remain.
-//
-// The body records of slots 0 and 1 that the immediate predecessor cannot write are loaded in the prologue too (plain kernels, kStagePrefetchBodies:
-// the predecessor is a stage of this solve and not the WarmStart of this same batch), so that the post-wait gather is the velocities alone:
-//   - WarmStart, integrating slot: local inertia (never written during a solve) and pose (written only by this batch's own WarmStart, a substep ago);
-//   - Solve: world inertia (and pose for kNeedsPose types), written only by the WarmStart stages of batches up to this one.
-// Sharded kernels load every body record after the wait: a peer's stores are only known to have arrived after shard_wait.
-// A WarmStart stage with kStageBodiesIntegrated (angular mode 0) writes no world inertia and no pose: the incremental contact update at the start
-// of the substep wrote them for every integrated body, and nothing else writes them before the substep's Solve stages. So such a stage loads the
-// world inertia of slots 0 and 1, for integrating and other lanes alike, before its wait, like a Solve stage, whenever its predecessor is not that
-// update (kStagePrefetchRows: behind a WarmStart stage of an earlier batch or the kinematic pass, which writes kinematic poses and velocities
-// only). Contact-only kernels only: no contact type reads a pose. Otherwise the flagged stage loads no body record before the wait.
-constexpr int kStagePrefetchRows = 1, kStagePrefetchBodies = 2, kStageBodiesIntegrated = 4;
+// body references (immutable during a solve) always, and what the launch flags say (resolve_stage_launch, DESIGN §3): the whole row block
+// (kLaunchPrefetchRows), which takes the bulk copy's latency off the critical path, and the body records of slots 0 and 1 (kLaunchEarlyWorld /
+// kLaunchEarlyOwned), so that the post-wait gather is the velocities alone.
 template <int STAGE, bool kContacts>
 BEPU_DI void load_early_bodies(int type_id, uint32_t enc0, uint32_t enc1, const BodyBuffers& B, EarlyBodies& e) {
     if ((int32_t)enc0 == kRefEmpty) return;
@@ -440,7 +426,7 @@ BEPU_DI void shard_wait(const ShardPeers& peers, int lane, uint32_t solve_index,
     }
     __syncwarp();
 }
-// Body part of the incremental contact update (kStageBodiesIntegrated, angular mode 0): thread i does the pose half of IntegratePoseAndVelocity
+// Body part of the incremental contact update (kLaunchBodiesIntegrated): thread i does the pose half of IntegratePoseAndVelocity
 // for body i if a constraint lane integrates it (first_batch set; kinematic bodies have none), so that the WarmStart stage of the body's first
 // batch only integrates its velocity. The velocity is loaded after the wait: the predecessor, the last stage of the previous substep, writes it.
 // Pose and local inertia are loaded before it: no stage that can precede an incremental update writes them (Solve writes velocities and
@@ -448,7 +434,7 @@ BEPU_DI void shard_wait(const ShardPeers& peers, int lane, uint32_t solve_index,
 // writes kinematic poses, is older than that predecessor).
 BEPU_DI void integrate_body_pose(int i, const BodyBuffers& B, const FrameParams* __restrict__ fpp) {
     const FrameParams fp = *fpp;
-    const bool owned = i < B.count && fp.angular_mode == 0 && (int32_t)ldg_nc_u32(B.first_batch + i) != 0x7fffffff;
+    const bool owned = i < B.count && (int32_t)ldg_nc_u32(B.first_batch + i) != 0x7fffffff;
     Inertia local;
     V3 pos;
     Q4 q;
@@ -473,7 +459,7 @@ BEPU_DI void constraint_stage_body(const WorkRecord* __restrict__ records, const
     constexpr bool kStaged = STAGE != kStageIncremental;
     constexpr int kWarps = kStageBlockThreads / 32;
     if constexpr (STAGE == kStageIncremental) {
-        // the CTAs past the bundles' (launch_stage_instance adds them with kStageBodiesIntegrated) hold one thread per body
+        // the CTAs past the bundles' (launch_stage adds them with kLaunchBodiesIntegrated) hold one thread per body
         const int bundle_blocks = (work_count + kWarps - 1) / kWarps;
         if ((int)blockIdx.x >= bundle_blocks) return integrate_body_pose(((int)blockIdx.x - bundle_blocks) * kStageBlockThreads + (int)threadIdx.x, B, fpp);
     }
@@ -488,7 +474,7 @@ BEPU_DI void constraint_stage_body(const WorkRecord* __restrict__ records, const
     const bool active = warp < work_count;
     const uint32_t slab_addr = kStaged ? smem_u32(slab) + warp_in_block * kStageSlabBytes : 0;
     const uint32_t bar = smem_u32(&bars[warp_in_block]);
-    const bool early_rows = kStaged && (flags & kStagePrefetchRows);
+    const bool early_rows = kStaged && (flags & kLaunchPrefetchRows);
     uint32_t prestep_bytes = 0, impulse_bytes = 0;
     EarlyBodies early{};
     if (active) {
@@ -510,17 +496,16 @@ BEPU_DI void constraint_stage_body(const WorkRecord* __restrict__ records, const
         enc0 = ldg_nc_u32(ref_rows + (size_t)warp * (2 * kLanes) + lane);
         enc1 = ldg_nc_u32(ref_rows + (size_t)warp * (2 * kLanes) + kLanes + lane);
         if constexpr (kStaged && kEarlyBodies) {
-            if (flags & kStagePrefetchBodies) {
-                if (!(flags & kStageBodiesIntegrated)) load_early_bodies<STAGE, kContacts>(rec.type_id, enc0, enc1, B, early);
-                else if (STAGE == kStageWarmStart && kContacts && !kExt && (flags & kStagePrefetchRows) && fpp->angular_mode == 0)
-                    load_early_bodies<kStageSolve, kContacts>(rec.type_id, enc0, enc1, B, early);  // world inertia of every slot, as a Solve stage does
-            }
+            // world mode on a WarmStart only in the instantiation the host launches it in: contact-only, without kExt
+            constexpr bool kWorld = STAGE == kStageSolve || (STAGE == kStageWarmStart && kContacts && !kExt), kOwned = STAGE != kStageSolve;
+            if (kOwned && (flags & kLaunchEarlyOwned)) load_early_bodies<STAGE, kContacts>(rec.type_id, enc0, enc1, B, early);
+            else if (kWorld && (flags & kLaunchEarlyWorld)) load_early_bodies<kStageSolve, kContacts>(rec.type_id, enc0, enc1, B, early);
         }
     }
     const FrameParams fp = *fpp;
     asm volatile("griddepcontrol.wait;" ::: "memory");
     asm volatile("griddepcontrol.launch_dependents;");
-    const bool integrated = STAGE == kStageWarmStart && !kExt && (flags & kStageBodiesIntegrated) && fp.angular_mode == 0;
+    const bool integrated = STAGE == kStageWarmStart && !kExt && (flags & kLaunchBodiesIntegrated);
     bool boundary = false;
     if constexpr (kSharded) {
         boundary = active && (rec.live_lanes & kRecordBoundaryBit) != 0;
@@ -550,7 +535,7 @@ BEPU_DI void constraint_stage_body(const WorkRecord* __restrict__ records, const
 }
 
 // The pre-wait body loads are compiled into the uncapped and the contact-only budgets. The deep budget (full switch at 80 registers) would spill
-// with them, and a batch several waves deep has only its first wave's CTAs in a prologue while the predecessor runs.
+// with them, and a batch several waves deep has only its first wave's CTAs in a prologue while the predecessor runs; the host never asks for them there.
 template <int STAGE, int MINB, bool kExt, bool kContacts>
 __global__ void __launch_bounds__(kStageBlockThreads, MINB) constraint_stage_kernel(const WorkRecord* __restrict__ records, const int32_t* __restrict__ ref_rows, int work_count, BodyBuffers B, const FrameParams* __restrict__ fpp, int flags) {
     constraint_stage_body<STAGE, false, kExt, kContacts, MINB == 1 || kContacts>(records, ref_rows, work_count, B, fpp, flags, nullptr, 0);

@@ -264,16 +264,12 @@ StageProgram build_stage_program(const TopologyPlan& plan, const std::vector<int
         for (size_t b = 0; b < plan.batches.size(); ++b) {
             const TopologyPlan::Batch& bw = plan.batches[b];
             if (bw.count > 0 || (peer_mode && (int)b < plan.sync_batch_count))
-                push(stage, bw.begin, bw.count, peer_mode ? (int32_t)b : kNoExchange, flags | (bw.contacts_only ? kLaunchContactsOnly : 0),
+                push(stage, bw.begin, bw.count, peer_mode ? (int32_t)b : kNoExchange, flags | (bw.contacts_only ? kOpContactsOnly : 0),
                      stage == kStageSolve ? solve_bytes[b] : warm_start_bytes[b]);
         }
     };
-    // In substeps > 0 the incremental contact update integrates the pose and world inertia of every body that a constraint lane integrates, and
-    // the WarmStart stages only integrate velocity. That update is exact there: a body's pose update depends on its pose, its local inertia and its
-    // velocity at the start of the substep, and nothing writes those between the start of the substep and the WarmStart of the body's first batch
-    // (the incremental update writes rows, the kinematic pass kinematic bodies, and earlier batches do not reference the body). Peer-sharded
-    // solves keep the integration in the owning lane, which also pushes the new records to the peers.
-    const int32_t bodies_integrated = plan.inc_count > 0 && !peer_mode ? kLaunchBodiesIntegrated : 0;
+    // peer-sharded solves keep the integration in the owning lane, which also pushes the new records to the peers
+    const int32_t integrable = plan.inc_count > 0 && !peer_mode ? kOpIntegrable : 0;
     const int64_t incremental_bytes = work_bytes(plan.inc_begin, plan.inc_count, &TypeInfo::incremental_bytes);
     const int64_t kinematic_bytes = (int64_t)kinematic_count * 108;  // per-body passes: 108 bytes per body
     const int substeps = (int)iterations.size();
@@ -281,7 +277,7 @@ StageProgram build_stage_program(const TopologyPlan& plan, const std::vector<int
         if (s > 0) {
             // peer sharding: what peers pushed in the last Solve stages must have arrived before the contact update reads velocities
             if (peer_mode) push(kStageKinematic, 0, 0, kRankBarrier, 0, 0);
-            if (plan.inc_count > 0) push(kStageIncremental, plan.inc_begin, plan.inc_count, kNoExchange, bodies_integrated, incremental_bytes);
+            if (plan.inc_count > 0) push(kStageIncremental, plan.inc_begin, plan.inc_count, kNoExchange, integrable, incremental_bytes);
             if (kinematic_count > 0) push(kStageKinematic, 0, kinematic_count, kNoExchange, 0, kinematic_bytes);
         } else if (integrate_velocity_for_kinematics && kinematic_count > 0) {
             push(kStageKinematicFirst, 0, kinematic_count, kNoExchange, 0, kinematic_bytes);
@@ -290,7 +286,7 @@ StageProgram build_stage_program(const TopologyPlan& plan, const std::vector<int
         // WarmStart stage stores into this rank's arrays
         if (peer_mode) push(kStageKinematic, 0, 0, kRankBarrier, 0, 0);
         if (s == 0) batch_stages(kStageWarmStartFirst, 0);
-        else batch_stages(kStageWarmStart, bodies_integrated);
+        else batch_stages(kStageWarmStart, integrable);
         for (int it = 0; it < iterations[(size_t)s]; ++it) batch_stages(kStageSolve, 0);
     }
     if (peer_mode) push(kStageKinematic, 0, 0, kRankBarrier, 0, 0);  // ... and before the final pose pass reads them
@@ -302,16 +298,11 @@ StageProgram build_stage_program(const TopologyPlan& plan, const std::vector<int
         if (op.exchange != kNoExchange) ++prog.exchange_count;
         if (op.exchange == kRankBarrier) continue;
         if (op.stage <= kStageIncremental) {
-            // Row prefetch in the PDL prologue (constraint_stage_kernel): allowed when the stage launched immediately before neither rewrites this
-            // stage's prestep rows (the incremental contact update does) nor its impulses (a stage of the same batch does: single-batch scenes).
+            // what the PDL prologue may read (DESIGN §3): not what the op launched just before writes
             if (op.stage != kStageIncremental && previous && previous->stage != kStageIncremental && !(previous->stage <= kStageSolve && previous->work_begin == op.work_begin))
-                op.launch_flags |= kLaunchPrefetchRows;
-            // Body-record loads in the PDL prologue (constraint_stage_body): allowed for a WarmStart / Solve stage when the stage launched immediately
-            // before belongs to this solve (what ran before the solve, such as a body upload, has no stage to order against) and is not the WarmStart
-            // of the same batch, the only stage that writes the records these loads read: world inertia and pose of this batch's bodies, the pose
-            // of an integrating one.
+                op.launch_flags |= kOpRowsFree;
             if (op.stage <= kStageSolve && previous && !(previous->stage <= kStageWarmStart && previous->work_begin == op.work_begin))
-                op.launch_flags |= kLaunchPrefetchBodies;
+                op.launch_flags |= kOpBodiesFree;
         }
         if (op.stage == kStageFinalPose ? body_count > 0 : op.work_count > 0) previous = &op;
         if (op.work_count > 0 || op.stage == kStageFinalPose) ++prog.stage_count;
@@ -321,6 +312,28 @@ StageProgram build_stage_program(const TopologyPlan& plan, const std::vector<int
     for (int32_t n : iterations) iterations_per_constraint += n;
     prog.constraint_iterations = plan.constraint_count * iterations_per_constraint;
     return prog;
+}
+
+StageLaunch resolve_stage_launch(const StageOp& op, const LaunchContext& lc) {
+    const int32_t ext = lc.integrator_extensions ? kLaunchIntegratorExtensions : 0;
+    if (op.stage > kStageIncremental) return {kKernelFull, ext};  // the per-body passes
+    const bool sharded = op.exchange != kNoExchange;
+    StageLaunch l{kKernelFull, 0};
+    if (op.stage != kStageIncremental && op.work_count >= kDeepBatchBundles) l.kernel = kKernelDeep;
+    else if ((op.launch_flags & kOpContactsOnly) && !sharded) l.kernel = kKernelContacts;
+    if (op.stage == kStageWarmStartFirst || op.stage == kStageWarmStart) l.flags |= ext;
+    // The momentum-conserving angular modes need the orientation before the update in the owning lane; the point-gravity term reads the pose, and
+    // loading it took the contact-only kExt WarmStart kernel past its register budget.
+    if ((op.launch_flags & kOpIntegrable) && lc.angular_mode == 0 && !ext) l.flags |= kLaunchBodiesIntegrated;
+    if (lc.profile) return l;
+    l.flags |= kLaunchPdl | ((op.launch_flags & kOpRowsFree) ? kLaunchPrefetchRows : 0);
+    // No body record before the wait on sharded kernels (a peer's stores are known to have arrived only after shard_wait) nor on deep ones (the
+    // loads would spill there). A flagged WarmStart writes no pose and no world inertia, so the contact-only one loads world inertia like a Solve
+    // stage unless its predecessor is the incremental update (which row prefetch excludes); no contact type reads a pose.
+    if (!(op.launch_flags & kOpBodiesFree) || sharded || l.kernel == kKernelDeep) return l;
+    if (!(l.flags & kLaunchBodiesIntegrated)) l.flags |= op.stage == kStageSolve ? kLaunchEarlyWorld : kLaunchEarlyOwned;
+    else if (l.kernel == kKernelContacts && (l.flags & kLaunchPrefetchRows)) l.flags |= kLaunchEarlyWorld;
+    return l;
 }
 
 int exchange_targets(const StageProgram& program, const std::vector<int32_t>& boundary_count, std::vector<unsigned long long>* targets, std::string* error) {

@@ -1,7 +1,7 @@
 // Constraint topology of libbepucuda, decided on the host without the CUDA runtime: the type registry, which device batch every constraint
 // runs in (synchronized batches, then the dependency levels of the sequential fallback batch), the work list the stage kernels walk, and the
-// stage program of one solve with the launch flags of every stage. bepucuda_api.cu turns a plan into device tables; tests/test_topology.py
-// checks plans on the CPU.
+// stage program of one solve, and how each of its stages is launched. bepucuda_api.cu turns a plan into device tables; tests/test_topology.py
+// checks plans and launches on the CPU.
 #pragma once
 #include <string>
 #include <vector>
@@ -68,10 +68,38 @@ struct StageOp {
     int32_t work_count;       // warps of work (constraint stages), bodies (final pose), kinematics (kinematic stages)
     int32_t exchange;         // peer sharding: kRankBarrier, the device batch of a sharded WarmStart / Solve stage, or kNoExchange
     uint32_t exchange_index;  // exchange points before this op in the solve (FrameParams::exchange_base, ShardStage)
-    int32_t launch_flags;     // kLaunchContactsOnly | kLaunchPrefetchRows | kLaunchPrefetchBodies | kLaunchBodiesIntegrated
+    int32_t launch_flags;     // kOp* below: facts about the op, from which resolve_stage_launch derives its launch
     int64_t algorithmic_bytes;  // SURVEY.md §8d bytes of the stage
 };
 constexpr int32_t kNoExchange = -1, kRankBarrier = -2;
+// Facts about a constraint op:
+//   kOpRowsFree: the op launched just before it writes neither this batch's prestep rows (the incremental contact update does) nor its impulses (a
+//   stage of the same batch does);
+//   kOpContactsOnly: every bundle of the device batch is a contact;
+//   kOpBodiesFree: the op launched just before it is a stage of this solve and not the WarmStart of the same batch, the only stage that writes
+//   the world inertia and pose of this batch's bodies, and the pose of those it integrates;
+//   kOpIntegrable: the incremental op and the WarmStart ops of substeps > 0 of a solve with contacts that is not peer-sharded. Their pose half of
+//   the integration may move from the WarmStart stages to the incremental update: a body's pose update depends on its pose, its local inertia and
+//   its velocity at the start of the substep, and nothing writes those between the start of the substep and the WarmStart of the body's first
+//   batch (the incremental update writes rows, the kinematic pass kinematic bodies, and earlier batches do not reference the body).
+constexpr int32_t kOpRowsFree = 2, kOpContactsOnly = 8, kOpBodiesFree = 16, kOpIntegrable = 32;
+// WarmStartFirst / WarmStart / Solve ops of at least this many bundles run the deep kernel (the deep budget in bepu_solver_kernels.cu, which
+// checks its copy of the threshold against this one).
+constexpr int32_t kDeepBatchBundles = 2150;
+
+// What a launch depends on besides its op. A captured graph bakes the resolved launches in, so it is rebuilt when any of these changes.
+struct LaunchContext {
+    bool integrator_extensions;  // per-body accelerations or point gravity are set
+    int32_t angular_mode;        // bepucuda_integrator_desc::angular_integration_mode
+    bool profile;                // bepucuda_profile_stages: every launch timed alone, without PDL and without prologue loads
+};
+struct StageLaunch {
+    int32_t kernel;  // StageKernel (constraint ops; kKernelFull otherwise)
+    int32_t flags;   // kLaunch*
+};
+// The one place that decides how an op of the stage program is launched: which instantiation runs, what its prologue loads before the
+// grid-dependency wait, and whether the incremental update integrates the bodies' poses.
+StageLaunch resolve_stage_launch(const StageOp& op, const LaunchContext& lc);
 
 struct StageProgram {
     std::vector<StageOp> ops;

@@ -248,8 +248,8 @@ void invalidate_graph(bepucuda_ctx* ctx) {
     ctx->graph_valid = false;
 }
 
-// Per-body accelerations or point gravity set: the WarmStart stages and the per-body passes launch the instantiations that apply them, so switching either on or
-// off changes the launch sequence (a captured graph is rebuilt); their values are frame parameters.
+// Per-body accelerations or point gravity set: an input of resolve_stage_launch, so switching either on or off changes the launch sequence (a
+// captured graph is rebuilt); their values are frame parameters.
 bool integrator_extensions(const bepucuda_ctx* ctx) { return ctx->accelerations_count >= 0 || ctx->point_gravity; }
 
 // Profiling sink of issue_stage_sequence: the launch of program op i sets launched[i] and is bracketed by events[2i] and events[2i + 1].
@@ -258,9 +258,8 @@ struct StageEvents {
     std::vector<int>& launched;
 };
 
-// Issues the whole stage sequence of one frame as individual launches on `s` (used directly in STREAM mode and under capture in GRAPH mode).
-// With `profile`, stages are launched without programmatic dependent launch and without prologue prefetch, so that each event pair times one
-// kernel alone.
+// Issues the whole stage sequence of one frame as individual launches on `s` (used directly in STREAM mode and under capture in GRAPH mode), each
+// as resolve_stage_launch says. With `profile`, each event pair times one kernel alone.
 void issue_stage_sequence(bepucuda_ctx* ctx, cudaStream_t s, int64_t* launches, const StageEvents* profile = nullptr) {
     const WorkRecord* records = ctx->record_table.as<WorkRecord>();
     const int32_t* ref_rows = ctx->ref_rows.as<int32_t>();
@@ -268,13 +267,14 @@ void issue_stage_sequence(bepucuda_ctx* ctx, cudaStream_t s, int64_t* launches, 
     const int32_t* kin = ctx->kinematics_dev.as<int32_t>();
     ShardLaunch shard{ctx->peers, (long long)(ctx->peer32.as<int32_t>() - ctx->refs32.as<int32_t>()), {0, ctx->error_dev.as<int32_t>()}};
     int64_t n = 0;
-    const int extensions = integrator_extensions(ctx) ? kLaunchIntegratorExtensions : 0;
+    const LaunchContext lc{integrator_extensions(ctx), ctx->integ.angular_integration_mode, profile != nullptr};
     for (size_t i = 0; i < ctx->program.ops.size(); ++i) {
         const StageOp& op = ctx->program.ops[i];
         const bool barrier = op.exchange == kRankBarrier;
         // A sharded stage without constraints on this rank launches nothing but still counts as an exchange point: nothing arrives from this
         // rank there, and its arrival targets say so.
         if (barrier || (op.stage == kStageFinalPose ? ctx->B.count > 0 : op.work_count > 0)) {
+            const StageLaunch launch = resolve_stage_launch(op, lc);
             if (profile) cudaEventRecord(profile->events[2 * i], s);
             if (barrier) {
                 // all ranks meet: before the first stage of a solve; around the incremental contact update, which reads the velocities of shared
@@ -284,15 +284,12 @@ void issue_stage_sequence(bepucuda_ctx* ctx, cudaStream_t s, int64_t* launches, 
                 // a sharded stage stores the records it writes for shared bodies into the ranks that reference them, and its boundary bundles wait
                 // for and announce arrivals themselves (ShardStage)
                 shard.stage.exchange_index = op.exchange_index;
-                // with per-body accelerations or point gravity the WarmStart stages keep the pose integration (warm_start_body)
-                const int op_flags = extensions ? op.launch_flags & ~kLaunchBodiesIntegrated : op.launch_flags;
-                const int flags = (profile ? op_flags & (kLaunchContactsOnly | kLaunchBodiesIntegrated) : kLaunchPdl | op_flags) | extensions;
-                ctx->launchers->constraint_stage(op.stage, records + op.work_begin, ref_rows + (size_t)op.work_begin * 64, op.work_count, ctx->B, fp, flags,
-                                                 op.exchange == kNoExchange ? nullptr : &shard, s);
+                ctx->launchers->constraint_stage(op.stage, launch.kernel, records + op.work_begin, ref_rows + (size_t)op.work_begin * 64, op.work_count, ctx->B, fp,
+                                                 launch.flags, op.exchange == kNoExchange ? nullptr : &shard, s);
             } else if (op.stage <= kStageKinematic) {
-                ctx->launchers->kinematic_stage(op.stage, kin, op.work_count, ctx->B, fp, extensions, s);
+                ctx->launchers->kinematic_stage(op.stage, kin, op.work_count, ctx->B, fp, launch.flags, s);
             } else {
-                ctx->launchers->final_pose(ctx->B, fp, extensions, s);
+                ctx->launchers->final_pose(ctx->B, fp, launch.flags, s);
             }
             if (profile) {
                 cudaEventRecord(profile->events[2 * i + 1], s);
@@ -542,6 +539,8 @@ int32_t bepucuda_set_integrator(bepucuda_ctx* ctx, const bepucuda_integrator_des
     if (!ctx || !desc) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "set_integrator: bad arguments");
     if (desc->angular_integration_mode < 0 || desc->angular_integration_mode > 2) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "set_integrator: unknown AngularIntegrationMode");
     const bool kin_changed = (desc->integrate_velocity_for_kinematics != 0) != (ctx->integ.integrate_velocity_for_kinematics != 0);
+    // whether the angular mode is 0 is an input of resolve_stage_launch, and a captured graph bakes the resolved launches in
+    if ((desc->angular_integration_mode != 0) != (ctx->integ.angular_integration_mode != 0)) invalidate_graph(ctx);
     ctx->integ = *desc;
     ctx->integ_set = true;
     if (kin_changed && ctx->constraints_ready) {

@@ -1,6 +1,6 @@
 """Pose and world-inertia integration in the incremental contact update (kLaunchBodiesIntegrated). In substeps > 0 of a solve with contacts,
 the launch of IncrementallyUpdateForSubstep carries one thread per body that integrates the pose and rotates the inverse inertia of every body a
-constraint lane integrates, and the WarmStart stages integrate velocity only. CPU: where the stage program sets the flag (topology shim of
+constraint lane integrates, and the WarmStart stages integrate velocity only. CPU: which ops the stage program marks (topology shim of
 tests/test_topology.py), and the shared pose arithmetic of csrc/bepu_integration.cuh compiled for the host against the oracle, bit for bit. GPU:
 the strict build against the oracle, bit for bit, on the scenes and schedules that exercise the split."""
 import ctypes as C
@@ -18,7 +18,6 @@ from tests import util
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 HERE = os.path.join(ROOT, "tests", "device_on_host")
 CSRC = os.path.join(ROOT, "bepuphysics2_b200", "csrc")
-BODIES_INTEGRATED = 32
 DT = 1.0 / 60.0
 f32 = np.float32
 
@@ -28,7 +27,7 @@ shim = topo.shim
 # ---- CPU: the stage program --------------------------------------------------------------------------------------------------------------------------
 
 def _flagged(ops):
-    return (ops[:, 5] & BODIES_INTEGRATED) != 0
+    return (ops[:, 5] & topo.INTEGRABLE) != 0
 
 
 @pytest.mark.parametrize("iterations", [[1], [2, 2], [0, 2, 1], [3, 0, 1, 2]])
@@ -202,3 +201,32 @@ def test_momentum_conserving_modes_keep_the_warm_start_integration(libs, angular
 @pytest.mark.gpu
 def test_joints_only_scene_bit_exact(libs):
     _parity(scenes.joint_zoo(800, 30, seed=19, kinematic_fraction=0.1), substeps=3, velocity_iterations=2, integrator=_integrator(kinematics=1))
+
+
+@pytest.mark.gpu
+def test_graph_follows_integrator_changes_between_solves(libs):
+    """A captured graph bakes in the resolved launches, whose inputs include whether the angular mode is 0 and whether per-body accelerations or
+    point gravity are set. One context in graph mode switches the angular mode 0 -> 1 -> 0, then accelerations with point gravity on -> off,
+    between solves; every frame matches the oracle bit for bit."""
+    scene = scenes.merge(scenes.shape_pile(1500, seed=20), scenes.ragdolls(4, seed=21))
+    kw = dict(substeps=3, velocity_iterations=2, integrator=_integrator(kinematics=1))
+    a, b = util.make_sim(scene, **kw), util.make_sim(scene, **kw)
+    acc = np.random.default_rng(32).uniform(-5, 5, size=(a.body_count, 8)).astype(f32)
+    center, strength = (1.0, -40.0, 2.0), 800.0
+    ts = native.CudaTimestepper(b, strict_fp=True, execution_mode=native.EXEC_GRAPH)
+    try:
+        ts.describe()
+        for f, (angular_mode, terms) in enumerate([(0, False), (1, False), (0, False), (0, True), (0, False)]):
+            d = _integrator(kinematics=1, angular_mode=angular_mode)
+            a.set_integrator(d)
+            ts._check(ts._cuda.bepucuda_set_integrator(ts._ctx, C.byref(d)))
+            ts.set_body_accelerations(acc if terms else None)
+            ts.set_point_gravity(center if terms else None, strength if terms else 0.0)
+            ob.solve(a, DT, **(dict(accelerations=acc, center=center, strength=strength) if terms else {}))
+            if f > 0:
+                ts.refresh()
+            ts.solve(DT, download=True)
+            ts.download_prestep()
+            util.compare(util.snapshot(a), util.snapshot(b), exact=True)
+    finally:
+        ts.close()

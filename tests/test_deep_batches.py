@@ -1,7 +1,7 @@
 """Deep batches: a device batch of kDeepBatchBundles bundles or more runs its WarmStartFirst / WarmStart / Solve stages in the deep register budget
 (constraint_stage_kernel<S, BEPU_DEEP_MINB, kExt, false> in csrc/bepu_solver_kernels.cu: the full type switch at 80 registers, every body record
 gathered after the grid-dependency wait). The 100 k-body pile never gets there; the 1 M-body pile of BASELINE C4 does in its first ten batches.
-CPU: the threshold and the budget read from the source, the topology plan (the shim of tests/test_topology.py) of every scene the GPU tests below
+CPU: the threshold and the budget read from the source, the launches resolve_stage_launch gives deep ops, the topology plan (the shim of tests/test_topology.py) of every scene the GPU tests below
 solve, and the registers and stack frames of the deep kernels in the built library. GPU: the strict build against the oracle, bit for bit, on a
 mixed deep scene with every registered type and on the C4 pile; the fast build within the suite's tolerances (max abs taken at the 99.9th
 percentile at this scale, see CONTACT_TOLERANCE) and run-to-run deterministic there.
@@ -21,7 +21,6 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CSRC = os.path.join(ROOT, "bepuphysics2_b200", "csrc")
 DT = 1.0 / 60.0
 f32 = np.float32
-BODIES_INTEGRATED = 32
 WS_FIRST, WS, SOLVE = topo.WS_FIRST, topo.WS, topo.SOLVE
 
 shim = topo.shim
@@ -32,14 +31,14 @@ def _read(name):
         return f.read()
 
 
-def _source_int(pattern):
-    m = re.search(pattern, _read("bepu_solver_kernels.cu"), re.M)
+def _source_int(name, pattern):
+    m = re.search(pattern, _read(name), re.M)
     assert m, pattern
     return int(m.group(1))
 
 
-DEEP_BUNDLES = _source_int(r"^constexpr int kDeepBatchBundles = (\d+);")
-DEEP_MINB = _source_int(r"^#define BEPU_DEEP_MINB (\d+)$")
+DEEP_BUNDLES = _source_int("bepu_topology.h", r"^constexpr int32_t kDeepBatchBundles = (\d+);")
+DEEP_MINB = _source_int("bepu_solver_kernels.cu", r"^#define BEPU_DEEP_MINB (\d+)$")
 
 
 def registered_type_ids():
@@ -125,11 +124,23 @@ def _deep(p):
 
 # ---- CPU: the threshold, the plans, the budget --------------------------------------------------------------------------------------------------------
 
-def test_threshold_and_budget_come_from_the_source():
-    assert DEEP_BUNDLES > 0 and DEEP_MINB > 1
-    # every WarmStartFirst / WarmStart / Solve launch at or above the threshold takes the deep budget, contact-only or not
-    assert re.search(r"if \(work_count >= kDeepBatchBundles\) return launch_stage_variant<STAGE, BEPU_DEEP_MINB, false>", _read("bepu_solver_kernels.cu"))
+def test_threshold_and_budget_come_from_the_source(libs, shim, c4_pile):
+    assert DEEP_BUNDLES > 0 and DEEP_MINB > 1 and shim.topology_deep_batch_bundles() == DEEP_BUNDLES
     assert len(registered_type_ids()) == 44
+    # every WarmStartFirst / WarmStart / Solve op at or above the threshold resolves to the deep kernel, contact-only or not, plain or sharded,
+    # and loads no body record before its wait; the other launch rules hold on the C4 plan too
+    sim = util.make_sim(c4_pile, **C4_KW)
+    sources = topo.sim_sources(sim)
+    for peer_mode in (False, True):
+        p = topo.plan(shim, sources, sim.bundle_width, sim.fallback_batch_threshold, sim.batch_count, sim.body_count, peer_mode=peer_mode)
+        for iterations in ([2, 2, 2, 2], [0, 2, 0, 1]):
+            ops, _ = p.program(iterations, len(sim.constrained_kinematics), True, peer_mode, sim.body_count)
+            deep = (ops[:, 0] <= SOLVE) & (ops[:, 2] >= DEEP_BUNDLES)
+            assert deep.sum() >= 2 * len(iterations) and ((ops[deep, 5] & topo.CONTACTS_ONLY) != 0).all()
+            for ext, mode, profile in topo.LAUNCH_CONTEXTS:
+                kernel, flags = topo.resolve(shim, ops[deep], ext, mode, profile).T
+                assert (kernel == topo.KERNEL_DEEP).all() and not (flags & (topo.EARLY_WORLD | topo.EARLY_OWNED)).any()
+            topo.check_launches(shim, ops, peer_mode)
 
 
 def test_mixed_scene_runs_every_type_in_deep_batches(libs, shim, mixed):
@@ -148,7 +159,7 @@ def test_mixed_scene_runs_every_type_in_deep_batches(libs, shim, mixed):
     for stage in (WS_FIRST, WS, SOLVE):
         on_deep = ops[(ops[:, 0] == stage) & np.isin(ops[:, 1], list(begins)) & (ops[:, 2] >= DEEP_BUNDLES)]
         assert len(on_deep) == len(deep) * {WS_FIRST: 1, WS: len(ITERATIONS) - 1, SOLVE: sum(ITERATIONS)}[stage]
-        flagged = (on_deep[:, 5] & BODIES_INTEGRATED) != 0
+        flagged = (on_deep[:, 5] & topo.INTEGRABLE) != 0
         assert flagged.all() if stage == WS else not flagged.any(), stage
         contacts = (on_deep[:, 5] & topo.CONTACTS_ONLY) != 0
         assert contacts.any() and not contacts.all(), stage

@@ -1,7 +1,8 @@
 """The constraint topology plan without a GPU: csrc/bepu_topology.cpp (which device batch every constraint runs in, the work list, the stage
-program and its launch flags) compiled for the host with g++ behind tests/topology/topology_shim.cpp, fed with the type batches of the host mirror.
+program and how each of its stages is launched) compiled for the host with g++ behind tests/topology/topology_shim.cpp, fed with the type batches of the host mirror.
 Every property is stated from the uploaded data: coverage of the work list, the fallback levelisation of DESIGN §2 and its minimality, the stage
-order of Solver_Solve.cs:L1419-1479, the exchange sequence of a sharded graph, and the prologue prefetch rule of DESIGN §3.
+order of Solver_Solve.cs:L1419-1479, the exchange sequence of a sharded graph, the launch rules of resolve_stage_launch and the prologue prefetch
+rule of DESIGN §3.
 TEST INFRASTRUCTURE: the product never loads the shim."""
 import ctypes as C
 import os
@@ -21,7 +22,9 @@ CSRC = os.path.join(ROOT, "bepuphysics2_b200", "csrc")
 CONTACT_TYPES = set(range(11)) | {15, 16, 17}
 WS_FIRST, WS, SOLVE, INCREMENTAL, KIN_FIRST, KIN, FINAL = range(7)
 NO_EXCHANGE, RANK_BARRIER = -1, -2
-PREFETCH_ROWS, CONTACTS_ONLY, PREFETCH_BODIES = 2, 8, 16
+ROWS_FREE, CONTACTS_ONLY, BODIES_FREE, INTEGRABLE = 2, 8, 16, 32  # facts of a program op (kOp*)
+KERNEL_FULL, KERNEL_CONTACTS, KERNEL_DEEP = range(3)  # StageKernel
+PDL, ROWS, EXT, EARLY_WORLD, EARLY_OWNED, BODIES_INTEGRATED = 1, 2, 4, 8, 16, 32  # launch flags (kLaunch*)
 KINEMATIC_BIT, INDEX_MASK = 1 << 30, 0x0FFFFFFF
 ERR_INVALID_ARGUMENT, ERR_BATCH_INVARIANT, ERR_BAD_STATE = -1, -5, -6
 
@@ -47,6 +50,7 @@ def shim():
     dll.topology_program_sizes.argtypes = [vp, vp]
     dll.topology_program_ops.argtypes = [vp, vp]
     dll.topology_program_free.argtypes = [vp]
+    dll.topology_resolve.argtypes = [vp, i32, i32, i32, i32, vp]
     return dll
 
 
@@ -69,7 +73,7 @@ class Plan:
         self.dll.topology_plan_free(self.handle)
 
     def program(self, iterations, kinematic_count, integrate_velocity_for_kinematics, peer_mode, body_count):
-        """ops[n, 7]: stage, work begin, work count, exchange, exchange index, launch flags, algorithmic bytes; and the per-solve totals."""
+        """ops[n, 7]: stage, work begin, work count, exchange, exchange index, facts, algorithmic bytes; and the per-solve totals."""
         its = np.asarray(iterations, dtype=np.int32)
         h = self.dll.topology_program(self.handle, its.size, its.ctypes.data, kinematic_count, int(integrate_velocity_for_kinematics), int(peer_mode), body_count)
         s = np.zeros(5, dtype=np.int64)
@@ -93,6 +97,48 @@ def plan(dll, sources, W, threshold, batch_count, body_count, peer_mode=False):
         dll.topology_plan_free(h)
         return rc, message.value.decode()
     return Plan(dll, h)
+
+
+def resolve(dll, ops, extensions, angular_mode, profile):
+    """resolve_stage_launch for every op: [n, 2] kernel, launch flags."""
+    ops = np.ascontiguousarray(ops, dtype=np.int64)
+    out = np.zeros((len(ops), 2), dtype=np.int32)
+    dll.topology_resolve(ops.ctypes.data, len(ops), int(extensions), angular_mode, int(profile), out.ctypes.data)
+    return out
+
+
+LAUNCH_CONTEXTS = [(ext, mode, profile) for ext in (False, True) for mode in (0, 1, 2) for profile in (False, True)]
+
+
+def check_launches(dll, ops, peer_mode):
+    """The launch rules of DESIGN §3 for every op of a program, in every context (integrator extensions, angular mode, profile)."""
+    stage, count, facts = ops[:, 0], ops[:, 2], ops[:, 5]
+    sharded = (stage <= SOLVE) & (ops[:, 3] != NO_EXCHANGE)
+    deep = (stage <= SOLVE) & (count >= dll.topology_deep_batch_bundles())
+    integrating = (stage == WS_FIRST) | (stage == WS)
+    has_contacts = bool((stage == INCREMENTAL).any())
+    for ext, mode, profile in LAUNCH_CONTEXTS:
+        kernel, flags = resolve(dll, ops, ext, mode, profile).T
+        early = (flags & (EARLY_WORLD | EARLY_OWNED)) != 0
+        integrated = (flags & BODIES_INTEGRATED) != 0
+        contacts_kernel = kernel == KERNEL_CONTACTS
+        assert ((kernel == KERNEL_DEEP) == deep).all(), "deep iff a WarmStart / Solve op at or above the threshold"
+        assert (contacts_kernel == ((stage <= SOLVE) & ((facts & CONTACTS_ONLY) != 0) & ~sharded & ~deep)).all()
+        assert (((flags & EXT) != 0) == (ext & (integrating | (stage >= KIN_FIRST)))).all(), "kExt on the integrating stages only"
+        assert not (early & (deep | sharded)).any() and not (profile and early.any()), "no body record before the wait on deep, sharded or profile launches"
+        assert (((flags & PDL) != 0) == (not profile) & (stage <= INCREMENTAL)).all()
+        assert (((flags & ROWS) != 0) == (not profile) & ((facts & ROWS_FREE) != 0)).all()
+        assert (integrated == (((facts & INTEGRABLE) != 0) & (mode == 0) & (not ext))).all()
+        assert not integrated.any() or (has_contacts and not peer_mode and mode == 0 and not ext)
+        assert not (integrated & (stage != INCREMENTAL) & (stage != WS)).any(), "the incremental op and later WarmStart ops only"
+        # what each instantiation compiles: owned loads in WarmStartFirst / WarmStart, world loads in Solve and the contact-only WarmStart
+        world, owned = (flags & EARLY_WORLD) != 0, (flags & EARLY_OWNED) != 0
+        assert not (world & owned).any() and not (owned & ~integrating).any() and not (world & (stage == WS_FIRST)).any()
+        assert (integrated & contacts_kernel & ((flags & ROWS) != 0))[world & (stage == WS)].all(), "world loads on a WarmStart only behind a flagged one"
+        # and every load the program allows is made (the prologue rule test below checks that each is sound)
+        allowed = ((facts & BODIES_FREE) != 0) & ~deep & ~sharded & (not profile)
+        assert (owned == allowed & integrating & ~integrated).all()
+        assert (world == allowed & ((stage == SOLVE) | ((stage == WS) & integrated & contacts_kernel & ((flags & ROWS) != 0)))).all()
 
 
 def sim_sources(sim):
@@ -275,6 +321,27 @@ def test_every_rank_of_a_partition_runs_the_same_exchange_sequence(libs, shim, r
         assert all(s == sequences[0] for s in sequences) and len(sequences[0]) > 2 * sim.batch_count
 
 
+@pytest.mark.parametrize("case", ["mixed", "single_batch", "joints_only", "peer"])
+def test_every_launch_follows_the_rules(libs, shim, case):
+    """resolve_stage_launch on every op of the programs of these scenes, with iteration schedules that contain zeros, in every launch context."""
+    if case == "peer":
+        sim = util.make_sim(scenes.merge(scenes.shape_pile(1500, seed=13), scenes.ragdolls(4, seed=14)))
+        shards, _, _, _ = sharding.partition(sim, 2)
+        plans = [plan(shim, [(d["batch_index"], d["type_batch_index"], d["type_id"], d["count"], d["refs"]) for d in shard], sim.bundle_width,
+                      sim.fallback_batch_threshold, sim.batch_count, sim.body_count, peer_mode=True) for shard in shards]
+    else:
+        scene = {"mixed": lambda: mixed_scene(7), "single_batch": lambda: single_batch(scenes.shape_pile(800, seed=17)),
+                 "joints_only": lambda: scenes.joint_zoo(600, 20, seed=4, kinematic_fraction=0.1)}[case]()
+        sim = util.make_sim(scene, fallback_batch_threshold=6)
+        plans = [plan(shim, sim_sources(sim), 8, 6, sim.batch_count, sim.body_count)]
+    assert (plans[0].inc_count == 0) == (case == "joints_only")
+    for p in plans:
+        for iterations in ([1], [2, 2], [0, 3, 1], [0, 0], [3, 0, 1, 2]):
+            for ivk in (False, True):
+                ops, _ = p.program(iterations, len(sim.constrained_kinematics), ivk, case == "peer", sim.body_count)
+                check_launches(shim, ops, case == "peer")
+
+
 def single_batch(scene):
     """The constraints of `scene` that share no body with an earlier one: the whole scene is one batch."""
     used, kept = set(), []
@@ -292,10 +359,12 @@ def single_batch(scene):
 @pytest.mark.parametrize("case", ["mixed", "single_batch"])
 def test_prologue_prefetch_only_reads_what_the_previous_stage_does_not_write(libs, shim, case):
     """DESIGN §3: a stage's prologue runs while its immediate predecessor is still running, so it may load only what that predecessor does not write.
-    What each stage writes: WarmStart(b) the velocities of b's bodies and the pose and world inertia of those it integrates (the lowest batch that
-    references a body integrates it); Solve(b) velocities and b's impulses; the incremental update the prestep of every contact bundle; the
-    kinematic passes the kinematic bodies. What a prologue loads: rows = b's prestep and impulses; bodies = for WarmStart the pose of the bodies b
-    integrates, for Solve the world inertia and pose of the bodies in slots 0 and 1. Nothing is known about what ran before the first stage."""
+    What each stage writes: WarmStart(b) the velocities of b's bodies, and the pose and world inertia of those it integrates (the lowest batch that
+    references a body integrates it) unless its launch has kLaunchBodiesIntegrated; Solve(b) velocities and b's impulses; the incremental update the
+    prestep of every contact bundle, and with kLaunchBodiesIntegrated the pose and world inertia of every integrated body; the kinematic passes the
+    velocities and (substeps > 0) poses of the kinematic bodies. The program's facts are checked against the writes of unflagged launches. What a
+    resolved launch loads: rows = b's prestep and impulses; world = world inertia of the bodies in slots 0 and 1, and their pose unless the kernel is
+    contact-only; owned = the pose of the bodies b integrates. Nothing is known about what ran before the first stage."""
     W = 8
     scene = mixed_scene(7) if case == "mixed" else single_batch(scenes.shape_pile(800, seed=17))
     sim = util.make_sim(scene, bundle_width=W, fallback_batch_threshold=6)
@@ -323,15 +392,27 @@ def test_prologue_prefetch_only_reads_what_the_previous_stage_does_not_write(lib
     contact_batches = {int(p.tbs[t, 2]) for t in p.work[p.inc_begin:, 0]}
     batch_of = {int(b): d for d, b in enumerate(p.batches[:, 0]) if p.batches[d, 1] > 0}
 
-    def writes(op):
+    every_integrated = set().union(*integrated)
+    world_loads_on_ws = 0
+
+    def writes(op, flags=0):
         stage, d = int(op[0]), batch_of.get(int(op[1]))
         if stage in (WS_FIRST, WS):
-            return {("velocity", x) for x in dynamic[d]} | {(what, x) for x in integrated[d] for what in ("pose", "inertia")}
+            return {("velocity", x) for x in dynamic[d]} | ({(what, x) for x in integrated[d] for what in ("pose", "inertia")} if not flags & BODIES_INTEGRATED else set())
         if stage == SOLVE:
             return {("velocity", x) for x in dynamic[d]} | {("impulses", d)}
         if stage == INCREMENTAL:
-            return {("prestep", c) for c in contact_batches}
-        return {(what, x) for x in kinematics for what in ("velocity", "pose", "inertia")}
+            return {("prestep", c) for c in contact_batches} | ({(what, x) for x in every_integrated for what in ("pose", "inertia")} if flags & BODIES_INTEGRATED else set())
+        return {(what, x) for x in kinematics for what in (("velocity", "pose") if stage == KIN else ("velocity",))}
+
+    def loads(op, kernel, flags):
+        d = batch_of[int(op[1])]
+        got = {("prestep", d), ("impulses", d)} if flags & ROWS else set()
+        if flags & EARLY_WORLD:
+            got |= {(what, x) for x in slot01[d] for what in (("inertia",) if kernel == KERNEL_CONTACTS else ("inertia", "pose"))}
+        if flags & EARLY_OWNED:
+            got |= {("pose", x) for x in integrated[d]}
+        return got
 
     for iterations in ([1], [2, 2], [0, 3, 1], [0, 0]):
         for ivk in (False, True):
@@ -344,9 +425,9 @@ def test_prologue_prefetch_only_reads_what_the_previous_stage_does_not_write(lib
                 if stage in (WS_FIRST, WS, SOLVE):
                     d = batch_of[int(op[1])]
                     rows_ok = previous is not None and not writes(previous) & {("prestep", d), ("impulses", d)}
-                    loads = {("pose", x) for x in integrated[d]} if stage != SOLVE else {(what, x) for x in slot01[d] for what in ("pose", "inertia")}
-                    bodies_ok = previous is not None and not writes(previous) & loads
-                    rows, bodies = bool(op[5] & PREFETCH_ROWS), bool(op[5] & PREFETCH_BODIES)
+                    bodies_ok = previous is not None and not writes(previous) & {("pose", x) for x in integrated[d]} if stage != SOLVE else \
+                        previous is not None and not writes(previous) & {(what, x) for x in slot01[d] for what in ("pose", "inertia")}
+                    rows, bodies = bool(op[5] & ROWS_FREE), bool(op[5] & BODIES_FREE)
                     assert rows_ok or not rows, "row prefetch behind a stage that writes the rows"
                     assert bodies_ok or not bodies, "body prefetch behind a stage that writes the records"
                     assert bodies == bodies_ok, "a body prefetch the rule allows is missing"
@@ -355,6 +436,22 @@ def test_prologue_prefetch_only_reads_what_the_previous_stage_does_not_write(lib
                         # behind a WarmStart of the same batch (single-batch scenes)
                         assert int(previous[0]) == INCREMENTAL or (int(previous[0]) in (WS_FIRST, WS) and previous[1] == op[1]), "a row prefetch the rule allows is missing"
                 elif stage == INCREMENTAL:
-                    assert op[5] & (PREFETCH_ROWS | PREFETCH_BODIES) == 0, "the incremental update reads its rows after the wait"
+                    assert op[5] & (ROWS_FREE | BODIES_FREE) == 0, "the incremental update reads its rows after the wait"
                 previous = op
-            assert ops[0, 5] & (PREFETCH_ROWS | PREFETCH_BODIES) == 0
+            assert ops[0, 5] & (ROWS_FREE | BODIES_FREE) == 0
+            # every load of every resolved launch avoids what the resolved launch before it writes
+            live = ops[(ops[:, 2] > 0) & (ops[:, 3] != RANK_BARRIER)]
+            for ext, mode, profile in LAUNCH_CONTEXTS:
+                resolved = resolve(shim, live, ext, mode, profile)
+                world_on_ws = 0
+                for i, op in enumerate(live):
+                    if int(op[0]) not in (WS_FIRST, WS, SOLVE):
+                        continue
+                    kernel, flags = (int(v) for v in resolved[i])
+                    got = loads(op, kernel, flags)
+                    assert i > 0 or not got, "a prologue load before the first stage of the solve"
+                    clash = got & writes(live[i - 1], int(resolved[i - 1, 1])) if i > 0 else set()
+                    assert not clash, "op %d (%s) loads %s that its predecessor writes" % (i, op.tolist(), sorted(clash)[:4])
+                    world_on_ws += int(op[0]) == WS and bool(flags & EARLY_WORLD)
+                world_loads_on_ws += world_on_ws
+    assert (world_loads_on_ws > 0) == (case == "mixed"), "the world-inertia load of a flagged WarmStart behind an earlier batch's is covered"

@@ -1,5 +1,5 @@
-// Test shim for tests/test_topology.py: plan_topology and build_stage_program of bepuphysics2_b200/csrc/bepu_topology.h behind a ctypes-friendly
-// C interface. Built with g++ together with bepu_topology.cpp; the product never loads it.
+// Test shim for tests/test_topology.py: plan_topology, build_stage_program and resolve_stage_launch of bepuphysics2_b200/csrc/bepu_topology.h
+// behind a ctypes-friendly C interface. Built with g++ together with bepu_topology.cpp; the product never loads it.
 #include <cstring>
 
 #include "bepu_topology.h"
@@ -79,7 +79,7 @@ void topology_program_sizes(void* h, int64_t* out) {
     const int64_t v[] = {(int64_t)p.ops.size(), p.exchange_count, p.stage_count, p.constraint_iterations, p.algorithmic_bytes};
     std::memcpy(out, v, sizeof(v));
 }
-// per op: stage, work_begin, work_count, exchange, exchange_index, launch_flags, algorithmic_bytes
+// per op: stage, work_begin, work_count, exchange, exchange_index, launch_flags (kOp* facts), algorithmic_bytes
 void topology_program_ops(void* h, int64_t* out) {
     for (const StageOp& op : ((StageProgram*)h)->ops) {
         const int64_t v[] = {op.stage, op.work_begin, op.work_count, op.exchange, op.exchange_index, op.launch_flags, op.algorithmic_bytes};
@@ -88,5 +88,17 @@ void topology_program_ops(void* h, int64_t* out) {
     }
 }
 void topology_program_free(void* h) { delete (StageProgram*)h; }
+
+// ops: n rows of topology_program_ops; out[i] = kernel, flags of op i
+void topology_resolve(const int64_t* ops, int n, int integrator_extensions, int angular_mode, int profile, int32_t* out) {
+    const LaunchContext lc{integrator_extensions != 0, angular_mode, profile != 0};
+    for (int i = 0; i < n; ++i, ops += 7) {
+        const StageOp op{(int32_t)ops[0], (int32_t)ops[1], (int32_t)ops[2], (int32_t)ops[3], (uint32_t)ops[4], (int32_t)ops[5], ops[6]};
+        const StageLaunch l = resolve_stage_launch(op, lc);
+        out[2 * i] = l.kernel;
+        out[2 * i + 1] = l.flags;
+    }
+}
+int topology_deep_batch_bundles() { return kDeepBatchBundles; }
 
 }  // extern "C"
