@@ -3,6 +3,7 @@
 //   - reference AOSOA-W type batch buffers (Constraints/TypeBatch.cs:L10-27)  <->  device AOSOA-32
 //   - integration ownership (Solver_Solve.cs:L951-1044,L1072-1388) and the batch invariant check
 #include "bepu_layout_kernels.h"
+#include "bepu_redistribute.cuh"
 
 namespace bepucuda {
 
@@ -44,8 +45,10 @@ __global__ void transpose_in_all_kernel(const DeviceTypeBatch* __restrict__ tbs,
     const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
     if (warp >= work_count) return;
     const WorkItem w = work[warp];
-    const DeviceTypeBatch tb = tbs[w.type_batch];
     const TransposeDesc d = descs[w.type_batch];
+    if (what & kTransposePending) what &= d.flags;
+    if (!(what & (kTransposeRefs | kTransposePrestep | kTransposeImpulses))) return;
+    const DeviceTypeBatch tb = tbs[w.type_batch];
     const int slot = w.bundle * 32 + lane;
     int c = d.map ? d.map[slot] : slot;
     if (c >= d.src_count) c = -1;
@@ -65,16 +68,13 @@ __global__ void transpose_in_all_kernel(const DeviceTypeBatch* __restrict__ tbs,
         float* dst = tb.prestep + (size_t)w.bundle * d.prestep_rows * 32 + lane;
         for (int r = 0; r < d.prestep_rows; ++r) dst[r * 32] = c < 0 ? 0.0f : d.src_prestep[(sb * d.prestep_rows + r) * W + sl];
     }
-    if ((what & kTransposeImpulses) && !(d.flags & kDescResidentImpulses)) {
+    if (what & kTransposeImpulses) {
         float* dst = tb.impulses + (size_t)w.bundle * d.impulse_rows * 32 + lane;
         for (int r = 0; r < d.impulse_rows; ++r) dst[r * 32] = c < 0 ? 0.0f : d.src_impulses[(sb * d.impulse_rows + r) * W + sl];
     }
 }
 
-// NarrowPhase.RedistributeImpulses (CollisionDetection/NarrowPhaseConstraintUpdate.cs:L81-135) on the device-resident penetration impulses of one
-// constraint: a new contact whose feature id matches an old one takes that contact's accumulated impulse; the impulse of unmatched old contacts is
-// shared equally among the unmatched new contacts. Same-type update: old and new contact counts are equal (L172-183). Penetration rows of the
-// accumulated impulses: convex types [2 + i] (after the two tangent rows, ContactConstraintAccessor.cs:L58-66), nonconvex types [3 i + 2] (L70-76).
+// NarrowPhase.RedistributeImpulses on the device-resident penetration impulses, one constraint per lane (bepu_redistribute.cuh).
 __global__ void redistribute_impulses_kernel(const DeviceTypeBatch* __restrict__ tbs, const TransposeDesc* __restrict__ descs, const WorkItem* __restrict__ work, int work_count) {
     const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
     if (warp >= work_count) return;
@@ -85,33 +85,12 @@ __global__ void redistribute_impulses_kernel(const DeviceTypeBatch* __restrict__
     const int slot = w.bundle * 32 + lane;
     const int c = d.map ? d.map[slot] : slot;
     if (c < 0 || c >= d.src_count) return;
-    const bool convex = tb.type_id < 8;
-    const int n = convex ? (tb.type_id & 3) + 1 : (tb.type_id < 15 ? tb.type_id - 6 : tb.type_id - 13);  // ids 0-7: 1-4 contacts; 8-10 / 15-17: 2-4
+    const int n = contact_count_of_type(tb.type_id);
     float* acc = tb.impulses + (size_t)w.bundle * d.impulse_rows * 32 + lane;
-    const int32_t* oldIds = d.features_old + (size_t)c * n;
-    const int32_t* newIds = d.features_new + (size_t)c * n;
     float oldImpulses[4], newImpulses[4];
-    for (int i = 0; i < n; ++i) oldImpulses[i] = acc[(convex ? 2 + i : 3 * i + 2) * 32];
-    int unmatchedCount = 0;
-    for (int i = 0; i < n; ++i) {
-        newImpulses[i] = -1.0f;  // accumulated impulses cannot be negative: negative = unmatched
-        for (int j = 0; j < n; ++j) {
-            if (oldIds[j] == newIds[i]) {
-                newImpulses[i] = oldImpulses[j];
-                oldImpulses[j] = 0.0f;  // not distributed to the unmatched contacts
-                break;
-            }
-        }
-        if (newImpulses[i] < 0.0f) ++unmatchedCount;
-    }
-    if (unmatchedCount > 0) {
-        float unmatchedImpulse = 0.0f;
-        for (int i = 0; i < n; ++i) unmatchedImpulse += oldImpulses[i];
-        const float impulsePerUnmatched = unmatchedImpulse / (float)unmatchedCount;
-        for (int i = 0; i < n; ++i)
-            if (newImpulses[i] < 0.0f) newImpulses[i] = impulsePerUnmatched;
-    }
-    for (int i = 0; i < n; ++i) acc[(convex ? 2 + i : 3 * i + 2) * 32] = newImpulses[i];
+    for (int i = 0; i < n; ++i) oldImpulses[i] = acc[penetration_impulse_row(tb.type_id, i) * 32];
+    redistribute_impulses(n, d.features_old + (size_t)c * n, oldImpulses, d.features_new + (size_t)c * n, newImpulses);
+    for (int i = 0; i < n; ++i) acc[penetration_impulse_row(tb.type_id, i) * 32] = newImpulses[i];
 }
 
 // One thread per float4 of the motion half of a BodyDynamics record (float4 0,1 -> pose, 2,3 -> velocity).

@@ -15,12 +15,14 @@ struct TransposeDesc {
     int32_t src_count;    // TypeBatch.ConstraintCount of the source
     int32_t bodies, prestep_rows, impulse_rows;
     int32_t src_bundle_base;  // index of the source type batch's first host-width bundle in the per-bundle flag array
-    int32_t flags;            // kDescResidentImpulses: the accumulated impulses live on the device (bepucuda_update_contacts), transpose_in skips them
+    int32_t flags;            // kTransposePrestep / kTransposeImpulses: rows uploaded since the last transposition; kDescRedistribute
     const int32_t* features_old;  // contact feature ids the resident impulses belong to / the frame's new ids ([constraint][contact]); null = none
     const int32_t* features_new;
 };
-constexpr int32_t kDescResidentImpulses = 1, kDescRedistribute = 2;
-enum { kTransposeRefs = 1, kTransposePrestep = 2, kTransposeImpulses = 4 };
+// what: the rows to transpose. kTransposePending restricts them, per type batch, to those its descriptor marks as uploaded; the other type batches
+// keep their device rows (accumulated impulses left by the last solve, depths the incremental update moved).
+enum { kTransposeRefs = 1, kTransposePrestep = 2, kTransposeImpulses = 4, kTransposePending = 8 };
+constexpr int32_t kDescRedistribute = 16;
 void launch_transpose_in_all(const DeviceTypeBatch* tbs, const TransposeDesc* descs, const WorkItem* work, int work_count, int W, int what, cudaStream_t s);
 void launch_transpose_out_all(const DeviceTypeBatch* tbs, const TransposeDesc* descs, const WorkItem* work, int work_count, int W, int what, cudaStream_t s);
 void launch_fill_i32(int32_t* p, size_t n, int32_t v, cudaStream_t s);

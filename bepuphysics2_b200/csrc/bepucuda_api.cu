@@ -79,7 +79,10 @@ struct SourceTypeBatch {
     int32_t* raw_features_old = nullptr;
     int32_t* raw_features_new = nullptr;
     size_t feature_bytes = 0;
-    bool resident_impulses = false, redistribute = false;
+    // rows uploaded since the last transposition (kTransposePrestep / kTransposeImpulses): refresh_device_rows transposes only these, so the rows
+    // of every other type batch, the accumulated impulses in particular, stay as the last solve left them on the device
+    int32_t pending = 0;
+    bool redistribute = false;
 };
 
 }  // namespace bepucuda
@@ -117,7 +120,7 @@ struct bepucuda_ctx {
     // constraints
     int W = 8;
     int batch_count = 0;
-    bool constraints_open = false, constraints_ready = false, data_dirty = false, descs_dirty = false;
+    bool constraints_open = false, constraints_ready = false, data_dirty = false;
     std::vector<SourceTypeBatch> sources;
     ChunkArena raw_arena, pinned_arena;
     DeviceBuffer record_table, ref_rows, source_bundle_flags, refs32, prestep32, impulses32, tb_table, tdesc_table, work_table, map_table, bodies_per_type, kinematics_dev, frame_params_dev, error_dev;
@@ -365,35 +368,35 @@ int check_accelerations(bepucuda_ctx* ctx, const char* what) {
 }
 
 // Brings the device AOSOA-32 rows up to date with what the host queued since the last solve (bepucuda_update_type_batch / bepucuda_update_contacts):
-// flushes the batched copies, re-uploads the transposition descriptors when a type batch switched to resident impulses, transposes, and
-// redistributes the resident penetration impulses of updated contact type batches from the old to the new feature ids.
+// flushes the batched copies, re-uploads the transposition descriptors when their pending rows, redistribution flags or feature ids changed,
+// transposes the pending rows only, and redistributes the resident penetration impulses of updated contact type batches from the old to the new
+// feature ids. A frame that refreshes every type batch in full (bepuhost_cuda_refresh) leaves the descriptors as end_constraints uploaded them.
 int refresh_device_rows(bepucuda_ctx* ctx) {
     if (!ctx->data_dirty) return BEPUCUDA_OK;
     { int rc = flush_chunks(ctx, ctx->pending_h2d); if (rc != BEPUCUDA_OK) return rc; }
-    bool any_redistribute = false;
-    if (ctx->descs_dirty) {
-        for (size_t tb = 0; tb < ctx->topo.tbs.size(); ++tb) {
-            const SourceTypeBatch& s = ctx->sources[(size_t)ctx->topo.tbs[tb].source];
-            TransposeDesc& d = ctx->tdescs[tb];
-            d.flags = (s.resident_impulses ? kDescResidentImpulses : 0) | (s.redistribute ? kDescRedistribute : 0);
+    bool any_redistribute = false, descs_changed = false;
+    for (size_t tb = 0; tb < ctx->topo.tbs.size(); ++tb) {
+        const SourceTypeBatch& s = ctx->sources[(size_t)ctx->topo.tbs[tb].source];
+        TransposeDesc& d = ctx->tdescs[tb];
+        const int32_t flags = s.pending | (s.redistribute ? kDescRedistribute : 0);
+        if (d.flags != flags || d.features_old != s.raw_features_old || d.features_new != s.raw_features_new) {
+            d.flags = flags;
             d.features_old = s.raw_features_old;
             d.features_new = s.raw_features_new;
-            any_redistribute |= s.redistribute;
+            descs_changed = true;
         }
-        CK(cudaMemcpyAsync(ctx->tdesc_table.ptr, ctx->tdescs.data(), ctx->tdescs.size() * sizeof(TransposeDesc), cudaMemcpyHostToDevice, ctx->stream));
+        any_redistribute |= s.redistribute;
     }
+    if (descs_changed)
+        CK(cudaMemcpyAsync(ctx->tdesc_table.ptr, ctx->tdescs.data(), ctx->tdescs.size() * sizeof(TransposeDesc), cudaMemcpyHostToDevice, ctx->stream));
     launch_transpose_in_all(ctx->tb_table.as<DeviceTypeBatch>(), ctx->tdesc_table.as<TransposeDesc>(), ctx->work_table.as<WorkItem>(), ctx->topo.all_work_count, ctx->W,
-                            kTransposePrestep | kTransposeImpulses, ctx->stream);
-    if (any_redistribute) {
+                            kTransposePrestep | kTransposeImpulses | kTransposePending, ctx->stream);
+    if (any_redistribute)
         launch_redistribute_impulses(ctx->tb_table.as<DeviceTypeBatch>(), ctx->tdesc_table.as<TransposeDesc>(), ctx->work_table.as<WorkItem>(), ctx->topo.all_work_count, ctx->stream);
-        for (SourceTypeBatch& s : ctx->sources)
-            if (s.redistribute) {
-                std::swap(s.raw_features_old, s.raw_features_new);  // the resident impulses now belong to the new ids
-                s.redistribute = false;
-            }
-        // descriptors still carry kDescRedistribute and the pre-swap pointers: they are rewritten by the next update (descs_dirty stays set)
-    } else {
-        ctx->descs_dirty = false;
+    for (SourceTypeBatch& s : ctx->sources) {
+        if (s.redistribute) std::swap(s.raw_features_old, s.raw_features_new);  // the resident impulses now belong to the new ids
+        s.redistribute = false;
+        s.pending = 0;
     }
     CK(cudaGetLastError());
     ctx->data_dirty = false;
@@ -723,7 +726,7 @@ int32_t bepucuda_end_constraints(bepucuda_ctx* ctx) {
         tbs[i] = {p.type_id, p.bundle_count, p.device_batch, 0, ctx->refs32.as<int32_t>() + p.refs_offset, ctx->prestep32.as<float>() + p.prestep_offset,
                   ctx->impulses32.as<float>() + p.impulse_offset};
         ctx->tdescs[i] = {s.raw_refs, s.raw_prestep, s.raw_impulses, p.map_offset < 0 ? nullptr : ctx->map_table.as<int32_t>() + p.map_offset, s.count, t->bodies, t->prestep_rows,
-                          t->impulse_rows, topo.source_bundle_base[(size_t)p.source], 0, nullptr, nullptr};
+                          t->impulse_rows, topo.source_bundle_base[(size_t)p.source], kTransposePrestep | kTransposeImpulses, nullptr, nullptr};
     }
     ctx->records = work_records(topo, ctx->refs32.as<int32_t>(), ctx->prestep32.as<float>(), ctx->impulses32.as<float>());
 
@@ -830,7 +833,8 @@ int32_t bepucuda_update_type_batch(bepucuda_ctx* ctx, int32_t batch_index, int32
             }
             ctx->h2d_accum += (int64_t)(s.prestep_bytes + s.impulse_bytes);
             s.host_impulses = accumulated_impulses;
-            if (s.resident_impulses) { s.resident_impulses = false; s.redistribute = false; ctx->descs_dirty = true; }  // the host took the impulses back
+            s.pending = kTransposePrestep | kTransposeImpulses;
+            s.redistribute = false;  // the host took the impulses back
             ctx->data_dirty = true;
             return BEPUCUDA_OK;
         }
@@ -860,6 +864,8 @@ int32_t bepucuda_set_contact_features(bepucuda_ctx* ctx, int32_t batch_index, in
     if (get_type_info(s->type_id)->contacts == 0) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "set_contact_features: not a contact constraint type");
     CK(cudaSetDevice(ctx->device));
     { int rc = ensure_feature_arrays(ctx, *s); if (rc != BEPUCUDA_OK) return rc; }
+    // from a mapped buffer the ids are only queued: the next solve copies them, before the host writes the next frame's ids into the same buffer
+    if (ctx->constraints_ready) ctx->data_dirty = true;
     return copy_in(ctx, s->raw_features_old, feature_ids, s->feature_bytes);
 }
 
@@ -868,6 +874,7 @@ int32_t bepucuda_update_contacts(bepucuda_ctx* ctx, int32_t batch_index, int32_t
     if (!ctx->constraints_ready) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, "update_contacts before end_constraints");
     SourceTypeBatch* s = find_source(ctx, batch_index, type_batch_index);
     if (!s) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "update_contacts: unknown type batch");
+    if (get_type_info(s->type_id)->contacts == 0) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "update_contacts: not a contact constraint type");
     if (!s->raw_features_old) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, "update_contacts: bepucuda_set_contact_features was never called for this type batch");
     if (s->redistribute) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, "update_contacts: called twice for the same type batch without a solve in between");
     CK(cudaSetDevice(ctx->device));
@@ -882,9 +889,8 @@ int32_t bepucuda_update_contacts(bepucuda_ctx* ctx, int32_t batch_index, int32_t
         else CK(cudaMemcpyAsync(dsts[i], srcs[i], sizes[i], cudaMemcpyHostToDevice, ctx->stream));
         ctx->h2d_accum += (int64_t)sizes[i];
     }
-    s->resident_impulses = true;
+    s->pending |= kTransposePrestep;  // the accumulated impulses stay resident
     s->redistribute = true;
-    ctx->descs_dirty = true;
     ctx->data_dirty = true;
     return BEPUCUDA_OK;
 }

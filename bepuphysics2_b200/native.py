@@ -88,6 +88,21 @@ class StageProfile(C.Structure):
 
 EXEC_GRAPH, EXEC_STREAM = 0, 2  # 1 and 3 (persistent / dataflow kernels) were removed: slower than the graph on every configuration
 
+# BEPUCUDA_ERR_* of include/bepucuda.h (BepuCudaError.code; checked against the header by the CPU test-suite)
+ERR_INVALID_ARGUMENT, ERR_NO_DEVICE, ERR_CUDA, ERR_UNSUPPORTED_TYPE, ERR_BATCH_INVARIANT, ERR_BAD_STATE, ERR_OUT_OF_MEMORY = -1, -2, -3, -4, -5, -6, -7
+
+
+def contact_count(type_id):
+    """Contacts per constraint of a contact constraint type id: 1-4 for the convex ids 0-7, 2-4 for the nonconvex ids 8-10 and 15-17; 0 for every
+    other type (joints)."""
+    if 0 <= type_id <= 7:
+        return (type_id & 3) + 1
+    if 8 <= type_id <= 10:
+        return type_id - 6
+    if 15 <= type_id <= 17:
+        return type_id - 13
+    return 0
+
 # Every symbol include/bepucuda.h declares (checked by the CPU test-suite).
 C_ABI_SYMBOLS = [
     "bepucuda_create", "bepucuda_destroy", "bepucuda_last_error", "bepucuda_type_info", "bepucuda_host_register", "bepucuda_host_unregister",
@@ -444,8 +459,8 @@ class CudaTimestepper:
     def contact_feature_pool(self, rng=None):
         """One int32 block with the feature ids of every contact type batch back to back in (batch, type batch) order (the layout
         bepuhost_cuda_update_contacts walks), plus {(batch, type batch): view}. Filled with random ids when an rng is given."""
-        count = lambda tid: (tid & 3) + 1 if tid <= 7 else (tid - 6 if tid <= 10 else tid - 13)
-        tbs = [tb for tb in self.sim.type_batches() if tb.type_id <= 17]
+        count = contact_count
+        tbs = [tb for tb in self.sim.type_batches() if count(tb.type_id)]
         total = max(1, sum(tb.constraint_count * count(tb.type_id) for tb in tbs))
         backing = np.zeros(total + 2048, dtype=np.int32)  # page-aligned start and a whole number of pages, like a pinned pool block
         skip = (-backing.ctypes.data % 4096) // 4
@@ -474,7 +489,8 @@ class CudaTimestepper:
 
     def update_contacts(self, features):
         """Per frame, same topology: the host's new prestep data + the new feature ids of every contact type batch; impulses are redistributed on the
-        device (NarrowPhaseConstraintUpdate.cs:L81-135). Type batches not named in `features` keep their device rows."""
+        device (NarrowPhaseConstraintUpdate.cs:L81-135). Type batches not named in `features` (joints included) keep their device rows: the
+        accumulated impulses and depths the last solve left."""
         by_key = {(tb.batch_index, tb.type_batch_index): tb for tb in self.sim.type_batches()}
         for (b, t), ids in features.items():
             ids = np.ascontiguousarray(ids, dtype=np.int32)

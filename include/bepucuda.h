@@ -172,7 +172,16 @@ int32_t bepucuda_update_type_batch(bepucuda_ctx* ctx, int32_t batch_index, int32
  * bepucuda_set_contact_features stores the ids that belong to the impulses uploaded with bepucuda_upload_type_batch (call it between
  * begin/end_constraints or any time after). bepucuda_update_contacts uploads the frame's prestep data and NEW feature ids; at the next solve the
  * penetration impulses are redistributed from the old to the new ids on the device (matched ids keep their impulse, the unmatched share the
- * remainder equally); friction impulses are kept, as in the reference. No impulse bytes cross the bus in either direction. */
+ * remainder equally); friction impulses are kept, as in the reference. No impulse bytes cross the bus in either direction.
+ * A solve transposes in only the rows uploaded since the previous one: every type batch the frame did not name (joint type batches, contact type
+ * batches without an update) keeps its device rows, accumulated impulses and incrementally updated depths included. bepucuda_update_type_batch
+ * on a contact type batch hands its impulses back to the host: the next solve uses the uploaded ones and does not redistribute, even when
+ * bepucuda_update_contacts was called for it in the same frame. The device then still takes the uploaded impulses to belong to the feature ids
+ * it held before that frame (the last bepucuda_set_contact_features or redistribution); if they belong to other ids (the host redistributed
+ * them itself), call bepucuda_set_contact_features with those ids before the next bepucuda_update_contacts.
+ * bepucuda_update_contacts returns BEPUCUDA_ERR_INVALID_ARGUMENT for a type batch without contacts, BEPUCUDA_ERR_BAD_STATE before
+ * bepucuda_set_contact_features or when called twice for a type batch without a solve in between. From a registered (mapped) buffer the ids are
+ * read by the next solve: keep the buffer unchanged until then. */
 int32_t bepucuda_set_contact_features(bepucuda_ctx* ctx, int32_t batch_index, int32_t type_batch_index, const int32_t* feature_ids);
 int32_t bepucuda_update_contacts(bepucuda_ctx* ctx, int32_t batch_index, int32_t type_batch_index, const float* prestep, const int32_t* new_feature_ids);
 /* The motion half of BodyDynamics only: floats 0-15 of every 128-B record (pose + velocity, BodyProperties.cs:L318-338); the inertia half does not

@@ -130,6 +130,24 @@ extern "C" int32_t device_on_host_eval_integration(int32_t op, const float* in, 
     return 0;
 }
 
+// Impulse carry-over of the device-side contact update (csrc/bepu_redistribute.cuh, what redistribute_impulses_kernel runs per constraint) over a
+// whole type batch in the reference AOSOA-W layout, with the operands of oracle_update_contact_impulses. Returns -1 for a type without contacts.
+#include "bepu_redistribute.cuh"
+extern "C" int32_t device_on_host_update_contact_impulses(int32_t type_id, int32_t constraint_count, int32_t W, float* accumulated_impulses, const int32_t* old_feature_ids,
+                                                          const int32_t* new_feature_ids) {
+    const int n = bepucuda::contact_count_of_type(type_id);
+    if (n == 0) return -1;
+    const int rows = type_id < 8 ? n + 3 : 3 * n;
+    for (int c = 0; c < constraint_count; ++c) {
+        float* bundle = accumulated_impulses + (size_t)(c / W) * rows * W + (c % W);
+        float oldImpulses[4], newImpulses[4];
+        for (int i = 0; i < n; ++i) oldImpulses[i] = bundle[bepucuda::penetration_impulse_row(type_id, i) * W];
+        bepucuda::redistribute_impulses(n, old_feature_ids + (size_t)c * n, oldImpulses, new_feature_ids + (size_t)c * n, newImpulses);
+        for (int i = 0; i < n; ++i) bundle[bepucuda::penetration_impulse_row(type_id, i) * W] = newImpulses[i];
+    }
+    return 0;
+}
+
 // PredictBoundingBoxes arithmetic of csrc/bepu_bounds_math.cuh (same operand layout as ref_convex_bounds of the transpiled reference's harness).
 #include "bepu_bounds_math.cuh"
 extern "C" int32_t device_on_host_convex_bounds(int32_t type, const float* dims, const float* margins, int32_t allow, const float* q, const float* pos, const float* lin, const float* ang,

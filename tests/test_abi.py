@@ -41,7 +41,26 @@ def test_type_registry_matches_oracle_and_reference_sizes(libs):
 
 def test_unsupported_type_is_reported(libs):
     cuda, _ = bp.load_libraries()
-    assert cuda.bepucuda_type_info(63, None, None, None) == -4  # BEPUCUDA_ERR_UNSUPPORTED_TYPE
+    assert cuda.bepucuda_type_info(63, None, None, None) == native.ERR_UNSUPPORTED_TYPE
+
+
+def test_error_codes_match_the_header():
+    header = open(os.path.join(ROOT, "include", "bepucuda.h")).read()
+    defined = {name: int(value) for name, value in re.findall(r"#define BEPUCUDA_ERR_([A-Z_]+) \((-?\d+)\)", header)}
+    assert len(defined) == 7
+    assert defined == {name[4:]: getattr(native, name) for name in dir(native) if name.startswith("ERR_")}
+
+
+def test_contact_count_matches_the_type_registry(libs):
+    """native.contact_count (the feature-id layout of bepucuda_set_contact_features / bepucuda_update_contacts) against the registered layouts:
+    contacts only for the contact type ids, and the accumulated impulses hold their penetration rows (convex: 2 tangent + n + 1 twist,
+    nonconvex: 3 per contact)."""
+    for type_id in range(64):
+        info, n = bp.type_info(type_id), native.contact_count(type_id)
+        if info is None or type_id >= 22:
+            assert n == 0, type_id
+            continue
+        assert n > 0 and info[2] == (n + 3 if type_id < 8 else 3 * n), type_id
 
 
 def test_no_cpu_fallback_without_a_device(libs):
@@ -52,7 +71,7 @@ def test_no_cpu_fallback_without_a_device(libs):
     sim = bp.Simulation()
     with pytest.raises(bp.BepuCudaError) as e:
         bp.CudaTimestepper(sim)
-    assert e.value.code == -2  # BEPUCUDA_ERR_NO_DEVICE
+    assert e.value.code == native.ERR_NO_DEVICE
 
 
 def test_product_sources_never_reference_the_oracle():

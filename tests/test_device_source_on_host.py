@@ -27,7 +27,7 @@ DT = 1.0 / 240.0  # a substep of the 8 x 2 configuration at 1/30 s
 def device_on_host():
     lib = os.path.join(HERE, "libdevice_on_host.so")
     defines = []
-    srcs = [os.path.join(HERE, "device_on_host.cpp"), os.path.join(HERE, "stubs", "cuda_runtime.h")] + [os.path.join(CSRC, f) for f in ("bepu_device_math.cuh", "bepu_contacts.cuh", "bepu_joints.cuh", "bepu_joints_more.cuh", "bepu_integration.cuh", "bepu_bounds_math.cuh")]
+    srcs = [os.path.join(HERE, "device_on_host.cpp"), os.path.join(HERE, "stubs", "cuda_runtime.h")] + [os.path.join(CSRC, f) for f in ("bepu_device_math.cuh", "bepu_contacts.cuh", "bepu_joints.cuh", "bepu_joints_more.cuh", "bepu_integration.cuh", "bepu_bounds_math.cuh", "bepu_redistribute.cuh")]
     if not os.path.exists(lib) or any(os.path.getmtime(s) > os.path.getmtime(lib) for s in srcs):
         subprocess.check_call(["/usr/bin/g++", "-O2", "-std=c++17", "-ffp-contract=off", "-fno-fast-math", "-march=x86-64-v3", "-Wall", "-Wno-unused-function", "-Wno-unknown-pragmas", "-pthread"] + defines +
                               ["-I", os.path.join(HERE, "stubs"), "-I", HERE, "-I", CSRC, "-shared", "-fPIC", "-o", lib, srcs[0]])
@@ -179,3 +179,94 @@ def test_bounds_source_reproduces_the_reference_vectors_bit_for_bit(device_on_ho
             assert np.array_equal(out.view(np.uint32), want[i].view(np.uint32)), "set %d sample %d (shape type %d)" % (k, i, types[i])
             checked += 1
     assert checked == 96
+
+
+def _redistribute_case_ids(n):
+    """Every id-equality pattern of n old and n new feature ids: (old, new) drawn from an alphabet of n + 1 symbols, (n + 1)^(2n) cases. The symbols
+    are the int32 edges and negative ids, so that the comparison is held at the values where a signed / unsigned mix-up would show."""
+    alphabet = np.array([np.iinfo(np.int32).min, -1, 0, np.iinfo(np.int32).max, -7][:n + 1], dtype=np.int32)
+    k = n + 1
+    digits = (np.arange(k ** (2 * n), dtype=np.int64)[:, None] // (k ** np.arange(2 * n, dtype=np.int64))[None, :]) % k
+    ids = alphabet[digits]
+    return np.ascontiguousarray(ids[:, :n]), np.ascontiguousarray(ids[:, n:])
+
+
+def _redistribute_float64(old_ids, old_imp, new_ids):
+    """RedistributeImpulses restated in float64 over many constraints at once: (new impulses where matched, NaN where unmatched; the float64
+    remainder per unmatched contact, NaN when nothing is unmatched; the float64 remainder)."""
+    cases, n = old_ids.shape
+    remaining = old_imp.astype(np.float64)
+    new = np.full((cases, n), np.nan)
+    rows = np.arange(cases)
+    for i in range(n):
+        eq = old_ids == new_ids[:, i:i + 1]
+        matched = eq.any(axis=1)
+        j = np.argmax(eq, axis=1)  # the first old contact with the id
+        new[matched, i] = remaining[rows[matched], j[matched]]
+        remaining[rows[matched], j[matched]] = 0.0
+    unmatched = np.isnan(new).sum(axis=1)
+    remainder = remaining.sum(axis=1)
+    with np.errstate(invalid="ignore", divide="ignore"):
+        share = np.where(unmatched > 0, remainder / np.maximum(unmatched, 1), np.nan)
+    return new, share, remainder
+
+
+def test_redistribution_source_matches_the_oracle_on_every_id_pattern(libs, device_on_host):
+    """csrc/bepu_redistribute.cuh (the per-constraint body of redistribute_impulses_kernel) against oracle_update_contact_impulses bit for bit, for
+    every id-equality pattern at n = 1-4 contacts (duplicates in old, in new and in both, nothing matched, all matched and permuted), with impulses
+    of 0, subnormals, ordinary values and values near FLT_MAX (remainders that overflow to inf). Then against float64: a matched contact carries
+    its old impulse exactly (0 included: it stays matched), an unmatched one the remainder / unmatched count to within fp32 rounding."""
+    dev, orc = device_on_host
+    i32p = C.POINTER(C.c_int32)
+    for lib, name in ((dev, "device_on_host_update_contact_impulses"), (orc, "oracle_update_contact_impulses")):
+        getattr(lib, name).argtypes = [C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
+    fmax = np.finfo(np.float32).max
+    pool = np.array([0.0, 0.0, 1e-45, 3e-39, 1.1754942e-38, 0.25, 1.5, 7.0, 1234.5, fmax * 0.3, fmax * 0.6, fmax], dtype=np.float32)
+    rng = np.random.default_rng(5)
+    checked = 0
+    for n in (1, 2, 3, 4):
+        old_ids, new_ids = _redistribute_case_ids(n)
+        cases = old_ids.shape[0]
+        assert cases == (n + 1) ** (2 * n)
+        # the type ids with n contacts: convex one- and two-body, nonconvex (2-4 contacts) one- and two-body
+        types = [n - 1, n + 3] + ([n + 6, n + 13] if n >= 2 else [])
+        for trial, type_id in enumerate(types):
+            bodies, _, impulse_rows = ob.type_info(type_id)
+            W = (1, 8, 16, 4)[trial]
+            bundles = (cases + W - 1) // W
+            old_imp = pool[rng.integers(0, pool.size, size=(cases, n))]
+            if trial == 0:
+                old_imp[:] = pool[rng.integers(0, 6, size=(cases, n))]  # zeros, subnormals and small values only: no overflow anywhere
+            else:
+                old_imp[::3] = pool[rng.integers(pool.size - 3, pool.size, size=old_imp[::3].shape)]  # near FLT_MAX only: remainders overflow
+            acc = rng.normal(0, 1, size=(bundles, impulse_rows, W)).astype(np.float32)  # tangent / twist rows: must come out untouched
+            penetration = [2 + i for i in range(n)] if type_id < 8 else [3 * i + 2 for i in range(n)]
+            c = np.arange(cases)
+            for i, r in enumerate(penetration):
+                acc[c // W, r, c % W] = old_imp[:, i]
+            a_dev, a_orc = acc.copy(), acc.copy()
+            assert dev.device_on_host_update_contact_impulses(type_id, cases, W, a_dev.ctypes.data, old_ids.ctypes.data, new_ids.ctypes.data) == 0
+            assert orc.oracle_update_contact_impulses(type_id, cases, W, a_orc.ctypes.data, old_ids.ctypes.data, new_ids.ctypes.data) == 0
+            what = "n = %d, type %d, W = %d" % (n, type_id, W)
+            assert np.array_equal(a_dev.view(np.uint32), a_orc.view(np.uint32)), what + ": device source differs from the oracle"
+            others = [r for r in range(impulse_rows) if r not in penetration]
+            assert np.array_equal(a_dev[:, others, :].view(np.uint32), acc[:, others, :].view(np.uint32)), what + ": a friction / twist row changed"
+            out = np.stack([a_dev[c // W, r, c % W] for r in penetration], axis=1)
+            new64, share64, remainder64 = _redistribute_float64(old_ids, old_imp, new_ids)
+            matched = ~np.isnan(new64)
+            assert np.array_equal(out[matched].astype(np.float64), new64[matched]), what + ": a matched contact did not carry its old impulse exactly"
+            unmatched = ~matched
+            share = np.broadcast_to(share64[:, None], out.shape)[unmatched]
+            got = out[unmatched].astype(np.float64)
+            finite = np.isfinite(got)
+            # n fp32 additions and one division, all of non-negative values: relative error <= (n + 1) 2^-24, plus n subnormal quanta
+            tol = (n + 1) * 2.0 ** -24 * share[finite] + n * 2.0 ** -149
+            assert (np.abs(got[finite] - share[finite]) <= tol).all(), what + ": remainder share off by more than fp32 rounding"
+            rem = np.broadcast_to(remainder64[:, None], out.shape)[unmatched]
+            assert (rem[~finite] > float(fmax) * (1 - 2.0 ** -23)).all(), what + ": an unmatched share overflowed although the remainder fits fp32"
+            if trial > 0 and n > 1:
+                assert (~finite).any(), what + ": no remainder overflowed to inf"
+            if n > 1:  # (a single contact has only four cases)
+                assert ((out == 0) & matched).any() and (unmatched.sum(axis=1) == n).any() and (unmatched.sum(axis=1) == 0).any(), what
+            checked += cases
+    assert checked == sum(((n + 1) ** (2 * n)) * (2 if n == 1 else 4) for n in (1, 2, 3, 4))
