@@ -208,6 +208,15 @@ __global__ void mark_kinematics_kernel(const int32_t* __restrict__ kinematics, i
     if (idx < 0 || idx >= body_count) { atomicExch(error_flag, 2); return; }
     constrained[idx] = 1;
 }
+// Peer sharding: the integration owner of a body is the lowest batch referencing it on any rank. `global` holds host batch indices, which are the
+// device batch indices of the synchronized batches on every rank. A body the whole graph first references in the fallback batch (global index at
+// or above the threshold) keeps the device batch pass 1 found: only the fallback rank has lanes there, and it numbers its levels itself.
+__global__ void merge_first_batch_kernel(int32_t* __restrict__ first_batch, const int32_t* __restrict__ global, int body_count, int fallback_threshold) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= body_count) return;
+    const int32_t g = global[i];
+    if (g < fallback_threshold) first_batch[i] = g;
+}
 __global__ void fill_i32_kernel(int32_t* p, size_t n, int32_t v) {
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n) p[i] = v;
@@ -344,6 +353,9 @@ void launch_ownership_pass1(const DeviceTypeBatch* tbs, const WorkItem* work, in
     if (work_count > 0)
         ownership_pass1_kernel<<<blocks_for((size_t)work_count * 32, 128), 128, 0, s>>>(tbs, work, work_count, bodies_per_type, sync_batch_count, body_count, first_batch,
                                                                                          sync_refcount, sync_mask, error_flag);
+}
+void launch_merge_first_batch(int32_t* first_batch, const int32_t* global_first_batch, int body_count, int fallback_threshold, cudaStream_t s) {
+    if (body_count > 0) merge_first_batch_kernel<<<blocks_for(body_count, 256), 256, 0, s>>>(first_batch, global_first_batch, body_count, fallback_threshold);
 }
 void launch_ownership_rest(const DeviceTypeBatch* tbs, const WorkItem* work, int work_count, const int32_t* bodies_per_type, int body_count, const int32_t* first_batch,
                            const int32_t* sync_refcount, const unsigned long long* sync_mask, uint8_t* constrained, const int32_t* kinematics, int kinematic_count,

@@ -40,6 +40,9 @@ struct CopyChunk {
 void launch_batched_copy(const CopyChunk* chunks, int chunk_count, cudaStream_t s);
 void launch_ownership_pass1(const DeviceTypeBatch* tbs, const WorkItem* work, int work_count, const int32_t* bodies_per_type, int sync_batch_count, int body_count,
                             int32_t* first_batch, int32_t* sync_refcount, unsigned long long* sync_mask, int32_t* error_flag, cudaStream_t s);
+// Peer sharding, between the ownership passes: first_batch[i] = global_first_batch[i] (host batch indices, lowest over every rank) unless that is
+// at or above fallback_threshold, where the device batch of pass 1 (a fallback level of the fallback rank) stays.
+void launch_merge_first_batch(int32_t* first_batch, const int32_t* global_first_batch, int body_count, int fallback_threshold, cudaStream_t s);
 void launch_ownership_rest(const DeviceTypeBatch* tbs, const WorkItem* work, int work_count, const int32_t* bodies_per_type, int body_count, const int32_t* first_batch,
                            const int32_t* sync_refcount, const unsigned long long* sync_mask, uint8_t* constrained, const int32_t* kinematics, int kinematic_count,
                            int32_t* error_flag, const TransposeDesc* descs, int W, int32_t* source_bundle_flags, cudaStream_t s);

@@ -65,9 +65,10 @@ const TypeInfo* get_type_info(int type_id) {
 static bool dynamic_ref(int32_t enc) { return enc >= 0 && !((uint32_t)enc & kRefKinematicBit); }
 
 int plan_topology(const std::vector<SourceView>& sources, int W, int fallback_threshold, int batch_count, int body_count, bool peer_mode, TopologyPlan* plan,
-                  std::string* error) {
+                  std::string* error, int rank, int fallback_rank) {
     TopologyPlan& p = *plan;
     p = TopologyPlan{};
+    p.fallback_rank = peer_mode ? fallback_rank : -1;
     // sources in (batch, type batch) order
     std::vector<int> order(sources.size());
     std::iota(order.begin(), order.end(), 0);
@@ -100,9 +101,12 @@ int plan_topology(const std::vector<SourceView>& sources, int W, int fallback_th
     if (peer_mode) {
         // every rank runs the exchange point of every batch, also of batches it has no constraint in
         while ((int)batch_tbs.size() < std::min(batch_count, fallback_threshold)) batch_tbs.emplace_back();
+        // the sequential fallback batch runs whole on one rank, the fallback rank, in the levels below
         for (const SourceView& s : sources)
-            if (s.batch_index >= fallback_threshold) {
-                *error = "end_constraints: the sequential fallback batch is not supported across ranks";
+            if (s.batch_index >= fallback_threshold && rank != p.fallback_rank) {
+                *error = p.fallback_rank < 0 ? "end_constraints: the sequential fallback batch is not supported across ranks"
+                                             : "end_constraints: a type batch of the sequential fallback batch was uploaded on rank " + std::to_string(rank) +
+                                                   ", but only the fallback rank " + std::to_string(p.fallback_rank) + " may run it";
                 return BEPUCUDA_ERR_BAD_STATE;
             }
     }
@@ -244,8 +248,10 @@ StageProgram build_stage_program(const TopologyPlan& plan, const std::vector<int
                                  bool peer_mode, int body_count) {
     StageProgram prog;
     std::vector<StageOp>& ops = prog.ops;
-    auto push = [&](int32_t stage, int32_t begin, int32_t count, int32_t exchange, int32_t flags, int64_t bytes) {
+    std::vector<char> joins;  // per op: it belongs to the exchange point of the op before it (a later level of a fallback section)
+    auto push = [&](int32_t stage, int32_t begin, int32_t count, int32_t exchange, int32_t flags, int64_t bytes, bool join = false) {
         ops.push_back({stage, begin, count, exchange, 0u, flags, bytes});
+        joins.push_back(join);
     };
     // algorithmic bytes of one pass over a slice of the work list, summed once per device batch (a program repeats every batch many times)
     auto work_bytes = [&](int32_t begin, int32_t count, int32_t TypeInfo::*per) {
@@ -259,14 +265,19 @@ StageProgram build_stage_program(const TopologyPlan& plan, const std::vector<int
         warm_start_bytes.push_back(work_bytes(bw.begin, bw.count, &TypeInfo::warm_start_bytes));
         solve_bytes.push_back(work_bytes(bw.begin, bw.count, &TypeInfo::solve_bytes));
     }
+    // Peer mode with a fallback rank: the fallback section of a pass (its levels, in order, on the fallback rank alone) is one exchange point.
+    // Boundary warps of every level wait for what peers pushed before the section, and the peers' next stage waits for every level's arrivals.
+    const bool fallback_section = peer_mode && plan.fallback_rank >= 0;
     auto batch_stages = [&](int32_t stage, int32_t flags) {
         // in peer mode every rank runs the exchange point of every batch, also of one it has no constraint in
         for (size_t b = 0; b < plan.batches.size(); ++b) {
             const TopologyPlan::Batch& bw = plan.batches[b];
             if (bw.count > 0 || (peer_mode && (int)b < plan.sync_batch_count))
                 push(stage, bw.begin, bw.count, peer_mode ? (int32_t)b : kNoExchange, flags | (bw.contacts_only ? kOpContactsOnly : 0),
-                     stage == kStageSolve ? solve_bytes[b] : warm_start_bytes[b]);
+                     stage == kStageSolve ? solve_bytes[b] : warm_start_bytes[b], fallback_section && (int)b > plan.sync_batch_count);
         }
+        // a rank without fallback levels holds the section's place, as empty synchronized batches do
+        if (fallback_section && plan.fallback_levels == 0) push(stage, plan.all_work_count, 0, plan.sync_batch_count, flags, 0);
     };
     // peer-sharded solves keep the integration in the owning lane, which also pushes the new records to the peers
     const int32_t integrable = plan.inc_count > 0 && !peer_mode ? kOpIntegrable : 0;
@@ -293,9 +304,10 @@ StageProgram build_stage_program(const TopologyPlan& plan, const std::vector<int
     push(kStageFinalPose, 0, body_count, kNoExchange, 0, (int64_t)body_count * 108);
 
     const StageOp* previous = nullptr;  // last launched stage (rank barriers write nothing)
-    for (StageOp& op : ops) {
-        op.exchange_index = prog.exchange_count;
-        if (op.exchange != kNoExchange) ++prog.exchange_count;
+    for (size_t i = 0; i < ops.size(); ++i) {
+        StageOp& op = ops[i];
+        op.exchange_index = joins[i] ? prog.exchange_count - 1 : prog.exchange_count;
+        if (op.exchange != kNoExchange && !joins[i]) ++prog.exchange_count;
         if (op.exchange == kRankBarrier) continue;
         if (op.stage <= kStageIncremental) {
             // what the PDL prologue may read (DESIGN §3): not what the op launched just before writes

@@ -45,6 +45,7 @@ struct TopologyPlan {
     int32_t inc_begin = 0, inc_count = 0;     // the incremental contact update: every contact bundle once
     int32_t all_work_count = 0;               // work[0 .. all_work_count) covers every bundle once
     int32_t sync_batch_count = 0, fallback_levels = 0;
+    int32_t fallback_rank = -1;               // peer sharding: the rank that runs the whole fallback batch, -1 = none (no rank may have one)
     int64_t constraint_count = 0;
     std::vector<int32_t> source_live;         // constraints actually present per source (fallback type batches may contain holes)
     std::vector<int32_t> source_bundle_base;  // per source: its first host-width bundle in the per-bundle flag array
@@ -52,11 +53,13 @@ struct TopologyPlan {
     size_t refs_words = 0, prestep_words = 0, impulse_words = 0;
 };
 
-// Plans the device batches of `sources` (bundle width W; batches from fallback_threshold on form the sequential fallback batch). Returns
-// BEPUCUDA_OK, or an error code with `error` set: BEPUCUDA_ERR_BAD_STATE for a fallback batch in peer mode, BEPUCUDA_ERR_INVALID_ARGUMENT for a
-// fallback body reference out of range, BEPUCUDA_ERR_BATCH_INVARIANT for a fallback bundle that holds a dynamic body twice.
+// Plans the device batches of `sources` (bundle width W; batches from fallback_threshold on form the sequential fallback batch). In peer mode,
+// `rank` is this rank and `fallback_rank` the rank that owns every fallback constraint (bepucuda_shard_set_fallback_rank; -1 = none): only that
+// rank may have fallback sources, and it levelises them as a single context does. Returns BEPUCUDA_OK, or an error code with `error` set:
+// BEPUCUDA_ERR_BAD_STATE for a fallback source in peer mode on a rank other than the fallback rank (or with none set), BEPUCUDA_ERR_INVALID_ARGUMENT
+// for a fallback body reference out of range, BEPUCUDA_ERR_BATCH_INVARIANT for a fallback bundle that holds a dynamic body twice.
 int plan_topology(const std::vector<SourceView>& sources, int W, int fallback_threshold, int batch_count, int body_count, bool peer_mode, TopologyPlan* plan,
-                  std::string* error);
+                  std::string* error, int rank = 0, int fallback_rank = -1);
 
 // What the solver kernels read per work item, with the plan's offsets applied to the arena bases.
 std::vector<WorkRecord> work_records(const TopologyPlan& plan, int32_t* refs, float* prestep, float* impulses);
@@ -109,12 +112,15 @@ struct StageProgram {
     int64_t algorithmic_bytes = 0;      // constraint stages and the final pose pass; neither the kinematic passes nor the per-body acceleration records
 };
 
-// Solver_Solve.cs:L1419-1479, then PoseIntegrator.IntegrateAfterSubstepping.
+// Solver_Solve.cs:L1419-1479, then PoseIntegrator.IntegrateAfterSubstepping. In peer mode with a fallback rank (TopologyPlan::fallback_rank), the
+// fallback part of every WarmStart and Solve pass is ONE exchange point on every rank: every level op of it carries the same exchange_index on the
+// fallback rank, and a zero-work op holds its place on the others.
 StageProgram build_stage_program(const TopologyPlan& plan, const std::vector<int32_t>& iterations, int kinematic_count, bool integrate_velocity_for_kinematics,
                                  bool peer_mode, int body_count);
 
 // Peer sharding: cumulative boundary bundles of this rank through each exchange point of one solve, kShardMaxExchanges slots, the last one the
-// per-solve total (ShardStage). BEPUCUDA_ERR_BAD_STATE when the program has too many exchange points.
+// per-solve total (ShardStage); the level ops of a fallback section add up into their one exchange point. BEPUCUDA_ERR_BAD_STATE when the program
+// has too many exchange points.
 int exchange_targets(const StageProgram& program, const std::vector<int32_t>& boundary_count, std::vector<unsigned long long>* targets, std::string* error);
 
 // Peer sharding: moves the boundary records (is_boundary[i] != 0) of every device batch to its front, marks them with kRecordBoundaryBit and

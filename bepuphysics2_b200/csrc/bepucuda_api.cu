@@ -136,7 +136,9 @@ struct bepucuda_ctx {
     std::vector<uint8_t> body_masks;                                // bepucuda_shard_set_body_masks: per body, the ranks that reference it
     std::vector<void*> opened_ipc;
     std::vector<int32_t> global_first_batch;
+    DeviceBuffer global_first_batch_dev;
     std::vector<uint8_t> global_constrained;
+    int32_t fallback_rank = -1;                                     // bepucuda_shard_set_fallback_rank: the rank that runs the fallback batch
     uint32_t exchange_counter = 0;                                  // exchange points executed so far (flag barrier sequence)
     std::vector<int32_t> kinematics;
     StageProgram program;
@@ -476,7 +478,7 @@ int32_t bepucuda_destroy(bepucuda_ctx* ctx) {
     if (ctx->stream) cudaStreamSynchronize(ctx->stream);
     invalidate_graph(ctx);
     for (void* p : ctx->opened_ipc) cudaIpcCloseMemHandle(p);
-    DeviceBuffer* bufs[] = {&ctx->shard_flags, &ctx->peer32, &ctx->body_masks_dev, &ctx->boundary_flags_dev, &ctx->raw_bodies, &ctx->pose, &ctx->velocity, &ctx->inertia_local, &ctx->inertia_world, &ctx->constrained, &ctx->first_batch, &ctx->sync_refcount,
+    DeviceBuffer* bufs[] = {&ctx->shard_flags, &ctx->peer32, &ctx->body_masks_dev, &ctx->boundary_flags_dev, &ctx->global_first_batch_dev, &ctx->raw_bodies, &ctx->pose, &ctx->velocity, &ctx->inertia_local, &ctx->inertia_world, &ctx->constrained, &ctx->first_batch, &ctx->sync_refcount,
                             &ctx->sync_mask, &ctx->chunk_table, &ctx->record_table, &ctx->ref_rows, &ctx->body_shapes, &ctx->body_activities, &ctx->body_bounds, &ctx->color_refs, &ctx->color_priorities, &ctx->color_body_min, &ctx->color_body_mask, &ctx->color_out, &ctx->color_lists, &ctx->color_counts, &ctx->source_bundle_flags, &ctx->refs32, &ctx->prestep32, &ctx->impulses32, &ctx->tb_table, &ctx->tdesc_table, &ctx->work_table, &ctx->map_table,
                             &ctx->bodies_per_type, &ctx->kinematics_dev, &ctx->frame_params_dev, &ctx->error_dev, &ctx->accelerations};
     for (auto b : bufs) b->release();
@@ -706,7 +708,7 @@ int32_t bepucuda_end_constraints(bepucuda_ctx* ctx) {
         for (const SourceTypeBatch& s : ctx->sources) views.push_back({s.batch_index, s.type_batch_index, s.type_id, s.count, s.host_refs.data()});
         TopologyPlan plan;
         std::string error;
-        const int rc = plan_topology(views, W, ctx->fallback_threshold, ctx->batch_count, ctx->body_count, ctx->peer_mode, &plan, &error);
+        const int rc = plan_topology(views, W, ctx->fallback_threshold, ctx->batch_count, ctx->body_count, ctx->peer_mode, &plan, &error, ctx->peers.rank, ctx->fallback_rank);
         if (rc != BEPUCUDA_OK) return fail(ctx, rc, error);
         ctx->topo = std::move(plan);
     }
@@ -767,9 +769,12 @@ int32_t bepucuda_end_constraints(bepucuda_ctx* ctx) {
                            ctx->body_count, ctx->first_batch.as<int32_t>(), ctx->sync_refcount.as<int32_t>(), (unsigned long long*)ctx->sync_mask.ptr, ctx->error_dev.as<int32_t>(),
                            ctx->stream);
     if (ctx->peer_mode && nb > 0) {
-        // peer sharding: the integration owner of a body is the lowest batch referencing it on ANY rank (computed by the host over the whole graph)
+        // peer sharding: the integration owner of a body is the lowest batch referencing it on ANY rank (computed by the host over the whole graph);
+        // a body the graph first references in the fallback batch keeps the level this rank, the fallback rank, found for it
         if ((int)ctx->global_first_batch.size() != ctx->body_count) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, "end_constraints: bepucuda_shard_set_global was not called for this body count");
-        CK(cudaMemcpyAsync(ctx->first_batch.ptr, ctx->global_first_batch.data(), (size_t)ctx->body_count * 4, cudaMemcpyHostToDevice, ctx->stream));
+        CK(ctx->global_first_batch_dev.reserve(nb * 4));
+        CK(cudaMemcpyAsync(ctx->global_first_batch_dev.ptr, ctx->global_first_batch.data(), (size_t)ctx->body_count * 4, cudaMemcpyHostToDevice, ctx->stream));
+        launch_merge_first_batch(ctx->first_batch.as<int32_t>(), ctx->global_first_batch_dev.as<int32_t>(), ctx->body_count, ctx->fallback_threshold, ctx->stream);
     }
     launch_ownership_rest(ctx->tb_table.as<DeviceTypeBatch>(), ctx->work_table.as<WorkItem>(), topo.all_work_count, ctx->bodies_per_type.as<int32_t>(), ctx->body_count,
                           ctx->first_batch.as<int32_t>(), ctx->sync_refcount.as<int32_t>(), (const unsigned long long*)ctx->sync_mask.ptr, ctx->constrained.as<uint8_t>(),
@@ -1309,6 +1314,15 @@ int32_t bepucuda_shard_set_global(bepucuda_ctx* ctx, const int32_t* first_batch,
 int32_t bepucuda_shard_set_body_masks(bepucuda_ctx* ctx, const uint8_t* rank_masks) {
     if (!ctx || !rank_masks) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "shard_set_body_masks: bad arguments");
     ctx->body_masks.assign(rank_masks, rank_masks + ctx->body_count);
+    if (ctx->constraints_ready) ctx->constraints_ready = false;
+    return BEPUCUDA_OK;
+}
+
+int32_t bepucuda_shard_set_fallback_rank(bepucuda_ctx* ctx, int32_t rank) {
+    if (!ctx) return BEPUCUDA_ERR_INVALID_ARGUMENT;
+    if (!ctx->peer_mode) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "shard_set_fallback_rank: the context is not in peer mode (bepucuda_shard_import*)");
+    if (rank < -1 || rank >= ctx->peers.rank_count) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "shard_set_fallback_rank: rank out of range");
+    ctx->fallback_rank = rank;
     if (ctx->constraints_ready) ctx->constraints_ready = false;
     return BEPUCUDA_OK;
 }

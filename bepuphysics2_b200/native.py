@@ -112,6 +112,7 @@ C_ABI_SYMBOLS = [
     "bepucuda_event_record", "bepucuda_event_elapsed_ms", "bepucuda_profile_stages",
     "bepucuda_set_contact_features", "bepucuda_update_contacts", "bepucuda_upload_body_motion", "bepucuda_download_body_motion",
     "bepucuda_shard_export", "bepucuda_shard_import", "bepucuda_shard_set_global", "bepucuda_shard_set_body_masks", "bepucuda_shard_import_contexts",
+    "bepucuda_shard_set_fallback_rank",
     "bepucuda_color_constraints", "bepucuda_color_hash", "bepucuda_set_body_shapes", "bepucuda_predict_bounding_boxes",
     "bepucuda_set_body_accelerations", "bepucuda_set_point_gravity",
 ]

@@ -5,6 +5,7 @@ into contiguous index slabs (the active set of a pile is spatially coherent in i
 cache-optimising sorts); a constraint belongs to the rank that owns its first dynamic body. Every rank uploads ALL bodies and only ITS constraints,
 compacted, under their original batch indices, so batch k means the same colour on every rank. What crosses GPUs after a (batch, stage): the records
 the stage wrote for bodies that another rank references too (direct NVLink peer stores from the lanes that computed them, then a flag barrier).
+The sequential fallback batch is the exception: one rank, the fallback rank, owns all of it and uploads its type batches as the host has them.
 """
 import ctypes as C
 
@@ -21,18 +22,11 @@ class IpcHandles(C.Structure):
     _fields_ = [("bytes", (C.c_ubyte * 64) * 4)]
 
 
-def partition(simulation, rank_count):
-    """Splits the host simulation's type batches by owner rank. Returns (shards, first_batch, constrained, masks):
-    shards[r] = list of dicts {batch_index, type_batch_index, type_id, count, refs, prestep, impulses, source (indices into the global type batch)};
-    first_batch[body] = lowest batch referencing it as a dynamic body (INT32_MAX if none); constrained[body]; masks[body] = bit r set when rank r references it."""
+def _constraint_owners(simulation, rank_count):
+    """Per type batch: (tb, flat refs [constraint, body slot], body indices, dynamic mask, owner rank: the slab of the constraint's first dynamic body,
+    rank 0 if it has none, -1 for a hole), and whether the constraint has a dynamic body."""
     n = simulation.body_count
-    W = simulation.bundle_width
     owner_of_body = (np.arange(n, dtype=np.int64) * rank_count) // max(n, 1)
-    first_batch = np.full(n, INT32_MAX, dtype=np.int32)
-    constrained = np.zeros(n, dtype=np.uint8)
-    masks = np.zeros(n, dtype=np.uint8)
-    shards = [[] for _ in range(rank_count)]
-    per_tb = []
     for tb in simulation.type_batches():
         refs = tb.body_references  # [bundles, bodies, W]
         nb = refs.shape[1]
@@ -40,19 +34,55 @@ def partition(simulation, rank_count):
         valid = flat[:, 0] >= 0
         idx = flat & INDEX_MASK
         dynamic = (flat >= 0) & ((flat & KINEMATIC_BIT) == 0)
-        # owner rank of a constraint: the slab of its first dynamic body (rank 0 if it has none)
         first_dyn = np.argmax(dynamic, axis=1)
         has_dyn = dynamic.any(axis=1)
-        owner = np.where(has_dyn, owner_of_body[idx[np.arange(idx.shape[0]), first_dyn]], 0)
-        owner = np.where(valid, owner, -1)
-        for s in range(nb):
-            sel = valid & dynamic[:, s]
+        first_body = np.where(has_dyn, idx[np.arange(idx.shape[0]), first_dyn], 0)  # holes of the fallback batch have no body
+        owner = np.where(has_dyn, owner_of_body[first_body], 0)
+        yield tb, flat, idx, dynamic, np.where(valid, owner, -1), valid & has_dyn
+
+
+def fallback_rank(simulation, rank_count):
+    """The rank that runs the whole sequential fallback batch (bepucuda_shard_set_fallback_rank), -1 when the graph has none: the rank whose body slab
+    holds the most first dynamic bodies of fallback constraints, the lowest on a tie. It depends on the scene alone, so every rank derives the same."""
+    counts, any_fallback = np.zeros(rank_count, dtype=np.int64), False
+    for tb, _, _, _, owner, has_dyn in _constraint_owners(simulation, rank_count):
+        if tb.batch_index >= simulation.fallback_batch_threshold and tb.constraint_count > 0:
+            any_fallback = True
+            counts += np.bincount(owner[has_dyn], minlength=rank_count)
+    return int(np.argmax(counts)) if any_fallback else -1
+
+
+def partition(simulation, rank_count):
+    """Splits the host simulation's type batches by owner rank. Returns (shards, first_batch, constrained, masks):
+    shards[r] = list of dicts {batch_index, type_batch_index, type_id, count, refs, prestep, impulses, source (indices into the global type batch)};
+    first_batch[body] = lowest batch referencing it as a dynamic body (INT32_MAX if none); constrained[body]; masks[body] = bit r set when rank r references it.
+    Every constraint of the sequential fallback batch belongs to fallback_rank(), whose type batches are the host's verbatim (source = identity):
+    the device levelises them by host bundle, so repacking would change the levels and the result."""
+    n = simulation.body_count
+    W = simulation.bundle_width
+    fallback = fallback_rank(simulation, rank_count)
+    first_batch = np.full(n, INT32_MAX, dtype=np.int32)
+    constrained = np.zeros(n, dtype=np.uint8)
+    masks = np.zeros(n, dtype=np.uint8)
+    shards = [[] for _ in range(rank_count)]
+    per_tb = []
+    for tb, flat, idx, dynamic, owner, _ in _constraint_owners(simulation, rank_count):
+        if tb.batch_index >= simulation.fallback_batch_threshold:
+            owner = np.where(owner >= 0, fallback, -1)
+        for s in range(flat.shape[1]):
+            sel = (owner >= 0) & dynamic[:, s]
             np.minimum.at(first_batch, idx[sel, s], tb.batch_index)
             constrained[idx[sel, s]] = 1
             np.bitwise_or.at(masks, idx[sel, s], (1 << owner[sel]).astype(np.uint8))
         per_tb.append((tb, flat, idx, dynamic, owner))
     constrained[np.asarray(simulation.constrained_kinematics, dtype=np.int64)] = 1
     for tb, flat, idx, dynamic, owner in per_tb:
+        if tb.batch_index >= simulation.fallback_batch_threshold:
+            if tb.constraint_count > 0:
+                shards[fallback].append({"batch_index": tb.batch_index, "type_batch_index": tb.type_batch_index, "type_id": tb.type_id, "count": tb.constraint_count,
+                                         "source": np.arange(tb.constraint_count), "refs": tb.body_references.copy(), "prestep": tb.prestep.copy(),
+                                         "impulses": tb.accumulated_impulses.copy(), "idx": idx, "dynamic": dynamic})
+            continue
         pre = tb.prestep.transpose(0, 2, 1).reshape(-1, tb.prestep.shape[1])[:tb.constraint_count]
         imp = tb.accumulated_impulses.transpose(0, 2, 1).reshape(-1, tb.accumulated_impulses.shape[1])[:tb.constraint_count]
         for r in range(rank_count):
@@ -85,7 +115,8 @@ class ShardedSolver:
         self._cuda, _ = native.load_libraries()
         for name, args in (("bepucuda_shard_export", [C.c_void_p, C.POINTER(IpcHandles)]), ("bepucuda_shard_import", [C.c_void_p, C.c_int32, C.c_int32, C.POINTER(IpcHandles)]),
                            ("bepucuda_shard_set_global", [C.c_void_p, C.c_void_p, C.c_void_p]),
-                           ("bepucuda_shard_set_body_masks", [C.c_void_p, C.c_void_p]), ("bepucuda_shard_import_contexts", [C.c_void_p, C.c_int32, C.c_int32, C.POINTER(C.c_void_p)])):
+                           ("bepucuda_shard_set_body_masks", [C.c_void_p, C.c_void_p]), ("bepucuda_shard_import_contexts", [C.c_void_p, C.c_int32, C.c_int32, C.POINTER(C.c_void_p)]),
+                           ("bepucuda_shard_set_fallback_rank", [C.c_void_p, C.c_int32])):
             getattr(self._cuda, name).argtypes = args
         self.sim, self.rank, self.rank_count = simulation, rank, rank_count
         cfg = native.Config()
@@ -96,6 +127,7 @@ class ShardedSolver:
             raise native.BepuCudaError(rc, "bepucuda_create failed")
         self._ctx = ctx
         self.shards, self.first_batch, self.constrained, self.masks = partition(simulation, rank_count)
+        self.fallback_rank = fallback_rank(simulation, rank_count)
         self.shard = self.shards[rank]
         self.bodies = simulation.bodies.copy()
 
@@ -127,6 +159,8 @@ class ShardedSolver:
     def describe(self):
         sim = self.sim
         self._check(self._cuda.bepucuda_shard_set_global(self._ctx, self.first_batch.ctypes.data, self.constrained.ctypes.data))
+        if self.fallback_rank >= 0:
+            self._check(self._cuda.bepucuda_shard_set_fallback_rank(self._ctx, self.fallback_rank))
         self._check(self._cuda.bepucuda_begin_constraints(self._ctx, sim.bundle_width, sim.batch_count))
         for tb in self.shard:
             self._check(self._cuda.bepucuda_upload_type_batch(self._ctx, tb["batch_index"], tb["type_batch_index"], tb["type_id"], tb["count"], tb["refs"].ctypes.data,

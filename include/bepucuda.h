@@ -296,11 +296,17 @@ uint32_t bepucuda_color_hash(uint32_t constraint_index);
  *   bepucuda_shard_set_global: per body, the lowest batch index that references it as a dynamic body on ANY rank (INT32_MAX if none) -- the owner of
  *     its integration, Solver_Solve.cs:L951-1044 -- and whether any rank constrains it (final pose pass, PoseIntegrator.cs:L537-693).
  *   bepucuda_shard_set_body_masks: rank_masks[body] has bit r set when rank r references the body (NULL: BEPUCUDA_ERR_INVALID_ARGUMENT).
- * Call order: upload_bodies, shard_export, (exchange handles), shard_import, shard_set_global, shard_set_body_masks, begin/upload/end_constraints.
+ *   bepucuda_shard_set_fallback_rank: the rank in [0, rank_count) that owns EVERY constraint of the sequential fallback batch, or -1 (the default) for
+ *     none; call it on every rank with the same value, before bepucuda_end_constraints. That rank uploads the fallback type batches as the host has
+ *     them (not compacted: the device levelises them by host bundle, Solver_Solve.cs:L546-583 runs them on one worker) and runs the whole fallback
+ *     part of every WarmStart / Solve pass, while the other ranks hand off once before and once after it. Out of range, or a context not in peer
+ *     mode: BEPUCUDA_ERR_INVALID_ARGUMENT.
+ * Call order: upload_bodies, shard_export, (exchange handles), shard_import, shard_set_global, shard_set_body_masks, shard_set_fallback_rank (graphs
+ * with a fallback batch), begin/upload/end_constraints.
  * In peer mode bepucuda_end_constraints returns BEPUCUDA_ERR_BAD_STATE when shard_set_body_masks was not called for the current body count, and when
- * a constraint lies in the sequential fallback batch, which is not supported across ranks. Every rank must have finished uploading a frame's bodies
- * before any rank's bepucuda_solve can complete its first stage: the solve starts with a rank barrier, so issuing upload and solve on each rank in
- * that order is enough. BEPUCUDA_EXEC_GRAPH or _STREAM. */
+ * a constraint of the sequential fallback batch is uploaded on a rank other than the fallback rank (or no fallback rank is set; the message names the
+ * fallback rank). Every rank must have finished uploading a frame's bodies before any rank's bepucuda_solve can complete its first stage: the solve
+ * starts with a rank barrier, so issuing upload and solve on each rank in that order is enough. BEPUCUDA_EXEC_GRAPH or _STREAM. */
 typedef struct bepucuda_ipc_handles {
     unsigned char bytes[4][64];
 } bepucuda_ipc_handles;
@@ -311,6 +317,7 @@ int32_t bepucuda_shard_import(bepucuda_ctx* ctx, int32_t rank, int32_t rank_coun
 int32_t bepucuda_shard_import_contexts(bepucuda_ctx* ctx, int32_t rank, int32_t rank_count, bepucuda_ctx* const* all_ranks);
 int32_t bepucuda_shard_set_global(bepucuda_ctx* ctx, const int32_t* first_batch_per_body, const uint8_t* constrained_per_body);
 int32_t bepucuda_shard_set_body_masks(bepucuda_ctx* ctx, const uint8_t* rank_masks);
+int32_t bepucuda_shard_set_fallback_rank(bepucuda_ctx* ctx, int32_t rank);
 
 #ifdef __cplusplus
 }

@@ -71,6 +71,8 @@ namespace BepuCuda
         [DllImport(Lib)] public static extern int bepucuda_shard_set_global(IntPtr ctx, int* firstBatchPerBody, byte* constrainedPerBody);
         [DllImport(Lib)] public static extern int bepucuda_shard_set_body_masks(IntPtr ctx, byte* rankMasks);
         [DllImport(Lib)] public static extern int bepucuda_shard_import_contexts(IntPtr ctx, int rank, int rankCount, IntPtr* allRanks);
+        /// <summary>The rank that runs the whole sequential fallback batch of a sharded graph (-1: none); same value on every rank, before end_constraints.</summary>
+        [DllImport(Lib)] public static extern int bepucuda_shard_set_fallback_rank(IntPtr ctx, int rank);
         /// <summary>PredictBoundingBoxes on the device: sleep candidacy + bounds and speculative margins of sphere / capsule / box / cylinder bodies from the resident body state.</summary>
         [DllImport(Lib)] public static extern int bepucuda_set_body_shapes(IntPtr ctx, BodyShape* shapes, int bodyCount);
         [DllImport(Lib)] public static extern int bepucuda_predict_bounding_boxes(IntPtr ctx, float dt, BodyActivity* activities, float* boundsOut);
