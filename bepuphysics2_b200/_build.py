@@ -99,9 +99,9 @@ def build(force=False, verbose=False, variant=None, defines=()):
     flavours = [("fast", ["-DBEPU_NS=bepu_fast", "-prec-sqrt=false"]), ("strict", ["-DBEPU_NS=bepu_strict", "-fmad=false"])]
     # (object, source, extra flags)
     units = [("solver_%s_%d.o" % (name, unit), "bepu_solver_kernels.cu", flags + ["-DBEPU_UNIT=%d" % unit]) for unit in (1, 0, 2, 3) for name, flags in flavours]
-    units += [("layout.o", "bepu_layout_kernels.cu", []), ("coloring.o", "bepu_coloring.cu", []), ("bounds.o", "bepu_bounds.cu", ["-fmad=false"]), ("api.o", "bepucuda_api.cu", []),
+    units += [("layout.o", "bepu_layout_kernels.cu", []), ("coloring.o", "bepu_coloring.cu", []), ("islands.o", "bepu_islands.cu", []), ("bounds.o", "bepu_bounds.cu", ["-fmad=false"]), ("api.o", "bepucuda_api.cu", []),
               ("topology.o", "bepu_topology.cpp", [])]
-    all_sources = [os.path.join(CSRC, f) for f in ("bepu_solver_kernels.cu", "bepu_layout_kernels.cu", "bepu_coloring.cu", "bepu_bounds.cu", "bepucuda_api.cu", "bepu_topology.cpp")] + headers
+    all_sources = [os.path.join(CSRC, f) for f in ("bepu_solver_kernels.cu", "bepu_layout_kernels.cu", "bepu_coloring.cu", "bepu_islands.cu", "bepu_bounds.cu", "bepucuda_api.cu", "bepu_topology.cpp")] + headers
     # Nothing to compile when the library was built from exactly these sources (content stamp written after a build: survives a snapshot that
     # does not keep modification times) or is newer than every source. Object files need not travel with a snapshot.
     stamp = LIB_CUDA + ".stamp"

@@ -9,6 +9,7 @@
 #include "../../include/bepucuda.h"
 #include "bepu_layout_kernels.h"
 #include "bepu_coloring.h"
+#include "bepu_islands.h"
 #include "bepu_bounds.h"
 #include "bepu_topology.h"
 
@@ -161,6 +162,7 @@ struct bepucuda_ctx {
     DeviceBuffer body_shapes, body_activities, body_bounds;  // bepucuda_set_body_shapes / bepucuda_predict_bounding_boxes
     int shape_count = -1;
     DeviceBuffer color_refs, color_priorities, color_body_min, color_body_mask, color_out, color_lists, color_counts;  // bepucuda_color_constraints
+    DeviceBuffer island_activities, island_label, island_blocked, island_count, island_flags, island_roots, island_counts, island_scalars, island_temp;  // bepucuda_find_sleepable_islands
     std::vector<cudaEvent_t> profile_events;
 };
 
@@ -479,7 +481,7 @@ int32_t bepucuda_destroy(bepucuda_ctx* ctx) {
     invalidate_graph(ctx);
     for (void* p : ctx->opened_ipc) cudaIpcCloseMemHandle(p);
     DeviceBuffer* bufs[] = {&ctx->shard_flags, &ctx->peer32, &ctx->body_masks_dev, &ctx->boundary_flags_dev, &ctx->global_first_batch_dev, &ctx->raw_bodies, &ctx->pose, &ctx->velocity, &ctx->inertia_local, &ctx->inertia_world, &ctx->constrained, &ctx->first_batch, &ctx->sync_refcount,
-                            &ctx->sync_mask, &ctx->chunk_table, &ctx->record_table, &ctx->ref_rows, &ctx->body_shapes, &ctx->body_activities, &ctx->body_bounds, &ctx->color_refs, &ctx->color_priorities, &ctx->color_body_min, &ctx->color_body_mask, &ctx->color_out, &ctx->color_lists, &ctx->color_counts, &ctx->source_bundle_flags, &ctx->refs32, &ctx->prestep32, &ctx->impulses32, &ctx->tb_table, &ctx->tdesc_table, &ctx->work_table, &ctx->map_table,
+                            &ctx->sync_mask, &ctx->chunk_table, &ctx->record_table, &ctx->ref_rows, &ctx->body_shapes, &ctx->body_activities, &ctx->body_bounds, &ctx->color_refs, &ctx->color_priorities, &ctx->color_body_min, &ctx->color_body_mask, &ctx->color_out, &ctx->color_lists, &ctx->color_counts, &ctx->island_activities, &ctx->island_label, &ctx->island_blocked, &ctx->island_count, &ctx->island_flags, &ctx->island_roots, &ctx->island_counts, &ctx->island_scalars, &ctx->island_temp, &ctx->source_bundle_flags, &ctx->refs32, &ctx->prestep32, &ctx->impulses32, &ctx->tb_table, &ctx->tdesc_table, &ctx->work_table, &ctx->map_table,
                             &ctx->bodies_per_type, &ctx->kinematics_dev, &ctx->frame_params_dev, &ctx->error_dev, &ctx->accelerations};
     for (auto b : bufs) b->release();
     if (ctx->accelerations_stage) cudaFreeHost(ctx->accelerations_stage);
@@ -1223,6 +1225,78 @@ int32_t bepucuda_color_constraints(bepucuda_ctx* ctx, int32_t constraint_count, 
     int32_t highest = -1;
     for (size_t i = 0; i < nc; ++i) highest = std::max(highest, batch_indices_out[i]);
     if (batch_count_out) *batch_count_out = highest + 1;
+    if (rounds_out) *rounds_out = (int32_t)std::min<int64_t>(rounds, 0x7fffffff);
+    return BEPUCUDA_OK;
+}
+
+int32_t bepucuda_find_sleepable_islands(bepucuda_ctx* ctx, const bepucuda_body_activity* activities, int32_t body_count, int32_t* island_of_body_out,
+                                        int32_t* sleepable_roots_out, int32_t* sleepable_body_counts_out, int32_t* sleepable_count_out, int32_t* rounds_out) {
+    if (!ctx) return BEPUCUDA_ERR_INVALID_ARGUMENT;
+    if (ctx->peer_mode) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, "find_sleepable_islands in peer mode: a rank holds only its own constraints and cannot see whole islands");
+    if (!ctx->constraints_ready) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, "find_sleepable_islands before end_constraints");
+    if (body_count != ctx->body_count) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "find_sleepable_islands: the body count must match the last upload_bodies");
+    if (!sleepable_count_out || (body_count > 0 && (!activities || !sleepable_roots_out || !sleepable_body_counts_out)))
+        return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "find_sleepable_islands: null buffer");
+    *sleepable_count_out = 0;
+    if (rounds_out) *rounds_out = 0;
+    if (body_count == 0) return BEPUCUDA_OK;
+    CK(cudaSetDevice(ctx->device));
+    const size_t n = (size_t)body_count;
+    CK(ctx->island_activities.reserve(n * sizeof(bepucuda_body_activity)));
+    CK(ctx->island_label.reserve(n * 4));
+    CK(ctx->island_blocked.reserve(n * 4));
+    CK(ctx->island_count.reserve(n * 4));
+    CK(ctx->island_flags.reserve(n));
+    CK(ctx->island_roots.reserve(n * 4));
+    CK(ctx->island_counts.reserve(n * 4));
+    CK(ctx->island_scalars.reserve(8));  // [0]: hook pass changed something, [1]: number of sleepable roots
+    IslandBuffers ib{};
+    ib.tbs = ctx->tb_table.as<DeviceTypeBatch>();
+    ib.work = ctx->work_table.as<WorkItem>();
+    ib.work_count = ctx->topo.all_work_count;
+    ib.bodies_per_type = ctx->bodies_per_type.as<int32_t>();
+    ib.activities = ctx->island_activities.as<uint8_t>();
+    ib.label = ctx->island_label.as<int32_t>();
+    ib.blocked = ctx->island_blocked.as<int32_t>();
+    ib.count = ctx->island_count.as<int32_t>();
+    ib.changed = ctx->island_scalars.as<unsigned int>();
+    ib.body_count = body_count;
+    int32_t* selected = ctx->island_scalars.as<int32_t>() + 1;
+    size_t temp_bytes = 0;
+    CK(launch_island_select(ib, nullptr, nullptr, nullptr, selected, nullptr, &temp_bytes, ctx->stream));
+    CK(ctx->island_temp.reserve(std::max(temp_bytes, (size_t)16)));
+    temp_bytes = ctx->island_temp.capacity;
+    CK(cudaMemcpyAsync(ctx->island_activities.ptr, activities, n * sizeof(bepucuda_body_activity), cudaMemcpyHostToDevice, ctx->stream));
+    launch_island_init(ib, ctx->stream);
+    CK(cudaGetLastError());
+    // every round that changes something joins at least two trees, so there are at most body_count of them; in practice O(log n)
+    int64_t rounds = 0;
+    if (ib.work_count > 0) {
+        for (;;) {
+            CK(cudaMemsetAsync(ib.changed, 0, 4, ctx->stream));
+            launch_island_round(ib, ctx->stream);
+            unsigned int changed = 0;
+            CK(cudaMemcpyAsync(&changed, ib.changed, 4, cudaMemcpyDeviceToHost, ctx->stream));
+            CK(cudaStreamSynchronize(ctx->stream));
+            CK(cudaGetLastError());
+            ++rounds;
+            if (!changed) break;
+            if (rounds > (int64_t)body_count) return fail(ctx, BEPUCUDA_ERR_CUDA, "find_sleepable_islands: no convergence (internal error)");
+        }
+    }
+    launch_island_verdict(ib, ctx->stream);
+    CK(launch_island_select(ib, ctx->island_flags.as<uint8_t>(), ctx->island_roots.as<int32_t>(), ctx->island_counts.as<int32_t>(), selected, ctx->island_temp.ptr, &temp_bytes,
+                            ctx->stream));
+    int32_t count = 0;
+    CK(cudaMemcpyAsync(&count, selected, 4, cudaMemcpyDeviceToHost, ctx->stream));
+    if (island_of_body_out) CK(cudaMemcpyAsync(island_of_body_out, ib.label, n * 4, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    if (count > 0) {
+        CK(cudaMemcpyAsync(sleepable_roots_out, ctx->island_roots.ptr, (size_t)count * 4, cudaMemcpyDeviceToHost, ctx->stream));
+        CK(cudaMemcpyAsync(sleepable_body_counts_out, ctx->island_counts.ptr, (size_t)count * 4, cudaMemcpyDeviceToHost, ctx->stream));
+        CK(cudaStreamSynchronize(ctx->stream));
+    }
+    *sleepable_count_out = count;
     if (rounds_out) *rounds_out = (int32_t)std::min<int64_t>(rounds, 0x7fffffff);
     return BEPUCUDA_OK;
 }

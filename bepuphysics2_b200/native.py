@@ -114,7 +114,7 @@ C_ABI_SYMBOLS = [
     "bepucuda_shard_export", "bepucuda_shard_import", "bepucuda_shard_set_global", "bepucuda_shard_set_body_masks", "bepucuda_shard_import_contexts",
     "bepucuda_shard_set_fallback_rank",
     "bepucuda_color_constraints", "bepucuda_color_hash", "bepucuda_set_body_shapes", "bepucuda_predict_bounding_boxes",
-    "bepucuda_set_body_accelerations", "bepucuda_set_point_gravity",
+    "bepucuda_set_body_accelerations", "bepucuda_set_point_gravity", "bepucuda_find_sleepable_islands",
 ]
 
 
@@ -180,6 +180,7 @@ def load_libraries():
     cuda.bepucuda_color_hash.restype = C.c_uint32
     cuda.bepucuda_set_body_accelerations.argtypes = [vp, vp, i32]
     cuda.bepucuda_set_point_gravity.argtypes = [vp, i32, vp, f32]
+    cuda.bepucuda_find_sleepable_islands.argtypes = [vp, vp, i32, vp, vp, vp, C.POINTER(i32), C.POINTER(i32)]
 
     host.bepuhost_create.restype = vp
     host.bepuhost_create.argtypes = [i32, i32]
@@ -432,6 +433,20 @@ class CudaTimestepper:
         bounds = np.zeros((max(activities.shape[0], 1), 8), dtype=np.float32)
         self._check(self._cuda.bepucuda_predict_bounding_boxes(self._ctx, dt, activities.ctypes.data, bounds.ctypes.data))
         return bounds[:activities.shape[0]]
+
+    def find_sleepable_islands(self, activities):
+        """bepucuda_find_sleepable_islands over the constraint graph of the last describe(): `activities` (BODY_ACTIVITY_DTYPE, one record per body;
+        only sleep_candidate is read). Returns (island_of_body, roots, counts, rounds): per body the smallest body index of its island, the
+        islands whose bodies are all sleep candidates in ascending order, their body counts, and the device rounds the search took."""
+        activities = np.ascontiguousarray(activities, dtype=BODY_ACTIVITY_DTYPE)
+        n = activities.shape[0]
+        labels = np.zeros(max(n, 1), dtype=np.int32)
+        roots = np.zeros(max(n, 1), dtype=np.int32)
+        counts = np.zeros(max(n, 1), dtype=np.int32)
+        count, rounds = C.c_int32(), C.c_int32()
+        self._check(self._cuda.bepucuda_find_sleepable_islands(self._ctx, activities.ctypes.data, n, labels.ctypes.data, roots.ctypes.data, counts.ctypes.data,
+                                                               C.byref(count), C.byref(rounds)))
+        return labels[:n], roots[:count.value].copy(), counts[:count.value].copy(), rounds.value
 
     def register_host_buffers(self):
         """Page-locks the simulation's buffers (a C# host would register its BufferPool blocks once)."""

@@ -281,6 +281,26 @@ int32_t bepucuda_color_constraints(bepucuda_ctx* ctx, int32_t constraint_count, 
 /* The hash behind BEPUCUDA_COLOR_HASHED_ORDER: h = i * 0x9E3779B1; h ^= h >> 15; h *= 0x85EBCA77; h ^= h >> 13; h *= 0xC2B2AE3D; h ^= h >> 16 (uint32). */
 uint32_t bepucuda_color_hash(uint32_t constraint_index);
 
+/* Sleepable islands on the device: the search of Simulation.Sleep (IslandSleeper.CollectIsland with the SleepPredicate,
+ * BepuPhysics/IslandSleeper.cs:L85-223), for every island of the constraint graph the device holds at once instead of from a sampled fraction of
+ * the active bodies (TestedFractionPerFrame, Update L925-963).
+ *   graph: two active-set bodies share an island when one constraint of the last bepucuda_end_constraints references both -- every batch, the
+ *     sequential fallback batch included, every body slot of 1- to 4-body types. Kinematic references connect islands like any other: CollectIsland
+ *     walks Solver.EnumerateConnectedBodyReferences, which reports decoded references (Solver.cs:L1781-1784). Empty lanes (-1) are skipped. A body
+ *     no constraint references is an island of its own.
+ *   island_of_body_out[b] (optional, body_count entries): the smallest active-set index in b's island. The label is unique, so the result does not
+ *     depend on the order of the device's atomics.
+ *   An island is sleepable when every body in it has activities[i].sleep_candidate != 0 -- exactly when CollectIsland(start, SleepPredicate)
+ *     returns true for any start body in it. sleepable_roots_out receives the labels of the sleepable islands in ascending order,
+ *     sleepable_body_counts_out their body counts (so the host can apply TargetSleptFraction itself), *sleepable_count_out how many there are;
+ *     both arrays need room for body_count entries. *rounds_out (optional): hook-and-shortcut rounds the device ran (each ends with one flag read by the host; they grow like log n,
+ *     not like the island's diameter).
+ * Reads only activities[i].sleep_candidate; reads and writes no body, impulse or prestep state and leaves the captured graph valid. Blocks until the
+ * outputs are written. BEPUCUDA_ERR_BAD_STATE before the first bepucuda_end_constraints and in peer mode (a rank holds only its own constraints);
+ * BEPUCUDA_ERR_INVALID_ARGUMENT when body_count differs from the last bepucuda_upload_bodies or a required pointer is NULL. */
+int32_t bepucuda_find_sleepable_islands(bepucuda_ctx* ctx, const bepucuda_body_activity* activities, int32_t body_count, int32_t* island_of_body_out,
+                                        int32_t* sleepable_roots_out, int32_t* sleepable_body_counts_out, int32_t* sleepable_count_out, int32_t* rounds_out);
+
 /* Multi-GPU, ONE constraint graph over several GPUs with direct NVLink peer stores (SURVEY.md §8e; replaces the reference's multithreaded batch
  * dispatch, Solver_Solve.cs:L458-654, where workers split the constraints of a batch). Bodies are partitioned into owner slabs by the host; every
  * rank (one context per GPU, normally one process per GPU) uploads ALL bodies (only its own slab and the halo it references are kept current) and
