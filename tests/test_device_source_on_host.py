@@ -23,14 +23,19 @@ LANES = 32
 DT = 1.0 / 240.0  # a substep of the 8 x 2 configuration at 1/30 s
 
 
+def compile_device_on_host(lib, optimisation=("-O2",)):
+    """The build recipe of the harness: g++ with the arithmetic of the strict build; `optimisation` replaces -O2 (the coverage build)."""
+    src = os.path.join(HERE, "device_on_host.cpp")
+    subprocess.check_call(["/usr/bin/g++"] + list(optimisation) + ["-std=c++17", "-ffp-contract=off", "-fno-fast-math", "-march=x86-64-v3", "-Wall", "-Wno-unused-function", "-Wno-unknown-pragmas", "-pthread",
+                                                                   "-I", os.path.join(HERE, "stubs"), "-I", HERE, "-I", CSRC, "-shared", "-fPIC", "-o", lib, src])
+
+
 @pytest.fixture(scope="module")
 def device_on_host():
     lib = os.path.join(HERE, "libdevice_on_host.so")
-    defines = []
     srcs = [os.path.join(HERE, "device_on_host.cpp"), os.path.join(HERE, "stubs", "cuda_runtime.h")] + [os.path.join(CSRC, f) for f in ("bepu_device_math.cuh", "bepu_contacts.cuh", "bepu_joints.cuh", "bepu_joints_more.cuh", "bepu_integration.cuh", "bepu_bounds_math.cuh", "bepu_redistribute.cuh")]
     if not os.path.exists(lib) or any(os.path.getmtime(s) > os.path.getmtime(lib) for s in srcs):
-        subprocess.check_call(["/usr/bin/g++", "-O2", "-std=c++17", "-ffp-contract=off", "-fno-fast-math", "-march=x86-64-v3", "-Wall", "-Wno-unused-function", "-Wno-unknown-pragmas", "-pthread"] + defines +
-                              ["-I", os.path.join(HERE, "stubs"), "-I", HERE, "-I", CSRC, "-shared", "-fPIC", "-o", lib, srcs[0]])
+        compile_device_on_host(lib)
     dev = C.CDLL(lib)
     fp = C.POINTER(C.c_float)
     dev.device_on_host_eval_lane.argtypes = [C.c_int32, C.c_int32, fp, C.c_float, fp, fp, fp]
