@@ -71,9 +71,14 @@ void launch_stage(int kernel, const WorkRecord* records, const int32_t* ref_rows
                                                                                      shard->stage);
             else if (kernel == kKernelDeep)
                 launch_stage_kernel<constraint_stage_kernel<STAGE, BEPU_DEEP_MINB, kExt, false>>(work_count, 0u, flags, s, records, ref_rows, work_count, B, fp, flags);
-            else if (kernel == kKernelContacts)
+            else if (kernel == kKernelContacts) {
+                if constexpr (STAGE == kStageWarmStart && !kExt) {
+                    if (bepucuda::integrated_warm_start_launch(STAGE, bepucuda::StageLaunch{kernel, flags}))
+                        return launch_stage_kernel<integrated_constraint_stage_kernel<STAGE, kContactMinb, false, true>>(work_count, 0u, flags, s, records, ref_rows, work_count, B, fp,
+                                                                                                                         flags);
+                }
                 launch_stage_kernel<constraint_stage_kernel<STAGE, kContactMinb, kExt, true>>(work_count, 0u, flags, s, records, ref_rows, work_count, B, fp, flags);
-            else launch_stage_kernel<constraint_stage_kernel<STAGE, 1, kExt, false>>(work_count, 0u, flags, s, records, ref_rows, work_count, B, fp, flags);
+            } else launch_stage_kernel<constraint_stage_kernel<STAGE, 1, kExt, false>>(work_count, 0u, flags, s, records, ref_rows, work_count, B, fp, flags);
         };
         if constexpr (STAGE != kStageSolve) {
             if (flags & kLaunchIntegratorExtensions) return launch(std::true_type{});

@@ -453,7 +453,9 @@ BEPU_DI void integrate_body_pose(int i, const BodyBuffers& B, const FrameParams*
     store_pose(B.pose, (uint32_t)i, pos, q);
     store_inertia(B.inertia_world, (uint32_t)i, world);
 }
-template <int STAGE, bool kSharded, bool kExt, bool kContacts, bool kEarlyBodies>
+// kIntegrated: the contact-only WarmStart of the launches with kLaunchBodiesIntegrated (integrated_constraint_stage_kernel). The other contact-only
+// WarmStart instantiation is launched only without that flag, so it compiles no integrated path; the full-switch kernels read the flag.
+template <int STAGE, bool kSharded, bool kExt, bool kContacts, bool kEarlyBodies, bool kIntegrated = false>
 BEPU_DI void constraint_stage_body(const WorkRecord* __restrict__ records, const int32_t* __restrict__ ref_rows, int work_count, const BodyBuffers& B, const FrameParams* __restrict__ fpp, int flags, const ShardPeers* peers,
                                    long long peer_delta, const ShardStage* shard = nullptr) {
     constexpr bool kStaged = STAGE != kStageIncremental;
@@ -496,8 +498,8 @@ BEPU_DI void constraint_stage_body(const WorkRecord* __restrict__ records, const
         enc0 = ldg_nc_u32(ref_rows + (size_t)warp * (2 * kLanes) + lane);
         enc1 = ldg_nc_u32(ref_rows + (size_t)warp * (2 * kLanes) + kLanes + lane);
         if constexpr (kStaged && kEarlyBodies) {
-            // world mode on a WarmStart only in the instantiation the host launches it in: contact-only, without kExt
-            constexpr bool kWorld = STAGE == kStageSolve || (STAGE == kStageWarmStart && kContacts && !kExt), kOwned = STAGE != kStageSolve;
+            // world mode on a WarmStart only in the instantiation the host launches it in (the integrated one), owned mode never there
+            constexpr bool kWorld = STAGE == kStageSolve || kIntegrated, kOwned = STAGE != kStageSolve && !kIntegrated;
             if (kOwned && (flags & kLaunchEarlyOwned)) load_early_bodies<STAGE, kContacts>(rec.type_id, enc0, enc1, B, early);
             else if (kWorld && (flags & kLaunchEarlyWorld)) load_early_bodies<kStageSolve, kContacts>(rec.type_id, enc0, enc1, B, early);
         }
@@ -505,7 +507,7 @@ BEPU_DI void constraint_stage_body(const WorkRecord* __restrict__ records, const
     const FrameParams fp = *fpp;
     asm volatile("griddepcontrol.wait;" ::: "memory");
     asm volatile("griddepcontrol.launch_dependents;");
-    const bool integrated = STAGE == kStageWarmStart && !kExt && (flags & kLaunchBodiesIntegrated);
+    const bool integrated = kIntegrated || (STAGE == kStageWarmStart && !kExt && !kContacts && (flags & kLaunchBodiesIntegrated));
     bool boundary = false;
     if constexpr (kSharded) {
         boundary = active && (rec.live_lanes & kRecordBoundaryBit) != 0;
@@ -539,6 +541,15 @@ BEPU_DI void constraint_stage_body(const WorkRecord* __restrict__ records, const
 template <int STAGE, int MINB, bool kExt, bool kContacts>
 __global__ void __launch_bounds__(kStageBlockThreads, MINB) constraint_stage_kernel(const WorkRecord* __restrict__ records, const int32_t* __restrict__ ref_rows, int work_count, BodyBuffers B, const FrameParams* __restrict__ fpp, int flags) {
     constraint_stage_body<STAGE, false, kExt, kContacts, MINB == 1 || kContacts>(records, ref_rows, work_count, B, fpp, flags, nullptr, 0);
+}
+// The contact-only WarmStart of the launches whose poses and world inertias the incremental update of the substep integrated
+// (integrated_warm_start_launch, bepu_topology.h): its integrating lanes integrate velocity only, so it carries no pose integration, no angular-mode
+// branch and no local-inertia or pose load, about 40 % of the code of the integrating instantiation. It takes the template arguments of
+// constraint_stage_kernel, so that tools which read kernel names (tests/tools/stage_timeline.py) see one more contact-only WarmStart.
+template <int STAGE, int MINB, bool kExt, bool kContacts>
+__global__ void __launch_bounds__(kStageBlockThreads, MINB) integrated_constraint_stage_kernel(const WorkRecord* __restrict__ records, const int32_t* __restrict__ ref_rows, int work_count, BodyBuffers B, const FrameParams* __restrict__ fpp, int flags) {
+    static_assert(STAGE == kStageWarmStart && !kExt && kContacts, "integrated WarmStart launches are contact-only and never carry kExt");
+    constraint_stage_body<STAGE, false, false, true, true, true>(records, ref_rows, work_count, B, fpp, flags, nullptr, 0);
 }
 // Peer-sharded variant (bepucuda_shard_*): the lane that writes a body another rank references stores the record into that rank's arrays too.
 template <int STAGE, int MINB, bool kExt>

@@ -103,6 +103,11 @@ struct StageLaunch {
 // The one place that decides how an op of the stage program is launched: which instantiation runs, what its prologue loads before the
 // grid-dependency wait, and whether the incremental update integrates the bodies' poses.
 StageLaunch resolve_stage_launch(const StageOp& op, const LaunchContext& lc);
+// Whether a resolved launch runs the contact-only WarmStart instantiation that has no pose integration (launch_stage, bepu_solver_kernels.cu):
+// the incremental update of its substep integrates the poses. Its prologue compiles the world-inertia loads only, and it has no kExt.
+constexpr bool integrated_warm_start_launch(int32_t stage, const StageLaunch& l) {
+    return stage == kStageWarmStart && l.kernel == kKernelContacts && (l.flags & kLaunchBodiesIntegrated) != 0;
+}
 
 struct StageProgram {
     std::vector<StageOp> ops;
