@@ -348,6 +348,12 @@ StageLaunch resolve_stage_launch(const StageOp& op, const LaunchContext& lc) {
     return l;
 }
 
+bool same_launches(const LaunchContext& a, const LaunchContext& b) {
+    // resolve_stage_launch reads the angular mode only as zero / non-zero, and only without integrator extensions
+    return a.integrator_extensions == b.integrator_extensions && a.profile == b.profile &&
+           (a.integrator_extensions || (a.angular_mode == 0) == (b.angular_mode == 0));
+}
+
 int exchange_targets(const StageProgram& program, const std::vector<int32_t>& boundary_count, std::vector<unsigned long long>* targets, std::string* error) {
     if (program.exchange_count + 1 > (uint32_t)kShardMaxExchanges) {
         *error = "peer sharding: more than 4095 exchange points per solve";

@@ -90,7 +90,8 @@ constexpr int32_t kOpRowsFree = 2, kOpContactsOnly = 8, kOpBodiesFree = 16, kOpI
 // checks its copy of the threshold against this one).
 constexpr int32_t kDeepBatchBundles = 2150;
 
-// What a launch depends on besides its op. A captured graph bakes the resolved launches in, so it is rebuilt when any of these changes.
+// What a launch depends on besides its op. A captured graph bakes the resolved launches in, so it is re-captured unless same_launches holds for
+// the context it was captured with and the current one.
 struct LaunchContext {
     bool integrator_extensions;  // per-body accelerations or point gravity are set
     int32_t angular_mode;        // bepucuda_integrator_desc::angular_integration_mode
@@ -103,6 +104,8 @@ struct StageLaunch {
 // The one place that decides how an op of the stage program is launched: which instantiation runs, what its prologue loads before the
 // grid-dependency wait, and whether the incremental update integrates the bodies' poses.
 StageLaunch resolve_stage_launch(const StageOp& op, const LaunchContext& lc);
+// Whether resolve_stage_launch launches every op alike in both contexts.
+bool same_launches(const LaunchContext& a, const LaunchContext& b);
 // Whether a resolved launch runs the contact-only WarmStart instantiation that has no pose integration (launch_stage, bepu_solver_kernels.cu):
 // the incremental update of its substep integrates the poses. Its prologue compiles the world-inertia loads only, and it has no kExt.
 constexpr bool integrated_warm_start_launch(int32_t stage, const StageLaunch& l) {

@@ -18,26 +18,32 @@ using namespace bepucuda;
 namespace bepucuda {
 
 // ---- small RAII helpers ------------------------------------------------------------------------------------------------------
-struct DeviceBuffer {
+// Memory that grows on demand (contents are not kept) and is freed with its owner: device memory, or page-locked host memory.
+template <bool kPinnedHost> struct GrowBuffer {
     void* ptr = nullptr;
     size_t capacity = 0;
+    GrowBuffer() = default;
+    GrowBuffer(const GrowBuffer&) = delete;
+    GrowBuffer& operator=(const GrowBuffer&) = delete;
+    ~GrowBuffer() { release(); }
     cudaError_t reserve(size_t bytes) {
         if (bytes <= capacity) return cudaSuccess;
-        if (ptr) cudaFree(ptr);
-        ptr = nullptr;
-        capacity = 0;
+        release();
         size_t want = bytes + bytes / 4 + 256;
-        cudaError_t e = cudaMalloc(&ptr, want);
+        cudaError_t e = kPinnedHost ? cudaMallocHost(&ptr, want) : cudaMalloc(&ptr, want);
         if (e == cudaSuccess) capacity = want;
+        else ptr = nullptr;
         return e;
     }
     void release() {
-        if (ptr) cudaFree(ptr);
+        if (ptr) kPinnedHost ? cudaFreeHost(ptr) : cudaFree(ptr);
         ptr = nullptr;
         capacity = 0;
     }
     template <class T> T* as() const { return (T*)ptr; }
 };
+using DeviceBuffer = GrowBuffer<false>;
+using PinnedBuffer = GrowBuffer<true>;
 
 // Bump allocator over chunks that are never reallocated (uploads are enqueued against their addresses).
 struct ChunkArena {
@@ -45,6 +51,12 @@ struct ChunkArena {
     std::vector<Chunk> chunks;
     bool pinned_host = false;
     size_t min_chunk = (size_t)64 << 20;
+    ChunkArena() = default;
+    ChunkArena(const ChunkArena&) = delete;
+    ChunkArena& operator=(const ChunkArena&) = delete;
+    ~ChunkArena() {
+        for (auto& c : chunks) { if (pinned_host) cudaFreeHost(c.base); else cudaFree(c.base); }
+    }
     void reset() { for (auto& c : chunks) c.used = 0; }
     void* alloc(size_t bytes, cudaError_t* err) {
         bytes = (bytes + 255) & ~(size_t)255;
@@ -62,10 +74,12 @@ struct ChunkArena {
         chunks.push_back(c);
         return chunks.back().base;
     }
-    void release() {
-        for (auto& c : chunks) { if (pinned_host) cudaFreeHost(c.base); else cudaFree(c.base); }
-        chunks.clear();
-    }
+};
+
+// Pinned copy of a host buffer that the caller may reuse as soon as the upload is enqueued, and the event after which the copy has read it.
+struct StagedUpload {
+    PinnedBuffer host;
+    cudaEvent_t done = nullptr;
 };
 
 struct SourceTypeBatch {
@@ -105,9 +119,7 @@ struct bepucuda_ctx {
     // bepucuda_set_body_accelerations: device copy, the body count it was set for (-1: not set), and the pinned staging of the last upload
     DeviceBuffer accelerations;
     int accelerations_count = -1;
-    void* accelerations_stage = nullptr;
-    size_t accelerations_stage_bytes = 0;
-    cudaEvent_t accelerations_staged = nullptr;
+    StagedUpload accelerations_stage;
     // bepucuda_set_point_gravity
     bool point_gravity = false;
     float attractor_center[3] = {0.0f, 0.0f, 0.0f};
@@ -143,11 +155,13 @@ struct bepucuda_ctx {
     uint32_t exchange_counter = 0;                                  // exchange points executed so far (flag barrier sequence)
     std::vector<int32_t> kinematics;
     StageProgram program;
-    FrameParams* frame_params_host = nullptr;   // pinned
+    PinnedBuffer frame_params_host;             // FrameParams
 
+    // the captured stage sequence of the program (dropped when the program is replaced), and what its launches bake in besides the program
     cudaGraph_t graph = nullptr;
     cudaGraphExec_t graph_exec = nullptr;
-    bool graph_valid = false;
+    BodyBuffers graph_bodies{};
+    LaunchContext graph_launch{};
 
     bepucuda_timings timings{};
     int64_t h2d_accum = 0;
@@ -155,8 +169,7 @@ struct bepucuda_ctx {
     std::vector<HostRange> host_ranges;    // page-locked + device-mapped host memory registered through bepucuda_host_register
     std::vector<CopyChunk> pending_h2d;    // batched copies waiting for the next flush
     DeviceBuffer chunk_table;
-    struct ChunkStage { void* host = nullptr; size_t capacity = 0; cudaEvent_t done = nullptr; };
-    ChunkStage chunk_stage[4];             // pinned ring for chunk tables (a table must outlive its H2D copy)
+    StagedUpload chunk_stage[4];           // pinned ring for chunk tables
     int chunk_stage_next = 0;
     cudaEvent_t user_events[16] = {};
     DeviceBuffer body_shapes, body_activities, body_bounds;  // bepucuda_set_body_shapes / bepucuda_predict_bounding_boxes
@@ -199,42 +212,40 @@ void queue_chunks(std::vector<CopyChunk>& list, void* dst, const void* src, size
     const size_t kChunk = (size_t)64 << 10;
     for (size_t off = 0; off < bytes; off += kChunk) list.push_back({(char*)dst + off, (const char*)src + off, std::min(kChunk, bytes - off)});
 }
-// Runs the queued chunks as one kernel. The chunk table travels through the pinned staging arena (recycled at begin_constraints / per flush).
+// H2D copy of `bytes` at `src` through the pinned staging buffer of `st`.
+int upload_staged(bepucuda_ctx* ctx, StagedUpload& st, void* dst, const void* src, size_t bytes) {
+    if (!st.done) CK(cudaEventCreateWithFlags(&st.done, cudaEventDisableTiming));
+    CK(cudaEventSynchronize(st.done));  // the previous upload has left the staging buffer
+    CK(st.host.reserve(bytes));
+    std::memcpy(st.host.ptr, src, bytes);
+    CK(cudaMemcpyAsync(dst, st.host.ptr, bytes, cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaEventRecord(st.done, ctx->stream));
+    return BEPUCUDA_OK;
+}
+
+// Runs the queued chunks as one kernel. The chunk table travels through a ring of pinned staging buffers.
 int flush_chunks(bepucuda_ctx* ctx, std::vector<CopyChunk>& list) {
     if (list.empty()) return BEPUCUDA_OK;
     const size_t bytes = list.size() * sizeof(CopyChunk);
     CK(ctx->chunk_table.reserve(bytes));
-    auto& st = ctx->chunk_stage[ctx->chunk_stage_next];
+    StagedUpload& st = ctx->chunk_stage[ctx->chunk_stage_next];
     ctx->chunk_stage_next = (ctx->chunk_stage_next + 1) & 3;
-    if (!st.done) CK(cudaEventCreateWithFlags(&st.done, cudaEventDisableTiming));
-    CK(cudaEventSynchronize(st.done));  // its previous use (4 flushes ago) is long finished
-    if (st.capacity < bytes) {
-        if (st.host) cudaFreeHost(st.host);
-        st.host = nullptr;
-        st.capacity = 0;
-        CK(cudaMallocHost(&st.host, bytes * 2));
-        st.capacity = bytes * 2;
-    }
-    std::memcpy(st.host, list.data(), bytes);
     // The device-side table is reused by every flush: stream order keeps the previous batched copy ahead of this overwrite.
-    CK(cudaMemcpyAsync(ctx->chunk_table.ptr, st.host, bytes, cudaMemcpyHostToDevice, ctx->stream));
+    { int rc = upload_staged(ctx, st, ctx->chunk_table.ptr, list.data(), bytes); if (rc != BEPUCUDA_OK) return rc; }
     launch_batched_copy(ctx->chunk_table.as<CopyChunk>(), (int)list.size(), ctx->stream);
     CK(cudaGetLastError());
-    CK(cudaEventRecord(st.done, ctx->stream));
     list.clear();
     return BEPUCUDA_OK;
 }
 
-// H2D copy of one host buffer into the raw arena. Small buffers are packed through pinned staging so that hundreds of
-// tiny type batches do not each pay a pageable-memory DMA setup; large ones go directly (fast when the host registered them).
+// The H2D copy of constraint rows and contact feature ids. A registered (mapped) host buffer is read by the batched copy kernel at the next flush.
+// While the constraints are being described, small buffers are packed through the pinned staging arena, so that hundreds of tiny type batches do
+// not each pay a pageable-memory DMA setup; begin_constraints recycles that arena, so after end_constraints every other copy goes directly.
 int copy_in(bepucuda_ctx* ctx, void* dst, const void* src, size_t bytes) {
     if (bytes == 0) return BEPUCUDA_OK;
     if (char* alias = map_host(ctx, src, bytes)) {
-        queue_chunks(ctx->pending_h2d, dst, alias, bytes);  // read straight from the mapped host buffer by the batched copy kernel at the next flush
-        ctx->h2d_accum += (int64_t)bytes;
-        return BEPUCUDA_OK;
-    }
-    if (bytes < ((size_t)256 << 10)) {
+        queue_chunks(ctx->pending_h2d, dst, alias, bytes);
+    } else if (ctx->constraints_open && bytes < ((size_t)256 << 10)) {
         cudaError_t e = cudaSuccess;
         void* stage = ctx->pinned_arena.alloc(bytes, &e);
         if (!stage) return cuda_fail(ctx, e, "pinned staging");
@@ -247,17 +258,29 @@ int copy_in(bepucuda_ctx* ctx, void* dst, const void* src, size_t bytes) {
     return BEPUCUDA_OK;
 }
 
+SourceTypeBatch* find_source(bepucuda_ctx* ctx, int32_t batch_index, int32_t type_batch_index) {
+    for (auto& s : ctx->sources)
+        if (s.batch_index == batch_index && s.type_batch_index == type_batch_index) return &s;
+    return nullptr;
+}
+
 void invalidate_graph(bepucuda_ctx* ctx) {
     if (ctx->graph_exec) cudaGraphExecDestroy(ctx->graph_exec);
     if (ctx->graph) cudaGraphDestroy(ctx->graph);
     ctx->graph_exec = nullptr;
     ctx->graph = nullptr;
-    ctx->graph_valid = false;
 }
 
-// Per-body accelerations or point gravity set: an input of resolve_stage_launch, so switching either on or off changes the launch sequence (a
-// captured graph is rebuilt); their values are frame parameters.
-bool integrator_extensions(const bepucuda_ctx* ctx) { return ctx->accelerations_count >= 0 || ctx->point_gravity; }
+// The optional velocity terms that are set (bepucuda_set_body_accelerations / bepucuda_set_point_gravity): kIntegrateAccelerations |
+// kIntegratePointGravity. Whether any is set is an input of resolve_stage_launch; their values are frame parameters.
+uint32_t integrate_extensions(const bepucuda_ctx* ctx) {
+    return (ctx->accelerations_count >= 0 ? kIntegrateAccelerations : 0u) | (ctx->point_gravity ? kIntegratePointGravity : 0u);
+}
+LaunchContext launch_context(const bepucuda_ctx* ctx, bool profile) { return {integrate_extensions(ctx) != 0, ctx->integ.angular_integration_mode, profile}; }
+bool same_bodies(const BodyBuffers& a, const BodyBuffers& b) {
+    return a.pose == b.pose && a.velocity == b.velocity && a.inertia_local == b.inertia_local && a.inertia_world == b.inertia_world && a.constrained == b.constrained &&
+           a.first_batch == b.first_batch && a.count == b.count;
+}
 
 // Profiling sink of issue_stage_sequence: the launch of program op i sets launched[i] and is bracketed by events[2i] and events[2i + 1].
 struct StageEvents {
@@ -274,7 +297,7 @@ void issue_stage_sequence(bepucuda_ctx* ctx, cudaStream_t s, int64_t* launches, 
     const int32_t* kin = ctx->kinematics_dev.as<int32_t>();
     ShardLaunch shard{ctx->peers, (long long)(ctx->peer32.as<int32_t>() - ctx->refs32.as<int32_t>()), {0, ctx->error_dev.as<int32_t>()}};
     int64_t n = 0;
-    const LaunchContext lc{integrator_extensions(ctx), ctx->integ.angular_integration_mode, profile != nullptr};
+    const LaunchContext lc = launch_context(ctx, profile != nullptr);
     for (size_t i = 0; i < ctx->program.ops.size(); ++i) {
         const StageOp& op = ctx->program.ops[i];
         const bool barrier = op.exchange == kRankBarrier;
@@ -308,7 +331,14 @@ void issue_stage_sequence(bepucuda_ctx* ctx, cudaStream_t s, int64_t* launches, 
     if (launches) *launches = n;
 }
 
+// Replaces the stage program and drops the graph captured from the old one. The constraints are ready for a solve only once this succeeds.
 int upload_program(bepucuda_ctx* ctx) {
+    // Before any early return: a failure below must not leave a graph of the old program, whose launches read tables end_constraints may have
+    // reallocated, nor a description that solve takes as ready.
+    ctx->constraints_ready = false;
+    // work issued under the previous program completes before that program and its graph are replaced
+    CK(cudaStreamSynchronize(ctx->stream));
+    invalidate_graph(ctx);
     ctx->program = build_stage_program(ctx->topo, ctx->iterations, (int)ctx->kinematics.size(), ctx->integ.integrate_velocity_for_kinematics != 0, ctx->peer_mode,
                                        ctx->body_count);
     if (ctx->peer_mode) {
@@ -318,49 +348,58 @@ int upload_program(bepucuda_ctx* ctx) {
         std::string error;
         const int rc = exchange_targets(ctx->program, ctx->boundary_count, &targets, &error);
         if (rc != BEPUCUDA_OK) return fail(ctx, rc, error);
-        CK(cudaStreamSynchronize(ctx->stream));
         for (int q = 0; q < ctx->peers.rank_count; ++q)
             if (q != ctx->peers.rank)
                 CK(cudaMemcpy(ctx->peers.flags[q] + kShardTargetSlot + (size_t)ctx->peers.rank * kShardMaxExchanges, targets.data(), targets.size() * 8, cudaMemcpyDefault));
         CK(cudaMemset((unsigned long long*)ctx->shard_flags.ptr + kShardCounterSlot, 0, kMaxShardRanks * 8));
         ctx->shard_solve_index = 0;
     }
-    // work issued under the previous program completes before that program and its graph are replaced
-    CK(cudaStreamSynchronize(ctx->stream));
-    invalidate_graph(ctx);
     ctx->timings.stage_count = ctx->program.stage_count;
+    ctx->constraints_ready = true;
     return BEPUCUDA_OK;
+}
+
+// Callbacks.PrepareForIntegration(dt): Demos/DemoCallbacks.cs:L79-86, and for point gravity gravityDt = dt * Gravity (PlanetDemo.cs:L36-40).
+struct IntegrationTerms {
+    float gravity_dt[3], linear_damping_dt, angular_damping_dt, attractor_dt;
+};
+IntegrationTerms prepare_for_integration(const bepucuda_ctx* ctx, float dt) {
+    auto clamp01 = [](float v) { return v < 0.f ? 0.f : (v > 1.f ? 1.f : v); };
+    IntegrationTerms t;
+    for (int i = 0; i < 3; ++i) t.gravity_dt[i] = ctx->integ.gravity[i] * dt;
+    t.linear_damping_dt = powf(clamp01(1 - ctx->integ.linear_damping), dt);
+    t.angular_damping_dt = powf(clamp01(1 - ctx->integ.angular_damping), dt);
+    t.attractor_dt = dt * ctx->attractor_strength;
+    return t;
 }
 
 void compute_frame_params(bepucuda_ctx* ctx, float dt, FrameParams* fp) {
     const int substeps = (int)ctx->iterations.size();
     const float substepDt = dt / substeps;  // Solver_Solve.cs:L1417
-    auto clamp01 = [](float v) { return v < 0.f ? 0.f : (v > 1.f ? 1.f : v); };
     const bepucuda_integrator_desc& d = ctx->integ;
+    const IntegrationTerms sub = prepare_for_integration(ctx, substepDt);
     fp->dt = substepDt;
     fp->inverse_dt = 1.0f / substepDt;
-    // PrepareForIntegration(substepDt): Demos/DemoCallbacks.cs:L79-86
-    fp->linear_damping_dt = powf(clamp01(1 - d.linear_damping), substepDt);
-    fp->angular_damping_dt = powf(clamp01(1 - d.angular_damping), substepDt);
-    for (int i = 0; i < 3; ++i) fp->gravity_dt[i] = d.gravity[i] * substepDt;
+    fp->linear_damping_dt = sub.linear_damping_dt;
+    fp->angular_damping_dt = sub.angular_damping_dt;
+    for (int i = 0; i < 3; ++i) fp->gravity_dt[i] = sub.gravity_dt[i];
+    fp->attractor_dt = sub.attractor_dt;
     // IntegrateAfterSubstepping: PoseIntegrator.cs:L707-712
     const float finalDt = d.allow_substeps_for_unconstrained ? substepDt : dt;
+    const IntegrationTerms fin = prepare_for_integration(ctx, finalDt);
     fp->final_dt = finalDt;
-    fp->final_linear_damping_dt = powf(clamp01(1 - d.linear_damping), finalDt);
-    fp->final_angular_damping_dt = powf(clamp01(1 - d.angular_damping), finalDt);
-    for (int i = 0; i < 3; ++i) fp->final_gravity_dt[i] = d.gravity[i] * finalDt;
+    fp->final_linear_damping_dt = fin.linear_damping_dt;
+    fp->final_angular_damping_dt = fin.angular_damping_dt;
+    for (int i = 0; i < 3; ++i) fp->final_gravity_dt[i] = fin.gravity_dt[i];
+    fp->final_attractor_dt = fin.attractor_dt;
     fp->final_steps = d.allow_substeps_for_unconstrained ? substeps : 1;
     fp->angular_mode = d.angular_integration_mode;
     fp->integrate_velocity_for_kinematics = d.integrate_velocity_for_kinematics;
-    // optional velocity terms (bepucuda_set_body_accelerations / bepucuda_set_point_gravity); PrepareForIntegration: gravityDt = dt * Gravity
-    // (PlanetDemo.cs:L36-40)
-    const unsigned long long accelerations = ctx->accelerations_count >= 0 ? (unsigned long long)ctx->accelerations.ptr : 0ull;
+    fp->integrate_extensions = integrate_extensions(ctx);
+    const unsigned long long accelerations = (fp->integrate_extensions & kIntegrateAccelerations) ? (unsigned long long)ctx->accelerations.ptr : 0ull;
     fp->accelerations[0] = (uint32_t)accelerations;
     fp->accelerations[1] = (uint32_t)(accelerations >> 32);
-    fp->integrate_extensions = (ctx->accelerations_count >= 0 ? kIntegrateAccelerations : 0u) | (ctx->point_gravity ? kIntegratePointGravity : 0u);
     for (int i = 0; i < 3; ++i) fp->attractor_center[i] = ctx->attractor_center[i];
-    fp->attractor_dt = substepDt * ctx->attractor_strength;
-    fp->final_attractor_dt = finalDt * ctx->attractor_strength;
 }
 
 // Accelerations set for another body count than the current one index the wrong bodies: solve, profile_stages and predict_bounding_boxes refuse
@@ -421,10 +460,11 @@ int prepare_frame(bepucuda_ctx* ctx, float dt) {
     // frame parameters (previous solve's copy has completed by stream order only after its graph, a stage profile's before it returned; wait for
     // it before reusing the pinned struct)
     CK(cudaEventSynchronize(ctx->ev_solve_end));
-    compute_frame_params(ctx, dt, ctx->frame_params_host);
-    ctx->frame_params_host->exchange_base = ctx->exchange_counter;
-    ctx->frame_params_host->shard_solve_index = ctx->shard_solve_index;
-    CK(cudaMemcpyAsync(ctx->frame_params_dev.ptr, ctx->frame_params_host, sizeof(FrameParams), cudaMemcpyHostToDevice, ctx->stream));
+    FrameParams* fp = ctx->frame_params_host.as<FrameParams>();
+    compute_frame_params(ctx, dt, fp);
+    fp->exchange_base = ctx->exchange_counter;
+    fp->shard_solve_index = ctx->shard_solve_index;
+    CK(cudaMemcpyAsync(ctx->frame_params_dev.ptr, fp, sizeof(FrameParams), cudaMemcpyHostToDevice, ctx->stream));
     return BEPUCUDA_OK;
 }
 
@@ -459,7 +499,7 @@ int32_t bepucuda_create(const bepucuda_config* cfg, bepucuda_ctx** out) {
     cudaEvent_t* evs[] = {&ctx->ev_solve_begin, &ctx->ev_solve_end, &ctx->ev_up_begin, &ctx->ev_up_end, &ctx->ev_down_begin, &ctx->ev_down_end};
     for (auto ev : evs)
         if (e == cudaSuccess) e = cudaEventCreate(ev);
-    if (e == cudaSuccess) e = cudaMallocHost((void**)&ctx->frame_params_host, sizeof(FrameParams));
+    if (e == cudaSuccess) e = ctx->frame_params_host.reserve(sizeof(FrameParams));
     if (e == cudaSuccess) e = ctx->frame_params_dev.reserve(sizeof(FrameParams));
     if (e == cudaSuccess) e = ctx->error_dev.reserve(8 * sizeof(int32_t));
     if (e != cudaSuccess) {
@@ -480,27 +520,16 @@ int32_t bepucuda_destroy(bepucuda_ctx* ctx) {
     if (ctx->stream) cudaStreamSynchronize(ctx->stream);
     invalidate_graph(ctx);
     for (void* p : ctx->opened_ipc) cudaIpcCloseMemHandle(p);
-    DeviceBuffer* bufs[] = {&ctx->shard_flags, &ctx->peer32, &ctx->body_masks_dev, &ctx->boundary_flags_dev, &ctx->global_first_batch_dev, &ctx->raw_bodies, &ctx->pose, &ctx->velocity, &ctx->inertia_local, &ctx->inertia_world, &ctx->constrained, &ctx->first_batch, &ctx->sync_refcount,
-                            &ctx->sync_mask, &ctx->chunk_table, &ctx->record_table, &ctx->ref_rows, &ctx->body_shapes, &ctx->body_activities, &ctx->body_bounds, &ctx->color_refs, &ctx->color_priorities, &ctx->color_body_min, &ctx->color_body_mask, &ctx->color_out, &ctx->color_lists, &ctx->color_counts, &ctx->island_activities, &ctx->island_label, &ctx->island_blocked, &ctx->island_count, &ctx->island_flags, &ctx->island_roots, &ctx->island_counts, &ctx->island_scalars, &ctx->island_temp, &ctx->source_bundle_flags, &ctx->refs32, &ctx->prestep32, &ctx->impulses32, &ctx->tb_table, &ctx->tdesc_table, &ctx->work_table, &ctx->map_table,
-                            &ctx->bodies_per_type, &ctx->kinematics_dev, &ctx->frame_params_dev, &ctx->error_dev, &ctx->accelerations};
-    for (auto b : bufs) b->release();
-    if (ctx->accelerations_stage) cudaFreeHost(ctx->accelerations_stage);
-    if (ctx->accelerations_staged) cudaEventDestroy(ctx->accelerations_staged);
-    ctx->raw_arena.release();
-    ctx->pinned_arena.release();
-    if (ctx->frame_params_host) cudaFreeHost(ctx->frame_params_host);
-    for (auto ev : ctx->user_events)
-        if (ev) cudaEventDestroy(ev);
-    for (auto& st : ctx->chunk_stage) {
-        if (st.host) cudaFreeHost(st.host);
-        if (st.done) cudaEventDestroy(st.done);
-    }
-    for (auto ev : ctx->profile_events) cudaEventDestroy(ev);
-    cudaEvent_t evs[] = {ctx->ev_solve_begin, ctx->ev_solve_end, ctx->ev_up_begin, ctx->ev_up_end, ctx->ev_down_begin, ctx->ev_down_end};
+    cudaEvent_t evs[] = {ctx->ev_solve_begin, ctx->ev_solve_end, ctx->ev_up_begin, ctx->ev_up_end, ctx->ev_down_begin, ctx->ev_down_end, ctx->accelerations_stage.done};
     for (auto ev : evs)
         if (ev) cudaEventDestroy(ev);
+    for (auto ev : ctx->user_events)
+        if (ev) cudaEventDestroy(ev);
+    for (auto& st : ctx->chunk_stage)
+        if (st.done) cudaEventDestroy(st.done);
+    for (auto ev : ctx->profile_events) cudaEventDestroy(ev);
     if (ctx->stream) cudaStreamDestroy(ctx->stream);
-    delete ctx;
+    delete ctx;  // the device and pinned buffers free themselves, on the device set above
     return BEPUCUDA_OK;
 }
 
@@ -546,8 +575,6 @@ int32_t bepucuda_set_integrator(bepucuda_ctx* ctx, const bepucuda_integrator_des
     if (!ctx || !desc) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "set_integrator: bad arguments");
     if (desc->angular_integration_mode < 0 || desc->angular_integration_mode > 2) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "set_integrator: unknown AngularIntegrationMode");
     const bool kin_changed = (desc->integrate_velocity_for_kinematics != 0) != (ctx->integ.integrate_velocity_for_kinematics != 0);
-    // whether the angular mode is 0 is an input of resolve_stage_launch, and a captured graph bakes the resolved launches in
-    if ((desc->angular_integration_mode != 0) != (ctx->integ.angular_integration_mode != 0)) invalidate_graph(ctx);
     ctx->integ = *desc;
     ctx->integ_set = true;
     if (kin_changed && ctx->constraints_ready) {
@@ -560,9 +587,7 @@ int32_t bepucuda_set_integrator(bepucuda_ctx* ctx, const bepucuda_integrator_des
 int32_t bepucuda_set_body_accelerations(bepucuda_ctx* ctx, const float* accelerations, int32_t body_count) {
     if (!ctx) return BEPUCUDA_ERR_INVALID_ARGUMENT;
     if (!accelerations) {
-        const bool was = integrator_extensions(ctx);
         ctx->accelerations_count = -1;
-        if (was != integrator_extensions(ctx)) invalidate_graph(ctx);
         return BEPUCUDA_OK;
     }
     if (body_count != ctx->body_count) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "set_body_accelerations: the body count must match the last upload_bodies");
@@ -572,28 +597,16 @@ int32_t bepucuda_set_body_accelerations(bepucuda_ctx* ctx, const float* accelera
     CK(ctx->accelerations.reserve(std::max(bytes, (size_t)32)));
     if (bytes > 0) {
         // through a pinned staging copy, so that the caller's buffer is free when the call returns without waiting for the device
-        if (!ctx->accelerations_staged) CK(cudaEventCreateWithFlags(&ctx->accelerations_staged, cudaEventDisableTiming));
-        CK(cudaEventSynchronize(ctx->accelerations_staged));  // the previous upload has left the staging buffer
-        if (ctx->accelerations_stage_bytes < bytes) {
-            if (ctx->accelerations_stage) cudaFreeHost(ctx->accelerations_stage);
-            ctx->accelerations_stage = nullptr;
-            ctx->accelerations_stage_bytes = 0;
-            CK(cudaMallocHost(&ctx->accelerations_stage, bytes));
-            ctx->accelerations_stage_bytes = bytes;
-        }
-        std::memcpy(ctx->accelerations_stage, accelerations, bytes);
-        CK(cudaMemcpyAsync(ctx->accelerations.ptr, ctx->accelerations_stage, bytes, cudaMemcpyHostToDevice, ctx->stream));
-        CK(cudaEventRecord(ctx->accelerations_staged, ctx->stream));
+        int rc = upload_staged(ctx, ctx->accelerations_stage, ctx->accelerations.ptr, accelerations, bytes);
+        if (rc != BEPUCUDA_OK) return rc;
         ctx->h2d_accum += (int64_t)bytes;
     }
-    if (!integrator_extensions(ctx)) invalidate_graph(ctx);
     ctx->accelerations_count = body_count;
     return BEPUCUDA_OK;
 }
 
 int32_t bepucuda_set_point_gravity(bepucuda_ctx* ctx, int32_t enabled, const float* center, float strength) {
     if (!ctx || (enabled && !center)) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "set_point_gravity: bad arguments");
-    if (ctx->point_gravity != (enabled != 0) && ctx->accelerations_count < 0) invalidate_graph(ctx);
     ctx->point_gravity = enabled != 0;
     for (int i = 0; i < 3; ++i) ctx->attractor_center[i] = enabled ? center[i] : 0.0f;
     ctx->attractor_strength = enabled ? strength : 0.0f;
@@ -606,11 +619,8 @@ int32_t bepucuda_upload_bodies(bepucuda_ctx* ctx, const void* body_dynamics, int
     CK(cudaSetDevice(ctx->device));
     open_upload_window(ctx);
     const size_t n = (size_t)body_count;
-    if (body_count != ctx->body_count) {
-        // constrained flags / ownership depend on the body count; force a rebuild of topology products.
-        if (ctx->constraints_ready) ctx->constraints_ready = false;
-        invalidate_graph(ctx);
-    }
+    // constrained flags / ownership depend on the body count; force a rebuild of topology products.
+    if (body_count != ctx->body_count) ctx->constraints_ready = false;
     CK(ctx->raw_bodies.reserve(n * 128));
     CK(ctx->pose.reserve(n * 32));
     CK(ctx->velocity.reserve(n * 32));
@@ -628,9 +638,6 @@ int32_t bepucuda_upload_bodies(bepucuda_ctx* ctx, const void* body_dynamics, int
     B.constrained = ctx->constrained.as<uint8_t>();
     B.first_batch = ctx->first_batch.as<int32_t>();
     B.count = body_count;
-    if (B.pose != ctx->B.pose || B.velocity != ctx->B.velocity || B.inertia_local != ctx->B.inertia_local || B.inertia_world != ctx->B.inertia_world ||
-        B.constrained != ctx->B.constrained || B.first_batch != ctx->B.first_batch || B.count != ctx->B.count)
-        invalidate_graph(ctx);  // kernel arguments are baked into graph nodes
     ctx->B = B;
     if (body_count > 0) {
         CK(cudaMemcpyAsync(ctx->raw_bodies.ptr, body_dynamics, n * 128, cudaMemcpyHostToDevice, ctx->stream));
@@ -654,7 +661,6 @@ int32_t bepucuda_begin_constraints(bepucuda_ctx* ctx, int32_t source_bundle_widt
     ctx->pinned_arena.reset();
     ctx->constraints_open = true;
     ctx->constraints_ready = false;
-    invalidate_graph(ctx);
     return BEPUCUDA_OK;
 }
 
@@ -759,7 +765,7 @@ int32_t bepucuda_end_constraints(bepucuda_ctx* ctx) {
     CK(ctx->first_batch.reserve(nb * 4));
     CK(ctx->sync_refcount.reserve(nb * 4));
     CK(ctx->sync_mask.reserve(nb * 8));
-    ctx->B.first_batch = ctx->first_batch.as<int32_t>();  // the graph is re-captured below (upload_program)
+    ctx->B.first_batch = ctx->first_batch.as<int32_t>();
     launch_fill_i32(ctx->first_batch.as<int32_t>(), nb, 0x7fffffff, ctx->stream);
     CK(cudaMemsetAsync(ctx->sync_refcount.ptr, 0, nb * 4, ctx->stream));
     CK(cudaMemsetAsync(ctx->sync_mask.ptr, 0, nb * 8, ctx->stream));
@@ -816,7 +822,6 @@ int32_t bepucuda_end_constraints(bepucuda_ctx* ctx) {
     ctx->timings.device_batch_count = (int)topo.batches.size();
     ctx->timings.fallback_level_count = topo.fallback_levels;
     ctx->constraints_open = false;
-    ctx->constraints_ready = true;
     ctx->data_dirty = false;
     return upload_program(ctx);
 }
@@ -824,35 +829,20 @@ int32_t bepucuda_end_constraints(bepucuda_ctx* ctx) {
 int32_t bepucuda_update_type_batch(bepucuda_ctx* ctx, int32_t batch_index, int32_t type_batch_index, const float* prestep, float* accumulated_impulses) {
     if (!ctx || !prestep || !accumulated_impulses) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "update_type_batch: bad arguments");
     if (!ctx->constraints_ready) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, "update_type_batch before end_constraints");
+    SourceTypeBatch* s = find_source(ctx, batch_index, type_batch_index);
+    if (!s) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "update_type_batch: unknown type batch");
     CK(cudaSetDevice(ctx->device));
     open_upload_window(ctx);
-    for (auto& s : ctx->sources)
-        if (s.batch_index == batch_index && s.type_batch_index == type_batch_index) {
-            char* alias_p = map_host(ctx, prestep, s.prestep_bytes);
-            char* alias_i = map_host(ctx, accumulated_impulses, s.impulse_bytes);
-            if (alias_p && alias_i) {
-                queue_chunks(ctx->pending_h2d, s.raw_prestep, alias_p, s.prestep_bytes);
-                queue_chunks(ctx->pending_h2d, s.raw_impulses, alias_i, s.impulse_bytes);
-            } else {
-                // Direct copies only: the pinned staging arena is recycled per begin_constraints, not per frame.
-                CK(cudaMemcpyAsync(s.raw_prestep, prestep, s.prestep_bytes, cudaMemcpyHostToDevice, ctx->stream));
-                CK(cudaMemcpyAsync(s.raw_impulses, accumulated_impulses, s.impulse_bytes, cudaMemcpyHostToDevice, ctx->stream));
-            }
-            ctx->h2d_accum += (int64_t)(s.prestep_bytes + s.impulse_bytes);
-            s.host_impulses = accumulated_impulses;
-            s.pending = kTransposePrestep | kTransposeImpulses;
-            s.redistribute = false;  // the host took the impulses back
-            ctx->data_dirty = true;
-            return BEPUCUDA_OK;
-        }
-    return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "update_type_batch: unknown type batch");
+    int rc;
+    if ((rc = copy_in(ctx, s->raw_prestep, prestep, s->prestep_bytes)) != BEPUCUDA_OK) return rc;
+    if ((rc = copy_in(ctx, s->raw_impulses, accumulated_impulses, s->impulse_bytes)) != BEPUCUDA_OK) return rc;
+    s->host_impulses = accumulated_impulses;
+    s->pending = kTransposePrestep | kTransposeImpulses;
+    s->redistribute = false;  // the host took the impulses back
+    ctx->data_dirty = true;
+    return BEPUCUDA_OK;
 }
 
-static SourceTypeBatch* find_source(bepucuda_ctx* ctx, int32_t batch_index, int32_t type_batch_index) {
-    for (auto& s : ctx->sources)
-        if (s.batch_index == batch_index && s.type_batch_index == type_batch_index) return &s;
-    return nullptr;
-}
 static int ensure_feature_arrays(bepucuda_ctx* ctx, SourceTypeBatch& s) {
     if (s.raw_features_old) return BEPUCUDA_OK;
     s.feature_bytes = (size_t)s.count * get_type_info(s.type_id)->contacts * sizeof(int32_t);
@@ -886,16 +876,9 @@ int32_t bepucuda_update_contacts(bepucuda_ctx* ctx, int32_t batch_index, int32_t
     if (s->redistribute) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, "update_contacts: called twice for the same type batch without a solve in between");
     CK(cudaSetDevice(ctx->device));
     open_upload_window(ctx);
-    // per-frame path: mapped (registered) host buffers go through the batched zero-copy kernel, anything else is copied directly -- never through the
-    // pinned staging arena, which is only recycled by bepucuda_begin_constraints
-    const void* srcs[2] = {prestep, new_feature_ids};
-    void* dsts[2] = {s->raw_prestep, s->raw_features_new};
-    const size_t sizes[2] = {s->prestep_bytes, s->feature_bytes};
-    for (int i = 0; i < 2; ++i) {
-        if (char* alias = map_host(ctx, srcs[i], sizes[i])) queue_chunks(ctx->pending_h2d, dsts[i], alias, sizes[i]);
-        else CK(cudaMemcpyAsync(dsts[i], srcs[i], sizes[i], cudaMemcpyHostToDevice, ctx->stream));
-        ctx->h2d_accum += (int64_t)sizes[i];
-    }
+    int rc;
+    if ((rc = copy_in(ctx, s->raw_prestep, prestep, s->prestep_bytes)) != BEPUCUDA_OK) return rc;
+    if ((rc = copy_in(ctx, s->raw_features_new, new_feature_ids, s->feature_bytes)) != BEPUCUDA_OK) return rc;
     s->pending |= kTransposePrestep;  // the accumulated impulses stay resident
     s->redistribute = true;
     ctx->data_dirty = true;
@@ -954,20 +937,21 @@ int32_t bepucuda_solve(bepucuda_ctx* ctx, float dt) {
     CK(cudaEventRecord(ctx->ev_solve_begin, ctx->stream));
     int64_t launches = 0;
     if (ctx->cfg.execution_mode == BEPUCUDA_EXEC_GRAPH) {
-        if (!ctx->graph_valid) {
+        const LaunchContext lc = launch_context(ctx, false);
+        if (!ctx->graph_exec || !same_bodies(ctx->graph_bodies, ctx->B) || !same_launches(ctx->graph_launch, lc)) {
+            invalidate_graph(ctx);
             CK(cudaStreamBeginCapture(ctx->stream, cudaStreamCaptureModeThreadLocal));
             int64_t n = 0;
             issue_stage_sequence(ctx, ctx->stream, &n);
             cudaError_t e = cudaStreamEndCapture(ctx->stream, &ctx->graph);
             if (e == cudaSuccess) e = cudaGraphInstantiate(&ctx->graph_exec, ctx->graph, 0);
             if (e != cudaSuccess) return cuda_fail(ctx, e, "graph capture");
-            ctx->graph_valid = true;
+            ctx->graph_bodies = ctx->B;
+            ctx->graph_launch = lc;
             ctx->timings.kernel_launches = n;
         }
-        if (ctx->graph_valid) {
-            CK(cudaGraphLaunch(ctx->graph_exec, ctx->stream));
-            launches = ctx->timings.kernel_launches;
-        }
+        CK(cudaGraphLaunch(ctx->graph_exec, ctx->stream));
+        launches = ctx->timings.kernel_launches;
     }
     if (ctx->cfg.execution_mode == BEPUCUDA_EXEC_STREAM) {
         issue_stage_sequence(ctx, ctx->stream, &launches);
@@ -1040,17 +1024,15 @@ int32_t bepucuda_download_impulses(bepucuda_ctx* ctx) {
 int32_t bepucuda_download_prestep(bepucuda_ctx* ctx, int32_t batch_index, int32_t type_batch_index, float* prestep_out) {
     if (!ctx || !prestep_out) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "download_prestep: bad arguments");
     if (!ctx->constraints_ready) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, "download_prestep before end_constraints");
+    const SourceTypeBatch* s = find_source(ctx, batch_index, type_batch_index);
+    if (!s) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "download_prestep: unknown type batch");
     CK(cudaSetDevice(ctx->device));
-    for (auto& s : ctx->sources)
-        if (s.batch_index == batch_index && s.type_batch_index == type_batch_index) {
-            launch_transpose_out_all(ctx->tb_table.as<DeviceTypeBatch>(), ctx->tdesc_table.as<TransposeDesc>(), ctx->work_table.as<WorkItem>(), ctx->topo.all_work_count, ctx->W,
-                                     kTransposePrestep, ctx->stream);
-            CK(cudaGetLastError());
-            CK(cudaMemcpyAsync(prestep_out, s.raw_prestep, s.prestep_bytes, cudaMemcpyDeviceToHost, ctx->stream));
-            CK(cudaStreamSynchronize(ctx->stream));
-            return BEPUCUDA_OK;
-        }
-    return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "download_prestep: unknown type batch");
+    launch_transpose_out_all(ctx->tb_table.as<DeviceTypeBatch>(), ctx->tdesc_table.as<TransposeDesc>(), ctx->work_table.as<WorkItem>(), ctx->topo.all_work_count, ctx->W,
+                             kTransposePrestep, ctx->stream);
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(prestep_out, s->raw_prestep, s->prestep_bytes, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    return BEPUCUDA_OK;
 }
 
 int32_t bepucuda_get_timings(bepucuda_ctx* ctx, bepucuda_timings* out) {
@@ -1134,17 +1116,17 @@ int32_t bepucuda_predict_bounding_boxes(bepucuda_ctx* ctx, float dt, bepucuda_bo
     CK(ctx->body_bounds.reserve((size_t)n * 32));
     CK(cudaMemcpyAsync(ctx->body_activities.ptr, activities, (size_t)n * sizeof(BodyActivityRecord), cudaMemcpyHostToDevice, ctx->stream));
     // PoseIntegrator.PredictBoundingBoxes calls Callbacks.PrepareForIntegration(dt) with the frame dt (PoseIntegrator.cs:L428)
-    auto clamp01 = [](float v) { return v < 0.f ? 0.f : (v > 1.f ? 1.f : v); };
+    const IntegrationTerms t = prepare_for_integration(ctx, dt);
     PredictParams p{};
     p.dt = dt;
-    for (int i = 0; i < 3; ++i) p.gravity_dt[i] = ctx->integ.gravity[i] * dt;
-    p.linear_damping_dt = powf(clamp01(1 - ctx->integ.linear_damping), dt);
-    p.angular_damping_dt = powf(clamp01(1 - ctx->integ.angular_damping), dt);
+    for (int i = 0; i < 3; ++i) p.gravity_dt[i] = t.gravity_dt[i];
+    p.linear_damping_dt = t.linear_damping_dt;
+    p.angular_damping_dt = t.angular_damping_dt;
     p.integrate_velocity_for_kinematics = ctx->integ.integrate_velocity_for_kinematics;
-    p.accelerations = ctx->accelerations_count >= 0 ? ctx->accelerations.as<float4>() : nullptr;
-    p.integrate_extensions = (ctx->accelerations_count >= 0 ? kIntegrateAccelerations : 0u) | (ctx->point_gravity ? kIntegratePointGravity : 0u);
+    p.integrate_extensions = integrate_extensions(ctx);
+    p.accelerations = (p.integrate_extensions & kIntegrateAccelerations) ? ctx->accelerations.as<float4>() : nullptr;
     for (int i = 0; i < 3; ++i) p.attractor_center[i] = ctx->attractor_center[i];
-    p.attractor_dt = dt * ctx->attractor_strength;
+    p.attractor_dt = t.attractor_dt;
     launch_predict_bounding_boxes(ctx->B, ctx->body_shapes.as<BodyShape>(), ctx->body_activities.as<BodyActivityRecord>(), ctx->body_bounds.as<float4>(), p, ctx->stream);
     CK(cudaGetLastError());
     CK(cudaMemcpyAsync(activities, ctx->body_activities.ptr, (size_t)n * sizeof(BodyActivityRecord), cudaMemcpyDeviceToHost, ctx->stream));
@@ -1342,7 +1324,6 @@ int32_t bepucuda_shard_import(bepucuda_ctx* ctx, int32_t rank, int32_t rank_coun
     ctx->peer_mode = true;
     ctx->exchange_counter = 0;
     if (ctx->constraints_ready) ctx->constraints_ready = false;
-    invalidate_graph(ctx);
     return BEPUCUDA_OK;
 }
 
@@ -1373,7 +1354,6 @@ int32_t bepucuda_shard_import_contexts(bepucuda_ctx* ctx, int32_t rank, int32_t 
     ctx->peer_mode = true;
     ctx->exchange_counter = 0;
     if (ctx->constraints_ready) ctx->constraints_ready = false;
-    invalidate_graph(ctx);
     return BEPUCUDA_OK;
 }
 

@@ -206,8 +206,8 @@ def test_joints_only_scene_bit_exact(libs):
 @pytest.mark.gpu
 def test_graph_follows_integrator_changes_between_solves(libs):
     """A captured graph bakes in the resolved launches, whose inputs include whether the angular mode is 0 and whether per-body accelerations or
-    point gravity are set. One context in graph mode switches the angular mode 0 -> 1 -> 0, then accelerations with point gravity on -> off,
-    between solves; every frame matches the oracle bit for bit."""
+    point gravity are set. One context in graph mode switches the angular mode 0 -> 1 -> 2 -> 1 -> 0, then accelerations with point gravity
+    on -> off, between solves; every frame matches the oracle bit for bit."""
     scene = scenes.merge(scenes.shape_pile(1500, seed=20), scenes.ragdolls(4, seed=21))
     kw = dict(substeps=3, velocity_iterations=2, integrator=_integrator(kinematics=1))
     a, b = util.make_sim(scene, **kw), util.make_sim(scene, **kw)
@@ -216,7 +216,7 @@ def test_graph_follows_integrator_changes_between_solves(libs):
     ts = native.CudaTimestepper(b, strict_fp=True, execution_mode=native.EXEC_GRAPH)
     try:
         ts.describe()
-        for f, (angular_mode, terms) in enumerate([(0, False), (1, False), (0, False), (0, True), (0, False)]):
+        for f, (angular_mode, terms) in enumerate([(0, False), (1, False), (2, False), (1, False), (0, False), (0, True), (0, False)]):
             d = _integrator(kinematics=1, angular_mode=angular_mode)
             a.set_integrator(d)
             ts._check(ts._cuda.bepucuda_set_integrator(ts._ctx, C.byref(d)))

@@ -384,6 +384,54 @@ def test_topology_change_after_resident_frames(libs):
     util.compare(util.snapshot(host), util.snapshot(dev), exact=True)
 
 
+def _resident_bytes():
+    with open("/proc/self/status") as f:
+        return next(int(line.split()[1]) << 10 for line in f if line.startswith("VmRSS:"))
+
+
+@pytest.mark.gpu
+def test_feature_ids_sent_again_every_frame_hold_no_host_memory(libs):
+    """bepucuda_set_contact_features after end_constraints from unregistered buffers, again and again, as a host that sends the feature ids every
+    frame does: type batches whose ids are each under 256 KB, 512 MB sent in all. The process's resident memory grows by far less than that, and
+    the ids of the last call are the ones the next update_contacts redistributes from: that frame matches the host path bit for bit."""
+    kw = dict(substeps=3, velocity_iterations=2)
+    host, dev = util.make_sim(_pile(0.3), **kw), util.make_sim(_pile(0.3), **kw)
+    rng_h, rng_d = np.random.default_rng(9), np.random.default_rng(9)
+    ts = bp.CudaTimestepper(dev, strict_fp=True)
+    try:
+        ts.describe()
+        feat_h, feat_d = _initial_features(host, rng_h), _initial_features(dev, rng_d)
+        ts.set_contact_features(feat_d)
+        ob.solve(host, DT)
+        ts.solve_device_only(DT)  # resident impulses that belong to feat_d
+        ts.download_body_motion()
+        assert max(ids.nbytes for ids in feat_d.values()) < 256 << 10
+        wrong = {key: ids + (1 << 21) for key, ids in feat_d.items()}  # match nothing: a device that kept these would redistribute differently
+        per_call = sum(ids.nbytes for ids in feat_d.values())
+        calls = -(-(512 << 20) // per_call)
+        before = _resident_bytes()
+        for i in range(calls):
+            ts.set_contact_features(feat_d if i == calls - 1 else wrong)
+        ts.synchronize()
+        grown = _resident_bytes() - before
+        assert grown < 32 << 20, "resident memory grew by %d MB while %d MB of feature ids were sent" % (grown >> 20, (calls * per_call) >> 20)
+        new_h = _narrow_phase_like_update(host, feat_h, rng_h)
+        for tb in host.type_batches():
+            key = (tb.batch_index, tb.type_batch_index)
+            if key in new_h:
+                ob.update_contact_impulses(tb, feat_h[key], new_h[key])
+        ts.upload_body_motion()
+        ts.update_contacts(_narrow_phase_like_update(dev, feat_d, rng_d))
+        ob.solve(host, DT)
+        ts.solve_device_only(DT)
+        ts.download_bodies()
+        ts.download_impulses()
+        ts.download_prestep()
+    finally:
+        ts.close()
+    util.compare(util.snapshot(host), util.snapshot(dev), exact=True)
+
+
 @pytest.mark.gpu
 def test_update_contacts_state_errors(libs):
     """update_contacts before set_contact_features and twice without a solve: BAD_STATE; on a joint type batch: INVALID_ARGUMENT. update_type_batch

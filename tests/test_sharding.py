@@ -214,3 +214,36 @@ def test_profile_stages_is_refused_in_peer_mode(libs):
     finally:
         for s in solvers:
             s.close()
+
+
+@pytest.mark.gpu
+def test_a_stage_program_that_fails_to_upload_leaves_nothing_to_solve(libs):
+    """A described peer-mode rank gets a schedule with more exchange points per solve than the arrival targets hold: bepucuda_set_solve_description
+    fails while it uploads the new stage program. The rank then holds no program a solve may run, neither the new one, whose targets no peer
+    received, nor a graph of the old one: calls that need the constraints refuse before any device work, and a new describe recovers."""
+    sim = util.make_sim(scenes.shape_pile(400, seed=4), substeps=2, velocity_iterations=1)
+    solvers = [sharding.ShardedSolver(sim, r, 2, 0, strict_fp=True) for r in range(2)]
+    try:
+        for s in solvers:
+            s.export_handles()
+        for s in solvers:
+            s.import_contexts(solvers)
+        for s in solvers:
+            s.describe()
+        s, cuda = solvers[0], solvers[0]._cuda
+        its = (ctypes.c_int32 * 64)(*([32] * 64))
+        with pytest.raises(native.BepuCudaError) as e:
+            s._check(cuda.bepucuda_set_solve_description(s._ctx, 64, its, sim.fallback_batch_threshold))
+        assert e.value.code == -6 and "exchange points" in str(e.value)  # BEPUCUDA_ERR_BAD_STATE
+        assert cuda.bepucuda_download_impulses(s._ctx) == -6
+        assert cuda.bepucuda_solve(s._ctx, ctypes.c_float(DT)) == -6
+        mine = s.referenced_bodies()
+        s._check(cuda.bepucuda_download_bodies(s._ctx, s.bodies.ctypes.data, sim.body_count))
+        assert np.array_equal(sim.bodies[mine][:, util.MOTION].view(np.uint32), s.bodies[mine][:, util.MOTION].view(np.uint32))
+        its = (ctypes.c_int32 * len(sim.velocity_iterations))(*sim.velocity_iterations)
+        s._check(cuda.bepucuda_set_solve_description(s._ctx, len(sim.velocity_iterations), its, sim.fallback_batch_threshold))
+        s.describe()
+        s._check(cuda.bepucuda_download_impulses(s._ctx))
+    finally:
+        for s in solvers:
+            s.close()

@@ -51,6 +51,7 @@ def shim():
     dll.topology_program_ops.argtypes = [vp, vp]
     dll.topology_program_free.argtypes = [vp]
     dll.topology_resolve.argtypes = [vp, i32, i32, i32, i32, vp]
+    dll.topology_same_launches.argtypes = [i32] * 6
     return dll
 
 
@@ -340,6 +341,20 @@ def test_every_launch_follows_the_rules(libs, shim, case):
             for ivk in (False, True):
                 ops, _ = p.program(iterations, len(sim.constrained_kinematics), ivk, case == "peer", sim.body_count)
                 check_launches(shim, ops, case == "peer")
+
+
+def test_same_launches_holds_exactly_when_every_op_launches_the_same(libs, shim):
+    """same_launches, which decides when a captured graph is re-captured, against resolve_stage_launch on a program with every op kind: for every
+    pair of launch contexts it holds exactly when every op resolves to the same launch in both."""
+    sim = util.make_sim(mixed_scene(7), fallback_batch_threshold=6)
+    p = plan(shim, sim_sources(sim), 8, 6, sim.batch_count, sim.body_count)
+    ops, _ = p.program([2, 1], len(sim.constrained_kinematics), True, False, sim.body_count)
+    assert set(ops[:, 0].tolist()) == {WS_FIRST, WS, SOLVE, INCREMENTAL, KIN_FIRST, KIN, FINAL} and ((ops[:, 5] & INTEGRABLE) != 0).any()
+    launches = {lc: resolve(shim, ops, *lc) for lc in LAUNCH_CONTEXTS}
+    for a in LAUNCH_CONTEXTS:
+        for b in LAUNCH_CONTEXTS:
+            same = shim.topology_same_launches(*(int(v) for v in a + b)) != 0
+            assert same == np.array_equal(launches[a], launches[b]), (a, b)
 
 
 def single_batch(scene):

@@ -1,4 +1,4 @@
-// Test shim for tests/test_topology.py: plan_topology, build_stage_program and resolve_stage_launch of bepuphysics2_b200/csrc/bepu_topology.h
+// Test shim for tests/test_topology.py: plan_topology, build_stage_program, resolve_stage_launch and same_launches of bepuphysics2_b200/csrc/bepu_topology.h
 // behind a ctypes-friendly C interface. Built with g++ together with bepu_topology.cpp; the product never loads it.
 #include <cstring>
 
@@ -98,6 +98,9 @@ void topology_resolve(const int64_t* ops, int n, int integrator_extensions, int 
         out[2 * i] = l.kernel;
         out[2 * i + 1] = l.flags;
     }
+}
+int topology_same_launches(int extensions_a, int angular_mode_a, int profile_a, int extensions_b, int angular_mode_b, int profile_b) {
+    return same_launches(LaunchContext{extensions_a != 0, angular_mode_a, profile_a != 0}, LaunchContext{extensions_b != 0, angular_mode_b, profile_b != 0});
 }
 int topology_deep_batch_bundles() { return kDeepBatchBundles; }
 
