@@ -6,9 +6,9 @@
 
 namespace bepu_oracle {
 
-// A view of one AOSOA bundle chunk: row r of the bundle starts at base + r * stride floats.
+// A view of one AOSOA bundle chunk: row r of the bundle starts at base + r * stride elements (float, or double for the float64 lane).
 template <class F> struct Rows {
-    float* base;
+    typename LaneTraits<F>::Scalar* base;
     int stride;
     inline F get(int r) const {
         F v;

@@ -10,8 +10,9 @@
 // known-answer vectors tests/golden/reference_vectors.npz. UNPINNED (by construction + closed-form tests only): the solver
 // driver in bepu_oracle.cpp (substep loop, batch order, integration responsibilities, gather/scatter, bundle loops).
 //
-// Everything is templated on a lane type F: `float` (scalar-per-lane checker) or `f8` (8 x fp32 GCC vector, the
-// AVX2 shape of System.Numerics.Vector<float> on the reference's usual hosts; used for the timed CPU baseline).
+// Everything is templated on a lane type F: `float` (scalar-per-lane checker), `f8` (8 x fp32 GCC vector, the
+// AVX2 shape of System.Numerics.Vector<float> on the reference's usual hosts; used for the timed CPU baseline) or
+// `double` (the same operations evaluated in float64: the precision yardstick of tests/precision/isolated_solve.cpp).
 // Compile with -ffp-contract=off: RyuJIT never contracts a*b+c in Vector<T> code.
 #pragma once
 #include <cmath>
@@ -28,24 +29,35 @@ typedef int32_t i8 __attribute__((vector_size(32)));
 
 // ---- lane traits -------------------------------------------------------------------------------------------------
 template <class F> struct LaneTraits;
+// Scalar: the element type of the rows a lane reads and writes (Rows<F>).
 template <> struct LaneTraits<float> {
     typedef bool Mask;
+    typedef float Scalar;
     static constexpr int Width = 1;
 };
 template <> struct LaneTraits<f8> {
     typedef i8 Mask;
+    typedef float Scalar;
     static constexpr int Width = 8;
+};
+template <> struct LaneTraits<double> {
+    typedef bool Mask;
+    typedef double Scalar;
+    static constexpr int Width = 1;
 };
 template <class F> using MaskOf = typename LaneTraits<F>::Mask;
 
 template <class F> inline F bc(float v);
 template <> inline float bc<float>(float v) { return v; }
 template <> inline f8 bc<f8>(float v) { return f8{v, v, v, v, v, v, v, v}; }
+template <> inline double bc<double>(float v) { return v; }
 
 inline float get_lane(float v, int) { return v; }
 inline float get_lane(const f8& v, int i) { return v[i]; }
 inline void set_lane(float& v, int, float x) { v = x; }
 inline void set_lane(f8& v, int i, float x) { v[i] = x; }
+inline double get_lane(double v, int) { return v; }
+inline void set_lane(double& v, int, double x) { v = x; }
 
 // Vector.SquareRoot / Math.Sqrt: IEEE correctly rounded.
 inline float vsqrt(float a) { return sqrtf(a); }
@@ -62,6 +74,17 @@ inline bool mand(bool a, bool b) { return a && b; }
 inline bool mor(bool a, bool b) { return a || b; }
 inline bool mnot(bool a) { return !a; }
 inline bool any(bool a) { return a; }
+// The float64 lane: the same operations in double. These must precede every template that calls them: a double argument
+// brings no namespace for argument-dependent lookup, so a template defined earlier would bind the float overloads and round.
+inline double vsqrt(double a) { return std::sqrt(a); }
+inline double vfloor(double a) { return std::floor(a); }
+inline double vabs(double a) { return std::fabs(a); }
+inline double vmin(double a, double b) { return a < b ? a : b; }
+inline double vmax(double a, double b) { return a > b ? a : b; }
+inline bool lt(double a, double b) { return a < b; }
+inline bool gt(double a, double b) { return a > b; }
+inline bool eq(double a, double b) { return a == b; }
+inline double sel(bool m, double a, double b) { return m ? a : b; }
 
 #if defined(__AVX2__)
 inline f8 vsqrt(f8 a) { return (f8)_mm256_sqrt_ps((__m256)a); }

@@ -83,10 +83,9 @@ def max_threads():
     return load().oracle_max_threads()
 
 
-def solve(simulation, dt, threads=1, simd=False, accelerations=None, center=None, strength=0.0):
-    """Runs the oracle's Simulation.Solve restatement in place on `simulation`'s buffers (bodies, prestep depths, accumulated impulses), with the
-    optional velocity terms of bepucuda_set_body_accelerations / bepucuda_set_point_gravity (see _terms)."""
-    lib = load()
+def scene(simulation, threads=1, simd=False, accelerations=None, center=None, strength=0.0):
+    """The oracle_scene of `simulation`'s buffers with the optional velocity terms (see _terms), and the ctypes objects it points into, which the
+    caller keeps alive while the scene is used."""
     tbs = simulation.type_batches()
     batch_count = simulation.batch_count
     per_batch = [[] for _ in range(batch_count)]
@@ -128,7 +127,15 @@ def solve(simulation, dt, threads=1, simd=False, accelerations=None, center=None
     sc.constrained_kinematic_count = int(kin.size)
     sc.threads = threads
     sc.simd = 1 if simd else 0
-    sc.terms, acc = _terms(simulation.body_count, accelerations, center, strength)  # acc stays alive until oracle_solve returns
+    sc.terms, acc = _terms(simulation.body_count, accelerations, center, strength)
+    return sc, (tbs, keep, batches, bodies, its, kin, acc)
+
+
+def solve(simulation, dt, threads=1, simd=False, accelerations=None, center=None, strength=0.0):
+    """Runs the oracle's Simulation.Solve restatement in place on `simulation`'s buffers (bodies, prestep depths, accumulated impulses), with the
+    optional velocity terms of bepucuda_set_body_accelerations / bepucuda_set_point_gravity (see _terms)."""
+    lib = load()
+    sc, keep = scene(simulation, threads, simd, accelerations, center, strength)  # keep: alive until oracle_solve returns
     rc = lib.oracle_solve(C.byref(sc), dt)
     if rc != 0:
         raise RuntimeError("oracle_solve failed: %d" % rc)

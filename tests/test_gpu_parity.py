@@ -120,7 +120,7 @@ def test_ragdolls_substepped_servo_variant_bit_exact(libs):
 
 def test_ragdolls_stream_mode_fast_within_tolerance(libs):
     """Fast build on joints: relative RMS error <= 1e-3, max abs error <= 2e-2 after one frame (the twist/servo angle
-    measurements go through acos near 1, which amplifies rounding: see tests/tools/fast_error_stats.py)."""
+    measurements go through acos near 1, which amplifies rounding: tests/test_fast_build_precision.py measures it against float64)."""
     _parity(scenes.ragdolls(60, seed=5), exact=False, mode=EXEC_STREAM, rel_rms=1e-3, max_abs=2e-2, substeps=1, velocity_iterations=4)
 
 

@@ -1,28 +1,32 @@
-"""Development diagnostic: error statistics of the FMA/approx-div build against the oracle after one frame."""
+"""Development diagnostic: per configuration of tests/test_fast_build_precision.py, each constraint type's lane error against the float64
+evaluation of the same solve, for the strict and the fast GPU build, with the flips and ill-conditioned lanes (see compare_builds there).
+Needs a GPU. Usage: python tests/tools/fast_error_stats.py [configuration ...]"""
 import os
 import sys
+import tempfile
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))))
-import numpy as np
 
-from bepuphysics2_b200 import scenes
-from bepuphysics2_b200.native import EXEC_GRAPH
-from tests import util
+from bepuphysics2_b200 import _build  # noqa: E402
+from oracle import binding as ob  # noqa: E402
+from tests import test_fast_build_precision as fp  # noqa: E402
 
-DT = 1 / 60
-for name, scene, kw in (("pile", scenes.shape_pile(3000, seed=5), dict(substeps=8, velocity_iterations=2)),
-                        ("ragdolls 1x4", scenes.ragdolls(60, seed=5), dict(substeps=1, velocity_iterations=4)),
-                        ("ragdolls 8x2", scenes.ragdolls(60, seed=5), dict(substeps=8, velocity_iterations=2)),
-                        ("ragdolls rest pose", scenes.ragdolls(60, seed=5, pose_noise=0.0), dict(substeps=1, velocity_iterations=4))):
-    a = util.make_sim(scene, **kw)
-    b = util.make_sim(scene, **kw)
-    ref = util.run_oracle(a, DT)
-    got = util.run_gpu(b, DT, strict=False, mode=EXEC_GRAPH)
-    for label, cols in (("pose", np.r_[0:7]), ("linear v", np.r_[8:11]), ("angular v", np.r_[12:15])):
-        x, y = ref["bodies"][:, cols].astype(np.float64), got["bodies"][:, cols].astype(np.float64)
-        d = np.abs(x - y)
-        print("%-20s %-10s rel rms %.2e  max abs %.2e  p99.9 %.2e  scale(max|x|) %.2f" % (name, label, np.sqrt((d ** 2).sum() / (x ** 2).sum()), d.max(), np.quantile(d, 0.999), np.abs(x).max()))
-    imp_ref = np.concatenate([t["impulses"].ravel() for t in ref["type_batches"]]).astype(np.float64)
-    imp_got = np.concatenate([t["impulses"].ravel() for t in got["type_batches"]]).astype(np.float64)
-    d = np.abs(imp_ref - imp_got)
-    print("%-20s %-10s rel rms %.2e  max abs %.2e  p99.9 %.2e  scale %.2f" % (name, "impulses", np.sqrt((d ** 2).sum() / (imp_ref ** 2).sum()), d.max(), np.quantile(d, 0.999), np.abs(imp_ref).max()))
+
+def main(names):
+    _build.build()
+    ob.build()
+    with tempfile.TemporaryDirectory() as d:
+        dll = fp.build_driver(d)
+        for name in names or fp.CONFIGS:
+            case = fp.Case(name)
+            x64 = case.lanes(case.f64(dll))
+            table = fp.compare_builds(case.lanes(case.gpu(strict=True)), case.lanes(case.gpu(strict=False)), x64)
+            print(fp.format_table(name, table))
+            for verdict in ("ok", "typical_ok"):
+                for line in fp.failures(table, verdict):
+                    print("  %s check fails: %s" % ("issue" if verdict == "ok" else "typical-lane", line))
+            print()
+
+
+if __name__ == "__main__":
+    main(sys.argv[1:])
