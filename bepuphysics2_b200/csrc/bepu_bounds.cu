@@ -23,8 +23,9 @@ __global__ void predict_bounding_boxes_kernel(BodyBuffers B, const BodyShape* __
     const Q4 orientation = {q4.x, q4.y, q4.z, q4.w};
     const V3 position = {p4.x, p4.y, p4.z};
     Velocity velocity = {{l4.x, l4.y, l4.z}, {w4.x, w4.y, w4.z}};
-    // Bodies.IsKinematic (Bodies.cs:L326-331): every bit of inverse mass and inverse inertia is zero
-    const bool kinematic = (__float_as_uint(i1.z) | __float_as_uint(i0.x) | __float_as_uint(i0.y) | __float_as_uint(i0.z) | __float_as_uint(i0.w) | __float_as_uint(i1.x) | __float_as_uint(i1.y)) == 0u;
+    // Bodies.IsKinematic (Bodies.cs:L326-331) compares the OR of the seven floats' bits with 0.0f as a float: inverse mass and inverse inertia
+    // are all +0 or -0, in any mix
+    const bool kinematic = i1.z == 0.0f && i0.x == 0.0f && i0.y == 0.0f && i0.z == 0.0f && i0.w == 0.0f && i1.x == 0.0f && i1.y == 0.0f;
     const bool integrate = p.integrate_velocity_for_kinematics != 0 || !kinematic;
     const float sleepEnergy = length_squared(velocity.lin) + length_squared(velocity.ang);
     // the integrated velocity is only used for the prediction; it is not stored (PoseIntegrator.cs:L339)

@@ -1,14 +1,15 @@
 // ORACLE — test infrastructure only (see bepu_math.h). Driver: body gather/scatter, embedded integration, the substep loop,
 // integration responsibilities and the final pose pass, restated from the reference's single-threaded executable spec.
-// Parity: the constraint / math / integration functions called from here are pinned to the reference's C# text (oracle/ref_transpile); THIS file's
-// driver logic (stage order, integration responsibilities, gather/scatter, bundle loops) is UNPINNED: fidelity by construction + closed-form tests.
+// Parity: the constraint / math / integration functions called from here are pinned to the reference's C# text (oracle/ref_transpile). THIS file's
+// driver logic (stage order, integration responsibilities, gather/scatter, bundle loops, the final pose pass, PredictBoundingBoxes' per-body glue,
+// impulse redistribution) is pinned to a second, independent restatement of the reference's single-threaded frame that runs on the transpiled
+// reference's own arithmetic (tests/reference_frame.py, tests/test_oracle_driver_pinned_to_reference.py), bit for bit on a scene matrix.
 #include "bepu_oracle.h"
 
 #include <algorithm>
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
-#include <cstring>
 #include <vector>
 #ifdef _OPENMP
 #include <omp.h>
@@ -987,8 +988,9 @@ extern "C" int32_t oracle_predict_bounding_boxes(int32_t body_count, const float
         const Q4<float> orientation = {b[0], b[1], b[2], b[3]};
         const V3<float> position = {b[4], b[5], b[6]};
         V3<float> linear = {b[8], b[9], b[10]}, angular = {b[12], b[13], b[14]};
-        bool kinematic = true;  // Bodies.IsKinematic, Bodies.cs:L326-331
-        for (int k = 16; k < 23; ++k) { uint32_t bits; std::memcpy(&bits, b + k, 4); kinematic = kinematic && bits == 0u; }
+        // Bodies.IsKinematic (Bodies.cs:L326-331) compares the OR of the seven floats' bits with 0.0f as a FLOAT: any mix of +0 and -0 is kinematic
+        bool kinematic = true;
+        for (int k = 16; k < 23; ++k) kinematic = kinematic && b[k] == 0.0f;
         const bool integrate = integrate_velocity_for_kinematics != 0 || !kinematic;
         const float sleepEnergy = length_squared(linear) + length_squared(angular);
         if (integrate) {  // IntegrateVelocity at the current pose (PoseIntegrator.cs:L339-341); the result is not stored

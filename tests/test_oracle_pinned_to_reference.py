@@ -12,8 +12,10 @@ oracle/_ref/libbepu_ref.so, compiled without FMA contraction like RyuJIT's Vecto
     made by tests/golden/make_reference_fresh_vectors.py where a checkout of the reference is at hand).
 All of it runs from the committed files alone.
 
-What stays outside the pin: the solver driver (substep loop, batch order, integration responsibilities, gather/scatter, the TypeProcessor bundle
-loops), which is generic / unsafe C# the transpiler does not cover; tests/test_oracle.py holds those to closed-form answers.
+What this file leaves to others: the solver driver (substep loop, batch order, integration responsibilities, gather/scatter, the TypeProcessor bundle
+loops, the final pose pass, PredictBoundingBoxes' per-body glue, impulse redistribution) is generic / unsafe C# the transpiler does not cover.
+tests/reference_frame.py restates it a second time from the C# text on top of the transpiled library, and
+tests/test_oracle_driver_pinned_to_reference.py holds the oracle to that restatement bit for bit; tests/test_oracle.py adds closed-form answers.
 TEST INFRASTRUCTURE: nothing in the product loads either library."""
 import ctypes as C
 import os
