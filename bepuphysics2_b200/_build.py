@@ -85,13 +85,23 @@ def _run(cmd):
     return r.stdout
 
 
+# Variants that __graft_entry__.build() compiles next to the shipped library. hazard: the PDL hazard harness (test infrastructure,
+# tests/tools/pdl_hazards.py): the stage kernels delay every post-wait access and can carry planted hazards; the shipped library compiles none of it.
+VARIANTS = {"hazard": ("-DBEPU_HAZARD",)}
+
+
+def variant_paths(variant):
+    """(object directory, library) of a variant build; of the shipped library for variant None."""
+    if not variant:
+        return BUILD, LIB_CUDA
+    return os.path.join(CSRC, "build_" + variant), os.path.join(HERE, "libbepucuda_%s.so" % variant)
+
+
 def build(force=False, verbose=False, variant=None, defines=()):
-    """variant/defines: development A/B builds (libbepucuda_<variant>.so with extra -D flags, selected at run time with BEPUCUDA_VARIANT)."""
-    global BUILD, LIB_CUDA
-    if variant:
-        BUILD = os.path.join(CSRC, "build_" + variant)
-        LIB_CUDA = os.path.join(HERE, "libbepucuda_%s.so" % variant)
-    os.makedirs(BUILD, exist_ok=True)
+    """variant/defines: libbepucuda_<variant>.so with extra -D flags, selected at run time with BEPUCUDA_VARIANT: the VARIANTS above, and development
+    A/B builds (tests/tools/ab_variants.py). A variant build leaves the module's BUILD / LIB_CUDA, the shipped library's paths, alone."""
+    build_dir, lib_cuda = variant_paths(variant)
+    os.makedirs(build_dir, exist_ok=True)
     headers = [os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith((".cuh", ".h", ".inc"))]
     headers.append(os.path.join(HERE, "..", "include", "bepucuda.h"))
     # fast keeps IEEE division: on an H100 the approximate one took the 100 k-body pile past the 8-frame drift bound the fast build is held to
@@ -104,16 +114,16 @@ def build(force=False, verbose=False, variant=None, defines=()):
     all_sources = [os.path.join(CSRC, f) for f in ("bepu_solver_kernels.cu", "bepu_layout_kernels.cu", "bepu_coloring.cu", "bepu_islands.cu", "bepu_bounds.cu", "bepucuda_api.cu", "bepu_topology.cpp")] + headers
     # Nothing to compile when the library was built from exactly these sources (content stamp written after a build: survives a snapshot that
     # does not keep modification times) or is newer than every source. Object files need not travel with a snapshot.
-    stamp = LIB_CUDA + ".stamp"
+    stamp = lib_cuda + ".stamp"
     digest = _digest(all_sources, [NVCC_FLAGS] + [f for _, f in flavours] + [list(defines)])
-    fresh = os.path.exists(LIB_CUDA) and (_stamp_matches(stamp, digest) or (not os.path.exists(stamp) and not _newer(LIB_CUDA, all_sources)))
-    if not force and not defines and fresh:
+    fresh = os.path.exists(lib_cuda) and (_stamp_matches(stamp, digest) or (not os.path.exists(stamp) and not _newer(lib_cuda, all_sources)))
+    if not force and fresh:  # the digest covers the defines
         units = []
         if not os.path.exists(stamp):
-            _write_stamp(stamp, digest, LIB_CUDA)
+            _write_stamp(stamp, digest, lib_cuda)
     jobs = []
     for obj, src, extra in units:
-        o = os.path.join(BUILD, obj)
+        o = os.path.join(build_dir, obj)
         s = os.path.join(CSRC, src)
         frozen = os.path.exists(o) and any(obj.endswith("_%s.o" % u) for u in os.environ.get("BEPUCUDA_FREEZE_UNITS", "").split(",") if u)
         if frozen:
@@ -125,20 +135,19 @@ def build(force=False, verbose=False, variant=None, defines=()):
             for out in ex.map(_run, jobs):
                 if verbose and out.strip():
                     print(out)
-    objs = [os.path.join(BUILD, u[0]) for u in units]
-    if units and (force or _newer(LIB_CUDA, objs) or not _stamp_matches(stamp, digest)):
-        _run([NVCC] + NVCC_FLAGS + ["-shared", "-o", LIB_CUDA] + objs)
+    objs = [os.path.join(build_dir, u[0]) for u in units]
+    if units and (force or _newer(lib_cuda, objs) or not _stamp_matches(stamp, digest)):
+        _run([NVCC] + NVCC_FLAGS + ["-shared", "-o", lib_cuda] + objs)
     if units and not os.environ.get("BEPUCUDA_FREEZE_UNITS"):
-        _write_stamp(stamp, digest, LIB_CUDA)
+        _write_stamp(stamp, digest, lib_cuda)
     if variant:
-        return LIB_CUDA, LIB_HOST
+        return lib_cuda, LIB_HOST
     host_src = os.path.join(CSRC, "host", "bepu_host.cpp")
-    if force or _newer(LIB_HOST, [host_src, LIB_CUDA] + headers):
+    if force or _newer(LIB_HOST, [host_src, lib_cuda] + headers):
         _run([GXX, "-O2", "-std=c++17", "-fPIC", "-shared", "-o", LIB_HOST, host_src, "-L" + HERE, "-lbepucuda", "-Wl,-rpath,$ORIGIN"])
-    return LIB_CUDA, LIB_HOST
+    return lib_cuda, LIB_HOST
 
 
 if __name__ == "__main__":
     _variant = next((a.split("=", 1)[1] for a in sys.argv if a.startswith("--variant=")), None)
-    build(force="--force" in sys.argv, verbose=True, variant=_variant, defines=[a for a in sys.argv if a.startswith("-D")])
-    print("built", LIB_CUDA, LIB_HOST)
+    print("built", *build(force="--force" in sys.argv, verbose=True, variant=_variant, defines=[a for a in sys.argv if a.startswith("-D")]))

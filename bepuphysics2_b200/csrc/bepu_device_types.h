@@ -101,6 +101,53 @@ enum StageKernel : int32_t {
 //   integrates, one thread per body, and the WarmStart stages integrate velocity only.
 constexpr int32_t kLaunchPdl = 1, kLaunchPrefetchRows = 2, kLaunchIntegratorExtensions = 4, kLaunchEarlyWorld = 8, kLaunchEarlyOwned = 16, kLaunchBodiesIntegrated = 32;
 
+// Hazard build (libbepucuda_hazard.so, -DBEPU_HAZARD; test infrastructure, tests/tools/pdl_hazards.py). Two fields above the launch flags, which
+// the shipped library never sets: bits 16-18 a planted hazard (canary), bits 20-27 a delay in units of 10 us that every thread spends after its
+// grid-dependency trigger and before any post-wait load or store. The rank barrier takes them in the high bits of its exchange index. Each canary
+// moves one load to the wrong side of the wait:
+//   kCanarySolveVelocity: Solve gathers the velocity of body slot 0 in its prologue;
+//   kCanaryRowPrefetch: the prologue prefetches the row block without kLaunchPrefetchRows;
+//   kCanaryEarlyWorldBehindIncremental: the integrated contact-only WarmStart loads world inertia in its prologue without kLaunchEarlyWorld;
+//   kCanaryIncrementalVelocity: the incremental update's body CTAs load the velocity before the wait;
+//   kCanarySkipShardWait: boundary warps of sharded stages do not wait for the peers' pushes.
+constexpr int kLaunchHazardCanaryShift = 16, kLaunchHazardDelayShift = 20;
+enum HazardCanary : int32_t {
+    kCanaryNone = 0,
+    kCanarySolveVelocity = 1,
+    kCanaryRowPrefetch = 2,
+    kCanaryEarlyWorldBehindIncremental = 3,
+    kCanaryIncrementalVelocity = 4,
+    kCanarySkipShardWait = 5,
+};
+#ifdef BEPU_HAZARD
+#define BEPU_CANARY(flags, which) ((((flags) >> kLaunchHazardCanaryShift) & 7) == (which))
+#else
+#define BEPU_CANARY(flags, which) false
+#endif
+
+#ifdef __CUDACC__
+// The one grid-dependency wait and trigger of every kernel launched with programmatic dependent launch (the stage kernels and the rank barrier).
+// The trigger comes after the wait, so the next grid's prologue runs only once this grid's predecessor has completed (DESIGN §3). In the hazard
+// build every thread then spins for the launch's delay before it touches memory again: the next grid's prologue loads all run before any store
+// of this grid, so a prologue that reads what this grid writes reads the old value every time.
+__device__ __forceinline__ void pdl_wait_then_trigger(int32_t launch_flags) {
+    asm volatile("griddepcontrol.wait;" ::: "memory");
+    asm volatile("griddepcontrol.launch_dependents;");
+#ifdef BEPU_HAZARD
+    const unsigned long long delay_ns = (unsigned long long)((launch_flags >> kLaunchHazardDelayShift) & 0xff) * 10000ull;
+    if (delay_ns) {
+        unsigned long long t0, t;
+        asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t0)::"memory");
+        do {
+            asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)::"memory");
+        } while (t - t0 < delay_ns);
+    }
+#else
+    (void)launch_flags;
+#endif
+}
+#endif
+
 // One entry per warp of a stage launch: which bundle of which device type batch.
 struct WorkItem {
     int32_t type_batch;

@@ -283,8 +283,10 @@ void launch_gather_body_motion(void* raw, int body_count, const BodyBuffers& B, 
 // which overlaps with the barrier below.
 __global__ void __launch_bounds__(256, 1)
 shard_barrier_kernel(ShardPeers peers, const FrameParams* __restrict__ fpp, uint32_t exchange_index, int32_t* error_flag) {
-    asm volatile("griddepcontrol.wait;" ::: "memory");
-    asm volatile("griddepcontrol.launch_dependents;");
+    pdl_wait_then_trigger((int32_t)exchange_index);  // the hazard build's delay field rides in the high bits of the exchange index
+#ifdef BEPU_HAZARD
+    exchange_index &= 0xffffu;
+#endif
     const unsigned long long seq = (unsigned long long)fpp->exchange_base + exchange_index + 1ull;
     const int p = threadIdx.x;
     if (p < peers.rank_count && p != peers.rank) {

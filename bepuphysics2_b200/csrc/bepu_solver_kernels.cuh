@@ -92,6 +92,9 @@ struct EarlyBodies {
     Inertia inertia[2];
     V3 pos[2];
     Q4 q[2];
+#ifdef BEPU_HAZARD
+    Velocity velocity0;  // kCanarySolveVelocity: the velocity of slot 0, gathered before the wait (bit 2 of `slots`)
+#endif
 };
 
 // GatherAndIntegrate for one body slot of one lane (TypeProcessor.cs:L1298-1397), after the velocity has been loaded. The lane integrates iff the
@@ -230,7 +233,11 @@ BEPU_DI void run_lane(const int32_t* refs, PR p, AR a, float* p_rw, uint32_t enc
 #pragma unroll
         for (int s = 0; s < NB; ++s) {
             const uint32_t idx = enc[s] & kRefIndexMask;
-            load_velocity(B.velocity, idx, v[s]);
+#ifdef BEPU_HAZARD
+            if (s == 0 && (early.slots & 4u)) v[s] = early.velocity0;
+            else
+#endif
+                load_velocity(B.velocity, idx, v[s]);
             if (s < 2 && (early.slots >> s & 1u)) {
                 b[s].inertia = early.inertia[s & 1];
                 if (T::kNeedsPose) b[s].pos = early.pos[s & 1], b[s].q = early.q[s & 1];
@@ -432,21 +439,22 @@ BEPU_DI void shard_wait(const ShardPeers& peers, int lane, uint32_t solve_index,
 // Pose and local inertia are loaded before it: no stage that can precede an incremental update writes them (Solve writes velocities and
 // impulses, WarmStartFirst and, with this flag, WarmStart velocities and world inertia only; the kinematic pass of the previous substep, which
 // writes kinematic poses, is older than that predecessor).
-BEPU_DI void integrate_body_pose(int i, const BodyBuffers& B, const FrameParams* __restrict__ fpp) {
+BEPU_DI void integrate_body_pose(int i, const BodyBuffers& B, const FrameParams* __restrict__ fpp, int flags) {
     const FrameParams fp = *fpp;
     const bool owned = i < B.count && (int32_t)ldg_nc_u32(B.first_batch + i) != 0x7fffffff;
     Inertia local;
     V3 pos;
     Q4 q;
+    Velocity v;
+    const bool early_velocity = owned && BEPU_CANARY(flags, kCanaryIncrementalVelocity);
     if (owned) {
         load_inertia(B.inertia_local, (uint32_t)i, local);
         load_pose(B.pose, (uint32_t)i, pos, q);
+        if (early_velocity) load_velocity(B.velocity, (uint32_t)i, v);
     }
-    asm volatile("griddepcontrol.wait;" ::: "memory");
-    asm volatile("griddepcontrol.launch_dependents;");
+    pdl_wait_then_trigger(flags);
     if (!owned) return;
-    Velocity v;
-    load_velocity(B.velocity, (uint32_t)i, v);
+    if (!early_velocity) load_velocity(B.velocity, (uint32_t)i, v);
     Inertia world;
     world.inv_mass = local.inv_mass;
     integrate_pose_and_inertia(v.lin, v.ang, fp.dt, local.t, pos, q, world.t);
@@ -463,7 +471,7 @@ BEPU_DI void constraint_stage_body(const WorkRecord* __restrict__ records, const
     if constexpr (STAGE == kStageIncremental) {
         // the CTAs past the bundles' (launch_stage adds them with kLaunchBodiesIntegrated) hold one thread per body
         const int bundle_blocks = (work_count + kWarps - 1) / kWarps;
-        if ((int)blockIdx.x >= bundle_blocks) return integrate_body_pose(((int)blockIdx.x - bundle_blocks) * kStageBlockThreads + (int)threadIdx.x, B, fpp);
+        if ((int)blockIdx.x >= bundle_blocks) return integrate_body_pose(((int)blockIdx.x - bundle_blocks) * kStageBlockThreads + (int)threadIdx.x, B, fpp, flags);
     }
     __shared__ __align__(128) float slab[kStaged ? kWarps * kStageSlabRows * kLanes : 1];
     __shared__ __align__(8) unsigned long long bars[kWarps];
@@ -476,7 +484,7 @@ BEPU_DI void constraint_stage_body(const WorkRecord* __restrict__ records, const
     const bool active = warp < work_count;
     const uint32_t slab_addr = kStaged ? smem_u32(slab) + warp_in_block * kStageSlabBytes : 0;
     const uint32_t bar = smem_u32(&bars[warp_in_block]);
-    const bool early_rows = kStaged && (flags & kLaunchPrefetchRows);
+    const bool early_rows = kStaged && ((flags & kLaunchPrefetchRows) || BEPU_CANARY(flags, kCanaryRowPrefetch));
     uint32_t prestep_bytes = 0, impulse_bytes = 0;
     EarlyBodies early{};
     if (active) {
@@ -501,18 +509,24 @@ BEPU_DI void constraint_stage_body(const WorkRecord* __restrict__ records, const
             // world mode on a WarmStart only in the instantiation the host launches it in (the integrated one), owned mode never there
             constexpr bool kWorld = STAGE == kStageSolve || kIntegrated, kOwned = STAGE != kStageSolve && !kIntegrated;
             if (kOwned && (flags & kLaunchEarlyOwned)) load_early_bodies<STAGE, kContacts>(rec.type_id, enc0, enc1, B, early);
-            else if (kWorld && (flags & kLaunchEarlyWorld)) load_early_bodies<kStageSolve, kContacts>(rec.type_id, enc0, enc1, B, early);
+            else if (kWorld && ((flags & kLaunchEarlyWorld) || (kIntegrated && BEPU_CANARY(flags, kCanaryEarlyWorldBehindIncremental))))
+                load_early_bodies<kStageSolve, kContacts>(rec.type_id, enc0, enc1, B, early);
         }
+#ifdef BEPU_HAZARD
+        if (STAGE == kStageSolve && BEPU_CANARY(flags, kCanarySolveVelocity) && (int32_t)enc0 != kRefEmpty) {
+            load_velocity(B.velocity, enc0 & kRefIndexMask, early.velocity0);
+            early.slots |= 4u;
+        }
+#endif
     }
     const FrameParams fp = *fpp;
-    asm volatile("griddepcontrol.wait;" ::: "memory");
-    asm volatile("griddepcontrol.launch_dependents;");
+    pdl_wait_then_trigger(flags);
     const bool integrated = kIntegrated || (STAGE == kStageWarmStart && !kExt && !kContacts && (flags & kLaunchBodiesIntegrated));
     bool boundary = false;
     if constexpr (kSharded) {
         boundary = active && (rec.live_lanes & kRecordBoundaryBit) != 0;
         // records other ranks pushed in the previous exchange point are read below: all of them must have arrived
-        if (boundary && shard->exchange_index > 0) shard_wait(*peers, lane, fp.shard_solve_index, shard->exchange_index - 1u, shard->error_flag);
+        if (boundary && shard->exchange_index > 0 && !BEPU_CANARY(flags, kCanarySkipShardWait)) shard_wait(*peers, lane, fp.shard_solve_index, shard->exchange_index - 1u, shard->error_flag);
     }
     if (!active) return;
     if constexpr (kStaged) {

@@ -2,6 +2,7 @@
 // C ABI declared in include/bepucuda.h. No CPU fallback lives here: without a usable CUDA device bepucuda_create fails.
 #include <algorithm>
 #include <cmath>
+#include <cstdlib>
 #include <cstring>
 #include <string>
 #include <vector>
@@ -156,6 +157,9 @@ struct bepucuda_ctx {
     std::vector<int32_t> kinematics;
     StageProgram program;
     PinnedBuffer frame_params_host;             // FrameParams
+#ifdef BEPU_HAZARD
+    int32_t hazard_canary = 0, hazard_delay_us = 0;  // BEPUCUDA_HAZARD at bepucuda_create (hazard build only, see hazard_launch_bits)
+#endif
 
     // the captured stage sequence of the program (dropped when the program is replaced), and what its launches bake in besides the program
     cudaGraph_t graph = nullptr;
@@ -276,6 +280,23 @@ void invalidate_graph(bepucuda_ctx* ctx) {
 uint32_t integrate_extensions(const bepucuda_ctx* ctx) {
     return (ctx->accelerations_count >= 0 ? kIntegrateAccelerations : 0u) | (ctx->point_gravity ? kIntegratePointGravity : 0u);
 }
+#ifdef BEPU_HAZARD
+// The hazard fields of every launch of this context (bepu_device_types.h): its canary, and its delay, which grows with the rank in peer mode so that
+// the ranks drift apart by one delay per stage wherever boundary warps do not wait for their peers.
+int32_t hazard_launch_bits(const bepucuda_ctx* ctx) {
+    const int delay_units = std::min(255, ctx->hazard_delay_us * (1 + (ctx->peer_mode ? ctx->peers.rank : 0)) / 10);
+    return (ctx->hazard_canary << kLaunchHazardCanaryShift) | (delay_units << kLaunchHazardDelayShift);
+}
+// BEPUCUDA_HAZARD="delay_us=<n>,canary=<k>" (either part optional)
+void read_hazard_environment(bepucuda_ctx* ctx) {
+    const char* env = std::getenv("BEPUCUDA_HAZARD");
+    if (!env) return;
+    const char* d = std::strstr(env, "delay_us=");
+    const char* c = std::strstr(env, "canary=");
+    if (d) ctx->hazard_delay_us = std::max(0, std::atoi(d + 9));
+    if (c) ctx->hazard_canary = std::atoi(c + 7) & 7;
+}
+#endif
 LaunchContext launch_context(const bepucuda_ctx* ctx, bool profile) { return {integrate_extensions(ctx) != 0, ctx->integ.angular_integration_mode, profile}; }
 bool same_bodies(const BodyBuffers& a, const BodyBuffers& b) {
     return a.pose == b.pose && a.velocity == b.velocity && a.inertia_local == b.inertia_local && a.inertia_world == b.inertia_world && a.constrained == b.constrained &&
@@ -298,6 +319,11 @@ void issue_stage_sequence(bepucuda_ctx* ctx, cudaStream_t s, int64_t* launches, 
     ShardLaunch shard{ctx->peers, (long long)(ctx->peer32.as<int32_t>() - ctx->refs32.as<int32_t>()), {0, ctx->error_dev.as<int32_t>()}};
     int64_t n = 0;
     const LaunchContext lc = launch_context(ctx, profile != nullptr);
+#ifdef BEPU_HAZARD
+    const int32_t hazard = hazard_launch_bits(ctx);
+#else
+    constexpr int32_t hazard = 0;
+#endif
     for (size_t i = 0; i < ctx->program.ops.size(); ++i) {
         const StageOp& op = ctx->program.ops[i];
         const bool barrier = op.exchange == kRankBarrier;
@@ -309,13 +335,13 @@ void issue_stage_sequence(bepucuda_ctx* ctx, cudaStream_t s, int64_t* launches, 
             if (barrier) {
                 // all ranks meet: before the first stage of a solve; around the incremental contact update, which reads the velocities of shared
                 // bodies; and before the final pose pass
-                launch_shard_barrier(ctx->peers, fp, op.exchange_index, ctx->error_dev.as<int32_t>(), s);
+                launch_shard_barrier(ctx->peers, fp, op.exchange_index | (uint32_t)hazard, ctx->error_dev.as<int32_t>(), s);
             } else if (op.stage <= kStageIncremental) {
                 // a sharded stage stores the records it writes for shared bodies into the ranks that reference them, and its boundary bundles wait
                 // for and announce arrivals themselves (ShardStage)
                 shard.stage.exchange_index = op.exchange_index;
                 ctx->launchers->constraint_stage(op.stage, launch.kernel, records + op.work_begin, ref_rows + (size_t)op.work_begin * 64, op.work_count, ctx->B, fp,
-                                                 launch.flags, op.exchange == kNoExchange ? nullptr : &shard, s);
+                                                 launch.flags | hazard, op.exchange == kNoExchange ? nullptr : &shard, s);
             } else if (op.stage <= kStageKinematic) {
                 ctx->launchers->kinematic_stage(op.stage, kin, op.work_count, ctx->B, fp, launch.flags, s);
             } else {
@@ -494,6 +520,9 @@ int32_t bepucuda_create(const bepucuda_config* cfg, bepucuda_ctx** out) {
     ctx->launchers = cfg->strict_fp ? get_launchers_bepu_strict() : get_launchers_bepu_fast();
     ctx->pinned_arena.pinned_host = true;
     ctx->pinned_arena.min_chunk = (size_t)16 << 20;
+#ifdef BEPU_HAZARD
+    read_hazard_environment(ctx);
+#endif
     cudaError_t e = cudaSetDevice(ctx->device);
     if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking);
     cudaEvent_t* evs[] = {&ctx->ev_solve_begin, &ctx->ev_solve_end, &ctx->ev_up_begin, &ctx->ev_up_end, &ctx->ev_down_begin, &ctx->ev_down_end};

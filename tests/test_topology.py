@@ -375,11 +375,14 @@ def single_batch(scene):
 def test_prologue_prefetch_only_reads_what_the_previous_stage_does_not_write(libs, shim, case):
     """DESIGN §3: a stage's prologue runs while its immediate predecessor is still running, so it may load only what that predecessor does not write.
     What each stage writes: WarmStart(b) the velocities of b's bodies, and the pose and world inertia of those it integrates (the lowest batch that
-    references a body integrates it) unless its launch has kLaunchBodiesIntegrated; Solve(b) velocities and b's impulses; the incremental update the
-    prestep of every contact bundle, and with kLaunchBodiesIntegrated the pose and world inertia of every integrated body; the kinematic passes the
-    velocities and (substeps > 0) poses of the kinematic bodies. The program's facts are checked against the writes of unflagged launches. What a
-    resolved launch loads: rows = b's prestep and impulses; world = world inertia of the bodies in slots 0 and 1, and their pose unless the kernel is
-    contact-only; owned = the pose of the bodies b integrates. Nothing is known about what ran before the first stage."""
+    references a body integrates it) unless its launch has kLaunchBodiesIntegrated; WarmStartFirst(b) the velocities of b's bodies and the world
+    inertia of those it integrates (IntegrateVelocity moves no pose); Solve(b) velocities and b's impulses; the incremental update the prestep of
+    every contact bundle, and with kLaunchBodiesIntegrated the pose and world inertia of every integrated body; the kinematic passes the velocities
+    and (substeps > 0) poses of the kinematic bodies. Nothing writes local inertia. The program's facts are checked against the writes of unflagged
+    launches. What a resolved launch loads before its wait: rows = b's prestep and impulses; world = world inertia of the bodies in slots 0 and 1,
+    and their pose unless the kernel is contact-only; owned = the local inertia and pose of the bodies b integrates; the incremental update with
+    kLaunchBodiesIntegrated (integrate_body_pose, launched with PDL) the local inertia and pose of every integrated body. Nothing is known about what
+    ran before the first stage."""
     W = 8
     scene = mixed_scene(7) if case == "mixed" else single_batch(scenes.shape_pile(800, seed=17))
     sim = util.make_sim(scene, bundle_width=W, fallback_batch_threshold=6)
@@ -409,10 +412,13 @@ def test_prologue_prefetch_only_reads_what_the_previous_stage_does_not_write(lib
 
     every_integrated = set().union(*integrated)
     world_loads_on_ws = 0
+    body_loads_behind = {WS_FIRST: 0, WS: 0, SOLVE: 0}  # incremental launches with pre-wait body loads, by the stage of their predecessor
 
     def writes(op, flags=0):
         stage, d = int(op[0]), batch_of.get(int(op[1]))
-        if stage in (WS_FIRST, WS):
+        if stage == WS_FIRST:
+            return {("velocity", x) for x in dynamic[d]} | {("inertia", x) for x in integrated[d]}
+        if stage == WS:
             return {("velocity", x) for x in dynamic[d]} | ({(what, x) for x in integrated[d] for what in ("pose", "inertia")} if not flags & BODIES_INTEGRATED else set())
         if stage == SOLVE:
             return {("velocity", x) for x in dynamic[d]} | {("impulses", d)}
@@ -421,15 +427,17 @@ def test_prologue_prefetch_only_reads_what_the_previous_stage_does_not_write(lib
         return {(what, x) for x in kinematics for what in (("velocity", "pose") if stage == KIN else ("velocity",))}
 
     def loads(op, kernel, flags):
+        if int(op[0]) == INCREMENTAL:
+            return {(what, x) for x in every_integrated for what in ("local", "pose")} if flags & BODIES_INTEGRATED and flags & PDL else set()
         d = batch_of[int(op[1])]
         got = {("prestep", d), ("impulses", d)} if flags & ROWS else set()
         if flags & EARLY_WORLD:
             got |= {(what, x) for x in slot01[d] for what in (("inertia",) if kernel == KERNEL_CONTACTS else ("inertia", "pose"))}
         if flags & EARLY_OWNED:
-            got |= {("pose", x) for x in integrated[d]}
+            got |= {(what, x) for x in integrated[d] for what in ("local", "pose")}
         return got
 
-    for iterations in ([1], [2, 2], [0, 3, 1], [0, 0]):
+    for iterations in ([1], [2, 2], [0, 3, 1], [0, 0], [2, 0, 2]):
         for ivk in (False, True):
             ops, _ = p.program(iterations, len(kinematics), ivk, False, sim.body_count)
             previous = None
@@ -460,7 +468,7 @@ def test_prologue_prefetch_only_reads_what_the_previous_stage_does_not_write(lib
                 resolved = resolve(shim, live, ext, mode, profile)
                 world_on_ws = 0
                 for i, op in enumerate(live):
-                    if int(op[0]) not in (WS_FIRST, WS, SOLVE):
+                    if int(op[0]) not in (WS_FIRST, WS, SOLVE, INCREMENTAL):
                         continue
                     kernel, flags = (int(v) for v in resolved[i])
                     got = loads(op, kernel, flags)
@@ -468,5 +476,9 @@ def test_prologue_prefetch_only_reads_what_the_previous_stage_does_not_write(lib
                     clash = got & writes(live[i - 1], int(resolved[i - 1, 1])) if i > 0 else set()
                     assert not clash, "op %d (%s) loads %s that its predecessor writes" % (i, op.tolist(), sorted(clash)[:4])
                     world_on_ws += int(op[0]) == WS and bool(flags & EARLY_WORLD)
+                    if got and int(op[0]) == INCREMENTAL:
+                        body_loads_behind[int(live[i - 1, 0])] += 1
                 world_loads_on_ws += world_on_ws
     assert (world_loads_on_ws > 0) == (case == "mixed"), "the world-inertia load of a flagged WarmStart behind an earlier batch's is covered"
+    # the incremental update's body CTAs were checked behind a Solve and, in the substeps without iterations, behind a WarmStart and a WarmStartFirst
+    assert body_loads_behind[SOLVE] > 0 and body_loads_behind[WS] > 0 and body_loads_behind[WS_FIRST] > 0, body_loads_behind

@@ -55,9 +55,10 @@ def compare(a, b, exact=True, rel_rms=1e-3, max_abs=5e-2):
     otherwise (FMA-contracted, approximate sqrt build): per quantity, relative RMS error <= rel_rms and max abs error <= max_abs."""
     def check(x, y, what):
         if exact:
-            same = np.array_equal(x, y) or np.array_equal(x.view(np.uint32), y.view(np.uint32))
-            if not same:
-                bad = np.argwhere(~((x == y) | (np.isnan(x) & np.isnan(y))))
+            # bit patterns only: -0.0 against +0.0 is a difference, and so are two NaNs with different payloads
+            bits_x, bits_y = np.ascontiguousarray(x).view(np.uint32), np.ascontiguousarray(y).view(np.uint32)
+            if not np.array_equal(bits_x, bits_y):
+                bad = np.argwhere(bits_x != bits_y)
                 diff = np.abs(x.astype(np.float64) - y.astype(np.float64))
                 raise AssertionError("%s differs at %d positions (first %s), max abs diff %g" % (what, bad.shape[0], bad[0].tolist(), np.nanmax(diff)))
         else:
