@@ -36,6 +36,10 @@ __global__ void merge_bodies_kernel(float4* __restrict__ raw, int body_count, Bo
     raw[t] = v;
 }
 
+// Row 0 of lane `lane` of bundle `bundle` of an AOSOA-32 array with `rows` rows per bundle (a device type batch's body references, prestep or
+// accumulated impulses); row r is at [r * 32]. A macro: as an inline function it changed the instructions nvcc selects for transpose_in_all_kernel.
+#define SLOT_ROW0(base, rows, bundle, lane) ((base) + (size_t)(bundle) * (rows) * 32 + (lane))
+
 // AOSOA-W (reference layout: [bundleW][row][W]) <-> AOSOA-32 for every device type batch in one launch.
 // One warp per destination bundle; lane = destination constraint slot. `map` (fallback levels only) gives the source
 // constraint index of each destination slot, -1 = padding; without a map slot i is source constraint i.
@@ -54,7 +58,7 @@ __global__ void transpose_in_all_kernel(const DeviceTypeBatch* __restrict__ tbs,
     if (c >= d.src_count) c = -1;
     const size_t sb = c < 0 ? 0 : (size_t)(c / W), sl = c < 0 ? 0 : (size_t)(c % W);
     if (what & kTransposeRefs) {
-        int32_t* dst = tb.refs + (size_t)w.bundle * d.bodies * 32 + lane;
+        int32_t* dst = SLOT_ROW0(tb.refs, d.bodies, w.bundle, lane);
         for (int r = 0; r < d.bodies; ++r) {
             int32_t v = kRefEmpty;
             if (c >= 0) {
@@ -65,11 +69,11 @@ __global__ void transpose_in_all_kernel(const DeviceTypeBatch* __restrict__ tbs,
         }
     }
     if (what & kTransposePrestep) {
-        float* dst = tb.prestep + (size_t)w.bundle * d.prestep_rows * 32 + lane;
+        float* dst = SLOT_ROW0(tb.prestep, d.prestep_rows, w.bundle, lane);
         for (int r = 0; r < d.prestep_rows; ++r) dst[r * 32] = c < 0 ? 0.0f : d.src_prestep[(sb * d.prestep_rows + r) * W + sl];
     }
     if (what & kTransposeImpulses) {
-        float* dst = tb.impulses + (size_t)w.bundle * d.impulse_rows * 32 + lane;
+        float* dst = SLOT_ROW0(tb.impulses, d.impulse_rows, w.bundle, lane);
         for (int r = 0; r < d.impulse_rows; ++r) dst[r * 32] = c < 0 ? 0.0f : d.src_impulses[(sb * d.impulse_rows + r) * W + sl];
     }
 }
@@ -124,13 +128,49 @@ __global__ void transpose_out_all_kernel(const DeviceTypeBatch* __restrict__ tbs
     if (c < 0 || c >= d.src_count) return;
     const size_t sb = (size_t)(c / W), sl = (size_t)(c % W);
     if (what & kTransposePrestep) {
-        const float* src = tb.prestep + (size_t)w.bundle * d.prestep_rows * 32 + lane;
+        const float* src = SLOT_ROW0(tb.prestep, d.prestep_rows, w.bundle, lane);
         for (int r = 0; r < d.prestep_rows; ++r) d.src_prestep[(sb * d.prestep_rows + r) * W + sl] = src[r * 32];
     }
     if (what & kTransposeImpulses) {
-        const float* src = tb.impulses + (size_t)w.bundle * d.impulse_rows * 32 + lane;
+        const float* src = SLOT_ROW0(tb.impulses, d.impulse_rows, w.bundle, lane);
         for (int r = 0; r < d.impulse_rows; ++r) d.src_impulses[(sb * d.impulse_rows + r) * W + sl] = src[r * 32];
     }
+}
+
+// bepucuda_read_constraints: one warp per request. Lane l gathers words l and l + 32 of the request's record from the rows of its slot, so the
+// warp stores the 256-B record as two coalesced 128-B rows; the only rows read are those of the requested constraints.
+// Record words (include/bepucuda.h): 0 type id, 1 live, 2-5 body references, 6-17 accumulated impulses, 18-52 prestep, 53-63 zero.
+constexpr int kRecordRefs = 2, kRecordImpulses = 6, kRecordPrestep = 18, kRecordEnd = 53;
+__global__ void read_constraints_kernel(const DeviceTypeBatch* __restrict__ tbs, const TransposeDesc* __restrict__ descs, const DeviceSlot* __restrict__ inverse,
+                                        const ReadRequest* __restrict__ requests, int count, int32_t* __restrict__ records) {
+    const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+    if (warp >= count) return;
+    const ReadRequest q = requests[warp];
+    const DeviceSlot at = q.at.type_batch < 0 ? inverse[q.at.slot] : q.at;
+    int32_t out[2] = {lane == 0 ? q.type_id : 0, 0};
+    if (at.type_batch >= 0) {
+        const TransposeDesc d = descs[at.type_batch];
+        const DeviceTypeBatch tb = tbs[at.type_batch];
+        const int bundle = at.slot >> 5, l = at.slot & 31;
+        for (int k = 0; k < 2; ++k) {
+            const int w = lane + 32 * k;
+            if (w == 1) {
+                out[k] = 1;
+            } else if (w >= kRecordRefs && w < kRecordImpulses) {
+                // the host's encoding: the device-only ownership bits (DESIGN §2) cleared, empty slots -1
+                const int r = w - kRecordRefs;
+                const int32_t v = r < d.bodies ? SLOT_ROW0(tb.refs, d.bodies, bundle, l)[r * 32] : kRefEmpty;
+                out[k] = v < 0 ? kRefEmpty : (int32_t)((uint32_t)v & (kRefIndexMask | kRefKinematicBit));
+            } else if (w >= kRecordImpulses && w < kRecordPrestep) {
+                if (w - kRecordImpulses < d.impulse_rows) out[k] = __float_as_int(SLOT_ROW0(tb.impulses, d.impulse_rows, bundle, l)[(w - kRecordImpulses) * 32]);
+            } else if (w >= kRecordPrestep && w < kRecordEnd) {
+                if (w - kRecordPrestep < d.prestep_rows) out[k] = __float_as_int(SLOT_ROW0(tb.prestep, d.prestep_rows, bundle, l)[(w - kRecordPrestep) * 32]);
+            }
+        }
+    }
+    int32_t* record = records + (size_t)warp * 64;
+    record[lane] = out[0];
+    record[lane + 32] = out[1];
 }
 
 // Pass 1 over every (constraint, body slot): first_batch[body] = min device batch referencing it as a dynamic body;
@@ -264,6 +304,11 @@ void launch_transpose_in_all(const DeviceTypeBatch* tbs, const TransposeDesc* de
 void launch_transpose_out_all(const DeviceTypeBatch* tbs, const TransposeDesc* descs, const WorkItem* work, int work_count, int W, int what, cudaStream_t s) {
     if (work_count <= 0) return;
     transpose_out_all_kernel<<<blocks_for((size_t)work_count * 32, 128), 128, 0, s>>>(tbs, descs, work, work_count, W, what);
+}
+void launch_read_constraints(const DeviceTypeBatch* tbs, const TransposeDesc* descs, const DeviceSlot* inverse, const ReadRequest* requests, int count, int32_t* records,
+                             cudaStream_t s) {
+    if (count <= 0) return;
+    read_constraints_kernel<<<blocks_for((size_t)count * 32, 128), 128, 0, s>>>(tbs, descs, inverse, requests, count, records);
 }
 void launch_redistribute_impulses(const DeviceTypeBatch* tbs, const TransposeDesc* descs, const WorkItem* work, int work_count, cudaStream_t s) {
     if (work_count <= 0) return;

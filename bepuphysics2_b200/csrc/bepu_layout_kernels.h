@@ -25,6 +25,19 @@ enum { kTransposeRefs = 1, kTransposePrestep = 2, kTransposeImpulses = 4, kTrans
 constexpr int32_t kDescRedistribute = 16;
 void launch_transpose_in_all(const DeviceTypeBatch* tbs, const TransposeDesc* descs, const WorkItem* work, int work_count, int W, int what, cudaStream_t s);
 void launch_transpose_out_all(const DeviceTypeBatch* tbs, const TransposeDesc* descs, const WorkItem* work, int work_count, int W, int what, cudaStream_t s);
+// Lane `slot % 32` of bundle `slot / 32` of device type batch `type_batch`.
+struct DeviceSlot {
+    int32_t type_batch, slot;
+};
+// One location of bepucuda_read_constraints, resolved on the host. A constraint of a synchronized type batch is its device slot (identity slots); one
+// of a fallback type batch is found on the device through the planner's inverse map: at = {-1, entry}, and the entry is {-1, -1} for a hole.
+struct ReadRequest {
+    int32_t type_id;
+    DeviceSlot at;
+};
+// bepucuda_read_constraints: the 64-word record of every request (include/bepucuda.h), read from the AOSOA-32 rows, into records[count][64].
+void launch_read_constraints(const DeviceTypeBatch* tbs, const TransposeDesc* descs, const DeviceSlot* inverse, const ReadRequest* requests, int count, int32_t* records,
+                             cudaStream_t s);
 void launch_fill_i32(int32_t* p, size_t n, int32_t v, cudaStream_t s);
 // RedistributeImpulses (NarrowPhaseConstraintUpdate.cs:L81-135) for every device type batch whose descriptor has kDescRedistribute, on the AOSOA-32 impulses.
 void launch_redistribute_impulses(const DeviceTypeBatch* tbs, const TransposeDesc* descs, const WorkItem* work, int work_count, cudaStream_t s);

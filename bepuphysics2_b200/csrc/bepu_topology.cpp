@@ -78,6 +78,8 @@ int plan_topology(const std::vector<SourceView>& sources, int W, int fallback_th
     });
     p.source_live.assign(sources.size(), 0);
     p.source_bundle_base.assign(sources.size(), 0);
+    p.source_type_batch.assign(sources.size(), -1);
+    p.source_inverse_offset.assign(sources.size(), -1);
     for (int si : order) {
         p.source_bundle_base[(size_t)si] = p.source_bundles;
         p.source_bundles += (sources[(size_t)si].count + W - 1) / W;
@@ -94,6 +96,7 @@ int plan_topology(const std::vector<SourceView>& sources, int W, int fallback_th
         const SourceView& s = sources[(size_t)si];
         if (s.batch_index >= fallback_threshold) continue;
         while ((int)batch_tbs.size() <= s.batch_index) batch_tbs.emplace_back();
+        p.source_type_batch[(size_t)si] = (int32_t)p.tbs.size();
         add_tb(si, s.batch_index, s.count, -1);
         p.source_live[(size_t)si] = s.count;
         p.constraint_count += s.count;
@@ -124,6 +127,8 @@ int plan_topology(const std::vector<SourceView>& sources, int W, int fallback_th
         const SourceView& s = sources[(size_t)order[rank]];
         if (s.batch_index < fallback_threshold) continue;
         if (last_level.empty()) last_level.assign((size_t)body_count, 0);
+        p.source_inverse_offset[(size_t)order[rank]] = (int64_t)p.inverse.size();
+        p.inverse.resize(p.inverse.size() + (size_t)s.count, DeviceSlot{-1, -1});  // holes keep {-1, -1}
         const int nb = get_type_info(s.type_id)->bodies;
         const int bundles = (s.count + W - 1) / W;
         auto ref = [&](int k, int b, int l) { return s.refs[((size_t)k * nb + b) * W + l]; };
@@ -180,8 +185,12 @@ int plan_topology(const std::vector<SourceView>& sources, int W, int fallback_th
             const int rank = slots[i].rank;
             size_t j = i;
             while (j < slots.size() && slots[j].level == level && slots[j].rank == rank) ++j;
-            add_tb(order[(size_t)rank], (int)batch_tbs.size() - 1, (int)(j - i), (int64_t)p.maps.size());
-            for (size_t q = i; q < j; ++q) p.maps.push_back(slots[q].constraint);
+            const int source = order[(size_t)rank];
+            add_tb(source, (int)batch_tbs.size() - 1, (int)(j - i), (int64_t)p.maps.size());
+            for (size_t q = i; q < j; ++q) {
+                p.maps.push_back(slots[q].constraint);
+                p.inverse[(size_t)p.source_inverse_offset[(size_t)source] + (size_t)slots[q].constraint] = {(int32_t)p.tbs.size() - 1, (int32_t)(q - i)};
+            }
             p.maps.resize((size_t)p.tbs.back().map_offset + (size_t)p.tbs.back().bundle_count * 32, -1);
             i = j;
         }

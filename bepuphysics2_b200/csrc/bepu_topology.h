@@ -38,6 +38,11 @@ struct PlannedTypeBatch {
 struct TopologyPlan {
     std::vector<PlannedTypeBatch> tbs;
     std::vector<int32_t> maps;                // per slot of a fallback level: the source constraint, -1 = padding
+    // The inverse, for reads by host location (bepucuda_read_constraints). A synchronized source is one device type batch with identity slots;
+    // the constraints of a fallback source are spread over the type batches of its levels.
+    std::vector<int32_t> source_type_batch;      // per source: its device type batch if synchronized, else -1
+    std::vector<int64_t> source_inverse_offset;  // per source: the first of its `count` entries in `inverse` if fallback, else -1
+    std::vector<DeviceSlot> inverse;             // per fallback source constraint: the slot that maps to it, {-1, -1} for a hole
     std::vector<WorkItem> work;               // grouped by device batch, then the incremental list
     std::vector<int32_t> bundle_live;         // live constraints per work item (parallel to `work`)
     struct Batch { int32_t begin, count, contacts_only; };

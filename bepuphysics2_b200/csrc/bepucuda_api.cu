@@ -180,6 +180,7 @@ struct bepucuda_ctx {
     int shape_count = -1;
     DeviceBuffer color_refs, color_priorities, color_body_min, color_body_mask, color_out, color_lists, color_counts;  // bepucuda_color_constraints
     DeviceBuffer island_activities, island_label, island_blocked, island_count, island_flags, island_roots, island_counts, island_scalars, island_temp;  // bepucuda_find_sleepable_islands
+    DeviceBuffer inverse_table, read_requests, read_records;  // bepucuda_read_constraints: the plan's inverse slot map, one call's requests and records
     std::vector<cudaEvent_t> profile_events;
 };
 
@@ -756,6 +757,7 @@ int32_t bepucuda_end_constraints(bepucuda_ctx* ctx) {
     CK(ctx->prestep32.reserve(topo.prestep_words * 4 + 4));
     CK(ctx->impulses32.reserve(topo.impulse_words * 4 + 4));
     CK(ctx->map_table.reserve(topo.maps.size() * 4 + 4));
+    CK(ctx->inverse_table.reserve(topo.inverse.size() * sizeof(DeviceSlot) + 8));
     std::vector<DeviceTypeBatch> tbs(topo.tbs.size());
     ctx->tdescs.resize(topo.tbs.size());
     for (size_t i = 0; i < topo.tbs.size(); ++i) {
@@ -783,6 +785,8 @@ int32_t bepucuda_end_constraints(bepucuda_ctx* ctx) {
     if (!topo.work.empty()) CK(cudaMemcpyAsync(ctx->work_table.ptr, topo.work.data(), topo.work.size() * sizeof(WorkItem), cudaMemcpyHostToDevice, ctx->stream));
     if (!ctx->records.empty()) CK(cudaMemcpyAsync(ctx->record_table.ptr, ctx->records.data(), ctx->records.size() * sizeof(WorkRecord), cudaMemcpyHostToDevice, ctx->stream));
     if (!topo.maps.empty()) CK(cudaMemcpyAsync(ctx->map_table.ptr, topo.maps.data(), topo.maps.size() * 4, cudaMemcpyHostToDevice, ctx->stream));
+    if (!topo.inverse.empty())
+        CK(cudaMemcpyAsync(ctx->inverse_table.ptr, topo.inverse.data(), topo.inverse.size() * sizeof(DeviceSlot), cudaMemcpyHostToDevice, ctx->stream));
     CK(cudaMemcpyAsync(ctx->bodies_per_type.ptr, bodies_per_type, sizeof(bodies_per_type), cudaMemcpyHostToDevice, ctx->stream));
     if (!ctx->kinematics.empty()) CK(cudaMemcpyAsync(ctx->kinematics_dev.ptr, ctx->kinematics.data(), ctx->kinematics.size() * 4, cudaMemcpyHostToDevice, ctx->stream));
 
@@ -978,6 +982,7 @@ int32_t bepucuda_solve(bepucuda_ctx* ctx, float dt) {
             ctx->graph_bodies = ctx->B;
             ctx->graph_launch = lc;
             ctx->timings.kernel_launches = n;
+            ++ctx->timings.graph_captures;
         }
         CK(cudaGraphLaunch(ctx->graph_exec, ctx->stream));
         launches = ctx->timings.kernel_launches;
@@ -1060,6 +1065,44 @@ int32_t bepucuda_download_prestep(bepucuda_ctx* ctx, int32_t batch_index, int32_
                              kTransposePrestep, ctx->stream);
     CK(cudaGetLastError());
     CK(cudaMemcpyAsync(prestep_out, s->raw_prestep, s->prestep_bytes, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    return BEPUCUDA_OK;
+}
+
+static_assert(sizeof(bepucuda_constraint_location) == 16, "bepucuda_constraint_location is four int32");
+
+int32_t bepucuda_read_constraints(bepucuda_ctx* ctx, int32_t count, const bepucuda_constraint_location* locations, int32_t* records_out) {
+    if (!ctx) return BEPUCUDA_ERR_INVALID_ARGUMENT;
+    if (ctx->peer_mode) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, "read_constraints in peer mode: a rank holds its constraints compacted, so host locations do not address them");
+    if (!ctx->constraints_ready) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, "read_constraints before end_constraints");
+    if (count < 0 || (count > 0 && (!locations || !records_out))) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "read_constraints: bad arguments");
+    if (count == 0) return BEPUCUDA_OK;
+    // (batch, type id) -> source; every location is checked before any device work, so a bad one leaves records_out untouched
+    std::vector<int32_t> source_of((size_t)ctx->batch_count * 64, -1);
+    for (size_t i = ctx->sources.size(); i-- > 0;) source_of[(size_t)ctx->sources[i].batch_index * 64 + (size_t)ctx->sources[i].type_id] = (int32_t)i;
+    std::vector<ReadRequest> requests((size_t)count);
+    for (int32_t i = 0; i < count; ++i) {
+        const bepucuda_constraint_location& l = locations[i];
+        const int32_t s = l.set_index == 0 && l.batch_index >= 0 && l.batch_index < ctx->batch_count && l.type_id >= 0 && l.type_id < 64
+                              ? source_of[(size_t)l.batch_index * 64 + (size_t)l.type_id] : -1;
+        if (s < 0 || l.index_in_type_batch < 0 || l.index_in_type_batch >= ctx->sources[(size_t)s].count)
+            return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "read_constraints: location " + std::to_string(i) + " (set " + std::to_string(l.set_index) + ", batch " +
+                                                                std::to_string(l.batch_index) + ", type " + std::to_string(l.type_id) + ", index " +
+                                                                std::to_string(l.index_in_type_batch) + ") names no constraint of the active set");
+        ReadRequest& q = requests[(size_t)i];
+        q.type_id = l.type_id;
+        q.at.type_batch = ctx->topo.source_type_batch[(size_t)s];
+        q.at.slot = q.at.type_batch >= 0 ? l.index_in_type_batch : (int32_t)(ctx->topo.source_inverse_offset[(size_t)s] + l.index_in_type_batch);
+    }
+    CK(cudaSetDevice(ctx->device));
+    const size_t n = (size_t)count;
+    CK(ctx->read_requests.reserve(n * sizeof(ReadRequest)));
+    CK(ctx->read_records.reserve(n * 256));
+    CK(cudaMemcpyAsync(ctx->read_requests.ptr, requests.data(), n * sizeof(ReadRequest), cudaMemcpyHostToDevice, ctx->stream));
+    launch_read_constraints(ctx->tb_table.as<DeviceTypeBatch>(), ctx->tdesc_table.as<TransposeDesc>(), ctx->inverse_table.as<DeviceSlot>(), ctx->read_requests.as<ReadRequest>(),
+                            count, ctx->read_records.as<int32_t>(), ctx->stream);
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(records_out, ctx->read_records.ptr, n * 256, cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
     return BEPUCUDA_OK;
 }

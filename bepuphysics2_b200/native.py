@@ -57,6 +57,7 @@ class Timings(C.Structure):
         ("d2h_bytes", C.c_int64),
         ("device_batch_count", C.c_int32),
         ("fallback_level_count", C.c_int32),
+        ("graph_captures", C.c_int64),
     ]
 
     def as_dict(self):
@@ -114,7 +115,7 @@ C_ABI_SYMBOLS = [
     "bepucuda_shard_export", "bepucuda_shard_import", "bepucuda_shard_set_global", "bepucuda_shard_set_body_masks", "bepucuda_shard_import_contexts",
     "bepucuda_shard_set_fallback_rank",
     "bepucuda_color_constraints", "bepucuda_color_hash", "bepucuda_set_body_shapes", "bepucuda_predict_bounding_boxes",
-    "bepucuda_set_body_accelerations", "bepucuda_set_point_gravity", "bepucuda_find_sleepable_islands",
+    "bepucuda_set_body_accelerations", "bepucuda_set_point_gravity", "bepucuda_find_sleepable_islands", "bepucuda_read_constraints",
 ]
 
 
@@ -181,6 +182,7 @@ def load_libraries():
     cuda.bepucuda_set_body_accelerations.argtypes = [vp, vp, i32]
     cuda.bepucuda_set_point_gravity.argtypes = [vp, i32, vp, f32]
     cuda.bepucuda_find_sleepable_islands.argtypes = [vp, vp, i32, vp, vp, vp, C.POINTER(i32), C.POINTER(i32)]
+    cuda.bepucuda_read_constraints.argtypes = [vp, i32, vp, vp]
 
     host.bepuhost_create.restype = vp
     host.bepuhost_create.argtypes = [i32, i32]
@@ -350,6 +352,13 @@ class Simulation:
                 out.append(TypeBatch(b, t, v, self.bundle_width))
         return out
 
+    def constraint_locations(self):
+        """Every location of the type batches, int32[n, 3] = (batch index, type id, index in the type batch), in type_batches() order: the
+        locations CudaTimestepper.read_constraints takes. Fallback holes are included (they read back as empty lanes)."""
+        parts = [np.stack([np.full(tb.constraint_count, tb.batch_index), np.full(tb.constraint_count, tb.type_id), np.arange(tb.constraint_count)], axis=1)
+                 for tb in self.type_batches()]
+        return np.concatenate(parts).astype(np.int32) if parts else np.zeros((0, 3), dtype=np.int32)
+
     @property
     def constrained_kinematics(self):
         n = self._host.bepuhost_constrained_kinematic_count(self._sim)
@@ -447,6 +456,20 @@ class CudaTimestepper:
         self._check(self._cuda.bepucuda_find_sleepable_islands(self._ctx, activities.ctypes.data, n, labels.ctypes.data, roots.ctypes.data, counts.ctypes.data,
                                                                C.byref(count), C.byref(rounds)))
         return labels[:n], roots[:count.value].copy(), counts[:count.value].copy(), rounds.value
+
+    def read_constraints(self, locations, out=None):
+        """bepucuda_read_constraints: int32[n, 64] records of the listed constraints from the device rows (include/bepucuda.h: type id, live,
+        body references, accumulated impulses, prestep). locations: int32[n, 3] (batch index, type id, index in the type batch) in the active set,
+        or int32[n, 4] with the set index first, the layout of bepucuda_constraint_location. out: a C-contiguous int32 array of at least n x 64
+        to write the records into (e.g. one kept registered across frames); a new array otherwise."""
+        loc = np.asarray(locations, dtype=np.int32)
+        if loc.ndim == 2 and loc.shape[1] == 3:
+            loc = np.concatenate([np.zeros((loc.shape[0], 1), dtype=np.int32), loc], axis=1)
+        loc = np.ascontiguousarray(loc.reshape(-1, 4))
+        records = np.zeros((max(loc.shape[0], 1), 64), dtype=np.int32) if out is None else out.reshape(-1, 64)
+        assert records.dtype == np.int32 and records.flags["C_CONTIGUOUS"] and records.shape[0] >= loc.shape[0]
+        self._check(self._cuda.bepucuda_read_constraints(self._ctx, loc.shape[0], loc.ctypes.data, records.ctypes.data))
+        return records[:loc.shape[0]]
 
     def register_host_buffers(self):
         """Page-locks the simulation's buffers (a C# host would register its BufferPool blocks once)."""

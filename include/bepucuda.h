@@ -86,6 +86,7 @@ typedef struct bepucuda_timings {
     int64_t d2h_bytes;              /* bytes copied device->host by the last downloads */
     int32_t device_batch_count;     /* synchronized batches + fallback dependency levels */
     int32_t fallback_level_count;   /* dependency levels the sequential fallback batch was split into */
+    int64_t graph_captures;         /* CUDA graphs this context has captured (BEPUCUDA_EXEC_GRAPH): one per stage program and launch context */
 } bepucuda_timings;
 
 /* Lifetime. Replaces: construction of Solver<TIntegrationCallbacks> in Simulation.Create (Simulation.cs:L135-141). */
@@ -205,6 +206,34 @@ int32_t bepucuda_download_bodies(bepucuda_ctx* ctx, void* body_dynamics_out, int
 int32_t bepucuda_download_impulses(bepucuda_ctx* ctx);
 /* Replaces: in-place prestep mutation by IncrementallyUpdateForSubstep (contact depths). Test/diagnostic use. */
 int32_t bepucuda_download_prestep(bepucuda_ctx* ctx, int32_t batch_index, int32_t type_batch_index, float* prestep_out);
+
+/* Read listed constraints straight from the device rows, without moving anything else: the state behind NarrowPhase.TryExtractSolverContactData
+ * (CollisionDetection/NarrowPhase.cs:L136-145) and Solver.EnumerateAccumulatedImpulses / GetAccumulatedImpulseMagnitude[Squared]
+ * (Solver.cs:L1535-1574) on the resident path, where the host's TypeBatch.AccumulatedImpulses and PrestepData go stale after the first frame.
+ *   bepucuda_constraint_location: Solver.HandleToConstraint[handle] (ConstraintLocation.cs). set_index 0 is the active set, the only one the device
+ *   holds; type_id selects the type batch of that id in batch batch_index.
+ *   records_out: count records of 64 int32 (256 B), in the order of `locations`; duplicates are allowed.
+ *     word 0      type id
+ *     word 1      1 = a live constraint, 0 = an empty lane (a hole of the sequential fallback batch); then words 2-63 are 0
+ *     words 2-5   the body references as TypeBatch.BodyReferences holds them: active-set index, bit 30 for a kinematic body, -1 for a slot the type
+ *                 does not have
+ *     words 6-17  accumulated impulses (float bits) in the row order of <Type>AccumulatedImpulses, EnumerateAccumulatedImpulses' order; then 0
+ *     words 18-52 prestep (float bits) in the row order of <Type>PrestepData; then 0
+ *     words 53-63 0
+ * The rows are the device's as of the later of the last bepucuda_end_constraints and the last bepucuda_solve / bepucuda_profile_stages: for contacts
+ * the impulses after redistribution and solve and the depths the incremental update left, what the reference's TypeBatch holds after Solver.Solve.
+ * Rows uploaded since then (bepucuda_update_type_batch, bepucuda_update_contacts) are pending and not visible before the next solve.
+ * Locations are resolved against the type batches of the last bepucuda_end_constraints. Read after the solve and before the host changes its
+ * constraint set: once collision detection has added or removed constraints (which moves IndexInTypeBatch), an index still in range names the
+ * device row of another constraint until the next describe.
+ * Writes no device state and no host memory but records_out, leaves the captured graph in place, and blocks until the records are written.
+ * BEPUCUDA_ERR_BAD_STATE before the first bepucuda_end_constraints and in peer mode (a rank holds its constraints compacted, so host locations do not
+ * address them). BEPUCUDA_ERR_INVALID_ARGUMENT for a NULL pointer with count > 0, set_index != 0, a batch out of range, a type id without a type batch
+ * in that batch, or an index at or beyond its ConstraintCount; all are checked before any device work and nothing is written. count == 0 is OK. */
+typedef struct bepucuda_constraint_location {
+    int32_t set_index, batch_index, type_id, index_in_type_batch;
+} bepucuda_constraint_location;
+int32_t bepucuda_read_constraints(bepucuda_ctx* ctx, int32_t count, const bepucuda_constraint_location* locations, int32_t* records_out);
 
 int32_t bepucuda_get_timings(bepucuda_ctx* ctx, bepucuda_timings* out);
 

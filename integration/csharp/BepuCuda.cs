@@ -23,6 +23,7 @@ namespace BepuCuda
         public float SolveMs, UploadMs, DownloadMs;
         public long ConstraintCount, ConstraintIterations, StageCount, KernelLaunches, AlgorithmicBytes, H2DBytes, D2HBytes;
         public int DeviceBatchCount, FallbackLevelCount;
+        public long GraphCaptures;
     }
 
     [StructLayout(LayoutKind.Sequential)]
@@ -32,6 +33,11 @@ namespace BepuCuda
         public fixed long Launches[8];
         public fixed long AlgorithmicBytes[8];
     }
+
+    /// <summary>bepucuda_constraint_location: Solver.HandleToConstraint[handle] (ConstraintLocation.cs); SetIndex 0 is the active set. Named apart
+    /// from BepuPhysics.ConstraintLocation so that code importing both namespaces still compiles.</summary>
+    [StructLayout(LayoutKind.Sequential)]
+    public struct CudaConstraintLocation { public int SetIndex, BatchIndex, TypeId, IndexInTypeBatch; }
 
     public static unsafe class Native
     {
@@ -62,6 +68,8 @@ namespace BepuCuda
         [DllImport(Lib)] public static extern int bepucuda_download_bodies(IntPtr ctx, void* bodyDynamicsOut, int bodyCount);
         [DllImport(Lib)] public static extern int bepucuda_download_impulses(IntPtr ctx);
         [DllImport(Lib)] public static extern int bepucuda_download_prestep(IntPtr ctx, int batchIndex, int typeBatchIndex, float* prestepOut);
+        /// <summary>Records of 64 ints (type id, live, body references, accumulated impulses, prestep) of the listed constraints, read from the device rows.</summary>
+        [DllImport(Lib)] public static extern int bepucuda_read_constraints(IntPtr ctx, int count, CudaConstraintLocation* locations, int* recordsOut);
         [DllImport(Lib)] public static extern int bepucuda_get_timings(IntPtr ctx, Timings* timings);
         [DllImport(Lib)] public static extern int bepucuda_event_record(IntPtr ctx, int slot);
         [DllImport(Lib)] public static extern int bepucuda_event_elapsed_ms(IntPtr ctx, int slotBegin, int slotEnd, float* ms);

@@ -141,6 +141,25 @@ public unsafe class CudaTimestepper<TCallbacks> : ITimestepper, IDisposable wher
         return true;
     }
 
+    /// <summary>The solver state of the listed constraints as the last device solve left it (bepucuda_read_constraints): 64 ints per handle, in
+    /// order, into records (length at least 64 * handles.Length). Words: 0 type id, 1 live, 2-5 body references, 6-17 accumulated impulses in
+    /// EnumerateAccumulatedImpulses' order, 18-52 prestep (float bits). The handles must belong to the active set. Call it after the frame's solve
+    /// and before the host changes the constraint set: the locations are resolved against the type batches the device was last described with, so
+    /// after collision detection has added or removed constraints an index still in range names another constraint.</summary>
+    public void ReadConstraints(Simulation simulation, ReadOnlySpan<ConstraintHandle> handles, Span<int> records)
+    {
+        if (records.Length < handles.Length * 64) throw new ArgumentException("records needs 64 ints per handle");
+        var locations = new CudaConstraintLocation[handles.Length];
+        for (int i = 0; i < handles.Length; ++i)
+        {
+            ref var l = ref simulation.Solver.HandleToConstraint[handles[i].Value];                                   // ConstraintLocation.cs
+            locations[i] = new CudaConstraintLocation { SetIndex = l.SetIndex, BatchIndex = l.BatchIndex, TypeId = l.TypeId, IndexInTypeBatch = l.IndexInTypeBatch };
+        }
+        fixed (CudaConstraintLocation* l = locations)
+        fixed (int* r = records)
+            Check(Native.bepucuda_read_constraints(ctx, handles.Length, l, r));
+    }
+
     // FNV-1a over everything bepucuda_end_constraints analyses: batch / type batch shape, every body reference, the constrained kinematics.
     // (~8 bytes per constraint body: a few hundred microseconds for 300 k contacts, against a graph re-capture per frame.)
     static ulong TopologySignature(Simulation simulation)
