@@ -41,14 +41,14 @@ def fresh_lane_cases():
     """(type id, states, velocities, impulses, prestep) per sample: 32 samples per type, prestep rows from the scene generators, random body
     states, velocities and impulses, plus degenerate lanes (zero velocities and impulses, a kinematic partner, identity orientations)."""
     from oracle import binding as ob
-    from tests.test_device_source_on_host import _prestep_samples, _random_states
+    from tests.device_source import prestep_samples, random_states
 
-    samples = _prestep_samples()
+    samples = prestep_samples()
     rng = np.random.default_rng(991)
     for type_id in sorted(samples):
         bodies, _, impulse_rows = ob.type_info(type_id)
         for n, prestep in enumerate(samples[type_id]):
-            states = _random_states(rng, bodies)
+            states = random_states(rng, bodies)
             vel = rng.normal(0, 1.5, (bodies, 6)).astype(np.float32)
             imp = np.abs(rng.normal(0, 0.2, impulse_rows)).astype(np.float32)
             if n % 8 == 5:

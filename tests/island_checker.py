@@ -1,15 +1,13 @@
 """Loader of tests/islands/collect_island.cpp, the CPU restatement of IslandSleeper.CollectIsland that bepucuda_find_sleepable_islands is held to.
-Compiled with g++ on first use into the temporary directory (keyed by the source's hash), so the tree stays as it is."""
+Compiled with g++ on first use into the temporary directory (tests/harness.py), so the tree stays as it is."""
 import ctypes as C
-import hashlib
 import os
-import subprocess
-import tempfile
 
 import numpy as np
 
+from tests import harness
+
 SRC = os.path.join(os.path.dirname(os.path.abspath(__file__)), "islands", "collect_island.cpp")
-_LIB = None
 
 
 class IslandTypeBatch(C.Structure):
@@ -17,18 +15,9 @@ class IslandTypeBatch(C.Structure):
 
 
 def load():
-    global _LIB
-    if _LIB is None:
-        with open(SRC, "rb") as f:
-            digest = hashlib.sha256(f.read()).hexdigest()[:16]
-        lib = os.path.join(tempfile.gettempdir(), "collect_island_%d_%s.so" % (os.getuid(), digest))
-        if not os.path.exists(lib):
-            partial = lib + ".%d" % os.getpid()
-            subprocess.check_call(["/usr/bin/g++", "-O2", "-std=c++17", "-Wall", "-shared", "-fPIC", "-o", partial, SRC])
-            os.replace(partial, lib)
-        _LIB = C.CDLL(lib)
-        _LIB.collect_sleepable_islands.argtypes = [C.POINTER(IslandTypeBatch), C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
-    return _LIB
+    lib = harness.load("collect_island", [SRC], ["-O2", "-std=c++17", "-Wall", "-shared", "-fPIC"])
+    lib.collect_sleepable_islands.argtypes = [C.POINTER(IslandTypeBatch), C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    return lib
 
 
 def find_sleepable_islands(type_batches, body_count, bundle_width, sleep_candidates):

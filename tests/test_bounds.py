@@ -14,13 +14,10 @@ import pytest
 import bepuphysics2_b200 as bp
 from bepuphysics2_b200 import native, scenes
 from oracle import binding as ob
+from tests import util
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 DT = 1.0 / 60.0
-
-
-def _bits(a):
-    return np.ascontiguousarray(a, dtype=np.float32).view(np.uint32)
 
 
 def _identity_callback():
@@ -59,7 +56,7 @@ def test_oracle_reproduces_the_reference_bounds_vectors_bit_for_bit(libs):
         inputs = [golden["set%d_%s" % (k, name)] for name in ("types", "dims", "margins", "allow", "q", "pos", "lin", "ang")]
         got = _oracle_on_inputs(*inputs, float(golden["set%d_dt" % k]))
         assert (got[:, 7] == 1.0).all()
-        assert np.array_equal(_bits(got[:, :7]), _bits(golden["set%d_out" % k])), "set %d" % k
+        assert np.array_equal(util.bits(got[:, :7]), util.bits(golden["set%d_out" % k])), "set %d" % k
         assert sorted(set(inputs[0].tolist())) == [0, 1, 2, 4]
     # the vectors reach the clamps: some margins sit on their bounds, some expansions are cut by the margin
     out, margins = golden["set0_out"], golden["set0_margins"]
@@ -73,7 +70,7 @@ def test_oracle_matches_the_transpiled_reference_on_fresh_inputs(libs):
 
     want = np.load(os.path.join(ROOT, "tests", "golden", "reference_fresh_vectors.npz"))["bounds_out"]
     got = _oracle_on_inputs(*gen.fresh_bounds_inputs(), gen.DT_BOUNDS)
-    assert np.array_equal(_bits(got[:, :7]), _bits(want))
+    assert np.array_equal(util.bits(got[:, :7]), util.bits(want))
 
 
 def test_known_answers_and_sleep_candidacy(libs):
@@ -141,7 +138,7 @@ def test_device_bounds_are_bit_identical_to_the_oracle(libs):
             for frame in range(3):  # the counters evolve over several frames
                 want = ob.predict_bounding_boxes(bodies, shapes, want_activities, DT, integ)
                 got = ts.predict_bounding_boxes(DT, activities)
-                assert np.array_equal(_bits(got), _bits(want)), "frame %d" % frame
+                assert np.array_equal(util.bits(got), util.bits(want)), "frame %d" % frame
                 assert np.array_equal(activities.view(np.uint8), want_activities.view(np.uint8))
             assert (got[:, 7] == np.isin(shapes["type"], [0, 1, 2, 4])).all()
             with pytest.raises(bp.BepuCudaError):
@@ -154,8 +151,6 @@ def test_device_bounds_are_bit_identical_to_the_oracle(libs):
 @pytest.mark.gpu
 def test_device_bounds_on_the_state_a_solve_leaves_resident(libs):
     """DefaultTimestepper order: ... Solve | next frame: PredictBoundingBoxes. The bounds come from the bodies the solve left on the device."""
-    from tests import util
-
     scene = scenes.shape_pile(3000, seed=4)
     a = util.make_sim(scene, substeps=2, velocity_iterations=2)
     b = util.make_sim(scene, substeps=2, velocity_iterations=2)
@@ -172,5 +167,5 @@ def test_device_bounds_on_the_state_a_solve_leaves_resident(libs):
         got = ts.predict_bounding_boxes(DT, activities)
     finally:
         ts.close()
-    assert np.array_equal(_bits(got), _bits(want))
+    assert np.array_equal(util.bits(got), util.bits(want))
     assert np.array_equal(activities.view(np.uint8), want_activities.view(np.uint8))

@@ -1,73 +1,34 @@
 """bepucuda_read_constraints: records of listed constraints read straight from the device rows (include/bepucuda.h), the state behind
 NarrowPhase.TryExtractSolverContactData and Solver.EnumerateAccumulatedImpulses on the resident path.
-CPU part: the planner's inverse slot map (csrc/bepu_topology.cpp) against its forward map, through the topology shim.
+CPU part: the planner's inverse slot map (csrc/bepu_topology.cpp) against its forward map, through the topology shim (tests/planner.py).
 GPU part: after resident frames with device-side redistribution, every record equals the host buffers after the full downloads, word for word; subsets
 come back in the order given; the call changes nothing; and each error leaves the output untouched."""
-import ctypes as C
-import os
-import subprocess
-
 import numpy as np
 import pytest
 
 import bepuphysics2_b200 as bp
-from bepuphysics2_b200 import _build, scenes, sharding
+from bepuphysics2_b200 import scenes, sharding
 from bepuphysics2_b200.native import ERR_BAD_STATE, ERR_INVALID_ARGUMENT, EXEC_GRAPH, EXEC_STREAM
 from tests import util
-from tests.test_contact_update import _initial_features, _narrow_phase_like_update, _push_bodies
-from tests.test_islands import punch_fallback_holes
-from tests.test_topology import constraints_of, plan, sim_sources
+from tests.planner import constraints_of, inverse_of, plan, sim_sources
+from tests.resident import initial_features, narrow_phase_like_update, push_bodies
 
 DT = 1.0 / 60.0
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-TOPOLOGY = os.path.join(ROOT, "tests", "topology")
-CSRC = os.path.join(ROOT, "bepuphysics2_b200", "csrc")
 CONVEX, NONCONVEX = set(range(8)), {8, 9, 10, 15, 16, 17}
 
 
 # ---- CPU: the inverse slot map -------------------------------------------------------------------------------------------------------------
-@pytest.fixture(scope="module")
-def inverse_shim():
-    lib = os.path.join(TOPOLOGY, "libreadback_shim.so")
-    srcs = [os.path.join(TOPOLOGY, "topology_shim.cpp"), os.path.join(TOPOLOGY, "readback_shim.cpp"), os.path.join(CSRC, "bepu_topology.cpp")]
-    deps = srcs + [os.path.join(CSRC, f) for f in ("bepu_topology.h", "bepu_device_types.h", "bepu_layout_kernels.h", "bepu_joint_registry.inc")]
-    if not os.path.exists(lib) or any(os.path.getmtime(s) > os.path.getmtime(lib) for s in deps):
-        cuda_include = os.path.join(os.path.dirname(os.path.dirname(_build.NVCC)), "include")
-        subprocess.check_call(["/usr/bin/g++", "-O2", "-std=c++17", "-Wall", "-shared", "-fPIC", "-I", CSRC, "-I", cuda_include, "-o", lib] + srcs)
-    dll = C.CDLL(lib)
-    vp, i32 = C.c_void_p, C.c_int32
-    dll.topology_plan.restype = vp
-    dll.topology_plan.argtypes = [i32, vp, vp, i32, i32, i32, i32, i32]
-    dll.topology_plan_error.argtypes = [vp, C.c_char_p, i32]
-    for name in ("sizes", "tbs", "maps", "work", "batches", "source_live"):
-        getattr(dll, "topology_plan_" + name).argtypes = [vp, vp]
-    dll.topology_plan_free.argtypes = [vp]
-    dll.topology_plan_inverse_size.restype = C.c_int64
-    dll.topology_plan_inverse_size.argtypes = [vp]
-    dll.topology_plan_inverse.argtypes = [vp, vp, vp, vp]
-    return dll
-
-
-def inverse_of(dll, p):
-    n_sources = len(p.source_live)
-    source_tb = np.zeros(n_sources, dtype=np.int32)
-    offsets = np.zeros(n_sources, dtype=np.int64)
-    inverse = np.zeros((max(int(dll.topology_plan_inverse_size(p.handle)), 1), 2), dtype=np.int32)
-    dll.topology_plan_inverse(p.handle, source_tb.ctypes.data, offsets.ctypes.data, inverse.ctypes.data)
-    return source_tb, offsets, inverse[:dll.topology_plan_inverse_size(p.handle)]
-
-
 @pytest.mark.parametrize("case", ["mixed_w8", "fallback_stress_w4", "holes_w16"])
-def test_inverse_map_sends_every_fallback_constraint_to_its_slot_and_holes_nowhere(libs, inverse_shim, case):
+def test_inverse_map_sends_every_fallback_constraint_to_its_slot_and_holes_nowhere(libs, case):
     scene, W, threshold = {"mixed_w8": (lambda: scenes.merge(scenes.shape_pile(1200, seed=3, nonconvex_fraction=0.3), scenes.joint_zoo(400, per_type=8, seed=4)), 8, 6),
                            "fallback_stress_w4": (lambda: scenes.fallback_stress(3000, hubs=6, seed=7), 4, 4),
                            "holes_w16": (lambda: scenes.merge(scenes.shape_pile(800, seed=5), scenes.joint_zoo(300, per_type=6, seed=6)), 16, 3)}[case]
     sim = util.make_sim(scene(), bundle_width=W, fallback_batch_threshold=threshold)
-    holes = punch_fallback_holes(sim) if case == "holes_w16" else 0
+    holes = util.punch_fallback_holes(sim) if case == "holes_w16" else 0
     sources = sim_sources(sim)
-    p = plan(inverse_shim, sources, W, threshold, sim.batch_count, sim.body_count)
+    p = plan(sources, W, threshold, sim.batch_count, sim.body_count)
     assert p.fallback_levels > 0
-    source_tb, offsets, inverse = inverse_of(inverse_shim, p)
+    source_tb, offsets, inverse = inverse_of(p)
     # the forward maps: (device type batch, slot) -> source constraint
     forward = {}
     for tb in range(len(p.tbs)):
@@ -119,17 +80,17 @@ def resident(scene, frames=3, bundle_width=8, fallback_batch_threshold=64, mode=
     incremental depth updates have moved the device rows away from the host's. Returns (simulation, timestepper)."""
     sim = util.make_sim(scene, bundle_width=bundle_width, fallback_batch_threshold=fallback_batch_threshold, substeps=substeps, velocity_iterations=velocity_iterations)
     if holes:
-        assert punch_fallback_holes(sim) > 0
+        assert util.punch_fallback_holes(sim) > 0
     rng = np.random.default_rng(seed)
     ts = bp.CudaTimestepper(sim, strict_fp=strict, execution_mode=mode)
     ts.register_host_buffers()
     ts.describe()
-    features = _initial_features(sim, rng)
+    features = initial_features(sim, rng)
     ts.set_contact_features(features)
     for frame in range(frames):
         if frame > 0:
-            new = _narrow_phase_like_update(sim, features, rng)
-            _push_bodies(sim, frame)
+            new = narrow_phase_like_update(sim, features, rng)
+            push_bodies(sim, frame)
             ts.upload_body_motion()
             ts.update_contacts(new)
             features.update(new)

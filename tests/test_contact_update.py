@@ -9,9 +9,9 @@ import pytest
 
 import bepuphysics2_b200 as bp
 from bepuphysics2_b200 import scenes
-from bepuphysics2_b200.native import ERR_BAD_STATE, ERR_INVALID_ARGUMENT, EXEC_GRAPH, EXEC_STREAM, contact_count
+from bepuphysics2_b200.native import ERR_BAD_STATE, ERR_INVALID_ARGUMENT, EXEC_STREAM, contact_count
 from oracle import binding as ob
-from tests import util
+from tests import resident, util
 
 DT = 1.0 / 60.0
 
@@ -50,144 +50,6 @@ def _penetration_rows(type_id):
     return [2 + i for i in range(n)] if type_id < 8 else [3 * i + 2 for i in range(n)]
 
 
-def _initial_features(sim, rng):
-    return {(tb.batch_index, tb.type_batch_index): rng.integers(0, 1 << 20, size=(tb.constraint_count, contact_count(tb.type_id)), dtype=np.int32)
-            for tb in sim.type_batches() if contact_count(tb.type_id)}
-
-
-def _narrow_phase_like_update(sim, features, rng):
-    """What a frame of collision detection does to an unchanged topology: new depths, and some contacts replaced by new features. Touches the
-    contact type batches named in `features` only."""
-    new = {}
-    for tb in sim.type_batches():
-        key = (tb.batch_index, tb.type_batch_index)
-        if key not in features:
-            continue
-        ids = features[key].copy()
-        n = ids.shape[1]
-        change = rng.random(ids.shape) < 0.2
-        ids[change] = rng.integers(1 << 20, 1 << 21, size=int(change.sum()), dtype=np.int32)
-        swap = rng.random(ids.shape[0]) < 0.3  # the narrow phase often reports the same features in another order
-        if n > 1:
-            ids[swap] = ids[swap][:, ::-1]
-        new[key] = ids
-        # depth rows: convex prestep rows 4 i + 3; nonconvex: after MaterialProperties (4 rows) [+ OffsetB (3 rows) for two bodies], contact i = 7 rows
-        # (Offset xyz, Depth, Normal xyz) with the depth at + 3 (tests/golden/type_layouts.json)
-        base = 4 if tb.type_id <= 10 else 7
-        rows = [4 * i + 3 for i in range(n)] if tb.type_id <= 7 else [base + 7 * i + 3 for i in range(n)]
-        for r in rows:  # the narrow phase writes fresh depths every frame (whatever the solver's incremental updates left in the row)
-            tb.prestep[:, r, :] = rng.uniform(-0.02, 0.05, size=tb.prestep[:, r, :].shape).astype(np.float32)
-    return new
-
-
-def _type_batch(sim, key):
-    return next(tb for tb in sim.type_batches() if (tb.batch_index, tb.type_batch_index) == key)
-
-
-def _update_type_batch(ts, tb):
-    """bepucuda_update_type_batch of one type batch from the simulation's own buffers (what bepuhost_cuda_refresh does for every type batch)."""
-    ts._check(ts._cuda.bepucuda_update_type_batch(ts._ctx, tb.batch_index, tb.type_batch_index, tb.prestep.ctypes.data, tb.accumulated_impulses.ctypes.data))
-
-
-KICK = 0.01  # m/s: far above the last bit of any velocity, small enough not to stress the joints
-
-
-def _push_bodies(sim, frame):
-    """What a host does to the bodies between frames (a character controller, a user drag): here a fifth of the bodies gets a small kick of
-    linear velocity. Applied to both twins, so a motion upload that did nothing would show."""
-    sim.bodies[frame % 5::5, 9] += np.float32(KICK)
-
-
-def _take_state(host, source, features, feat_h):
-    """The host twin takes the state of `source` (a simulation whose device run was downloaded): bodies, prestep, accumulated impulses, and the
-    feature ids those impulses belong to."""
-    host.bodies[:] = source.bodies
-    for th, src in zip(host.type_batches(), source.type_batches()):
-        th.prestep[:] = src.prestep
-        th.accumulated_impulses[:] = src.accumulated_impulses
-    feat_h.clear()
-    feat_h.update({key: ids.copy() for key, ids in features.items()})
-
-
-def _resident_frames(scene, frames=4, bundle_width=8, fallback_batch_threshold=64, mode=EXEC_GRAPH, strict=True, register=True, pool=False, named=None,
-                     joint_reset=False, seed=77, take_state=None, push=True):
-    """Frames of f2 through the device path next to the oracle's host path on a twin simulation. Host: narrow-phase-like update, RedistributeImpulses
-    (ob.update_contact_impulses), solve. Device: upload_body_motion + update_contacts (or update_contacts_from_pool, the sequence bench.py times),
-    solve_device_only, download_body_motion; the motion halves must agree bit for bit after every frame (strict build). One download_bodies,
-    download_impulses and download_prestep at the end. named(frame, keys): the contact type batches a frame updates (all by default); the others
-    keep what the last solve left on both sides. joint_reset: every frame also zeroes the accumulated impulses of one joint type batch on both
-    twins (a re-created joint) and sends it through bepucuda_update_type_batch. push: before every update both twins' bodies get the same velocity
-    kick (_push_bodies). take_state = (frame, source simulation, its feature ids): after that frame the host twin takes that state (_take_state), so
-    that the frame after it can be held to one-frame tolerances in the fast build. Returns (host, dev, device timings, replaced contact count,
-    the device's feature ids)."""
-    kw = dict(bundle_width=bundle_width, fallback_batch_threshold=fallback_batch_threshold, substeps=3, velocity_iterations=2)
-    host, dev = util.make_sim(scene, **kw), util.make_sim(scene, **kw)
-    rng_h, rng_d = np.random.default_rng(seed), np.random.default_rng(seed)
-    ts = bp.CudaTimestepper(dev, strict_fp=strict, execution_mode=mode)
-    try:
-        if register:
-            ts.register_host_buffers()
-        ts.describe()
-        feat_h, feat_d = _initial_features(host, rng_h), _initial_features(dev, rng_d)
-        if pool:
-            pool_d, views = ts.contact_feature_pool()
-            ts.register_array(pool_d)
-            assert sorted(views) == sorted(feat_d)
-            for key, ids in feat_d.items():
-                views[key][:] = ids
-            ts.set_contact_feature_pool(pool_d)
-        else:
-            ts.set_contact_features(feat_d)
-        joints = [(tb.batch_index, tb.type_batch_index) for tb in host.type_batches() if not contact_count(tb.type_id)]
-        assert joints or not joint_reset
-        replaced = 0
-        for frame in range(frames):
-            if frame > 0:
-                keys = sorted(feat_h) if named is None else named(frame, sorted(feat_h))
-                new_h = _narrow_phase_like_update(host, {k: feat_h[k] for k in keys}, rng_h)
-                new_d = _narrow_phase_like_update(dev, {k: feat_d[k] for k in keys}, rng_d)
-                if pool:
-                    for key, ids in new_d.items():
-                        views[key][:] = ids
-                    new_h = {key: views[key] for key in new_h}  # the host redistributes through the pool's views
-                for tb in host.type_batches():
-                    key = (tb.batch_index, tb.type_batch_index)
-                    if key in new_h:
-                        ob.update_contact_impulses(tb, feat_h[key], new_h[key])
-                        replaced += int((new_h[key] >= (1 << 20)).sum())
-                feat_h.update({key: ids.copy() for key, ids in new_h.items()})
-                if push:
-                    _push_bodies(host, frame)
-                    _push_bodies(dev, frame)
-                if pool:
-                    ts.update_contacts_from_pool(pool_d)
-                else:
-                    ts.upload_body_motion()
-                    ts.update_contacts(new_d)
-                feat_d.update(new_d)
-                if joint_reset:
-                    key = joints[frame % len(joints)]
-                    _type_batch(host, key).accumulated_impulses[:] = 0.0
-                    tb = _type_batch(dev, key)
-                    tb.accumulated_impulses[:] = 0.0
-                    _update_type_batch(ts, tb)
-            ob.solve(host, DT)
-            ts.solve_device_only(DT)
-            ts.download_body_motion()
-            t = ts.timings()
-            assert t.d2h_bytes == dev.body_count * 64
-            assert np.array_equal(host.bodies[:, util.MOTION].view(np.uint32), dev.bodies[:, util.MOTION].view(np.uint32)) or not strict, "frame %d" % frame
-            if take_state is not None and frame == take_state[0]:
-                _take_state(host, take_state[1], take_state[2], feat_h)
-        ts.download_bodies()  # the motion-only download leaves the host's world-inertia half untouched: fetch it once for the full comparison
-        ts.download_impulses()
-        ts.download_prestep()
-        timings = ts.timings()
-    finally:
-        ts.close()
-    return host, dev, timings, replaced, feat_d
-
-
 def _pile(nonconvex=0.0):
     return scenes.shape_pile(3000, seed=31, nonconvex_fraction=nonconvex)
 
@@ -196,7 +58,7 @@ def _mixed():
     return scenes.merge(scenes.shape_pile(1500, seed=41, nonconvex_fraction=0.3), scenes.joint_zoo(600, per_type=20, seed=42), scenes.ragdolls(20, seed=43))
 
 
-# scene, keyword arguments of _resident_frames
+# scene, keyword arguments of resident.resident_frames
 RESIDENT_CASES = {
     "pile": (lambda: _pile(0.0), {}),
     "pile_nonconvex": (lambda: _pile(0.5), {}),
@@ -221,7 +83,7 @@ def test_resident_impulses_with_device_side_redistribution_bit_exact(libs, case)
     batches (slot map), joints solved next to the contacts (their impulses stay resident and warm-start the next frame as on the host), both
     execution modes, both upload routes (mapped host buffers and cudaMemcpy2DAsync through the staging image) and the feature-pool walker."""
     make, kw = RESIDENT_CASES[case]
-    host, dev, timings, replaced, _ = _resident_frames(make(), **kw)
+    host, dev, timings, replaced, _ = resident.resident_frames(make(), **kw)
     util.compare(util.snapshot(host), util.snapshot(dev), exact=True)
     contacts = sum(tb.constraint_count * contact_count(tb.type_id) for tb in host.type_batches())
     assert replaced > 0.2 * contacts  # the test really replaced contacts
@@ -242,7 +104,7 @@ def test_partial_frames_keep_the_device_rows_of_type_batches_not_sent(libs, join
     """Frames that name only every other contact type batch (alternating): the others keep on the device the depths and impulses the last solve
     left, as the host does. With joint_reset one joint type batch per frame also goes up through bepucuda_update_type_batch with zeroed impulses,
     and only that one: the other joints keep warm-starting from their resident impulses."""
-    host, dev, _, _, _ = _resident_frames(_mixed(), frames=5, named=_every_other, joint_reset=joint_reset)
+    host, dev, _, _, _ = resident.resident_frames(_mixed(), frames=5, named=_every_other, joint_reset=joint_reset)
     util.compare(util.snapshot(host), util.snapshot(dev), exact=True)
 
 
@@ -360,17 +222,17 @@ def test_topology_change_after_resident_frames(libs):
                     for type_id, handles, prestep in extra["constraints"]:
                         sim.add_constraints(type_id, handles + base, prestep)
             ts.describe()
-            feat_h, feat_d = _initial_features(host, rng_h), _initial_features(dev, rng_d)
+            feat_h, feat_d = resident.initial_features(host, rng_h), resident.initial_features(dev, rng_d)
             ts.set_contact_features(feat_d)
             for frame in range(3):
                 if frame > 0:
-                    new_h = _narrow_phase_like_update(host, feat_h, rng_h)
+                    new_h = resident.narrow_phase_like_update(host, feat_h, rng_h)
                     for tb in host.type_batches():
                         key = (tb.batch_index, tb.type_batch_index)
                         if key in new_h:
                             ob.update_contact_impulses(tb, feat_h[key], new_h[key])
                     feat_h = new_h
-                    feat_d = _narrow_phase_like_update(dev, feat_d, rng_d)
+                    feat_d = resident.narrow_phase_like_update(dev, feat_d, rng_d)
                     ts.upload_body_motion()
                     ts.update_contacts(feat_d)
                 ob.solve(host, DT)
@@ -400,7 +262,7 @@ def test_feature_ids_sent_again_every_frame_hold_no_host_memory(libs):
     ts = bp.CudaTimestepper(dev, strict_fp=True)
     try:
         ts.describe()
-        feat_h, feat_d = _initial_features(host, rng_h), _initial_features(dev, rng_d)
+        feat_h, feat_d = resident.initial_features(host, rng_h), resident.initial_features(dev, rng_d)
         ts.set_contact_features(feat_d)
         ob.solve(host, DT)
         ts.solve_device_only(DT)  # resident impulses that belong to feat_d
@@ -415,13 +277,13 @@ def test_feature_ids_sent_again_every_frame_hold_no_host_memory(libs):
         ts.synchronize()
         grown = _resident_bytes() - before
         assert grown < 32 << 20, "resident memory grew by %d MB while %d MB of feature ids were sent" % (grown >> 20, (calls * per_call) >> 20)
-        new_h = _narrow_phase_like_update(host, feat_h, rng_h)
+        new_h = resident.narrow_phase_like_update(host, feat_h, rng_h)
         for tb in host.type_batches():
             key = (tb.batch_index, tb.type_batch_index)
             if key in new_h:
                 ob.update_contact_impulses(tb, feat_h[key], new_h[key])
         ts.upload_body_motion()
-        ts.update_contacts(_narrow_phase_like_update(dev, feat_d, rng_d))
+        ts.update_contacts(resident.narrow_phase_like_update(dev, feat_d, rng_d))
         ob.solve(host, DT)
         ts.solve_device_only(DT)
         ts.download_bodies()
@@ -442,7 +304,7 @@ def test_update_contacts_state_errors(libs):
     ts = bp.CudaTimestepper(dev, strict_fp=True)
     try:
         ts.describe()
-        feats = _initial_features(dev, rng)
+        feats = resident.initial_features(dev, rng)
         key = sorted(feats)[0]
         with pytest.raises(bp.BepuCudaError) as e:
             ts.update_contacts({key: feats[key]})
@@ -465,7 +327,7 @@ def test_update_contacts_state_errors(libs):
         assert e.value.code == ERR_BAD_STATE
         for tb in dev.type_batches():  # the host takes every contact type batch back, with its own impulses (the ones the last solve left)
             if contact_count(tb.type_id):
-                _update_type_batch(ts, tb)
+                resident.update_type_batch(ts, tb)
         ts.solve_device_only(DT)
         ob.solve(host, DT)  # no redistribution on the host either
         ts.download_bodies()
@@ -507,9 +369,9 @@ def test_fast_build_resident_frames_with_joints_deterministic_and_within_toleran
     instead of kept. No velocity kicks here (the strict cases cover the motion upload): the bounds are for the solver's rounding, and from the
     settled third frame single joint type batches already reach 2e-3 relative RMS on their own (measured on an H100); a rewound frame is off
     by 0.4 relative RMS and 2.8 in a body velocity."""
-    runs = [_resident_frames(_mixed(), strict=False) for _ in range(2)]
+    runs = [resident.resident_frames(_mixed(), strict=False) for _ in range(2)]
     a, b = (util.snapshot(run[1]) for run in runs)
     util.compare(a, b, exact=True)
-    _, source, _, _, features = _resident_frames(_mixed(), frames=3, strict=False, push=False)
-    host, dev, _, _, _ = _resident_frames(_mixed(), frames=4, strict=False, take_state=(2, source, features), push=False)
+    _, source, _, _, features = resident.resident_frames(_mixed(), frames=3, strict=False, push=False)
+    host, dev, _, _, _ = resident.resident_frames(_mixed(), frames=4, strict=False, take_state=(2, source, features), push=False)
     _within_one_frame_tolerances(util.snapshot(host), util.snapshot(dev))

@@ -7,76 +7,19 @@ The GPU parity tests remain the check of the binary that ships (kernels, gather/
 math be changed and re-verified on a machine without a GPU. TEST INFRASTRUCTURE: the product never loads either library."""
 import ctypes as C
 import os
-import subprocess
 
 import numpy as np
-import pytest
 
-from bepuphysics2_b200 import scenes
 from oracle import binding as ob
-from tests import util
+from tests import device_source, util
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-HERE = os.path.join(ROOT, "tests", "device_on_host")
-CSRC = os.path.join(ROOT, "bepuphysics2_b200", "csrc")
-LANES = 32
 DT = 1.0 / 240.0  # a substep of the 8 x 2 configuration at 1/30 s
 
 
-def compile_device_on_host(lib, optimisation=("-O2",)):
-    """The build recipe of the harness: g++ with the arithmetic of the strict build; `optimisation` replaces -O2 (the coverage build)."""
-    src = os.path.join(HERE, "device_on_host.cpp")
-    subprocess.check_call(["/usr/bin/g++"] + list(optimisation) + ["-std=c++17", "-ffp-contract=off", "-fno-fast-math", "-march=x86-64-v3", "-Wall", "-Wno-unused-function", "-Wno-unknown-pragmas", "-pthread",
-                                                                   "-I", os.path.join(HERE, "stubs"), "-I", HERE, "-I", CSRC, "-shared", "-fPIC", "-o", lib, src])
-
-
-@pytest.fixture(scope="module")
-def device_on_host():
-    lib = os.path.join(HERE, "libdevice_on_host.so")
-    srcs = [os.path.join(HERE, "device_on_host.cpp"), os.path.join(HERE, "stubs", "cuda_runtime.h")] + [os.path.join(CSRC, f) for f in ("bepu_device_math.cuh", "bepu_contacts.cuh", "bepu_joints.cuh", "bepu_joints_more.cuh", "bepu_integration.cuh", "bepu_bounds_math.cuh", "bepu_redistribute.cuh")]
-    if not os.path.exists(lib) or any(os.path.getmtime(s) > os.path.getmtime(lib) for s in srcs):
-        compile_device_on_host(lib)
-    dev = C.CDLL(lib)
-    fp = C.POINTER(C.c_float)
-    dev.device_on_host_eval_lane.argtypes = [C.c_int32, C.c_int32, fp, C.c_float, fp, fp, fp]
-    dev.device_on_host_type_info.argtypes = [C.c_int32] + [C.POINTER(C.c_int32)] * 4
-    orc = ob.load()
-    orc.oracle_eval_lane.argtypes = [C.c_int32, C.c_int32, fp, C.c_float, fp, fp, fp, C.c_int32]
-    dev.device_on_host_eval_integration.argtypes = [C.c_int32, fp, fp]
-    orc.oracle_eval_integration.argtypes = [C.c_int32, fp, fp]
-    return dev, orc
-
-
-def _ptr(a):
-    return a.ctypes.data_as(C.POINTER(C.c_float))
-
-
-def _random_states(rng, bodies):
-    """Per body: position, unit orientation, a symmetric positive definite world inverse inertia, inverse mass."""
-    out = np.zeros((bodies, 14), dtype=np.float32)
-    out[:, 0:3] = rng.normal(0, 2, (bodies, 3))
-    q = rng.normal(0, 1, (bodies, 4))
-    out[:, 3:7] = q / np.linalg.norm(q, axis=1, keepdims=True)
-    for b in range(bodies):
-        r = np.linalg.qr(rng.normal(0, 1, (3, 3)))[0]
-        m = r @ np.diag(rng.uniform(0.5, 4.0, 3)) @ r.T
-        out[b, 7:13] = (m[0, 0], m[1, 0], m[1, 1], m[2, 0], m[2, 1], m[2, 2])
-    out[:, 13] = rng.uniform(0.3, 2.0, bodies)
-    return out
-
-
-def _prestep_samples():
-    """type id -> float32[samples, prestep rows] of valid prestep data, from the same generators the GPU tests and the bench use."""
-    samples = {}
-    for scene in (scenes.shape_pile(1500, seed=21, nonconvex_fraction=0.5), scenes.joint_zoo(600, per_type=24, seed=21), scenes.ragdolls(6, seed=21), scenes.ragdolls(6, seed=22, motor="servo")):
-        for type_id, _, prestep in scene["constraints"]:
-            samples.setdefault(int(type_id), []).append(np.asarray(prestep, dtype=np.float32)[:24])
-    return {k: np.concatenate(v)[:32] for k, v in samples.items()}
-
-
-def test_device_constraint_source_matches_the_oracle_bit_for_bit(libs, device_on_host):
-    dev, orc = device_on_host
-    samples = _prestep_samples()
+def test_device_constraint_source_matches_the_oracle_bit_for_bit(libs):
+    dev, orc = device_source.load()
+    samples = device_source.prestep_samples()
     supported = sorted(t for t in range(64) if ob.type_info(t) is not None)
     assert sorted(samples) == supported, "the scene generators cover every registered type"
     rng = np.random.default_rng(7)
@@ -88,21 +31,21 @@ def test_device_constraint_source_matches_the_oracle_bit_for_bit(libs, device_on
         assert (info[0].value, info[1].value, info[2].value) == (bodies, prestep_rows, impulse_rows)
         for prestep in samples[type_id]:
             assert prestep.shape == (prestep_rows,)
-            states = _random_states(rng, bodies)
+            states = device_source.random_states(rng, bodies)
             velocities = rng.normal(0, 1.5, (bodies, 6)).astype(np.float32)
             impulses = np.abs(rng.normal(0, 0.2, impulse_rows)).astype(np.float32)
             for stage in (0, 1, 2):
                 if stage == 2 and not info[3].value:
                     continue
                 # device layout: row r of the lane at [r * 32]; the oracle reads the same buffers with that row stride
-                p_dev = np.zeros(prestep_rows * LANES, dtype=np.float32)
-                p_dev[::LANES] = prestep
-                a_dev = np.zeros(impulse_rows * LANES, dtype=np.float32)
-                a_dev[::LANES] = impulses
+                p_dev = np.zeros(prestep_rows * device_source.LANES, dtype=np.float32)
+                p_dev[::device_source.LANES] = prestep
+                a_dev = np.zeros(impulse_rows * device_source.LANES, dtype=np.float32)
+                a_dev[::device_source.LANES] = impulses
                 v_dev = velocities.copy()
                 p_orc, a_orc, v_orc = p_dev.copy(), a_dev.copy(), v_dev.copy()
-                assert dev.device_on_host_eval_lane(type_id, stage, _ptr(states), DT, _ptr(p_dev), _ptr(a_dev), _ptr(v_dev)) == 0
-                assert orc.oracle_eval_lane(type_id, stage, _ptr(states), DT, _ptr(p_orc), _ptr(a_orc), _ptr(v_orc), LANES) == 0
+                assert dev.device_on_host_eval_lane(type_id, stage, util.float_ptr(states), DT, util.float_ptr(p_dev), util.float_ptr(a_dev), util.float_ptr(v_dev)) == 0
+                assert orc.oracle_eval_lane(type_id, stage, util.float_ptr(states), DT, util.float_ptr(p_orc), util.float_ptr(a_orc), util.float_ptr(v_orc), device_source.LANES) == 0
                 what = "type %d stage %d" % (type_id, stage)
                 assert np.isfinite(v_orc).all() and np.isfinite(a_orc).all(), what
                 assert np.array_equal(v_dev.view(np.uint32), v_orc.view(np.uint32)), what + ": velocities"
@@ -114,11 +57,11 @@ def test_device_constraint_source_matches_the_oracle_bit_for_bit(libs, device_on
     assert checked > 44 * 2 * 16
 
 
-def test_device_integration_source_matches_the_oracle_bit_for_bit(libs, device_on_host):
+def test_device_integration_source_matches_the_oracle_bit_for_bit(libs):
     """csrc/bepu_integration.cuh (orientation integration through the custom sin / cos, inertia rotation, both momentum-conserving angular
     updates, the velocity callback, the optional per-body acceleration and point-gravity terms) against the oracle's restatement of
     PoseIntegrator.cs:L146-253, DemoCallbacks.cs, PerBodyGravityDemo.cs and PlanetDemo.cs, function by function."""
-    dev, orc = device_on_host
+    dev, orc = device_source.load()
     rng = np.random.default_rng(11)
 
     def unit_q():
@@ -146,8 +89,8 @@ def test_device_integration_source_matches_the_oracle_bit_for_bit(libs, device_o
         for op, operands in cases.items():
             operands = np.ascontiguousarray(operands, dtype=np.float32)
             a, b = np.zeros(6, dtype=np.float32), np.zeros(6, dtype=np.float32)
-            assert dev.device_on_host_eval_integration(op, _ptr(operands), _ptr(a)) == 0
-            assert orc.oracle_eval_integration(op, _ptr(operands), _ptr(b)) == 0
+            assert dev.device_on_host_eval_integration(op, util.float_ptr(operands), util.float_ptr(a)) == 0
+            assert orc.oracle_eval_integration(op, util.float_ptr(operands), util.float_ptr(b)) == 0
             assert np.isfinite(b).all()
             assert np.array_equal(a.view(np.uint32), b.view(np.uint32)), "integration op %d, trial %d: %s vs %s" % (op, trial, a, b)
 
@@ -161,16 +104,16 @@ def test_device_integration_source_matches_the_oracle_bit_for_bit(libs, device_o
         operands[19] = rng.uniform(-100, 100)
         operands[20], operands[21] = (trial >> 1) & 1, 1 if trial % 4 != 1 else 0
         a, b = np.zeros(6, dtype=np.float32), np.zeros(6, dtype=np.float32)
-        assert dev.device_on_host_eval_integration(5, _ptr(operands), _ptr(a)) == 0
-        assert orc.oracle_eval_integration(5, _ptr(operands), _ptr(b)) == 0
+        assert dev.device_on_host_eval_integration(5, util.float_ptr(operands), util.float_ptr(a)) == 0
+        assert orc.oracle_eval_integration(5, util.float_ptr(operands), util.float_ptr(b)) == 0
         assert np.isfinite(b).all()
         assert np.array_equal(a.view(np.uint32), b.view(np.uint32)), "integration op 5, trial %d: %s -> %s vs %s" % (trial, operands, a, b)
 
 
-def test_bounds_source_reproduces_the_reference_vectors_bit_for_bit(device_on_host):
+def test_bounds_source_reproduces_the_reference_vectors_bit_for_bit():
     """csrc/bepu_bounds_math.cuh (the arithmetic of bepucuda_predict_bounding_boxes) compiled for the host against the known-answer vectors generated
     from the reference's own C# text (tests/golden/reference_bounds_vectors.npz): the CUDA source of f4 is pinned to the reference without a GPU."""
-    dev, _ = device_on_host
+    dev, _ = device_source.load()
     fp = C.POINTER(C.c_float)
     dev.device_on_host_convex_bounds.argtypes = [C.c_int32, fp, fp, C.c_int32, fp, fp, fp, fp, C.c_float, fp]
     golden = np.load(os.path.join(ROOT, "tests", "golden", "reference_bounds_vectors.npz"))
@@ -180,7 +123,7 @@ def test_bounds_source_reproduces_the_reference_vectors_bit_for_bit(device_on_ho
         dt, want = float(golden["set%d_dt" % k]), golden["set%d_out" % k]
         for i in range(types.shape[0]):
             out = np.zeros(7, dtype=np.float32)
-            assert dev.device_on_host_convex_bounds(int(types[i]), _ptr(dims[i]), _ptr(margins[i]), int(allow[i]), _ptr(q[i]), _ptr(pos[i]), _ptr(lin[i]), _ptr(ang[i]), dt, _ptr(out)) == 0
+            assert dev.device_on_host_convex_bounds(int(types[i]), util.float_ptr(dims[i]), util.float_ptr(margins[i]), int(allow[i]), util.float_ptr(q[i]), util.float_ptr(pos[i]), util.float_ptr(lin[i]), util.float_ptr(ang[i]), dt, util.float_ptr(out)) == 0
             assert np.array_equal(out.view(np.uint32), want[i].view(np.uint32)), "set %d sample %d (shape type %d)" % (k, i, types[i])
             checked += 1
     assert checked == 96
@@ -216,12 +159,12 @@ def _redistribute_float64(old_ids, old_imp, new_ids):
     return new, share, remainder
 
 
-def test_redistribution_source_matches_the_oracle_on_every_id_pattern(libs, device_on_host):
+def test_redistribution_source_matches_the_oracle_on_every_id_pattern(libs):
     """csrc/bepu_redistribute.cuh (the per-constraint body of redistribute_impulses_kernel) against oracle_update_contact_impulses bit for bit, for
     every id-equality pattern at n = 1-4 contacts (duplicates in old, in new and in both, nothing matched, all matched and permuted), with impulses
     of 0, subnormals, ordinary values and values near FLT_MAX (remainders that overflow to inf). Then against float64: a matched contact carries
     its old impulse exactly (0 included: it stays matched), an unmatched one the remainder / unmatched count to within fp32 rounding."""
-    dev, orc = device_on_host
+    dev, orc = device_source.load()
     i32p = C.POINTER(C.c_int32)
     for lib, name in ((dev, "device_on_host_update_contact_impulses"), (orc, "oracle_update_contact_impulses")):
         getattr(lib, name).argtypes = [C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]

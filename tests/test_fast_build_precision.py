@@ -13,7 +13,6 @@ measured FINDINGS, which are held to the typical-lane check and reported. DESIGN
 import ctypes as C
 import os
 import re
-import subprocess
 
 import numpy as np
 import pytest
@@ -21,9 +20,8 @@ import pytest
 from bepuphysics2_b200 import native, scenes
 from bepuphysics2_b200.native import EXEC_GRAPH
 from oracle import binding as ob
-from tests import test_topology as topo
-from tests import util
-from tests.test_deep_batches import DEEP_BUNDLES
+from tests import harness, planner, util
+from tests.planner import DEEP_BUNDLES
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 DRIVER = os.path.join(ROOT, "tests", "precision", "isolated_solve.cpp")
@@ -36,24 +34,24 @@ ALL_TYPES = CONTACT_TYPES | RAGDOLL_TYPES | set(scenes.JOINT_ZOO_TYPES)
 BODY_QUANTITIES = {"position": np.r_[4:7], "orientation": np.r_[0:4], "linear velocity": np.r_[8:11], "angular velocity": np.r_[12:15]}
 OFF_SIDE = 1e-3  # a lane error above this is on the other side of a clamp, cone or limit
 CENTER, STRENGTH = (1.0, -40.0, 2.0), 800.0
-shim = topo.shim
 
 
-def build_driver(directory):
-    """Compiles the driver with oracle/Makefile's CXXFLAGS and -Werror=float-conversion into `directory`; returns the loaded library."""
+def _makefile_flags():
     with open(os.path.join(ROOT, "oracle", "Makefile")) as f:
-        flags = re.search(r"^CXXFLAGS = (.*)$", f.read(), re.M).group(1).split()
-    lib = os.path.join(directory, "libisolated_solve.so")
-    subprocess.check_call(["/usr/bin/g++"] + flags + ["-Werror=float-conversion", "-I", os.path.join(ROOT, "oracle"), "-shared", "-o", lib, DRIVER])
-    dll = C.CDLL(lib)
+        return re.search(r"^CXXFLAGS = (.*)$", f.read(), re.M).group(1)
+
+
+def build_driver():
+    """The driver built with oracle/Makefile's CXXFLAGS and -Werror=float-conversion."""
+    dll = harness.load("isolated_solve", [DRIVER], _makefile_flags().split() + ["-Werror=float-conversion", "-shared"], [os.path.join(ROOT, "oracle")])
     dll.isolated_solve_f32.argtypes = [C.POINTER(ob.OracleScene), C.c_float]
     dll.isolated_solve_f64.argtypes = [C.POINTER(ob.OracleScene), C.c_float, C.c_void_p, C.c_void_p, C.c_void_p]
     return dll
 
 
 @pytest.fixture(scope="module")
-def driver(tmp_path_factory):
-    return build_driver(str(tmp_path_factory.mktemp("precision")))
+def driver():
+    return build_driver()
 
 
 # ---- scenes -----------------------------------------------------------------------------------------------------------------------------------
@@ -317,26 +315,26 @@ def test_double_driver_computes_in_double(cases):
 
 
 @pytest.mark.parametrize("name", sorted(CONFIGS))
-def test_configuration_reaches_its_stage_kernel(libs, shim, cases, name):
+def test_configuration_reaches_its_stage_kernel(libs, cases, name):
     """(a) the contact-only WarmStartFirst, integrated WarmStart and incremental update with bodies; (b) the full switch; (c) the deep kernels;
     (d) the kExt launches; (e) the full switch in angular modes 1 and 2."""
     case = cases[name][0]
     sim = case.sim
-    p = topo.plan(shim, topo.sim_sources(sim), sim.bundle_width, sim.fallback_batch_threshold, sim.batch_count, sim.body_count)
+    p = planner.plan(planner.sim_sources(sim), sim.bundle_width, sim.fallback_batch_threshold, sim.batch_count, sim.body_count)
     ops, _ = p.program(sim.velocity_iterations, len(sim.constrained_kinematics), True, False, sim.body_count)
     ops = ops[ops[:, 2] > 0]
-    kernel, flags = topo.resolve(shim, ops, bool(case.terms), case.mode, False).T
+    kernel, flags = planner.resolve(ops, bool(case.terms), case.mode, False).T
     stage = ops[:, 0]
-    constraint_stages = stage <= topo.SOLVE
+    constraint_stages = stage <= planner.SOLVE
     if name.startswith("a"):
-        assert (kernel[constraint_stages] == topo.KERNEL_CONTACTS).all()
-        for s in (topo.WS, topo.INCREMENTAL):
-            assert (stage == s).any() and (flags[stage == s] & topo.BODIES_INTEGRATED).all(), s
+        assert (kernel[constraint_stages] == planner.KERNEL_CONTACTS).all()
+        for s in (planner.WS, planner.INCREMENTAL):
+            assert (stage == s).any() and (flags[stage == s] & planner.BODIES_INTEGRATED).all(), s
     else:
-        want = topo.KERNEL_DEEP if name.startswith("c") else topo.KERNEL_FULL
+        want = planner.KERNEL_DEEP if name.startswith("c") else planner.KERNEL_FULL
         assert (kernel[constraint_stages] == want).all(), kernel.tolist()
-    integrating = (stage == topo.WS_FIRST) | (stage == topo.WS)
-    assert (((flags[integrating] & topo.EXT) != 0) == bool(case.terms)).all()
+    integrating = (stage == planner.WS_FIRST) | (stage == planner.WS)
+    assert (((flags[integrating] & planner.EXT) != 0) == bool(case.terms)).all()
 
 
 def test_the_check_fails_on_a_joint_tolerance_error_and_passes_one_ulp(cases):
@@ -361,22 +359,19 @@ def test_the_check_fails_on_a_joint_tolerance_error_and_passes_one_ulp(cases):
             assert [(r["type"], r["quantity"]) for r in compare_builds(l32, bad, l64) if not r[verdict]] == [key], verdict
 
 
-def contracted_driver(directory):
+def contracted_driver():
     """The driver built like build_driver but with -ffp-contract=fast: the same arithmetic with a*b+c fused where GCC chooses, IEEE square roots."""
-    with open(os.path.join(ROOT, "oracle", "Makefile")) as f:
-        flags = re.search(r"^CXXFLAGS = (.*)$", f.read(), re.M).group(1).replace("-ffp-contract=off", "-ffp-contract=fast").split()
-    lib = os.path.join(directory, "libisolated_solve_contracted.so")
-    subprocess.check_call(["/usr/bin/g++"] + flags + ["-I", os.path.join(ROOT, "oracle"), "-shared", "-o", lib, DRIVER])
-    dll = C.CDLL(lib)
+    flags = _makefile_flags().replace("-ffp-contract=off", "-ffp-contract=fast").split()
+    dll = harness.load("isolated_solve_contracted", [DRIVER], flags + ["-shared"], [os.path.join(ROOT, "oracle")])
     dll.isolated_solve_f32.argtypes = [C.POINTER(ob.OracleScene), C.c_float]
     return dll
 
 
-def test_a_build_that_only_contracts_differently_passes_the_typical_lane_check(cases, tmp_path_factory):
+def test_a_build_that_only_contracts_differently_passes_the_typical_lane_check(cases):
     """The same arithmetic with FMA contraction and IEEE square roots passes the typical-lane check on every configuration. It speaks to
     contraction only, not to the approximate square root. How many groups it fails under the issue's check is printed next to the count per
     configuration, for comparison with the fast build's FINDINGS; that count depends on the compiler's contraction choices and is not asserted."""
-    dll = contracted_driver(str(tmp_path_factory.mktemp("contracted")))
+    dll = contracted_driver()
     for name, (case, _, l32, l64) in cases.items():
         lc = case.lanes(case.f32(dll))
         assert any(not np.array_equal(lc[k], l32[k]) for k in l32), "the contracted build rounds differently"

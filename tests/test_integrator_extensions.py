@@ -17,17 +17,6 @@ DT = 1.0 / 60.0
 f32 = np.float32
 
 
-def _integrator(gravity=(0.0, -10.0, 0.0), damping=0.03, angular_mode=0, allow_substeps=0, kinematics=0):
-    d = native.IntegratorDesc.default()
-    for i in range(3):
-        d.gravity[i] = gravity[i]
-    d.linear_damping = d.angular_damping = damping
-    d.angular_integration_mode = angular_mode
-    d.allow_substeps_for_unconstrained = allow_substeps
-    d.integrate_velocity_for_kinematics = kinematics
-    return d
-
-
 def _accelerations(n, seed, scale=5.0):
     a = np.random.default_rng(seed).uniform(-scale, scale, size=(n, 8)).astype(np.float32)
     a[:, 3] = a[:, 7] = 0.0
@@ -50,7 +39,7 @@ def test_unconstrained_body_takes_a_times_dt(libs, allow_substeps):
     g = f32(-10.0)
     a = _accelerations(1, 1)
     sim = util.make_sim(_one_body((1, 2, 3), (0.5, -1.0, 2.0), (0.25, -0.5, 0.75)), substeps=substeps, velocity_iterations=1,
-                        integrator=_integrator(gravity=(0.0, -10.0, 0.0), damping=0.0, allow_substeps=allow_substeps))
+                        integrator=util.integrator(gravity=(0.0, -10.0, 0.0), linear_damping=0.0, angular_damping=0.0, allow_substeps_for_unconstrained=allow_substeps))
     v = sim.bodies[0, 8:11].copy()
     w = sim.bodies[0, 12:15].copy()
     p = sim.bodies[0, 4:7].copy()
@@ -69,7 +58,7 @@ def test_unconstrained_body_takes_a_times_dt(libs, allow_substeps):
 def test_point_gravity_one_step(libs):
     """PlanetDemo's callback for one step: v' = v - (dt * strength * offset) * (1 / max(1, |offset|^3))."""
     center, strength = np.array([0.5, -20.0, 3.0], dtype=f32), f32(1000.0)
-    sim = util.make_sim(_one_body((4, 7, -2), (0.0, 0.0, 0.0), (0.0, 0.0, 0.0)), integrator=_integrator(gravity=(0, 0, 0), damping=0.0))
+    sim = util.make_sim(_one_body((4, 7, -2), (0.0, 0.0, 0.0), (0.0, 0.0, 0.0)), integrator=util.integrator(gravity=(0, 0, 0), linear_damping=0.0, angular_damping=0.0))
     pos = sim.bodies[0, 4:7].copy()
     ob.solve(sim, DT, center=center, strength=strength)
     offset = pos - center
@@ -87,7 +76,7 @@ def _mixed_scene():
 @pytest.mark.parametrize("angular_mode", [0, 1, 2])
 def test_scalar_and_eight_wide_oracle_agree_with_both_terms(libs, angular_mode):
     scene = _mixed_scene()
-    integ = _integrator(angular_mode=angular_mode, kinematics=1)
+    integ = util.integrator(angular_integration_mode=angular_mode, integrate_velocity_for_kinematics=1)
     a, b = (util.make_sim(scene, substeps=3, velocity_iterations=2, integrator=integ) for _ in range(2))
     acc = _accelerations(a.body_count, 5)
     for _ in range(2):
@@ -102,8 +91,8 @@ def test_per_body_acceleration_equal_to_gravity_matches_uniform_gravity(libs):
     extra = scenes.make_bodies(np.array([[50, 5, 0], [60, 5, 0]], dtype=np.float32), linear=np.array([[1, 2, 3], [0, 1, 0]], dtype=np.float32),
                                inverse_mass=np.array([1, 1], dtype=np.float32), inverse_inertia=np.array([[2, 0, 2, 0, 0, 2]] * 2, dtype=np.float32))
     scene["bodies"] = np.concatenate([scene["bodies"], extra])
-    uniform = util.make_sim(scene, substeps=4, velocity_iterations=2, integrator=_integrator(gravity=(0, -10, 0), damping=0.0))
-    per_body = util.make_sim(scene, substeps=4, velocity_iterations=2, integrator=_integrator(gravity=(0, 0, 0), damping=0.0))
+    uniform = util.make_sim(scene, substeps=4, velocity_iterations=2, integrator=util.integrator(gravity=(0, -10, 0), linear_damping=0.0, angular_damping=0.0))
+    per_body = util.make_sim(scene, substeps=4, velocity_iterations=2, integrator=util.integrator(gravity=(0, 0, 0), linear_damping=0.0, angular_damping=0.0))
     acc = np.zeros((per_body.body_count, 8), dtype=np.float32)
     acc[:, 1] = -10.0
     for _ in range(2):
@@ -116,7 +105,7 @@ def test_per_body_acceleration_equal_to_gravity_matches_uniform_gravity(libs):
 def test_no_extension_is_oracle_solve_bit_for_bit(libs):
     """Zero accelerations and point gravity of strength 0 run the terms at every integration site and must change nothing."""
     scene = _mixed_scene()
-    a, b = (util.make_sim(scene, substeps=2, velocity_iterations=2, integrator=_integrator(kinematics=1)) for _ in range(2))
+    a, b = (util.make_sim(scene, substeps=2, velocity_iterations=2, integrator=util.integrator(integrate_velocity_for_kinematics=1)) for _ in range(2))
     ob.solve(a, DT)
     ob.solve(b, DT, accelerations=np.zeros((b.body_count, 8), dtype=np.float32), center=(0, -30, 0), strength=0.0)
     util.compare(util.snapshot(a), util.snapshot(b), exact=True)
@@ -130,24 +119,9 @@ CENTER, STRENGTH = (1.0, -40.0, 2.0), 800.0
 def _gpu_parity(scene, frames=2, mode=native.EXEC_GRAPH, exact=True, resident=False, rel_rms=1e-3, max_abs=5e-2, **kw):
     a, b = util.make_sim(scene, **kw), util.make_sim(scene, **kw)
     acc = _accelerations(a.body_count, 11)
-    for _ in range(frames):
-        ob.solve(a, DT, accelerations=acc, center=CENTER, strength=STRENGTH)
-    ts = native.CudaTimestepper(b, strict_fp=exact, execution_mode=mode)
-    try:
-        ts.describe()
-        ts.set_body_accelerations(acc)
-        ts.set_point_gravity(CENTER, STRENGTH)
-        for f in range(frames):
-            if resident and f < frames - 1:
-                ts.solve_device_only(DT)
-                continue
-            if f > 0 and not resident:
-                ts.refresh()
-            ts.solve(DT, download=True)
-            ts.download_prestep()
-    finally:
-        ts.close()
-    util.compare(util.snapshot(a), util.snapshot(b), exact=exact, rel_rms=rel_rms, max_abs=max_abs)
+    ref = util.run_oracle(a, DT, frames=frames, accelerations=acc, center=CENTER, strength=STRENGTH)
+    got = util.run_gpu(b, DT, frames=frames, strict=exact, mode=mode, terms=(acc, CENTER, STRENGTH), resident=resident)
+    util.compare(ref, got, exact=exact, rel_rms=rel_rms, max_abs=max_abs)
 
 
 GPU_SCENES = {
@@ -161,7 +135,7 @@ GPU_SCENES = {
 @pytest.mark.parametrize("scene", sorted(GPU_SCENES))
 @pytest.mark.parametrize("mode", [native.EXEC_GRAPH, native.EXEC_STREAM])
 def test_scenes_bit_exact(libs, scene, mode):
-    _gpu_parity(GPU_SCENES[scene](), mode=mode, substeps=3, velocity_iterations=2, integrator=_integrator(kinematics=1))
+    _gpu_parity(GPU_SCENES[scene](), mode=mode, substeps=3, velocity_iterations=2, integrator=util.integrator(integrate_velocity_for_kinematics=1))
 
 
 @pytest.mark.gpu
@@ -173,13 +147,13 @@ def test_angular_modes_and_unconstrained_bodies_bit_exact(libs, angular_mode, al
                                angular=np.array([[0.5, 0.1, -0.3], [0, 1, 0], [0, 0, 0]], dtype=np.float32), inverse_mass=np.array([1, 0, 1], dtype=np.float32),
                                inverse_inertia=np.array([[2, 0, 2, 0, 0, 2], [0, 0, 0, 0, 0, 0], [1, 0.1, 2, 0, 0.2, 3]], dtype=np.float32))
     scene["bodies"] = np.concatenate([scene["bodies"], extra])
-    _gpu_parity(scene, substeps=3, velocity_iterations=1, integrator=_integrator(angular_mode=angular_mode, allow_substeps=allow_substeps, kinematics=1))
+    _gpu_parity(scene, substeps=3, velocity_iterations=1, integrator=util.integrator(angular_integration_mode=angular_mode, allow_substeps_for_unconstrained=allow_substeps, integrate_velocity_for_kinematics=1))
 
 
 @pytest.mark.gpu
 def test_resident_frames_bit_exact(libs):
     _gpu_parity(scenes.merge(scenes.box_stacks(6, 8), scenes.ragdolls(10, seed=2)), frames=4, resident=True, substeps=2, velocity_iterations=2,
-                integrator=_integrator(kinematics=1))
+                integrator=util.integrator(integrate_velocity_for_kinematics=1))
 
 
 @pytest.mark.gpu
@@ -191,7 +165,7 @@ def test_fast_build_within_joint_tolerance(libs):
 @pytest.mark.gpu
 def test_predict_bounding_boxes_with_both_terms(libs):
     rng = np.random.default_rng(3)
-    sim = util.make_sim(scenes.shape_pile(600, seed=2), substeps=1, velocity_iterations=1, integrator=_integrator(kinematics=1))
+    sim = util.make_sim(scenes.shape_pile(600, seed=2), substeps=1, velocity_iterations=1, integrator=util.integrator(integrate_velocity_for_kinematics=1))
     n = sim.body_count
     shapes = np.zeros(n, dtype=native.BODY_SHAPE_DTYPE)
     shapes["type"] = rng.choice([0, 1, 2, 4], size=n)
@@ -220,7 +194,7 @@ def test_predict_bounding_boxes_with_both_terms(libs):
 @pytest.mark.gpu
 def test_profile_stages_advances_like_solve(libs):
     scene = scenes.merge(scenes.box_stacks(6, 8), scenes.joint_zoo(400, 20, seed=6))
-    a, b = (util.make_sim(scene, substeps=2, velocity_iterations=2, integrator=_integrator(kinematics=1)) for _ in range(2))
+    a, b = (util.make_sim(scene, substeps=2, velocity_iterations=2, integrator=util.integrator(integrate_velocity_for_kinematics=1)) for _ in range(2))
     acc = _accelerations(a.body_count, 12)
     ob.solve(a, DT, accelerations=acc, center=CENTER, strength=STRENGTH)
     ts = native.CudaTimestepper(b, strict_fp=True)
@@ -240,7 +214,7 @@ def test_profile_stages_advances_like_solve(libs):
 @pytest.mark.gpu
 def test_two_shard_ranks_bit_exact(libs):
     """Every rank holds every body and is given the whole acceleration array; the owning lane's results travel through the peer stores."""
-    sim = util.make_sim(scenes.merge(scenes.shape_pile(1200, seed=21), scenes.ragdolls(12, seed=22)), substeps=3, velocity_iterations=2, integrator=_integrator())
+    sim = util.make_sim(scenes.merge(scenes.shape_pile(1200, seed=21), scenes.ragdolls(12, seed=22)), substeps=3, velocity_iterations=2, integrator=util.integrator())
     acc = _accelerations(sim.body_count, 13)
     solvers = [sharding.ShardedSolver(sim, r, 2, 0, strict_fp=True) for r in range(2)]
     try:
@@ -294,7 +268,7 @@ def test_argument_and_state_errors(libs):
 @pytest.mark.gpu
 def test_cleared_terms_equal_a_context_that_never_set_them(libs):
     scene = scenes.merge(scenes.box_stacks(4, 6), scenes.joint_zoo(300, 20, seed=2))
-    a, b = (util.make_sim(scene, substeps=2, velocity_iterations=2, integrator=_integrator(kinematics=1)) for _ in range(2))
+    a, b = (util.make_sim(scene, substeps=2, velocity_iterations=2, integrator=util.integrator(integrate_velocity_for_kinematics=1)) for _ in range(2))
     ref = util.run_gpu(a, DT, frames=2)
     ts = native.CudaTimestepper(b, strict_fp=True)
     try:

@@ -111,19 +111,6 @@ def checker(sim, candidates):
     return island_checker.find_sleepable_islands(sim.type_batches(), sim.body_count, sim.bundle_width, candidates)
 
 
-def punch_fallback_holes(sim, every=5):
-    """Empties every `every`-th lane of the fallback type batches in place (what removing a constraint from the fallback batch leaves behind)."""
-    punched = 0
-    for tb in sim.type_batches():
-        if tb.batch_index < sim.fallback_batch_threshold:
-            continue
-        W = tb.body_references.shape[2]
-        for i in range(0, tb.constraint_count - 1, every):  # interior lanes: the last one keeps ConstraintCount meaningful
-            tb.body_references[i // W, :, i % W] = -1
-            punched += 1
-    return punched
-
-
 def candidates_for(n, seed, p_block=0.002):
     rng = np.random.default_rng(seed)
     return (rng.random(n) >= p_block).astype(np.uint8)
@@ -155,7 +142,7 @@ def test_checker_kinematic_bridge_joins_two_piles(libs):
 
 def test_checker_skips_empty_fallback_lanes(libs):
     sim = util.make_sim(scenes.fallback_stress(600, hubs=3, seed=5), fallback_batch_threshold=8)
-    assert punch_fallback_holes(sim) > 10
+    assert util.punch_fallback_holes(sim) > 10
     check_against_scipy(sim, candidates_for(sim.body_count, 3))
 
 
@@ -233,7 +220,7 @@ def test_device_matches_the_checker_on_random_graphs_at_every_bundle_width(libs)
         c[400] = 0
         check_device(sim, c)
         sim = util.make_sim(scenes.fallback_stress(600, hubs=3, seed=5), bundle_width=W, fallback_batch_threshold=8)
-        punch_fallback_holes(sim)
+        util.punch_fallback_holes(sim)
         check_device(sim, candidates_for(sim.body_count, W))
 
 

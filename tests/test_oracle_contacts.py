@@ -8,7 +8,6 @@ types act against the static world, two-body types against a kinematic ground bo
 import numpy as np
 import pytest
 
-import bepuphysics2_b200 as bp
 from bepuphysics2_b200 import scenes
 from tests import util
 
@@ -28,14 +27,6 @@ CONTACT_TYPES = (
     + [(scenes.NONCONVEX_TWO_BODY[n], n, "nonconvex", 2) for n in (2, 3, 4)]
 )
 IDS = ["type%d" % t[0] for t in CONTACT_TYPES]
-
-
-def _integrator():
-    d = bp.IntegratorDesc.default()
-    d.gravity[0], d.gravity[1], d.gravity[2] = 0.0, -G, 0.0
-    d.linear_damping = 0.0
-    d.angular_damping = 0.0
-    return d
 
 
 def _scene(type_id, contacts, family, body_count, friction, depth=0.0, linear=(0, 0, 0), angular=(0, 0, 0), inverse_inertia=(6.0, 0, 6.0, 0, 0, 6.0), max_recovery=2.0):
@@ -69,7 +60,7 @@ def _penetration_impulses(sim, contacts, family):
 
 @pytest.mark.parametrize("type_id,contacts,family,body_count", CONTACT_TYPES, ids=IDS)
 def test_resting_contact_carries_the_weight(libs, type_id, contacts, family, body_count):
-    sim = util.make_sim(_scene(type_id, contacts, family, body_count, friction=1.0), substeps=1, velocity_iterations=4, integrator=_integrator())
+    sim = util.make_sim(_scene(type_id, contacts, family, body_count, friction=1.0), substeps=1, velocity_iterations=4, integrator=util.integrator(gravity=(0.0, -G, 0.0), linear_damping=0.0, angular_damping=0.0))
     for _ in range(120):
         util.ob.solve(sim, DT)
     pen = _penetration_impulses(sim, contacts, family)
@@ -88,7 +79,7 @@ def test_sliding_friction_decelerates_at_mu_g(libs, type_id, contacts, family, b
     cone = mu / contacts if family == "convex" else mu  # see the module docstring
     # rotation locked (zero inverse inertia) so that the friction force acting below the centre of mass does not tip the body
     scene = _scene(type_id, contacts, family, body_count, friction=mu, linear=(3.0, 0, 1.0), inverse_inertia=(0, 0, 0, 0, 0, 0))
-    sim = util.make_sim(scene, substeps=1, velocity_iterations=4, integrator=_integrator())
+    sim = util.make_sim(scene, substeps=1, velocity_iterations=4, integrator=util.integrator(gravity=(0.0, -G, 0.0), linear_damping=0.0, angular_damping=0.0))
     speeds = []
     for _ in range(40):
         util.ob.solve(sim, DT)
@@ -103,7 +94,7 @@ def test_twist_friction_decelerates_the_spin(libs, type_id, contacts, family, bo
     """TwistFriction: |impulse| <= mu / N * sum(penetration impulses) ... * distances (ContactConvexTypes.cs, premultiplied friction coefficient)."""
     mu, inverse_inertia_y = 0.3, 6.0
     scene = _scene(type_id, contacts, family, body_count, friction=mu, angular=(0, 6.0, 0))
-    sim = util.make_sim(scene, substeps=1, velocity_iterations=4, integrator=_integrator())
+    sim = util.make_sim(scene, substeps=1, velocity_iterations=4, integrator=util.integrator(gravity=(0.0, -G, 0.0), linear_damping=0.0, angular_damping=0.0))
     spin = []
     for _ in range(30):
         util.ob.solve(sim, DT)
@@ -120,7 +111,7 @@ def test_twist_friction_decelerates_the_spin(libs, type_id, contacts, family, bo
 @pytest.mark.parametrize("type_id,contacts,family,body_count", CONTACT_TYPES, ids=IDS)
 def test_penetration_recovery_is_speed_limited(libs, type_id, contacts, family, body_count):
     """A deep contact pushes out at MaximumRecoveryVelocity at most (PenetrationLimit.cs:L78-131: bias = min(depth * ERP, maxRecovery))."""
-    integ = _integrator()
+    integ = util.integrator(gravity=(0.0, -G, 0.0), linear_damping=0.0, angular_damping=0.0)
     integ.gravity[1] = 0.0
     scene = _scene(type_id, contacts, family, body_count, friction=1.0, depth=0.5, max_recovery=0.75)
     sim = util.make_sim(scene, substeps=1, velocity_iterations=8, integrator=integ)
@@ -129,7 +120,7 @@ def test_penetration_recovery_is_speed_limited(libs, type_id, contacts, family, 
     assert float(sim.bodies[0, 9]) == pytest.approx(0.75, rel=2e-2)
     # and a separated contact (negative depth beyond what the body can close in a step) applies nothing
     scene = _scene(type_id, contacts, family, body_count, friction=1.0, depth=-1.0)
-    sim = util.make_sim(scene, substeps=1, velocity_iterations=4, integrator=_integrator())
+    sim = util.make_sim(scene, substeps=1, velocity_iterations=4, integrator=util.integrator(gravity=(0.0, -G, 0.0), linear_damping=0.0, angular_damping=0.0))
     util.ob.solve(sim, DT)
     assert float(sim.bodies[0, 9]) == pytest.approx(-G * DT, rel=1e-6)
     assert np.abs(_penetration_impulses(sim, contacts, family)).max() == 0.0
@@ -141,7 +132,7 @@ def test_speculative_contact_only_removes_the_velocity_that_would_penetrate(libs
     that is still `gap` away is slowed towards the approach speed gap / dt that just closes the gap this step, and a slower one is left
     alone. Each contact is a soft row (SpringSettings.cs:L37-55: softness = extra / (1 + extra) per unit effective mass, extra =
     1 / (w dt (w dt + 2 zeta))): the converged impulses of one step are the solution of a small linear system, solved here in float64."""
-    integ = _integrator()
+    integ = util.integrator(gravity=(0.0, -G, 0.0), linear_damping=0.0, angular_damping=0.0)
     integ.gravity[1] = 0.0
     gap = 0.01
     sim = util.make_sim(_scene(type_id, contacts, family, body_count, friction=0.0, depth=-gap, linear=(0, -1.0, 0)), substeps=1, velocity_iterations=30, integrator=integ)

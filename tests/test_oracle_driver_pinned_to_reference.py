@@ -36,17 +36,6 @@ FRAMES = 2
 needs_reference = pytest.mark.skipif(rf.library() is None, reason="the transpiled reference (oracle/_ref/libbepu_ref.so) is not built here")
 
 
-def _integrator(gravity=(0.0, -10.0, 0.0), damping=0.03, angular_mode=0, allow_substeps=0, kinematics=0):
-    d = native.IntegratorDesc.default()
-    for i in range(3):
-        d.gravity[i] = gravity[i]
-    d.linear_damping = d.angular_damping = damping
-    d.angular_integration_mode = angular_mode
-    d.allow_substeps_for_unconstrained = allow_substeps
-    d.integrate_velocity_for_kinematics = kinematics
-    return d
-
-
 def _loose_bodies(seed):
     """Unconstrained bodies: dynamic ones, +0 kinematic ones and one kinematic with -0.0 components, all moving."""
     rng = np.random.default_rng(seed)
@@ -77,28 +66,28 @@ def _cases():
         "joints_w4_kinematics_integrated": ("the joint zoo at width 4 with constrained kinematics, integrate_velocity_for_kinematics = 1, angular mode 1, "
                                             "point gravity, schedule [2, 0, 1]",
                                             scenes.joint_zoo(150, 4, seed=2, kinematic_fraction=0.1),
-                                            dict(bundle_width=4, substeps=3, velocity_iterations=[2, 0, 1], integrator=_integrator(angular_mode=1, kinematics=1)),
+                                            dict(bundle_width=4, substeps=3, velocity_iterations=[2, 0, 1], integrator=util.integrator(angular_integration_mode=1, integrate_velocity_for_kinematics=1)),
                                             dict(center=(0.0, -30.0, 0.0), strength=500.0)),
         "joints_w16_kinematics_not_integrated": ("the joint zoo at width 16, constrained kinematics with integrate_velocity_for_kinematics = 0, angular mode 2",
                                                  scenes.joint_zoo(150, 4, seed=3, kinematic_fraction=0.1),
-                                                 dict(bundle_width=16, substeps=2, velocity_iterations=1, integrator=_integrator(angular_mode=2))),
+                                                 dict(bundle_width=16, substeps=2, velocity_iterations=1, integrator=util.integrator(angular_integration_mode=2))),
         "ragdolls_four_substeps": ("ragdolls with motors and servos (types 22, 25-27, 29, 30, 46, 47) in a kinematic tube, loose bodies between them, "
                                    "4 substeps [1, 0, 2, 1], allow_substeps_for_unconstrained = 1, both velocity terms",
                                    scenes.merge(scenes.ragdolls(2, seed=4), loose(7), scenes.ragdolls(1, seed=5, motor="servo")),
-                                   dict(bundle_width=8, substeps=4, velocity_iterations=[1, 0, 2, 1], integrator=_integrator(allow_substeps=1, kinematics=1)),
+                                   dict(bundle_width=8, substeps=4, velocity_iterations=[1, 0, 2, 1], integrator=util.integrator(allow_substeps_for_unconstrained=1, integrate_velocity_for_kinematics=1)),
                                    dict(accelerations=True, center=(0.0, -40.0, 0.0), strength=300.0)),
         "fallback_w8": ("a fallback batch (threshold 3) with holes, hubs in several of its type batches, bodies first seen in batches > 0",
                         scenes.fallback_stress(100, hubs=3, seed=5), dict(bundle_width=8, substeps=2, velocity_iterations=1, fallback_batch_threshold=3), {}),
         "fallback_w16_angular": ("a fallback batch at threshold 2 and width 16, angular mode 1, three substeps",
                                  scenes.fallback_stress(70, hubs=2, seed=8), dict(bundle_width=16, substeps=3, velocity_iterations=[1, 1, 0], fallback_batch_threshold=2,
-                                                                                  integrator=_integrator(angular_mode=1))),
+                                                                                  integrator=util.integrator(angular_integration_mode=1))),
         "loose_bodies_allow0": ("unconstrained dynamic and kinematic bodies (one with -0.0 inertia) in body bundles with constrained ones, "
                                 "allow_substeps_for_unconstrained = 0, angular mode 1, kinematics not integrated",
                                 scenes.merge(scenes.joint_zoo(40, 1, seed=9, kinematic_fraction=0.1), loose(10), scenes.shape_pile(30, seed=9), loose(11)),
-                                dict(bundle_width=8, substeps=3, velocity_iterations=[1, 2, 1], integrator=_integrator(angular_mode=1)), dict(center=(5.0, -20.0, 0.0), strength=200.0)),
+                                dict(bundle_width=8, substeps=3, velocity_iterations=[1, 2, 1], integrator=util.integrator(angular_integration_mode=1)), dict(center=(5.0, -20.0, 0.0), strength=200.0)),
         "loose_bodies_allow1": ("the same bodies with allow_substeps_for_unconstrained = 1, angular mode 2, kinematics integrated, per-body accelerations",
                                 scenes.merge(scenes.joint_zoo(40, 1, seed=9, kinematic_fraction=0.1), loose(10), scenes.shape_pile(30, seed=9), loose(11)),
-                                dict(bundle_width=4, substeps=3, velocity_iterations=[0, 2, 1], integrator=_integrator(angular_mode=2, allow_substeps=1, kinematics=1)),
+                                dict(bundle_width=4, substeps=3, velocity_iterations=[0, 2, 1], integrator=util.integrator(angular_integration_mode=2, allow_substeps_for_unconstrained=1, integrate_velocity_for_kinematics=1)),
                                 dict(accelerations=True)),
     }
 
@@ -175,7 +164,7 @@ def bounds_case(seed, kinematics, terms):
     activities["timesteps_under_threshold_count"] = rng.choice([0, 1, 254, 255], size=n)
     activities["sleep_candidate"] = rng.integers(0, 2, size=n)
     kw = dict(accelerations=_accelerations(n, seed), center=(1.0, -25.0, 2.0), strength=400.0) if terms else {}
-    return bodies, shapes, activities, _integrator(kinematics=kinematics), kw
+    return bodies, shapes, activities, util.integrator(integrate_velocity_for_kinematics=kinematics), kw
 
 
 BOUNDS_CASES = {"kinematics0": (11, 0, False), "kinematics1": (12, 1, False), "kinematics0_terms": (13, 0, True), "kinematics1_terms": (14, 1, True)}
@@ -260,7 +249,7 @@ def test_matrix_covers_what_it_claims(libs):
             fallback = fallback or (tb.batch_index == sim.fallback_batch_threshold and (tb.body_references[:, 0, :] == -1).any())
     assert sorted(types) == sorted(t for t in range(64) if ob.type_info(t) is not None) and len(types) == 44
     assert widths == {4, 8, 16} and fallback
-    modes = {CASES[n][2].get("integrator", _integrator()).angular_integration_mode for n in CASES}
+    modes = {CASES[n][2].get("integrator", util.integrator()).angular_integration_mode for n in CASES}
     assert modes == {0, 1, 2}
     assert set(_digests()["solve"]) == set(CASES) and set(_digests()["bounds"]) == set(BOUNDS_CASES)
 

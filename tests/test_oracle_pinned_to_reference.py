@@ -25,19 +25,12 @@ import numpy as np
 import pytest
 
 from oracle import binding as ob
+from tests import util
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "tests", "golden"))
 FP = C.POINTER(C.c_float)
 DT = 1.0 / 240.0
-
-
-def _ptr(a):
-    return a.ctypes.data_as(FP)
-
-
-def _bits(a):
-    return np.ascontiguousarray(a, dtype=np.float32).view(np.uint32)
 
 
 @pytest.fixture(scope="module")
@@ -70,11 +63,11 @@ def test_oracle_reproduces_the_reference_constraint_functions_bit_for_bit(oracle
             for stage in (0, 1, 2):
                 v, a, p = vel[i].copy(), imp[i].copy(), pre[i].copy()
                 st = np.ascontiguousarray(states[i])
-                assert oracle.oracle_eval_lane(type_id, stage, _ptr(st), DT, _ptr(p), _ptr(a), _ptr(v), 1) == 0
+                assert oracle.oracle_eval_lane(type_id, stage, util.float_ptr(st), DT, util.float_ptr(p), util.float_ptr(a), util.float_ptr(v), 1) == 0
                 what = "type %d stage %d sample %d" % (type_id, stage, i)
-                assert np.array_equal(_bits(v), _bits(golden[key + "out%d_velocities" % stage][i])), what + ": velocities"
-                assert np.array_equal(_bits(a), _bits(golden[key + "out%d_impulses" % stage][i])), what + ": accumulated impulses"
-                assert np.array_equal(_bits(p), _bits(golden[key + "out%d_prestep" % stage][i])), what + ": prestep"
+                assert np.array_equal(util.bits(v), util.bits(golden[key + "out%d_velocities" % stage][i])), what + ": velocities"
+                assert np.array_equal(util.bits(a), util.bits(golden[key + "out%d_impulses" % stage][i])), what + ": accumulated impulses"
+                assert np.array_equal(util.bits(p), util.bits(golden[key + "out%d_prestep" % stage][i])), what + ": prestep"
                 checked += 1
         # the vectors exercise the functions: WarmStart and Solve moved the velocities
         assert not np.array_equal(golden[key + "out1_velocities"], vel)
@@ -88,8 +81,8 @@ def test_oracle_reproduces_the_reference_pose_integration_bit_for_bit(oracle, go
         ins, outs = golden["integration_%d_in" % op], golden["integration_%d_out" % op]
         for i in range(ins.shape[0]):
             got = np.zeros(outs.shape[1], dtype=np.float32)
-            assert oracle.oracle_eval_integration(op, _ptr(np.ascontiguousarray(ins[i])), _ptr(got)) == 0
-            assert np.array_equal(_bits(got), _bits(outs[i])), "integration function %d sample %d" % (op, i)
+            assert oracle.oracle_eval_integration(op, util.float_ptr(np.ascontiguousarray(ins[i])), util.float_ptr(got)) == 0
+            assert np.array_equal(util.bits(got), util.bits(outs[i])), "integration function %d sample %d" % (op, i)
 
 
 def test_oracle_reproduces_the_reference_benchmark_chains_bit_for_bit(oracle, golden):
@@ -103,11 +96,11 @@ def test_oracle_reproduces_the_reference_benchmark_chains_bit_for_bit(oracle, go
         st, p = np.ascontiguousarray(golden[k + "states"]), golden[k + "prestep"].copy()
         v, a = np.zeros_like(golden[k + "out_velocities"]), np.zeros_like(golden[k + "out_impulses"])
         for _ in range(1000):
-            oracle.oracle_eval_lane(tid, 0, _ptr(st), 1.0 / 60.0, _ptr(p), _ptr(a), _ptr(v), 1)
-            oracle.oracle_eval_lane(tid, 1, _ptr(st), 1.0 / 60.0, _ptr(p), _ptr(a), _ptr(v), 1)
+            oracle.oracle_eval_lane(tid, 0, util.float_ptr(st), 1.0 / 60.0, util.float_ptr(p), util.float_ptr(a), util.float_ptr(v), 1)
+            oracle.oracle_eval_lane(tid, 1, util.float_ptr(st), 1.0 / 60.0, util.float_ptr(p), util.float_ptr(a), util.float_ptr(v), 1)
         assert np.isfinite(v).all(), name
-        assert np.array_equal(_bits(v), _bits(golden[k + "out_velocities"])), name + ": velocities after 1000 iterations"
-        assert np.array_equal(_bits(a), _bits(golden[k + "out_impulses"])), name + ": accumulated impulses after 1000 iterations"
+        assert np.array_equal(util.bits(v), util.bits(golden[k + "out_velocities"])), name + ": velocities after 1000 iterations"
+        assert np.array_equal(util.bits(a), util.bits(golden[k + "out_impulses"])), name + ": accumulated impulses after 1000 iterations"
 
 
 @pytest.fixture(scope="module")
@@ -119,7 +112,7 @@ def fresh():
 def test_transpiled_reference_covers_all_types_and_reproduces_the_committed_vectors(oracle, golden, fresh):
     assert sorted(fresh["covered_types"].tolist()) == sorted(t for t in range(64) if ob.type_info(t) is not None)
     # both committed files come from the same transpiled library: its Solve on the first type-7 sample, stored with the fresh answers, is the vector
-    assert np.array_equal(_bits(fresh["lane07_out1_velocities"]), _bits(golden["lane_07_out1_velocities"][0]))
+    assert np.array_equal(util.bits(fresh["lane07_out1_velocities"]), util.bits(golden["lane_07_out1_velocities"][0]))
 
 
 def test_oracle_matches_the_transpiled_reference_on_fresh_inputs(oracle, fresh):

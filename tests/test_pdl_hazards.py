@@ -15,9 +15,7 @@ import sys
 import pytest
 
 from bepuphysics2_b200 import _build, sharding
-from tests import test_topology as topo
-from tests.test_topology import shim  # noqa: F401  (a fixture)
-from tests.test_sharded_fallback import peer_shim, plan_peer, shard_sources  # noqa: F401  (peer_shim is a fixture)
+from tests import planner
 from tests.tools import pdl_hazards as hz
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -86,7 +84,7 @@ def _launch_context(name):
     return kind == "terms", integrator.angular_integration_mode if integrator is not None else 0
 
 
-def config_launches(shim, peer, name):
+def config_launches(name):
     """Per context of configuration `name` (one, or one per rank): rows stage, kernel, flags, warps of every launch the GPU run makes with PDL or
     that precedes one, in program order; the body count."""
     sim = hz.make_sim(name)
@@ -95,58 +93,58 @@ def config_launches(shim, peer, name):
     if ranks:
         shards, _, _, _ = sharding.partition(sim, ranks)
         fallback = sharding.fallback_rank(sim, ranks)
-        plans = [plan_peer(peer, shard_sources(shards[r]), sim.bundle_width, sim.fallback_batch_threshold, sim.batch_count, sim.body_count, r, fallback)
-                 for r in range(ranks)]
+        plans = [planner.plan(planner.shard_sources(shards[r]), sim.bundle_width, sim.fallback_batch_threshold, sim.batch_count, sim.body_count, True, r,
+                              fallback) for r in range(ranks)]
     else:
-        plans = [topo.plan(shim, topo.sim_sources(sim), sim.bundle_width, sim.fallback_batch_threshold, sim.batch_count, sim.body_count)]
+        plans = [planner.plan(planner.sim_sources(sim), sim.bundle_width, sim.fallback_batch_threshold, sim.batch_count, sim.body_count)]
     out = []
     for p in plans:
         ops, _ = p.program(sim.velocity_iterations, len(sim.constrained_kinematics), True, bool(ranks), sim.body_count)
-        ops = ops[(ops[:, 2] > 0) | (ops[:, 3] == topo.RANK_BARRIER)]
-        kernel, flags = topo.resolve(shim, ops, ext, mode, False).T
+        ops = ops[(ops[:, 2] > 0) | (ops[:, 3] == planner.RANK_BARRIER)]
+        kernel, flags = planner.resolve(ops, ext, mode, False).T
         rows = []
         for op, k, f in zip(ops, kernel, flags):
             stage = int(op[0])
-            if int(op[3]) == topo.RANK_BARRIER:
+            if int(op[3]) == planner.RANK_BARRIER:
                 rows.append((stage, BARRIER, 0, 8))
-            elif stage <= topo.INCREMENTAL:
-                ctas = (int(op[2]) + 1) // 2 + ((sim.body_count + 63) // 64 if f & topo.BODIES_INTEGRATED and stage == topo.INCREMENTAL else 0)
+            elif stage <= planner.INCREMENTAL:
+                ctas = (int(op[2]) + 1) // 2 + ((sim.body_count + 63) // 64 if f & planner.BODIES_INTEGRATED and stage == planner.INCREMENTAL else 0)
                 rows.append((stage, int(k), int(f), 2 * ctas))
             else:
-                rows.append((stage, topo.KERNEL_FULL, int(f), 0))  # kinematic and final pose passes: launched without PDL
+                rows.append((stage, planner.KERNEL_FULL, int(f), 0))  # kinematic and final pose passes: launched without PDL
         out.append((rows, sim.body_count, bool(ranks), p))
     return out
 
 
-def test_gpu_configurations_reach_every_launch_flag_and_instantiation(libs, shim, peer_shim):
+def test_gpu_configurations_reach_every_launch_flag_and_instantiation(libs):
     """Across the configurations the GPU check runs, with their launch contexts: row prefetch, world loads on a Solve and on a WarmStart, owned
     loads, the bodies-integrated flag; the full, contact-only, integrated WarmStart, deep, kExt and sharded instantiations; the incremental update's
     body CTAs; a rank barrier. Without them the check would hold the rule only where it is easy."""
     seen = set()
     for name in hz.CONFIGS:
-        for rows, _, sharded, _ in config_launches(shim, peer_shim, name):
+        for rows, _, sharded, _ in config_launches(name):
             for stage, kernel, flags, _ in rows:
                 if kernel == BARRIER:
                     seen.add("rank barrier")
                     continue
-                if stage > topo.INCREMENTAL:
+                if stage > planner.INCREMENTAL:
                     continue
-                seen |= {what for bit, what in ((topo.ROWS, "prefetch rows"), (topo.EARLY_OWNED, "early owned"), (topo.BODIES_INTEGRATED, "bodies integrated"))
+                seen |= {what for bit, what in ((planner.ROWS, "prefetch rows"), (planner.EARLY_OWNED, "early owned"), (planner.BODIES_INTEGRATED, "bodies integrated"))
                          if flags & bit}
-                if flags & topo.EARLY_WORLD:
-                    seen.add("early world on %s" % ("Solve" if stage == topo.SOLVE else "WarmStart"))
-                if stage == topo.INCREMENTAL:
-                    seen.add("incremental body CTAs" if flags & topo.BODIES_INTEGRATED else "incremental")
+                if flags & planner.EARLY_WORLD:
+                    seen.add("early world on %s" % ("Solve" if stage == planner.SOLVE else "WarmStart"))
+                if stage == planner.INCREMENTAL:
+                    seen.add("incremental body CTAs" if flags & planner.BODIES_INTEGRATED else "incremental")
                     continue
                 if sharded:
                     seen.add("sharded")
-                elif kernel == topo.KERNEL_DEEP:
+                elif kernel == planner.KERNEL_DEEP:
                     seen.add("deep")
-                elif kernel == topo.KERNEL_CONTACTS:
-                    seen.add("integrated WarmStart" if stage == topo.WS and flags & topo.BODIES_INTEGRATED else "contact-only")
+                elif kernel == planner.KERNEL_CONTACTS:
+                    seen.add("integrated WarmStart" if stage == planner.WS and flags & planner.BODIES_INTEGRATED else "contact-only")
                 else:
                     seen.add("full")
-                if flags & topo.EXT:
+                if flags & planner.EXT:
                     seen.add("kExt")
     want = {"prefetch rows", "early world on Solve", "early world on WarmStart", "early owned", "bodies integrated", "full", "contact-only",
             "integrated WarmStart", "deep", "kExt", "sharded", "incremental body CTAs", "rank barrier"}
@@ -155,7 +153,7 @@ def test_gpu_configurations_reach_every_launch_flag_and_instantiation(libs, shim
 
 # Warps per SM each instantiation keeps resident (its __launch_bounds__): the full switch 16, the contact-only kernels 20 (their WarmStart budget;
 # the Solve one keeps 24), the deep kernels 24; the rank barrier is one 256-thread CTA.
-RESIDENT_WARPS = {topo.KERNEL_FULL: 16, topo.KERNEL_CONTACTS: 20, topo.KERNEL_DEEP: 24, BARRIER: 64}
+RESIDENT_WARPS = {planner.KERNEL_FULL: 16, planner.KERNEL_CONTACTS: 20, planner.KERNEL_DEEP: 24, BARRIER: 64}
 
 
 def residency_failures(launches, sm_count):
@@ -164,15 +162,15 @@ def residency_failures(launches, sm_count):
     that loads body records before its wait is checked, and it needs only the start of its first wave (one CTA per SM) beside the predecessor's
     last wave: the deep kernels themselves load no body record before their wait."""
     worst = {}
-    deep = any(k == topo.KERNEL_DEEP for rows, _, _, _ in launches for _, k, _, _ in rows)
+    deep = any(k == planner.KERNEL_DEEP for rows, _, _, _ in launches for _, k, _, _ in rows)
     for rows, _, _, _ in launches:
         for i in range(1, len(rows)):
             (s0, k0, _, w0), (s1, k1, f1, w1) = rows[i - 1], rows[i]
-            if (s1 > topo.INCREMENTAL and k1 != BARRIER) or (s0 > topo.INCREMENTAL and k0 != BARRIER):
+            if (s1 > planner.INCREMENTAL and k1 != BARRIER) or (s0 > planner.INCREMENTAL and k0 != BARRIER):
                 continue  # a launch without PDL on either side: no overlap
             c0, c1 = RESIDENT_WARPS[k0] * sm_count, RESIDENT_WARPS[k1] * sm_count
             if deep:
-                if not f1 & (topo.EARLY_WORLD | topo.EARLY_OWNED | topo.BODIES_INTEGRATED):
+                if not f1 & (planner.EARLY_WORLD | planner.EARLY_OWNED | planner.BODIES_INTEGRATED):
                     continue  # the deep scene: only dependents that load body records before their wait
                 # several waves deep: one dependent CTA per SM must start beside the predecessor's last wave
                 need = (w0 % c0 or c0) / c0 + min(w1, 2 * sm_count) / c1
@@ -183,14 +181,14 @@ def residency_failures(launches, sm_count):
 
 
 @pytest.mark.gpu
-def test_pdl_hazards_on_the_h100(libs, shim, peer_shim):
+def test_pdl_hazards_on_the_h100(libs):
     """With the delay on: every configuration's pair of consecutive PDL launches fits on the device together, every configuration in both execution
     modes equals the oracle bit for bit, and every canary makes its scene differ. Whether a canary also differed with plain timing is reported."""
     import torch
 
     sm_count = torch.cuda.get_device_properties(0).multi_processor_count
     for name in hz.CONFIGS:
-        bad = residency_failures(config_launches(shim, peer_shim, name), sm_count)
+        bad = residency_failures(config_launches(name), sm_count)
         assert not bad, "%s: launches that do not fit beside their predecessor on %d SMs: %s" % (name, sm_count, sorted(bad.items())[:5])
     assert os.path.exists(os.path.join(os.path.dirname(_build.LIB_CUDA), "libbepucuda_hazard.so")), "__graft_entry__.build() builds the hazard variant"
     env = dict(os.environ, BEPUCUDA_VARIANT="hazard")

@@ -13,7 +13,6 @@ from tests import util
 
 DT = 1.0 / 60.0
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-EXECUTION_MODES = {"graph": native.EXEC_GRAPH, "stream": native.EXEC_STREAM}
 
 
 def _global_rows(sim):
@@ -97,60 +96,21 @@ def test_two_gloo_ranks_derive_the_same_global_tables(tmp_path):
     assert r.returncode == 0 and "OK" in r.stdout, r.stdout[-3000:]
 
 
-def _one_process_ranks(sim_scene, rank_count, frames, mode, libs, **kw):
-    """`rank_count` contexts on device 0, wired to one another with bepucuda_shard_import_contexts; every rank's referenced bodies and its own
-    impulses and prestep rows (contact depths written by the incremental update) against the oracle run on the whole graph."""
-    from oracle import binding as ob
-
-    sim = util.make_sim(sim_scene, **kw)
-    solvers = [sharding.ShardedSolver(sim, r, rank_count, 0, strict_fp=True, execution_mode=EXECUTION_MODES[mode]) for r in range(rank_count)]
-    try:
-        for s in solvers:
-            s.export_handles()
-        for s in solvers:
-            s.import_contexts(solvers)
-        for s in solvers:
-            s.describe()
-        for s in solvers:
-            s.synchronize()
-        for _ in range(frames):
-            ob.solve(sim, DT)
-            for s in solvers:  # asynchronous launches: the ranks' frames run side by side on the device and meet at their exchange points
-                s.solve(DT)
-        by_key = {(tb.batch_index, tb.type_batch_index): tb for tb in sim.type_batches()}
-        for s in solvers:
-            got = s.download()
-            mine = s.referenced_bodies()
-            assert mine.size > 0
-            assert np.array_equal(sim.bodies[mine][:, util.MOTION].view(np.uint32), got[mine][:, util.MOTION].view(np.uint32)), "rank %d bodies (%s)" % (s.rank, mode)
-            for tb in s.shard:
-                g = by_key[(tb["batch_index"], tb["type_batch_index"])]
-                for what, ref_rows in (("impulses", g.accumulated_impulses), ("prestep", g.prestep)):
-                    ref = ref_rows.transpose(0, 2, 1).reshape(-1, ref_rows.shape[1])[tb["source"]]
-                    have = tb[what].transpose(0, 2, 1).reshape(-1, tb[what].shape[1])[:tb["count"]]
-                    assert np.array_equal(ref.view(np.uint32), have.view(np.uint32)), "rank %d %s of batch %d (%s)" % (s.rank, what, tb["batch_index"], mode)
-        shared = int(((solvers[0].masks & (solvers[0].masks - 1)) != 0).sum())
-        assert shared > 0
-    finally:
-        for s in solvers:
-            s.close()
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("rank_count,mode", [(2, "graph"), (3, "graph"), (2, "stream")])
 def test_one_graph_over_several_ranks_bit_exact(libs, rank_count, mode):
-    _one_process_ranks(scenes.shape_pile(2500, seed=6), rank_count, frames=3, mode=mode, libs=libs, substeps=4, velocity_iterations=2)
+    util.run_ranks(scenes.shape_pile(2500, seed=6), rank_count, frames=3, mode=mode, substeps=4, velocity_iterations=2)
 
 
 @pytest.mark.gpu
 def test_one_graph_over_two_ranks_ragdolls_bit_exact(libs):
-    _one_process_ranks(scenes.ragdolls(60, seed=2), 2, frames=2, mode="graph", libs=libs, substeps=2, velocity_iterations=2)
+    util.run_ranks(scenes.ragdolls(60, seed=2), 2, frames=2, mode="graph", substeps=2, velocity_iterations=2)
 
 
 @pytest.mark.gpu
 def test_one_graph_over_two_ranks_joint_zoo_bit_exact(libs):
     """Three- and four-body constraints, kinematic bodies, every joint type: the pushes of body slots 2 and 3 and the kinematic stages."""
-    _one_process_ranks(scenes.joint_zoo(1200, per_type=60, seed=8), 2, frames=2, mode="graph", libs=libs, substeps=3, velocity_iterations=2)
+    util.run_ranks(scenes.joint_zoo(1200, per_type=60, seed=8), 2, frames=2, mode="graph", substeps=3, velocity_iterations=2)
 
 
 @pytest.mark.gpu
@@ -159,7 +119,7 @@ def test_one_graph_over_two_ranks_mixed_scene_bit_exact(libs):
     reads velocities that other ranks stored, and each rank's contact depths must still match the oracle bit for bit."""
     scene = scenes.merge(scenes.shape_pile(1200, seed=21), scenes.ragdolls(12, seed=22), scenes.joint_zoo(300, 20, seed=23))
     for mode in ("graph", "stream"):
-        _one_process_ranks(scene, 2, frames=2, mode=mode, libs=libs, substeps=3, velocity_iterations=2)
+        util.run_ranks(scene, 2, frames=2, mode=mode, substeps=3, velocity_iterations=2)
 
 
 @pytest.mark.gpu

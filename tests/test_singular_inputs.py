@@ -23,10 +23,9 @@ import pytest
 from bepuphysics2_b200 import native, scenes
 from bepuphysics2_b200.native import EXEC_GRAPH, EXEC_STREAM
 from oracle import binding as ob
-from tests import test_topology as topo
-from tests import util
-from tests.test_deep_batches import DEEP_BUNDLES
-from tests.test_device_source_on_host import CSRC, LANES, _ptr, compile_device_on_host, device_on_host  # noqa: F401 (device_on_host: fixture)
+from tests import device_source, harness, planner, util
+from tests.device_source import CSRC, LANES
+from tests.planner import DEEP_BUNDLES
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLDEN = os.path.join(ROOT, "tests", "golden", "reference_singular_vectors.npz")
@@ -35,7 +34,6 @@ DT = 1.0 / 60.0
 HEADERS = ("bepu_device_math.cuh", "bepu_contacts.cuh", "bepu_joints.cuh", "bepu_joints_more.cuh", "bepu_integration.cuh")
 CONTACT_TYPES = (0, 1, 2, 3, 4, 5, 6, 7, 8, 9, 10, 15, 16, 17)
 ONE_BODY_CONTACTS, TWO_BODY_CONTACTS = (0, 1, 2, 3, 8, 9, 10), (4, 5, 6, 7, 15, 16, 17)
-shim = topo.shim
 
 
 @pytest.fixture(scope="module")
@@ -58,7 +56,7 @@ def _eval(fn, g, i, stage, stride, takes_stride):
     a[::stride] = g["impulses"][i][:impulse_rows]
     v = g["velocities"][i].copy()
     states = np.ascontiguousarray(g["states"][i])
-    args = [type_id, stage, _ptr(states), DT_LANE, _ptr(p), _ptr(a), _ptr(v)]
+    args = [type_id, stage, util.float_ptr(states), DT_LANE, util.float_ptr(p), util.float_ptr(a), util.float_ptr(v)]
     assert (fn(*args, stride) if takes_stride else fn(*args)) == 0
     return v, a[::stride], p[::stride]
 
@@ -95,8 +93,8 @@ def test_oracle_reproduces_the_reference_on_singular_inputs(libs, golden):
     assert _check_against_golden(orc.oracle_eval_lane, golden, LANES, True) > 1000
 
 
-def test_device_source_reproduces_the_reference_on_singular_inputs(libs, golden, device_on_host):
-    dev, _ = device_on_host
+def test_device_source_reproduces_the_reference_on_singular_inputs(libs, golden):
+    dev, _ = device_source.load()
     assert _check_against_golden(dev.device_on_host_eval_lane, golden, LANES, False) > 1000
 
 
@@ -277,7 +275,7 @@ def coverage(tmp_path_factory, golden):
     """gcov's per-line branch counts {(header, line): [taken counts]} of the -O0 --coverage build after evaluating every singular case."""
     d = tmp_path_factory.mktemp("coverage")
     lib = str(d / "libdevice_on_host_cov.so")
-    compile_device_on_host(lib, ("-O0", "--coverage"))
+    harness.build(lib, [device_source.SOURCE], device_source.flags(("-O0", "--coverage")), device_source.INCLUDES)
     # the counters are written when the process that ran the code exits
     subprocess.run([sys.executable, "-c", CHILD, lib, GOLDEN, str(LANES)], cwd=str(d), check=True)
     gcda = [f for f in os.listdir(d) if f.endswith(".gcda")]
@@ -361,7 +359,7 @@ def make_singular_sim(g, scene, first, **kw):
     """A host simulation of the scene with every constraint's accumulated impulses set to its case's (the moving cases start warm)."""
     sim = util.make_sim(scene, integrator=_no_gravity(), **kw)
     for tb in sim.type_batches():
-        refs = tb.body_references[:, 0, :] & topo.INDEX_MASK
+        refs = tb.body_references[:, 0, :] & planner.INDEX_MASK
         for bundle, lane in zip(*np.nonzero(tb.body_references[:, 0, :] >= 0)):
             i = first[int(refs[bundle, lane])]
             tb.accumulated_impulses[bundle, :, lane] = g["impulses"][i][:tb.impulse_rows]
@@ -405,19 +403,19 @@ def scenes_of_cases(golden):
     return {kind: _scene(golden, kind) for kind in ("mixed", "contacts", "deep", "clamped", "unclamped")}
 
 
-def test_scenes_reach_the_full_the_contact_only_and_the_deep_kernels(libs, shim, golden, scenes_of_cases):
+def test_scenes_reach_the_full_the_contact_only_and_the_deep_kernels(libs, golden, scenes_of_cases):
     """The mixed scene runs in full-switch launches, the contact-only scene in contact-only launches, the replicated one in deep launches."""
     for kind, (scene, first) in scenes_of_cases.items():
         if kind in ("clamped", "unclamped"):
             continue
         sim = make_singular_sim(golden, scene, first, **KW)
         assert sim.batch_count == 1, kind  # every constraint has bodies of its own
-        p = topo.plan(shim, topo.sim_sources(sim), sim.bundle_width, sim.fallback_batch_threshold, sim.batch_count, sim.body_count)
+        p = planner.plan(planner.sim_sources(sim), sim.bundle_width, sim.fallback_batch_threshold, sim.batch_count, sim.body_count)
         ops, _ = p.program(sim.velocity_iterations, len(sim.constrained_kinematics), True, False, sim.body_count)
-        stages = ops[ops[:, 0] <= topo.SOLVE]
-        for ext, mode, profile in topo.LAUNCH_CONTEXTS:
-            kernel = topo.resolve(shim, stages, ext, mode, profile)[:, 0]
-            want = {"mixed": topo.KERNEL_FULL, "contacts": topo.KERNEL_CONTACTS, "deep": topo.KERNEL_DEEP}[kind]
+        stages = ops[ops[:, 0] <= planner.SOLVE]
+        for ext, mode, profile in planner.LAUNCH_CONTEXTS:
+            kernel = planner.resolve(stages, ext, mode, profile)[:, 0]
+            want = {"mixed": planner.KERNEL_FULL, "contacts": planner.KERNEL_CONTACTS, "deep": planner.KERNEL_DEEP}[kind]
             assert (kernel == want).all(), (kind, ext, mode, profile, kernel.tolist())
         count = int(p.batches[0, 1])
         assert (count >= DEEP_BUNDLES) == (kind == "deep"), (kind, count)

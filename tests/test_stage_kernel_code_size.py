@@ -14,7 +14,7 @@ import subprocess
 
 import pytest
 
-from tests.test_stage_kernel_resources import LIB, MAX_STACK_BYTES, MIN_WARPS_PER_SM, REGISTER_BUDGET, resident_warps, resource_usage
+from tests.kernel_resources import LIB, MAX_STACK_BYTES, MIN_WARPS_PER_SM, REGISTER_BUDGET, resident_warps, resource_usage
 
 KERNEL = re.compile(r"_ZN\d+(bepu_fast|bepu_strict)\d+(constraint_stage_kernel|integrated_constraint_stage_kernel)ILi1ELi\d+ELb0ELb1EE")
 BUDGET = {"bepu_fast": 5000, "bepu_strict": 5850}

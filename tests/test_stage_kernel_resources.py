@@ -3,59 +3,11 @@
 The contact-only WarmStart / Solve instantiations (kContacts, launched for batches whose every bundle is a contact) exist to be resident at 20 warps
 per SM or more (WarmStart 20 at 96 registers, Solve 24 at 80), so that the next stage's CTAs find free slots while a head batch still runs. A
 source change that pushes them past their budget, or makes them spill, silently takes that away; this test catches it without a GPU."""
-import os
 import re
-import shutil
-import subprocess
 
-import pytest
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-LIB = os.path.join(ROOT, "bepuphysics2_b200", "libbepucuda.so")
-
-# H100 (sm_90) per-SM limits
-REGS_PER_SM = 65536
-REG_ALLOC_UNIT = 256  # registers are allocated per warp in units of 256
-SMEM_PER_SM = 228 * 1024
-SMEM_RESERVED_PER_CTA = 1024
-MAX_WARPS_PER_SM = 64
-CTA_WARPS = 2  # kStageBlockThreads = 64
-
-REGISTER_BUDGET = 96  # WarmStartFirst / WarmStart
-MIN_WARPS_PER_SM = 20
-SOLVE_REGISTER_BUDGET = 80
-SOLVE_MIN_WARPS_PER_SM = 24
-# The WarmStart kernels pass argument structs to the out-of-line angular-momentum integrators on the stack (48 B); any larger frame is spill.
-MAX_STACK_BYTES = 48
+from tests.kernel_resources import MAX_STACK_BYTES, MIN_WARPS_PER_SM, REGISTER_BUDGET, SOLVE_MIN_WARPS_PER_SM, SOLVE_REGISTER_BUDGET, resident_warps, resource_usage
 
 CONTACT_KERNEL = re.compile(r"_ZN\d+(bepu_fast|bepu_strict)23constraint_stage_kernelILi(\d)ELi(\d+)ELb([01])ELb1EE")
-
-
-def resource_usage():
-    tool = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
-    if not os.path.exists(LIB):
-        pytest.skip("libbepucuda.so has not been built")
-    if not os.path.exists(tool):
-        pytest.skip("cuobjdump is not available")
-    out = subprocess.run([tool, "--dump-resource-usage", LIB], stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, check=True).stdout
-    kernels = {}
-    name = None
-    for line in out.splitlines():
-        m = re.match(r"\s*Function (\S+):", line)
-        if m:
-            name = m.group(1)
-            continue
-        if name and "REG:" in line:
-            kernels[name] = {k: int(v) for k, v in re.findall(r"(REG|STACK|SHARED|LOCAL):(\d+)", line)}
-            name = None
-    return kernels
-
-
-def resident_warps(regs, shared):
-    per_warp = -(-regs * 32 // REG_ALLOC_UNIT) * REG_ALLOC_UNIT
-    ctas_by_regs = REGS_PER_SM // (per_warp * CTA_WARPS)
-    ctas_by_smem = SMEM_PER_SM // (shared + SMEM_RESERVED_PER_CTA)
-    return min(min(ctas_by_regs, ctas_by_smem) * CTA_WARPS, MAX_WARPS_PER_SM)
 
 
 def contact_kernels():

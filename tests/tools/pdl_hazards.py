@@ -23,7 +23,7 @@ if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
 from bepuphysics2_b200 import native, scenes  # noqa: E402
-from tests import util  # noqa: E402
+from tests import planner, resident, util  # noqa: E402
 
 DT = 1.0 / 60.0
 DELAY_US = 50  # the delay of the checked runs; the residency precondition says what it has to cover
@@ -59,19 +59,15 @@ def mixed(seed=7):
 
 
 def single_batch_pile():
-    from tests.test_topology import single_batch
-
-    return single_batch(scenes.shape_pile(800, seed=17))
+    return planner.single_batch(scenes.shape_pile(800, seed=17))
 
 
 def deep():
     """A reduced copy of the deep-batch scene of tests/test_deep_batches.py: a 160 k-body pile whose head batches are deep, with every joint type
     in its first two batches and moving constrained kinematics."""
-    from tests.test_deep_batches import _in_first_batches
-
     joints = scenes.merge(scenes.joint_zoo(3000, per_type=60, seed=22), scenes.ragdolls(30, seed=23))
     joints["constraints"] = joints["constraints"][::-1]
-    scene = scenes.merge(scenes.shape_pile(DEEP_PILE_BODIES, seed=21, nonconvex_fraction=0.3), _in_first_batches(joints, 2))
+    scene = scenes.merge(scenes.shape_pile(DEEP_PILE_BODIES, seed=21, nonconvex_fraction=0.3), planner.in_first_batches(joints, 2))
     kin = np.flatnonzero(scene["bodies"][:, 22] == 0)
     rng = np.random.default_rng(25)
     scene["bodies"][kin, 8:11] = rng.uniform(-0.3, 0.3, size=(kin.size, 3)).astype(f32)
@@ -80,12 +76,6 @@ def deep():
 
 
 DEEP_PILE_BODIES = 160_000
-
-
-def integrator(angular_mode=0):
-    d = native.IntegratorDesc.default()
-    d.angular_integration_mode = angular_mode
-    return d
 
 
 def terms(n):
@@ -103,13 +93,13 @@ CONFIGS = {
     "joint_zoo": (lambda: scenes.joint_zoo(600, 20, seed=4, kinematic_fraction=0.1), dict(substeps=2, velocity_iterations=2), "single", None),
     "schedule_0_3_1": (lambda: mixed(5), dict(substeps=3, velocity_iterations=[0, 3, 1], fallback_batch_threshold=6), "single", None),
     "schedule_2_0_2": (lambda: with_kinematics(pile(), 0.03, 8), dict(substeps=3, velocity_iterations=[2, 0, 2]), "single", None),
-    "angular_mode_1": (mixed, dict(substeps=2, velocity_iterations=2, integrator=integrator(1)), "single", None),
+    "angular_mode_1": (mixed, dict(substeps=2, velocity_iterations=2, integrator=util.integrator(angular_integration_mode=1)), "single", None),
     "accelerations_point_gravity": (mixed, dict(substeps=2, velocity_iterations=2), "terms", None),
     "resident_frames": (lambda: scenes.shape_pile(3000, seed=31, nonconvex_fraction=0.3), {}, "resident", None),
     "ranks_2": (lambda: scenes.shape_pile(2500, seed=6), dict(substeps=4, velocity_iterations=2), "ranks", 2),
     "ranks_3_fallback": (lambda: scenes.fallback_stress(3000, hubs=6, seed=7), dict(fallback_batch_threshold=4, substeps=2, velocity_iterations=2),
                          "fallback_ranks", 3),
-    "deep": (deep, dict(substeps=3, velocity_iterations=[2, 0, 1], integrator=integrator()), "single", None),
+    "deep": (deep, dict(substeps=3, velocity_iterations=[2, 0, 1], integrator=util.integrator()), "single", None),
 }
 # canary: (name, the configurations it must be caught on). Row prefetch is caught twice: behind a stage of the same batch (Solve after Solve in a
 # single-batch pile) and behind the incremental update (the first WarmStart's depth rows, in a pile without kinematic passes).
@@ -125,25 +115,6 @@ CANARIES = {
 def make_sim(name):
     make, kw, _, _ = CONFIGS[name]
     return util.make_sim(make(), **kw)
-
-
-def _device_single(scene, kw, frames, mode, with_terms):
-    sim = util.make_sim(scene, **kw)
-    ts = native.CudaTimestepper(sim, strict_fp=True, execution_mode=mode)
-    try:
-        ts.describe()
-        if with_terms:
-            acc, center, strength = terms(sim.body_count)
-            ts.set_body_accelerations(acc)
-            ts.set_point_gravity(center, strength)
-        for f in range(frames):
-            if f > 0:
-                ts.refresh()
-            ts.solve(DT, download=True)
-            ts.download_prestep()
-    finally:
-        ts.close()
-    return util.snapshot(sim)
 
 
 _ORACLE = {}
@@ -166,21 +137,14 @@ def run(name, mode, hazard):
     try:
         if kind in ("single", "terms"):
             frames = 1 if name == "deep" else 2
-            got = _device_single(scene, kw, frames, MODES[mode], kind == "terms")
+            sim = util.make_sim(scene, **kw)
+            got = util.run_gpu(sim, DT, frames=frames, mode=MODES[mode], terms=terms(sim.body_count) if kind == "terms" else None)
             util.compare(_oracle(name, scene, kw, frames, kind == "terms"), got, exact=True)
         elif kind == "resident":
-            from tests.test_contact_update import _resident_frames
-
-            host, dev, _, _, _ = _resident_frames(scene, frames=2, mode=MODES[mode])
+            host, dev, _, _, _ = resident.resident_frames(scene, frames=2, mode=MODES[mode])
             util.compare(util.snapshot(host), util.snapshot(dev), exact=True)
-        elif kind == "ranks":
-            from tests.test_sharding import _one_process_ranks
-
-            _one_process_ranks(scene, extra, frames=2, mode=mode, libs=True, **kw)
         else:
-            from tests.test_sharded_fallback import _one_process_ranks
-
-            _one_process_ranks(scene, extra, frames=2, mode=mode, **kw)
+            util.run_ranks(scene, extra, frames=2, mode=mode, **kw)
     except AssertionError as e:
         return str(e).split("\n")[0][:300]
     finally:

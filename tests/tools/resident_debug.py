@@ -9,14 +9,14 @@ import bepuphysics2_b200 as bp
 from bepuphysics2_b200 import scenes
 from oracle import binding as ob
 from tests import util
-from tests.test_contact_update import _initial_features, _narrow_phase_like_update
+from tests.resident import initial_features, narrow_phase_like_update
 
 DT = 1 / 60.0
 scene = scenes.shape_pile(3000, seed=31)
 kw = dict(substeps=3, velocity_iterations=2)
 host, dev = util.make_sim(scene, **kw), util.make_sim(scene, **kw)
 rng_h, rng_d = np.random.default_rng(77), np.random.default_rng(77)
-feat_h, feat_d = _initial_features(host, rng_h), _initial_features(dev, rng_d)
+feat_h, feat_d = initial_features(host, rng_h), initial_features(dev, rng_d)
 ts = bp.CudaTimestepper(dev, strict_fp=True)
 ts.register_host_buffers()
 ts.describe()
@@ -36,12 +36,12 @@ def rows_equal(tag):
     print(tag, "impulse words differing:", bad_i, "prestep words differing:", bad_p, flush=True)
 for frame in range(4):
     if frame > 0:
-        new_h = _narrow_phase_like_update(host, feat_h, rng_h)
+        new_h = narrow_phase_like_update(host, feat_h, rng_h)
         for tb in host.type_batches():
             key = (tb.batch_index, tb.type_batch_index)
             ob.update_contact_impulses(tb, feat_h[key], new_h[key])
         feat_h = new_h
-        new_d = _narrow_phase_like_update(dev, feat_d, rng_d)
+        new_d = narrow_phase_like_update(dev, feat_d, rng_d)
         print("new ids equal:", all(np.array_equal(new_h[k], new_d[k]) for k in new_h))
         ts.upload_body_motion()
         ts.update_contacts(new_d)

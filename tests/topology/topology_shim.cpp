@@ -1,5 +1,6 @@
-// Test shim for tests/test_topology.py: plan_topology, build_stage_program, resolve_stage_launch and same_launches of bepuphysics2_b200/csrc/bepu_topology.h
-// behind a ctypes-friendly C interface. Built with g++ together with bepu_topology.cpp; the product never loads it.
+// Test shim of the planner tests (loaded by tests/planner.py): plan_topology (plain and per rank), its inverse slot map, build_stage_program,
+// exchange_targets, resolve_stage_launch, same_launches and integrated_warm_start_launch of bepuphysics2_b200/csrc/bepu_topology.h behind a
+// ctypes-friendly C interface. Built with g++ together with bepu_topology.cpp; the product never loads it.
 #include <cstring>
 
 #include "bepu_topology.h"
@@ -14,12 +15,14 @@ struct PlanHandle {
 
 extern "C" {
 
-// meta: per source (batch_index, type_batch_index, type_id, count); refs[i]: its host references (AOSOA-W) or null
-void* topology_plan(int n, const int32_t* meta, const int32_t* const* refs, int W, int fallback_threshold, int batch_count, int body_count, int peer_mode) {
+// meta: per source (batch_index, type_batch_index, type_id, count); refs[i]: its host references (AOSOA-W) or null. In peer mode the plan is
+// `rank`'s, with `fallback_rank` the rank that owns the fallback batch (-1 = none).
+void* topology_plan(int n, const int32_t* meta, const int32_t* const* refs, int W, int fallback_threshold, int batch_count, int body_count, int peer_mode,
+                    int rank, int fallback_rank) {
     std::vector<SourceView> sources;
     for (int i = 0; i < n; ++i) sources.push_back({meta[4 * i], meta[4 * i + 1], meta[4 * i + 2], meta[4 * i + 3], refs[i]});
     PlanHandle* h = new PlanHandle;
-    h->rc = plan_topology(sources, W, fallback_threshold, batch_count, body_count, peer_mode != 0, &h->plan, &h->error);
+    h->rc = plan_topology(sources, W, fallback_threshold, batch_count, body_count, peer_mode != 0, &h->plan, &h->error, rank, fallback_rank);
     return h;
 }
 int topology_plan_error(void* h, char* message, int capacity) {
@@ -67,6 +70,17 @@ void topology_plan_source_live(void* h, int32_t* out) {
     const TopologyPlan& p = ((PlanHandle*)h)->plan;
     if (!p.source_live.empty()) std::memcpy(out, p.source_live.data(), p.source_live.size() * 4);
 }
+int64_t topology_plan_inverse_size(void* h) { return (int64_t)((PlanHandle*)h)->plan.inverse.size(); }
+// per source: its device type batch (synchronized) and its first inverse entry (fallback); per entry: device type batch, slot
+void topology_plan_inverse(void* h, int32_t* source_type_batch, int64_t* source_inverse_offset, int32_t* inverse) {
+    const TopologyPlan& p = ((PlanHandle*)h)->plan;
+    std::memcpy(source_type_batch, p.source_type_batch.data(), p.source_type_batch.size() * 4);
+    std::memcpy(source_inverse_offset, p.source_inverse_offset.data(), p.source_inverse_offset.size() * 8);
+    for (size_t i = 0; i < p.inverse.size(); ++i) {
+        inverse[2 * i] = p.inverse[i].type_batch;
+        inverse[2 * i + 1] = p.inverse[i].slot;
+    }
+}
 void topology_plan_free(void* h) { delete (PlanHandle*)h; }
 
 void* topology_program(void* plan, int substeps, const int32_t* iterations, int kinematic_count, int integrate_velocity_for_kinematics, int peer_mode, int body_count) {
@@ -89,6 +103,20 @@ void topology_program_ops(void* h, int64_t* out) {
 }
 void topology_program_free(void* h) { delete (StageProgram*)h; }
 
+// exchange_targets of the peer-mode program of `plan` with per-device-batch boundary counts; out: kShardMaxExchanges cumulative targets
+int topology_exchange_targets(void* plan, int substeps, const int32_t* iterations, int kinematic_count, int integrate_velocity_for_kinematics, int body_count,
+                              const int32_t* boundary_count, unsigned long long* out) {
+    const TopologyPlan& p = ((PlanHandle*)plan)->plan;
+    const StageProgram prog = build_stage_program(p, std::vector<int32_t>(iterations, iterations + substeps), kinematic_count, integrate_velocity_for_kinematics != 0, true,
+                                                  body_count);
+    std::vector<unsigned long long> targets;
+    std::string error;
+    const int rc = exchange_targets(prog, std::vector<int32_t>(boundary_count, boundary_count + p.batches.size()), &targets, &error);
+    if (rc == 0) std::memcpy(out, targets.data(), targets.size() * sizeof(unsigned long long));
+    return rc;
+}
+int topology_max_exchanges() { return kShardMaxExchanges; }
+
 // ops: n rows of topology_program_ops; out[i] = kernel, flags of op i
 void topology_resolve(const int64_t* ops, int n, int integrator_extensions, int angular_mode, int profile, int32_t* out) {
     const LaunchContext lc{integrator_extensions != 0, angular_mode, profile != 0};
@@ -103,5 +131,7 @@ int topology_same_launches(int extensions_a, int angular_mode_a, int profile_a, 
     return same_launches(LaunchContext{extensions_a != 0, angular_mode_a, profile_a != 0}, LaunchContext{extensions_b != 0, angular_mode_b, profile_b != 0});
 }
 int topology_deep_batch_bundles() { return kDeepBatchBundles; }
+// which contact-only WarmStart instantiation launch_stage (csrc/bepu_solver_kernels.cu) runs for a resolved launch: 1 = the integrated one
+int topology_integrated_warm_start_launch(int stage, int kernel, int flags) { return integrated_warm_start_launch(stage, StageLaunch{kernel, flags}) ? 1 : 0; }
 
 }  // extern "C"
