@@ -139,8 +139,7 @@ __global__ void transpose_out_all_kernel(const DeviceTypeBatch* __restrict__ tbs
 
 // bepucuda_read_constraints: one warp per request. Lane l gathers words l and l + 32 of the request's record from the rows of its slot, so the
 // warp stores the 256-B record as two coalesced 128-B rows; the only rows read are those of the requested constraints.
-// Record words (include/bepucuda.h): 0 type id, 1 live, 2-5 body references, 6-17 accumulated impulses, 18-52 prestep, 53-63 zero.
-constexpr int kRecordRefs = 2, kRecordImpulses = 6, kRecordPrestep = 18, kRecordEnd = 53;
+// Record words: kRecord* (bepu_layout_kernels.h).
 __global__ void read_constraints_kernel(const DeviceTypeBatch* __restrict__ tbs, const TransposeDesc* __restrict__ descs, const DeviceSlot* __restrict__ inverse,
                                         const ReadRequest* __restrict__ requests, int count, int32_t* __restrict__ records) {
     const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
@@ -171,6 +170,18 @@ __global__ void read_constraints_kernel(const DeviceTypeBatch* __restrict__ tbs,
     int32_t* record = records + (size_t)warp * 64;
     record[lane] = out[0];
     record[lane + 32] = out[1];
+}
+
+// bepucuda_write_constraints: one warp per queued write; lane r writes prestep rows r and r + 32 of the write's slot. Only the written constraints'
+// prestep rows are touched: their accumulated impulses and body references stay as they are.
+__global__ void write_constraints_kernel(const DeviceTypeBatch* __restrict__ tbs, const TransposeDesc* __restrict__ descs, const PrestepWrite* __restrict__ writes,
+                                         const float* __restrict__ rows, int count) {
+    const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+    if (warp >= count) return;
+    const PrestepWrite q = writes[warp];
+    const int n = descs[q.at.type_batch].prestep_rows;
+    float* dst = SLOT_ROW0(tbs[q.at.type_batch].prestep, n, q.at.slot >> 5, q.at.slot & 31);
+    for (int r = lane; r < n; r += 32) dst[r * 32] = rows[q.row0 + r];
 }
 
 // Pass 1 over every (constraint, body slot): first_batch[body] = min device batch referencing it as a dynamic body;
@@ -309,6 +320,10 @@ void launch_read_constraints(const DeviceTypeBatch* tbs, const TransposeDesc* de
                              cudaStream_t s) {
     if (count <= 0) return;
     read_constraints_kernel<<<blocks_for((size_t)count * 32, 128), 128, 0, s>>>(tbs, descs, inverse, requests, count, records);
+}
+void launch_write_constraints(const DeviceTypeBatch* tbs, const TransposeDesc* descs, const PrestepWrite* writes, const float* rows, int count, cudaStream_t s) {
+    if (count <= 0) return;
+    write_constraints_kernel<<<blocks_for((size_t)count * 32, 128), 128, 0, s>>>(tbs, descs, writes, rows, count);
 }
 void launch_redistribute_impulses(const DeviceTypeBatch* tbs, const TransposeDesc* descs, const WorkItem* work, int work_count, cudaStream_t s) {
     if (work_count <= 0) return;

@@ -38,6 +38,17 @@ struct ReadRequest {
 // bepucuda_read_constraints: the 64-word record of every request (include/bepucuda.h), read from the AOSOA-32 rows, into records[count][64].
 void launch_read_constraints(const DeviceTypeBatch* tbs, const TransposeDesc* descs, const DeviceSlot* inverse, const ReadRequest* requests, int count, int32_t* records,
                              cudaStream_t s);
+// Words of the 64-word record of bepucuda_read_constraints / bepucuda_write_constraints (include/bepucuda.h): 0 type id, 1 live, 2-5 body references,
+// 6-17 accumulated impulses, 18-52 prestep (as many rows as the largest type has), 53-63 zero.
+constexpr int kRecordRefs = 2, kRecordImpulses = 6, kRecordPrestep = 18, kRecordEnd = 53;
+constexpr int kRecordPrestepWords = kRecordEnd - kRecordPrestep;
+// One queued write of bepucuda_write_constraints: the constraint at `at` takes the prestep rows rows[row0 .. row0 + its type's prestep_rows).
+struct PrestepWrite {
+    DeviceSlot at;
+    int32_t row0;
+};
+// bepucuda_write_constraints: the prestep rows of every write into the AOSOA-32 rows of its slot (impulses and body references untouched).
+void launch_write_constraints(const DeviceTypeBatch* tbs, const TransposeDesc* descs, const PrestepWrite* writes, const float* rows, int count, cudaStream_t s);
 void launch_fill_i32(int32_t* p, size_t n, int32_t v, cudaStream_t s);
 // RedistributeImpulses (NarrowPhaseConstraintUpdate.cs:L81-135) for every device type batch whose descriptor has kDescRedistribute, on the AOSOA-32 impulses.
 void launch_redistribute_impulses(const DeviceTypeBatch* tbs, const TransposeDesc* descs, const WorkItem* work, int work_count, cudaStream_t s);

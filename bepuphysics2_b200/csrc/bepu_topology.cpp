@@ -80,6 +80,13 @@ int plan_topology(const std::vector<SourceView>& sources, int W, int fallback_th
     p.source_bundle_base.assign(sources.size(), 0);
     p.source_type_batch.assign(sources.size(), -1);
     p.source_inverse_offset.assign(sources.size(), -1);
+    p.source_count.assign(sources.size(), 0);
+    p.location_source.assign((size_t)std::max(batch_count, 0) * 64, -1);
+    for (size_t i = sources.size(); i-- > 0;) {  // the first type batch of a (batch, type id) answers for it
+        const SourceView& s = sources[i];
+        p.source_count[i] = s.count;
+        if (s.batch_index >= 0 && s.batch_index < batch_count && s.type_id >= 0 && s.type_id < 64) p.location_source[(size_t)s.batch_index * 64 + (size_t)s.type_id] = (int32_t)i;
+    }
     for (int si : order) {
         p.source_bundle_base[(size_t)si] = p.source_bundles;
         p.source_bundles += (sources[(size_t)si].count + W - 1) / W;
@@ -234,6 +241,51 @@ int plan_topology(const std::vector<SourceView>& sources, int W, int fallback_th
         if (get_type_info(p.tbs[tb].type_id)->contacts > 0) add_bundles((int)tb);
     p.inc_count = (int)p.work.size() - p.inc_begin;
     return BEPUCUDA_OK;
+}
+
+int resolve_location(const TopologyPlan& plan, const bepucuda_constraint_location& l, ResolvedLocation* out) {
+    const size_t key = (size_t)l.batch_index * 64 + (size_t)l.type_id;
+    const int32_t s = l.set_index == 0 && l.batch_index >= 0 && l.type_id >= 0 && l.type_id < 64 && key < plan.location_source.size() ? plan.location_source[key] : -1;
+    if (s < 0 || l.index_in_type_batch < 0 || l.index_in_type_batch >= plan.source_count[(size_t)s]) return BEPUCUDA_ERR_INVALID_ARGUMENT;
+    out->source = s;
+    const int32_t tb = plan.source_type_batch[(size_t)s];
+    if (tb >= 0) {
+        out->at = {tb, l.index_in_type_batch};
+        out->inverse_entry = -1;
+    } else {
+        out->inverse_entry = plan.source_inverse_offset[(size_t)s] + l.index_in_type_batch;
+        out->at = plan.inverse[(size_t)out->inverse_entry];
+    }
+    return BEPUCUDA_OK;
+}
+
+void PrestepWriteQueue::plan(const TopologyPlan& p) {
+    writes.clear();
+    rows.clear();
+    entry_of_slot_.clear();
+    slot_base_.resize(p.tbs.size());
+    slots_ = 0;
+    for (size_t i = 0; i < p.tbs.size(); ++i) {
+        slot_base_[i] = slots_;
+        slots_ += (int64_t)p.tbs[i].bundle_count * 32;
+    }
+}
+
+void PrestepWriteQueue::put(DeviceSlot at, const float* r, int count) {
+    if (entry_of_slot_.empty()) entry_of_slot_.assign((size_t)slots_, -1);
+    int32_t& entry = entry_of_slot_[(size_t)(slot_base_[(size_t)at.type_batch] + at.slot)];
+    if (entry < 0) {
+        entry = (int32_t)writes.size();
+        writes.push_back({at, (int32_t)rows.size()});
+        rows.resize(rows.size() + (size_t)count);
+    }
+    std::memcpy(rows.data() + writes[(size_t)entry].row0, r, (size_t)count * sizeof(float));
+}
+
+void PrestepWriteQueue::clear() {
+    for (const PrestepWrite& w : writes) entry_of_slot_[(size_t)(slot_base_[(size_t)w.at.type_batch] + w.at.slot)] = -1;
+    writes.clear();
+    rows.clear();
 }
 
 std::vector<WorkRecord> work_records(const TopologyPlan& plan, int32_t* refs, float* prestep, float* impulses) {

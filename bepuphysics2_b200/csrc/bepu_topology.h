@@ -6,6 +6,7 @@
 #include <string>
 #include <vector>
 
+#include "../../include/bepucuda.h"
 #include "bepu_layout_kernels.h"
 
 namespace bepucuda {
@@ -43,6 +44,8 @@ struct TopologyPlan {
     std::vector<int32_t> source_type_batch;      // per source: its device type batch if synchronized, else -1
     std::vector<int64_t> source_inverse_offset;  // per source: the first of its `count` entries in `inverse` if fallback, else -1
     std::vector<DeviceSlot> inverse;             // per fallback source constraint: the slot that maps to it, {-1, -1} for a hole
+    std::vector<int32_t> source_count;           // per source: its ConstraintCount, holes of a fallback source included
+    std::vector<int32_t> location_source;        // per host batch index * 64 + type id: the source of that type batch, -1 = none
     std::vector<WorkItem> work;               // grouped by device batch, then the incremental list
     std::vector<int32_t> bundle_live;         // live constraints per work item (parallel to `work`)
     struct Batch { int32_t begin, count, contacts_only; };
@@ -65,6 +68,35 @@ struct TopologyPlan {
 // for a fallback body reference out of range, BEPUCUDA_ERR_BATCH_INVARIANT for a fallback bundle that holds a dynamic body twice.
 int plan_topology(const std::vector<SourceView>& sources, int W, int fallback_threshold, int batch_count, int body_count, bool peer_mode, TopologyPlan* plan,
                   std::string* error, int rank = 0, int fallback_rank = -1);
+
+// A host location (bepucuda_constraint_location, Solver.HandleToConstraint) resolved against a plan.
+struct ResolvedLocation {
+    int32_t source;         // index into the planned sources
+    DeviceSlot at;          // the device slot of the constraint; {-1, -1} for a hole of the sequential fallback batch
+    int64_t inverse_entry;  // a fallback source's constraint: its entry in TopologyPlan::inverse; -1 for a synchronized source
+};
+// The one resolution of bepucuda_read_constraints and bepucuda_write_constraints: the source by (batch, type id), then the identity slot of a
+// synchronized type batch or the inverse map of the fallback levels. BEPUCUDA_ERR_INVALID_ARGUMENT (out untouched) when the location names no
+// constraint of the active set: set_index != 0, a batch out of range, a type id without a type batch in that batch, or an index outside
+// [0, ConstraintCount).
+int resolve_location(const TopologyPlan& plan, const bepucuda_constraint_location& location, ResolvedLocation* out);
+
+// The prestep writes of bepucuda_write_constraints waiting for the next solve, one per device slot: a later write to a slot replaces the earlier
+// one, in place, so the queue holds each written constraint once, in the order the slots were first written.
+struct PrestepWriteQueue {
+    std::vector<PrestepWrite> writes;
+    std::vector<float> rows;              // the prestep rows of every write, back to back (PrestepWrite::row0)
+    // Takes the device type batches of a new plan (bepucuda_end_constraints) and drops every write.
+    void plan(const TopologyPlan& p);
+    // rows: the `count` prestep floats of the constraint at `at`, a slot of the plan (count: its type's prestep_rows)
+    void put(DeviceSlot at, const float* rows, int count);
+    void clear();
+
+  private:
+    std::vector<int64_t> slot_base_;      // per device type batch: its first slot in entry_of_slot_
+    int64_t slots_ = 0;
+    std::vector<int32_t> entry_of_slot_;  // per device slot: its entry of `writes`, -1 = none (allocated by the first write of a plan)
+};
 
 // What the solver kernels read per work item, with the plan's offsets applied to the arena bases.
 std::vector<WorkRecord> work_records(const TopologyPlan& plan, int32_t* refs, float* prestep, float* impulses);

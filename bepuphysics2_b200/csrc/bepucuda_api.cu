@@ -181,6 +181,9 @@ struct bepucuda_ctx {
     DeviceBuffer color_refs, color_priorities, color_body_min, color_body_mask, color_out, color_lists, color_counts;  // bepucuda_color_constraints
     DeviceBuffer island_activities, island_label, island_blocked, island_count, island_flags, island_roots, island_counts, island_scalars, island_temp;  // bepucuda_find_sleepable_islands
     DeviceBuffer inverse_table, read_requests, read_records;  // bepucuda_read_constraints: the plan's inverse slot map, one call's requests and records
+    PrestepWriteQueue prestep_writes;  // bepucuda_write_constraints since the last solve, applied by refresh_device_rows
+    DeviceBuffer write_table, write_rows;
+    StagedUpload write_stage, write_rows_stage;
     std::vector<cudaEvent_t> profile_events;
 };
 
@@ -429,6 +432,12 @@ void compute_frame_params(bepucuda_ctx* ctx, float dt, FrameParams* fp) {
     for (int i = 0; i < 3; ++i) fp->attractor_center[i] = ctx->attractor_center[i];
 }
 
+// The error message of a location that resolve_location rejects (bepucuda_read_constraints / bepucuda_write_constraints).
+std::string no_constraint_at(int32_t i, const bepucuda_constraint_location& l) {
+    return "location " + std::to_string(i) + " (set " + std::to_string(l.set_index) + ", batch " + std::to_string(l.batch_index) + ", type " + std::to_string(l.type_id) +
+           ", index " + std::to_string(l.index_in_type_batch) + ") names no constraint of the active set";
+}
+
 // Accelerations set for another body count than the current one index the wrong bodies: solve, profile_stages and predict_bounding_boxes refuse
 // to run before any device work.
 int check_accelerations(bepucuda_ctx* ctx, const char* what) {
@@ -437,14 +446,15 @@ int check_accelerations(bepucuda_ctx* ctx, const char* what) {
     return BEPUCUDA_OK;
 }
 
-// Brings the device AOSOA-32 rows up to date with what the host queued since the last solve (bepucuda_update_type_batch / bepucuda_update_contacts):
-// flushes the batched copies, re-uploads the transposition descriptors when their pending rows, redistribution flags or feature ids changed,
-// transposes the pending rows only, and redistributes the resident penetration impulses of updated contact type batches from the old to the new
-// feature ids. A frame that refreshes every type batch in full (bepuhost_cuda_refresh) leaves the descriptors as end_constraints uploaded them.
+// Brings the device AOSOA-32 rows up to date with what the host queued since the last solve (bepucuda_update_type_batch / bepucuda_update_contacts /
+// bepucuda_write_constraints): flushes the batched copies, re-uploads the transposition descriptors when their pending rows, redistribution flags
+// or feature ids changed, transposes the pending rows only, redistributes the resident penetration impulses of updated contact type batches from
+// the old to the new feature ids, and then writes the queued prestep rows of single constraints, so that they win over a whole-type-batch upload
+// of the same frame. A frame that refreshes every type batch in full (bepuhost_cuda_refresh) leaves the descriptors as end_constraints uploaded them.
 int refresh_device_rows(bepucuda_ctx* ctx) {
     if (!ctx->data_dirty) return BEPUCUDA_OK;
     { int rc = flush_chunks(ctx, ctx->pending_h2d); if (rc != BEPUCUDA_OK) return rc; }
-    bool any_redistribute = false, descs_changed = false;
+    bool any_pending = false, any_redistribute = false, descs_changed = false;
     for (size_t tb = 0; tb < ctx->topo.tbs.size(); ++tb) {
         const SourceTypeBatch& s = ctx->sources[(size_t)ctx->topo.tbs[tb].source];
         TransposeDesc& d = ctx->tdescs[tb];
@@ -455,14 +465,28 @@ int refresh_device_rows(bepucuda_ctx* ctx) {
             d.features_new = s.raw_features_new;
             descs_changed = true;
         }
+        any_pending |= s.pending != 0;
         any_redistribute |= s.redistribute;
     }
     if (descs_changed)
         CK(cudaMemcpyAsync(ctx->tdesc_table.ptr, ctx->tdescs.data(), ctx->tdescs.size() * sizeof(TransposeDesc), cudaMemcpyHostToDevice, ctx->stream));
-    launch_transpose_in_all(ctx->tb_table.as<DeviceTypeBatch>(), ctx->tdesc_table.as<TransposeDesc>(), ctx->work_table.as<WorkItem>(), ctx->topo.all_work_count, ctx->W,
-                            kTransposePrestep | kTransposeImpulses | kTransposePending, ctx->stream);
+    if (any_pending)  // a frame whose only change is a constraint write (or a feature-id upload) transposes nothing
+        launch_transpose_in_all(ctx->tb_table.as<DeviceTypeBatch>(), ctx->tdesc_table.as<TransposeDesc>(), ctx->work_table.as<WorkItem>(), ctx->topo.all_work_count, ctx->W,
+                                kTransposePrestep | kTransposeImpulses | kTransposePending, ctx->stream);
     if (any_redistribute)
         launch_redistribute_impulses(ctx->tb_table.as<DeviceTypeBatch>(), ctx->tdesc_table.as<TransposeDesc>(), ctx->work_table.as<WorkItem>(), ctx->topo.all_work_count, ctx->stream);
+    PrestepWriteQueue& q = ctx->prestep_writes;
+    if (!q.writes.empty()) {
+        const size_t bytes = q.writes.size() * sizeof(PrestepWrite), row_bytes = q.rows.size() * sizeof(float);
+        CK(ctx->write_table.reserve(bytes));
+        CK(ctx->write_rows.reserve(row_bytes));
+        { int rc = upload_staged(ctx, ctx->write_stage, ctx->write_table.ptr, q.writes.data(), bytes); if (rc != BEPUCUDA_OK) return rc; }
+        { int rc = upload_staged(ctx, ctx->write_rows_stage, ctx->write_rows.ptr, q.rows.data(), row_bytes); if (rc != BEPUCUDA_OK) return rc; }
+        ctx->h2d_accum += (int64_t)(bytes + row_bytes);
+        launch_write_constraints(ctx->tb_table.as<DeviceTypeBatch>(), ctx->tdesc_table.as<TransposeDesc>(), ctx->write_table.as<PrestepWrite>(), ctx->write_rows.as<float>(),
+                                 (int)q.writes.size(), ctx->stream);
+        q.clear();
+    }
     for (SourceTypeBatch& s : ctx->sources) {
         if (s.redistribute) std::swap(s.raw_features_old, s.raw_features_new);  // the resident impulses now belong to the new ids
         s.redistribute = false;
@@ -687,6 +711,7 @@ int32_t bepucuda_begin_constraints(bepucuda_ctx* ctx, int32_t source_bundle_widt
     ctx->batch_count = batch_count;
     ctx->sources.clear();
     ctx->pending_h2d.clear();  // queued refreshes target raw-arena addresses that are recycled below; a re-describe uploads everything anyway
+    ctx->prestep_writes.clear();  // slots of the old plan; the describe uploads the host's prestep, which ApplyDescription already wrote
     ctx->raw_arena.reset();
     ctx->pinned_arena.reset();
     ctx->constraints_open = true;
@@ -749,6 +774,7 @@ int32_t bepucuda_end_constraints(bepucuda_ctx* ctx) {
         const int rc = plan_topology(views, W, ctx->fallback_threshold, ctx->batch_count, ctx->body_count, ctx->peer_mode, &plan, &error, ctx->peers.rank, ctx->fallback_rank);
         if (rc != BEPUCUDA_OK) return fail(ctx, rc, error);
         ctx->topo = std::move(plan);
+        ctx->prestep_writes.plan(ctx->topo);
     }
     const TopologyPlan& topo = ctx->topo;
 
@@ -1077,22 +1103,16 @@ int32_t bepucuda_read_constraints(bepucuda_ctx* ctx, int32_t count, const bepucu
     if (!ctx->constraints_ready) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, "read_constraints before end_constraints");
     if (count < 0 || (count > 0 && (!locations || !records_out))) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "read_constraints: bad arguments");
     if (count == 0) return BEPUCUDA_OK;
-    // (batch, type id) -> source; every location is checked before any device work, so a bad one leaves records_out untouched
-    std::vector<int32_t> source_of((size_t)ctx->batch_count * 64, -1);
-    for (size_t i = ctx->sources.size(); i-- > 0;) source_of[(size_t)ctx->sources[i].batch_index * 64 + (size_t)ctx->sources[i].type_id] = (int32_t)i;
+    // every location is checked before any device work, so a bad one leaves records_out untouched
     std::vector<ReadRequest> requests((size_t)count);
     for (int32_t i = 0; i < count; ++i) {
         const bepucuda_constraint_location& l = locations[i];
-        const int32_t s = l.set_index == 0 && l.batch_index >= 0 && l.batch_index < ctx->batch_count && l.type_id >= 0 && l.type_id < 64
-                              ? source_of[(size_t)l.batch_index * 64 + (size_t)l.type_id] : -1;
-        if (s < 0 || l.index_in_type_batch < 0 || l.index_in_type_batch >= ctx->sources[(size_t)s].count)
-            return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "read_constraints: location " + std::to_string(i) + " (set " + std::to_string(l.set_index) + ", batch " +
-                                                                std::to_string(l.batch_index) + ", type " + std::to_string(l.type_id) + ", index " +
-                                                                std::to_string(l.index_in_type_batch) + ") names no constraint of the active set");
+        ResolvedLocation r;
+        if (resolve_location(ctx->topo, l, &r) != BEPUCUDA_OK) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "read_constraints: " + no_constraint_at(i, l));
         ReadRequest& q = requests[(size_t)i];
         q.type_id = l.type_id;
-        q.at.type_batch = ctx->topo.source_type_batch[(size_t)s];
-        q.at.slot = q.at.type_batch >= 0 ? l.index_in_type_batch : (int32_t)(ctx->topo.source_inverse_offset[(size_t)s] + l.index_in_type_batch);
+        // a fallback constraint, a hole included, is looked up on the device through its inverse entry
+        q.at = r.inverse_entry < 0 ? r.at : DeviceSlot{-1, (int32_t)r.inverse_entry};
     }
     CK(cudaSetDevice(ctx->device));
     const size_t n = (size_t)count;
@@ -1104,6 +1124,32 @@ int32_t bepucuda_read_constraints(bepucuda_ctx* ctx, int32_t count, const bepucu
     CK(cudaGetLastError());
     CK(cudaMemcpyAsync(records_out, ctx->read_records.ptr, n * 256, cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
+    return BEPUCUDA_OK;
+}
+
+int32_t bepucuda_write_constraints(bepucuda_ctx* ctx, int32_t count, const bepucuda_constraint_location* locations, const int32_t* records) {
+    if (!ctx) return BEPUCUDA_ERR_INVALID_ARGUMENT;
+    if (ctx->peer_mode) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, "write_constraints in peer mode: a rank holds its constraints compacted, so host locations do not address them");
+    if (!ctx->constraints_ready) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, "write_constraints before end_constraints");
+    if (count < 0 || (count > 0 && (!locations || !records))) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "write_constraints: bad arguments");
+    if (count == 0) return BEPUCUDA_OK;
+    // every location and record is checked before anything is queued, so a failing call changes nothing
+    std::vector<DeviceSlot> slots((size_t)count);
+    for (int32_t i = 0; i < count; ++i) {
+        const bepucuda_constraint_location& l = locations[i];
+        ResolvedLocation r;
+        if (resolve_location(ctx->topo, l, &r) != BEPUCUDA_OK) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "write_constraints: " + no_constraint_at(i, l));
+        if (r.at.type_batch < 0) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "write_constraints: " + no_constraint_at(i, l) + " (a hole of the fallback batch)");
+        if (records[(size_t)i * 64] != l.type_id)
+            return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "write_constraints: record " + std::to_string(i) + " has type id " + std::to_string(records[(size_t)i * 64]) +
+                                                                ", its location type id " + std::to_string(l.type_id));
+        slots[(size_t)i] = r.at;
+    }
+    CK(cudaSetDevice(ctx->device));
+    open_upload_window(ctx);
+    for (int32_t i = 0; i < count; ++i)
+        ctx->prestep_writes.put(slots[(size_t)i], (const float*)(records + (size_t)i * 64 + kRecordPrestep), get_type_info(locations[i].type_id)->prestep_rows);
+    ctx->data_dirty = true;
     return BEPUCUDA_OK;
 }
 

@@ -116,6 +116,7 @@ C_ABI_SYMBOLS = [
     "bepucuda_shard_set_fallback_rank",
     "bepucuda_color_constraints", "bepucuda_color_hash", "bepucuda_set_body_shapes", "bepucuda_predict_bounding_boxes",
     "bepucuda_set_body_accelerations", "bepucuda_set_point_gravity", "bepucuda_find_sleepable_islands", "bepucuda_read_constraints",
+    "bepucuda_write_constraints",
 ]
 
 
@@ -183,6 +184,7 @@ def load_libraries():
     cuda.bepucuda_set_point_gravity.argtypes = [vp, i32, vp, f32]
     cuda.bepucuda_find_sleepable_islands.argtypes = [vp, vp, i32, vp, vp, vp, C.POINTER(i32), C.POINTER(i32)]
     cuda.bepucuda_read_constraints.argtypes = [vp, i32, vp, vp]
+    cuda.bepucuda_write_constraints.argtypes = [vp, i32, vp, vp]
 
     host.bepuhost_create.restype = vp
     host.bepuhost_create.argtypes = [i32, i32]
@@ -457,19 +459,33 @@ class CudaTimestepper:
                                                                C.byref(count), C.byref(rounds)))
         return labels[:n], roots[:count.value].copy(), counts[:count.value].copy(), rounds.value
 
+    @staticmethod
+    def _locations(locations):
+        """int32[n, 4] bepucuda_constraint_location rows from int32[n, 3] (batch index, type id, index in the type batch) or int32[n, 4]."""
+        loc = np.asarray(locations, dtype=np.int32)
+        if loc.ndim == 2 and loc.shape[1] == 3:
+            loc = np.concatenate([np.zeros((loc.shape[0], 1), dtype=np.int32), loc], axis=1)
+        return np.ascontiguousarray(loc.reshape(-1, 4))
+
     def read_constraints(self, locations, out=None):
         """bepucuda_read_constraints: int32[n, 64] records of the listed constraints from the device rows (include/bepucuda.h: type id, live,
         body references, accumulated impulses, prestep). locations: int32[n, 3] (batch index, type id, index in the type batch) in the active set,
         or int32[n, 4] with the set index first, the layout of bepucuda_constraint_location. out: a C-contiguous int32 array of at least n x 64
         to write the records into (e.g. one kept registered across frames); a new array otherwise."""
-        loc = np.asarray(locations, dtype=np.int32)
-        if loc.ndim == 2 and loc.shape[1] == 3:
-            loc = np.concatenate([np.zeros((loc.shape[0], 1), dtype=np.int32), loc], axis=1)
-        loc = np.ascontiguousarray(loc.reshape(-1, 4))
+        loc = self._locations(locations)
         records = np.zeros((max(loc.shape[0], 1), 64), dtype=np.int32) if out is None else out.reshape(-1, 64)
         assert records.dtype == np.int32 and records.flags["C_CONTIGUOUS"] and records.shape[0] >= loc.shape[0]
         self._check(self._cuda.bepucuda_read_constraints(self._ctx, loc.shape[0], loc.ctypes.data, records.ctypes.data))
         return records[:loc.shape[0]]
+
+    def write_constraints(self, locations, records):
+        """bepucuda_write_constraints: queues the prestep rows (words 18 on) of int32[n, 64] records, in the layout read_constraints returns, for
+        the listed constraints; the next solve writes them into the device rows and leaves the accumulated impulses alone (Solver.ApplyDescription
+        on the resident path). Word 0 of each record must be its location's type id. locations: as for read_constraints."""
+        loc = self._locations(locations)
+        rec = np.ascontiguousarray(records, dtype=np.int32).reshape(-1, 64)
+        assert rec.shape[0] == loc.shape[0]
+        self._check(self._cuda.bepucuda_write_constraints(self._ctx, loc.shape[0], loc.ctypes.data, rec.ctypes.data))
 
     def register_host_buffers(self):
         """Page-locks the simulation's buffers (a C# host would register its BufferPool blocks once)."""

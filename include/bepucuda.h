@@ -235,6 +235,30 @@ typedef struct bepucuda_constraint_location {
 } bepucuda_constraint_location;
 int32_t bepucuda_read_constraints(bepucuda_ctx* ctx, int32_t count, const bepucuda_constraint_location* locations, int32_t* records_out);
 
+/* Write the prestep rows of listed constraints straight into the device rows, leaving their accumulated impulses as they are. Replaces
+ * Solver.ApplyDescriptionWithoutWaking(ConstraintReference, description) (Solver.cs:L1149-1180) against the device rows on the resident path, where
+ * bepucuda_update_type_batch would also send the host's stale accumulated impulses of the whole type batch: the host calls Solver.ApplyDescription
+ * on its own buffers as before (waking stays with the host; the device holds the active set only), then forwards the changed lanes here.
+ *   locations: as for bepucuda_read_constraints (Solver.HandleToConstraint[handle]), resolved against the type batches of the last
+ *   bepucuda_end_constraints.
+ *   records: count records of 64 int32 in the layout bepucuda_read_constraints returns, so a record read, patched and written back works as is.
+ *   Word 0 must equal the location's type id; words 18 .. 18 + P - 1 are applied, P = prestep_floats of the type (bepucuda_type_info), the
+ *   <Type>PrestepData rows in the reference's order. Every other word is ignored: no body reference and no accumulated impulse is written, as
+ *   ApplyDescription writes neither. The caller's buffers are free when the call returns.
+ * Writes are queued and applied by the next bepucuda_solve / bepucuda_profile_stages, after that frame's whole-type-batch rows
+ * (bepucuda_update_type_batch, bepucuda_update_contacts) are transposed in and the impulses redistributed: a write wins over a whole-type-batch upload
+ * of the same frame, whichever was called first. Several writes to one constraint before a solve, in one call or across calls, resolve to the last.
+ * Until that solve a write is pending: bepucuda_read_constraints and bepucuda_download_prestep do not see it. bepucuda_begin_constraints drops the
+ * pending writes (the describe uploads the host's buffers, which already hold what ApplyDescription wrote). Writing a contact's prestep sets its
+ * depths to the written values, as the reference's ApplyDescription does.
+ * The solve uploads 12 B per distinct constraint written plus its P prestep floats (bepucuda_timings h2d_bytes), inside the upload window
+ * (upload_ms); a write does not re-capture the graph.
+ * BEPUCUDA_ERR_BAD_STATE before the first bepucuda_end_constraints, between begin and end, and in peer mode. BEPUCUDA_ERR_INVALID_ARGUMENT for every
+ * location bepucuda_read_constraints rejects, a location that names a hole of the sequential fallback batch, a word 0 other than the location's
+ * type id, a NULL pointer with count > 0, and count < 0. All are checked before anything is queued, and a failing call queues nothing. count == 0
+ * is OK and changes nothing. */
+int32_t bepucuda_write_constraints(bepucuda_ctx* ctx, int32_t count, const bepucuda_constraint_location* locations, const int32_t* records);
+
 int32_t bepucuda_get_timings(bepucuda_ctx* ctx, bepucuda_timings* out);
 
 /* Replaces SimulationProfiler.Start/End (SimulationProfiler.cs:L25-60): CUDA events on the context stream, 16 slots. */

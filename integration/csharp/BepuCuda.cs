@@ -70,6 +70,9 @@ namespace BepuCuda
         [DllImport(Lib)] public static extern int bepucuda_download_prestep(IntPtr ctx, int batchIndex, int typeBatchIndex, float* prestepOut);
         /// <summary>Records of 64 ints (type id, live, body references, accumulated impulses, prestep) of the listed constraints, read from the device rows.</summary>
         [DllImport(Lib)] public static extern int bepucuda_read_constraints(IntPtr ctx, int count, CudaConstraintLocation* locations, int* recordsOut);
+        /// <summary>Queues the prestep rows (words 18 on) of records in the read layout for the listed constraints; the next solve writes them into the
+        /// device rows and keeps their accumulated impulses (Solver.ApplyDescription on the resident path).</summary>
+        [DllImport(Lib)] public static extern int bepucuda_write_constraints(IntPtr ctx, int count, CudaConstraintLocation* locations, int* records);
         [DllImport(Lib)] public static extern int bepucuda_get_timings(IntPtr ctx, Timings* timings);
         [DllImport(Lib)] public static extern int bepucuda_event_record(IntPtr ctx, int slot);
         [DllImport(Lib)] public static extern int bepucuda_event_elapsed_ms(IntPtr ctx, int slotBegin, int slotEnd, float* ms);
