@@ -538,4 +538,11 @@ BEPU_CONTACT_LOOP
     }
 };
 
+// BatchTypeId -> contact type (Contact/ContactConvexTypes.cs, ContactNonconvexTypes.cs)
+#define BEPU_CONTACT_TYPES(X)                                                                                                     \
+    X(0, ConvexOneBody<1>) X(1, ConvexOneBody<2>) X(2, ConvexOneBody<3>) X(3, ConvexOneBody<4>)                                   \
+    X(4, ConvexTwoBody<1>) X(5, ConvexTwoBody<2>) X(6, ConvexTwoBody<3>) X(7, ConvexTwoBody<4>)                                   \
+    X(8, NonconvexOneBody<2>) X(9, NonconvexOneBody<3>) X(10, NonconvexOneBody<4>)                                                \
+    X(15, NonconvexTwoBody<2>) X(16, NonconvexTwoBody<3>) X(17, NonconvexTwoBody<4>)
+
 }  // namespace BEPU_NS

@@ -8,6 +8,7 @@
 // error differs between CPU vendors; the portable definition the reference carries for other targets (1/v, 1/sqrt(v)) is what is used here.
 #pragma once
 #include "bepu_joints.cuh"
+#include "bepu_type_table.h"
 
 namespace BEPU_NS {
 
@@ -961,5 +962,20 @@ struct VolumeConstraint {
     X(35, CenterDistanceConstraint) X(36, AreaConstraint) X(37, PointOnLineServo) X(38, LinearAxisServo) X(39, LinearAxisMotor) X(40, LinearAxisLimit) \
     X(41, AngularAxisMotor) X(42, OneBodyAngularServo) X(43, OneBodyAngularMotor) X(44, OneBodyLinearServo) X(45, OneBodyLinearMotor)                  \
     X(52, BallSocketMotor) X(53, BallSocketServo) X(54, AngularAxisGearMotor) X(55, CenterDistanceLimit)
+
+// Every build of the device types holds them to the type table the planner sizes the arenas from: each listed struct has its id's bodies and
+// rows, and the lists name exactly the table's ids (a duplicate id in the lists is a duplicate case of the type switch).
+#define BEPU_CHECK_TYPE(ID, T)                                                                                                                       \
+    static_assert(bepucuda::type_row(ID) && bepucuda::type_row(ID)->bodies == T::kBodies && bepucuda::type_row(ID)->prestep_rows == T::kPrestepRows && \
+                      bepucuda::type_row(ID)->impulse_rows == T::kImpulseRows,                                                                       \
+                  "type " #ID " (" #T "): kBodies, kPrestepRows, kImpulseRows differ from its row of bepu_type_table.h");
+BEPU_CONTACT_TYPES(BEPU_CHECK_TYPE)
+BEPU_JOINT_TYPES(BEPU_CHECK_TYPE)
+BEPU_JOINT_TYPES_MORE(BEPU_CHECK_TYPE)
+#undef BEPU_CHECK_TYPE
+#define BEPU_COUNT_TYPE(ID, T) +1
+static_assert(0 BEPU_CONTACT_TYPES(BEPU_COUNT_TYPE) BEPU_JOINT_TYPES(BEPU_COUNT_TYPE) BEPU_JOINT_TYPES_MORE(BEPU_COUNT_TYPE) == bepucuda::kTypeCount,
+              "the device type lists and bepu_type_table.h name different type ids");
+#undef BEPU_COUNT_TYPE
 
 }  // namespace BEPU_NS

@@ -300,13 +300,6 @@ BEPU_DI WorkRecord load_record(const WorkRecord* r) {
     return w;
 }
 
-// Type registry: BatchTypeId constants of the reference (Contact/ContactConvexTypes.cs, ContactNonconvexTypes.cs, joint files).
-#define BEPU_CONTACT_TYPES(X)                                                                                                     \
-    X(0, ConvexOneBody<1>) X(1, ConvexOneBody<2>) X(2, ConvexOneBody<3>) X(3, ConvexOneBody<4>)                                   \
-    X(4, ConvexTwoBody<1>) X(5, ConvexTwoBody<2>) X(6, ConvexTwoBody<3>) X(7, ConvexTwoBody<4>)                                   \
-    X(8, NonconvexOneBody<2>) X(9, NonconvexOneBody<3>) X(10, NonconvexOneBody<4>)                                                \
-    X(15, NonconvexTwoBody<2>) X(16, NonconvexTwoBody<3>) X(17, NonconvexTwoBody<4>)
-
 // kContacts: the switch covers the contact types only (kKernelContacts, for device batches whose every bundle is a contact); it is about half the code of the full switch and fits a smaller register budget (bepu_solver_kernels.cu).
 template <int STAGE, bool kSharded, bool kExt, bool kContacts, class PR, class AR>
 BEPU_DI void run_bundle_rows(const WorkRecord& rec, int lane, PR p, AR a, uint32_t enc0, uint32_t enc1, const BodyBuffers& B, const FrameParams& fp, bool integrated,

@@ -3,62 +3,32 @@
 #include "bepu_topology.h"
 
 #include <algorithm>
+#include <array>
 #include <cstring>
 #include <numeric>
 
 #include "../../include/bepucuda.h"
+#include "bepu_type_table.h"
 
 namespace bepucuda {
 
 // ---- type registry -------------------------------------------------------------------------------------------------------
-// SURVEY.md §8d algorithmic bytes:
-//   solve       = 4 * (P + 2D + n + sum(R_i + W_i))        R/W from the type's Solve access filters
-//   warm start  = 4 * (P + D + n + sum(R'_i + W'_i))       (non-integrating lane, WarmStart filters)
-//   incremental = 4 * (P_read + contacts_written + n + 6n)
-// Filters (IBodyAccessFilter.cs:L38-126): pos 3, orientation 4, lin 3, ang 3, inertia tensor 6, mass 1.
-static TypeInfo make_contact(int bodies, int prestep, int impulses, int contacts, const char* name) {
-    TypeInfo t{};
-    t.bodies = bodies; t.prestep_rows = prestep; t.impulse_rows = impulses; t.contacts = contacts; t.name = name;
-    const int body_rw = 13 + 6;  // AccessNoPose: velocity 6 + inertia 7 read, velocity 6 written
-    t.solve_bytes = 4 * (prestep + 2 * impulses + bodies + bodies * body_rw);
-    t.warm_start_bytes = 4 * (prestep + impulses + bodies + bodies * body_rw);
-    t.incremental_bytes = 4 * (prestep + contacts + bodies + 6 * bodies);
-    return t;
-}
-static TypeInfo make_joint(int bodies, int prestep, int impulses, int solve_r, int solve_w, int ws_r, int ws_w, const char* name) {
-    TypeInfo t{};
-    t.bodies = bodies; t.prestep_rows = prestep; t.impulse_rows = impulses; t.contacts = 0; t.name = name;
-    t.solve_bytes = 4 * (prestep + 2 * impulses + bodies + solve_r + solve_w);
-    t.warm_start_bytes = 4 * (prestep + impulses + bodies + ws_r + ws_w);
-    t.incremental_bytes = 0;
-    return t;
-}
-struct Registry {
-    TypeInfo types[64];
-    bool present[64];
-    Registry() {
-        std::memset(present, 0, sizeof(present));
-        auto add = [&](int id, TypeInfo t) { types[id] = t; present[id] = true; };
-        add(0, make_contact(1, 11, 4, 1, "Contact1OneBody")); add(1, make_contact(1, 15, 5, 2, "Contact2OneBody"));
-        add(2, make_contact(1, 19, 6, 3, "Contact3OneBody")); add(3, make_contact(1, 23, 7, 4, "Contact4OneBody"));
-        add(4, make_contact(2, 14, 4, 1, "Contact1")); add(5, make_contact(2, 18, 5, 2, "Contact2"));
-        add(6, make_contact(2, 22, 6, 3, "Contact3")); add(7, make_contact(2, 26, 7, 4, "Contact4"));
-        add(8, make_contact(1, 18, 6, 2, "Contact2NonconvexOneBody")); add(9, make_contact(1, 25, 9, 3, "Contact3NonconvexOneBody"));
-        add(10, make_contact(1, 32, 12, 4, "Contact4NonconvexOneBody"));
-        add(15, make_contact(2, 21, 6, 2, "Contact2Nonconvex")); add(16, make_contact(2, 28, 9, 3, "Contact3Nonconvex"));
-        add(17, make_contact(2, 35, 12, 4, "Contact4Nonconvex"));
-#define BEPU_REGISTER_JOINTS
-#include "bepu_joint_registry.inc"
-#undef BEPU_REGISTER_JOINTS
-    }
-};
-static const Registry& registry() {
-    static Registry r;
-    return r;
-}
+// SURVEY.md §8d algorithmic bytes, from the rows of bepu_type_table.h (R / W: floats the access filters read / write, summed over the bodies):
+//   solve       = 4 * (P + 2D + n + R + W)
+//   warm start  = 4 * (P + D + n + R' + W')              (non-integrating lane, WarmStart filters)
+//   incremental = 4 * (P_read + contacts_written + n + 6n)  contacts only; joints have no incremental update
 const TypeInfo* get_type_info(int type_id) {
-    if (type_id < 0 || type_id >= 64 || !registry().present[type_id]) return nullptr;
-    return &registry().types[type_id];
+    static const std::array<TypeInfo, 64> types = [] {
+        std::array<TypeInfo, 64> t{};
+        for (const TypeRow& r : kTypeTable) {
+            const int32_t P = r.prestep_rows, D = r.impulse_rows, n = r.bodies;
+            t[(size_t)r.id] = {n, P, D, r.contacts, 4 * (P + 2 * D + n + r.solve_read + r.solve_written), 4 * (P + D + n + r.warm_start_read + r.warm_start_written),
+                               r.contacts > 0 ? 4 * (P + r.contacts + n + 6 * n) : 0, r.name};
+        }
+        return t;
+    }();
+    if (type_id < 0 || type_id >= 64 || !types[(size_t)type_id].name) return nullptr;
+    return &types[(size_t)type_id];
 }
 
 // ---- device batches and work list ----------------------------------------------------------------------------------------

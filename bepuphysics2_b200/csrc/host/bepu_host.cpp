@@ -16,6 +16,7 @@
 #include <vector>
 
 #include "../../../include/bepucuda.h"
+#include "../bepu_type_table.h"
 
 namespace {
 
@@ -432,12 +433,6 @@ int32_t bepuhost_cuda_refresh(void* simp, bepucuda_ctx* ctx) {
 // Per-frame refresh through the device-side contact update (bepucuda_update_contacts): body motion + new prestep + new contact feature ids; the
 // accumulated impulses stay on the device. `feature_pool` holds the ids of every CONTACT type batch back to back in (batch, type batch) order,
 // [constraint][contact] each (what a PairCache walk produces). set_only != 0: bepucuda_set_contact_features (the ids of the uploaded impulses).
-static int contact_count_of(int type_id) {
-    if (type_id >= 0 && type_id <= 7) return (type_id & 3) + 1;
-    if (type_id >= 8 && type_id <= 10) return type_id - 6;
-    if (type_id >= 15 && type_id <= 17) return type_id - 13;
-    return 0;
-}
 int32_t bepuhost_cuda_update_contacts(void* simp, bepucuda_ctx* ctx, const int32_t* feature_pool, int32_t set_only) {
     Simulation& sim = *(Simulation*)simp;
     int32_t rc;
@@ -446,7 +441,7 @@ int32_t bepuhost_cuda_update_contacts(void* simp, bepucuda_ctx* ctx, const int32
     for (int b = 0; b < (int)sim.batches.size(); ++b) {
         auto& tbs = sim.batches[b]->type_batches;
         for (int t = 0; t < (int)tbs.size(); ++t) {
-            const int n = contact_count_of(tbs[t]->type_id);
+            const int n = bepucuda::type_row(tbs[t]->type_id)->contacts;
             if (n == 0) continue;
             rc = set_only ? bepucuda_set_contact_features(ctx, b, t, feature_pool + at) : bepucuda_update_contacts(ctx, b, t, tbs[t]->prestep.data, feature_pool + at);
             if (rc != 0) return rc;

@@ -32,13 +32,6 @@ template <class T> static void call_incremental(float dt, const Velocity* v, flo
     }
 }
 
-// Same id -> type table as BEPU_CONTACT_TYPES in csrc/bepu_solver_kernels.cuh (the joint tables come from the joint headers themselves).
-#define DEVICE_ON_HOST_CONTACT_TYPES(X)                                                                                           \
-    X(0, ConvexOneBody<1>) X(1, ConvexOneBody<2>) X(2, ConvexOneBody<3>) X(3, ConvexOneBody<4>)                                   \
-    X(4, ConvexTwoBody<1>) X(5, ConvexTwoBody<2>) X(6, ConvexTwoBody<3>) X(7, ConvexTwoBody<4>)                                   \
-    X(8, NonconvexOneBody<2>) X(9, NonconvexOneBody<3>) X(10, NonconvexOneBody<4>)                                                \
-    X(15, NonconvexTwoBody<2>) X(16, NonconvexTwoBody<3>) X(17, NonconvexTwoBody<4>)
-
 template <class T> static int eval(int stage, const float* body_states, float dt, float* prestep, float* impulses, float* velocities) {
     constexpr int NB = T::kBodies;
     BodyState b[NB];
@@ -75,7 +68,7 @@ extern "C" int32_t device_on_host_eval_lane(int32_t type_id, int32_t stage, cons
     switch (type_id) {
 #define CASE(ID, T) \
     case ID: return eval<T>(stage, body_states, dt, prestep, impulses, velocities);
-        DEVICE_ON_HOST_CONTACT_TYPES(CASE)
+        BEPU_CONTACT_TYPES(CASE)
         BEPU_JOINT_TYPES(CASE)
         BEPU_JOINT_TYPES_MORE(CASE)
 #undef CASE
@@ -86,7 +79,7 @@ extern "C" int32_t device_on_host_type_info(int32_t type_id, int32_t* bodies, in
     switch (type_id) {
 #define CASE(ID, T) \
     case ID: *bodies = T::kBodies; *prestep_rows = T::kPrestepRows; *impulse_rows = T::kImpulseRows; *incremental = T::kIncremental ? 1 : 0; return 0;
-        DEVICE_ON_HOST_CONTACT_TYPES(CASE)
+        BEPU_CONTACT_TYPES(CASE)
         BEPU_JOINT_TYPES(CASE)
         BEPU_JOINT_TYPES_MORE(CASE)
 #undef CASE

@@ -68,8 +68,18 @@ def shim():
     dll.topology_resolve.argtypes = [vp, i32, i32, i32, i32, vp]
     dll.topology_same_launches.argtypes = [i32] * 6
     dll.topology_integrated_warm_start_launch.argtypes = [i32] * 3
+    dll.topology_type_info.restype = C.c_char_p
+    dll.topology_type_info.argtypes = [i32, vp]
     _SHIM = dll
     return dll
+
+
+def type_info(type_id):
+    """The planner's get_type_info of a type id and the access-filter float counts of its type table row, by name; None for an id without a type."""
+    out = np.zeros(11, dtype=np.int64)
+    name = shim().topology_type_info(type_id, out.ctypes.data)
+    fields = "bodies prestep_rows impulse_rows contacts solve_bytes warm_start_bytes incremental_bytes solve_read solve_written warm_start_read warm_start_written"
+    return None if name is None else dict(zip(fields.split(), out.tolist()), name=name.decode())
 
 
 class Plan:

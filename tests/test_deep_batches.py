@@ -23,9 +23,8 @@ DEEP_MINB = planner.source_int("bepu_solver_kernels.cu", r"^#define BEPU_DEEP_MI
 
 
 def registered_type_ids():
-    """The type ids the device registers: the contact types of bepu_topology.cpp and the joints of bepu_joint_registry.inc."""
-    ids = {int(t) for t in re.findall(r"add\((\d+), make_contact\(", planner.read_source("bepu_topology.cpp"))}
-    return ids | {int(t) for t in re.findall(r"^add\((\d+), make_joint\(", planner.read_source("bepu_joint_registry.inc"), re.M)}
+    """The type ids the device registers: those of the type table, as the planner holds them."""
+    return {t for t in range(64) if planner.type_info(t)}
 
 
 # ---- the scenes --------------------------------------------------------------------------------------------------------------------------------------

@@ -11,6 +11,7 @@ import numpy as np
 import bepuphysics2_b200 as bp
 from bepuphysics2_b200 import scenes
 from oracle import binding as ob
+from tests import planner
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 with open(os.path.join(ROOT, "tests", "golden", "type_layouts.json")) as f:
@@ -113,40 +114,25 @@ def test_contact_prestep_generators_write_rows_in_reference_order():
 
 
 def test_roofline_byte_model_uses_the_reference_access_filters():
-    """The SURVEY.md §8d algorithmic bytes per evaluation behind `roofline.achieved` (csrc/bepu_joint_registry.inc, make_contact in
-    csrc/bepu_topology.cpp): per-body read / written float counts must be the sums over the access filters the reference declares for each type
-    (fixture: parsed from the processor declarations and IBodyAccessFilter.cs), and the resulting bytes must reproduce the worked examples of
-    SURVEY.md §8d."""
+    """The SURVEY.md §8d algorithmic bytes per evaluation behind `roofline.achieved`, as the compiled planner holds them (get_type_info of
+    csrc/bepu_topology.cpp, built from csrc/bepu_type_table.h): per-type read / written float counts must be the sums over the access filters the
+    reference declares for each type (fixture: parsed from the processor declarations and IBodyAccessFilter.cs), the bytes must follow from them
+    and reproduce the worked examples of SURVEY.md §8d, and the incremental contact update must read every prestep row and write every depth."""
     with open(os.path.join(ROOT, "tests", "golden", "type_layouts.json")) as f:
         filters = json.load(f)["access_filters"]
-    csrc = os.path.join(ROOT, "bepuphysics2_b200", "csrc")
-    inc = open(os.path.join(csrc, "bepu_joint_registry.inc")).read()
-    api = open(os.path.join(csrc, "bepu_topology.cpp")).read()
-    solve_bytes, warm_start_bytes = {}, {}
-    seen = set()
-    for m in re.finditer(r"add\((\d+),\s*make_joint\((\d+),\s*(\d+),\s*(\d+),\s*(\d+),\s*(\d+),\s*(\d+),\s*(\d+),", inc):
-        type_id, bodies, prestep, impulses, solve_r, solve_w, ws_r, ws_w = (int(g) for g in m.groups())
-        ref = FIXTURE[type_id]
-        assert (bodies, prestep, impulses) == (ref["bodies"], len(ref["prestep_rows"]), len(ref["impulse_rows"])), type_id
-        assert solve_r == sum(filters[f]["read"] for f in ref["solve_filters"]), "type %d: Solve reads %s" % (type_id, ref["solve_filters"])
-        assert solve_w == sum(filters[f]["write"] for f in ref["solve_filters"]), "type %d: Solve writes %s" % (type_id, ref["solve_filters"])
-        assert ws_r == sum(filters[f]["read"] for f in ref["warm_start_filters"]), "type %d: WarmStart reads %s" % (type_id, ref["warm_start_filters"])
-        assert ws_w == sum(filters[f]["write"] for f in ref["warm_start_filters"]), "type %d: WarmStart writes %s" % (type_id, ref["warm_start_filters"])
-        solve_bytes[type_id] = 4 * (prestep + 2 * impulses + bodies + solve_r + solve_w)
-        warm_start_bytes[type_id] = 4 * (prestep + impulses + bodies + ws_r + ws_w)
-        seen.add(type_id)
-    # contacts: one formula, NoPose for every body and stage
-    assert re.search(r"const int body_rw = 13 \+ 6;", api) and "t.solve_bytes = 4 * (prestep + 2 * impulses + bodies + bodies * body_rw);" in api
-    assert "t.solve_bytes = 4 * (prestep + 2 * impulses + bodies + solve_r + solve_w);" in api
-    for m in re.finditer(r"add\((\d+),\s*make_contact\((\d+),\s*(\d+),\s*(\d+),\s*(\d+),", api):
-        type_id, bodies, prestep, impulses, contacts = (int(g) for g in m.groups())
-        ref = FIXTURE[type_id]
-        assert (bodies, prestep, impulses) == (ref["bodies"], len(ref["prestep_rows"]), len(ref["impulse_rows"])), type_id
-        assert set(ref["solve_filters"] + ref["warm_start_filters"]) == {"AccessNoPose"}
-        assert filters["AccessNoPose"] == {"read": 13, "write": 6}
-        assert contacts == sum(1 for r in ref["prestep_rows"] if r.endswith(".Depth"))
-        solve_bytes[type_id] = 4 * (prestep + 2 * impulses + bodies + bodies * 19)
-        seen.add(type_id)
-    assert seen == set(FIXTURE)
+    moved = lambda names: (sum(filters[f]["read"] for f in names), sum(filters[f]["write"] for f in names))  # read, written
+    infos = {t: planner.type_info(t) for t in range(64)}
+    assert {t for t, info in infos.items() if info} == set(FIXTURE), "the planner's types and the reference's registered type processors differ"
+    for type_id, ref in FIXTURE.items():
+        t = infos[type_id]
+        bodies, prestep, impulses = ref["bodies"], len(ref["prestep_rows"]), len(ref["impulse_rows"])
+        assert (t["bodies"], t["prestep_rows"], t["impulse_rows"]) == (bodies, prestep, impulses), type_id
+        assert (t["solve_read"], t["solve_written"]) == moved(ref["solve_filters"]), "type %d: Solve filters %s" % (type_id, ref["solve_filters"])
+        assert (t["warm_start_read"], t["warm_start_written"]) == moved(ref["warm_start_filters"]), "type %d: WarmStart filters %s" % (type_id, ref["warm_start_filters"])
+        assert t["solve_bytes"] == 4 * (prestep + 2 * impulses + bodies + t["solve_read"] + t["solve_written"]), type_id
+        assert t["warm_start_bytes"] == 4 * (prestep + impulses + bodies + t["warm_start_read"] + t["warm_start_written"]), type_id
+        contacts = sum(1 for r in ref["prestep_rows"] if r.endswith(".Depth"))
+        assert t["contacts"] == contacts, type_id
+        assert t["incremental_bytes"] == (4 * (prestep + contacts + bodies + 6 * bodies) if contacts else 0), type_id
     # SURVEY.md §8d worked examples
-    assert {k: solve_bytes[k] for k in (7, 4, 3, 22, 47, 31, 25, 27, 30, 29)} == {7: 320, 4: 248, 3: 228, 22: 272, 47: 312, 31: 300, 25: 180, 27: 192, 30: 164, 29: 196}
+    assert {k: infos[k]["solve_bytes"] for k in (7, 4, 3, 22, 47, 31, 25, 27, 30, 29)} == {7: 320, 4: 248, 3: 228, 22: 272, 47: 312, 31: 300, 25: 180, 27: 192, 30: 164, 29: 196}

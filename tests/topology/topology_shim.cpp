@@ -1,9 +1,10 @@
-// Test shim of the planner tests (loaded by tests/planner.py): plan_topology (plain and per rank), its inverse slot map, build_stage_program,
-// exchange_targets, resolve_stage_launch, same_launches and integrated_warm_start_launch of bepuphysics2_b200/csrc/bepu_topology.h behind a
-// ctypes-friendly C interface. Built with g++ together with bepu_topology.cpp; the product never loads it.
+// Test shim of the planner tests (loaded by tests/planner.py): get_type_info, plan_topology (plain and per rank), its inverse slot map,
+// build_stage_program, exchange_targets, resolve_stage_launch, same_launches and integrated_warm_start_launch of bepuphysics2_b200/csrc/
+// bepu_topology.h behind a ctypes-friendly C interface. Built with g++ together with bepu_topology.cpp; the product never loads it.
 #include <cstring>
 
 #include "bepu_topology.h"
+#include "bepu_type_table.h"
 
 using namespace bepucuda;
 
@@ -131,6 +132,16 @@ int topology_same_launches(int extensions_a, int angular_mode_a, int profile_a, 
     return same_launches(LaunchContext{extensions_a != 0, angular_mode_a, profile_a != 0}, LaunchContext{extensions_b != 0, angular_mode_b, profile_b != 0});
 }
 int topology_deep_batch_bundles() { return kDeepBatchBundles; }
+// get_type_info: the name (null for an id without a type); out: the other TypeInfo fields in order, then the filter counts of the table row
+const char* topology_type_info(int type_id, int64_t* out) {
+    const TypeInfo* t = get_type_info(type_id);
+    if (!t) return nullptr;
+    const TypeRow& r = *type_row(type_id);
+    const int64_t v[] = {t->bodies, t->prestep_rows, t->impulse_rows, t->contacts, t->solve_bytes, t->warm_start_bytes, t->incremental_bytes,
+                         r.solve_read, r.solve_written, r.warm_start_read, r.warm_start_written};
+    std::memcpy(out, v, sizeof(v));
+    return t->name;
+}
 // which contact-only WarmStart instantiation launch_stage (csrc/bepu_solver_kernels.cu) runs for a resolved launch: 1 = the integrated one
 int topology_integrated_warm_start_launch(int stage, int kernel, int flags) { return integrated_warm_start_launch(stage, StageLaunch{kernel, flags}) ? 1 : 0; }
 
