@@ -42,7 +42,7 @@ struct DeviceTypeBatch {
     int32_t type_id;
     int32_t bundle_count;      // 32-lane bundles
     int32_t device_batch;      // index of the device batch (synchronized batches, then fallback levels)
-    int32_t pad;
+    int32_t bodies;            // body slots per constraint of the type (bepu_type_table.h)
     int32_t* refs;             // [bundle][body slot][32]
     float* prestep;            // [bundle][prestep row][32]
     float* impulses;           // [bundle][impulse row][32]

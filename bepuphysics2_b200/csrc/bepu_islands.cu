@@ -41,7 +41,7 @@ __global__ void island_hook_kernel(IslandBuffers ib) {
     if (warp >= ib.work_count) return;
     const WorkItem w = ib.work[warp];
     const DeviceTypeBatch tb = ib.tbs[w.type_batch];
-    const int nb = ib.bodies_per_type[tb.type_id];
+    const int nb = tb.bodies;
     const int32_t* refs = tb.refs + (size_t)w.bundle * nb * 32 + lane;
     int32_t roots[4];
     int32_t lowest = 0x7fffffff;

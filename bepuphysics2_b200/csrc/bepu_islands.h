@@ -15,7 +15,6 @@ struct IslandBuffers {
     const DeviceTypeBatch* tbs;            // the resident type batches, read through the work list (work[0 .. work_count) covers every bundle once)
     const WorkItem* work;
     int32_t work_count;
-    const int32_t* bodies_per_type;
     const uint8_t* activities;             // bepucuda_body_activity records, 8 bytes per body; only sleep_candidate (byte 6) is read
     int32_t* label;                        // per body: a body of the same island with a smaller index, or itself for the island's root
     int32_t* blocked;                      // per root: nonzero when a body of its island is not a sleep candidate

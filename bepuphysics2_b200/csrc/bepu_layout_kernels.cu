@@ -89,7 +89,7 @@ __global__ void redistribute_impulses_kernel(const DeviceTypeBatch* __restrict__
     const int slot = w.bundle * 32 + lane;
     const int c = d.map ? d.map[slot] : slot;
     if (c < 0 || c >= d.src_count) return;
-    const int n = contact_count_of_type(tb.type_id);
+    const int n = d.contacts;
     float* acc = tb.impulses + (size_t)w.bundle * d.impulse_rows * 32 + lane;
     float oldImpulses[4], newImpulses[4];
     for (int i = 0; i < n; ++i) oldImpulses[i] = acc[penetration_impulse_row(tb.type_id, i) * 32];
@@ -186,13 +186,13 @@ __global__ void write_constraints_kernel(const DeviceTypeBatch* __restrict__ tbs
 
 // Pass 1 over every (constraint, body slot): first_batch[body] = min device batch referencing it as a dynamic body;
 // per-body reference count and bitmask of synchronized batches for the batch-invariant check.
-__global__ void ownership_pass1_kernel(const DeviceTypeBatch* __restrict__ tbs, const WorkItem* __restrict__ work, int work_count, const int32_t* __restrict__ bodies_per_type,
-                                       int sync_batch_count, int body_count, int32_t* first_batch, int32_t* sync_refcount, unsigned long long* sync_mask, int32_t* error_flag) {
+__global__ void ownership_pass1_kernel(const DeviceTypeBatch* __restrict__ tbs, const WorkItem* __restrict__ work, int work_count, int sync_batch_count, int body_count,
+                                       int32_t* first_batch, int32_t* sync_refcount, unsigned long long* sync_mask, int32_t* error_flag) {
     const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
     if (warp >= work_count) return;
     const WorkItem w = work[warp];
     const DeviceTypeBatch tb = tbs[w.type_batch];
-    const int nb = bodies_per_type[tb.type_id];
+    const int nb = tb.bodies;
     for (int s = 0; s < nb; ++s) {
         const int32_t enc = tb.refs[((size_t)w.bundle * nb + s) * 32 + lane];
         if (enc < 0 || (enc & kRefKinematicBit)) continue;
@@ -206,13 +206,13 @@ __global__ void ownership_pass1_kernel(const DeviceTypeBatch* __restrict__ tbs, 
     }
 }
 // Pass 2: set the integrate bit on the owning lane, mark constrained bodies.
-__global__ void ownership_pass2_kernel(const DeviceTypeBatch* __restrict__ tbs, const WorkItem* __restrict__ work, int work_count, const int32_t* __restrict__ bodies_per_type,
-                                       int body_count, const int32_t* __restrict__ first_batch, uint8_t* constrained) {
+__global__ void ownership_pass2_kernel(const DeviceTypeBatch* __restrict__ tbs, const WorkItem* __restrict__ work, int work_count, int body_count,
+                                       const int32_t* __restrict__ first_batch, uint8_t* constrained) {
     const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
     if (warp >= work_count) return;
     const WorkItem w = work[warp];
     const DeviceTypeBatch tb = tbs[w.type_batch];
-    const int nb = bodies_per_type[tb.type_id];
+    const int nb = tb.bodies;
     for (int s = 0; s < nb; ++s) {
         int32_t* r = tb.refs + ((size_t)w.bundle * nb + s) * 32 + lane;
         const int32_t enc = *r;
@@ -383,12 +383,15 @@ void launch_fill_peer_masks(const int32_t* refs, uint32_t* peer_masks, size_t co
     if (count == 0) return;
     fill_peer_masks_kernel<<<blocks_for(count, 256), 256, 0, s>>>(refs, peer_masks, count, body_masks, rank);
 }
-__global__ void boundary_flags_kernel(const WorkRecord* __restrict__ records, int count, const int32_t* __restrict__ bodies_per_type, long long peer_delta, uint8_t* __restrict__ flags) {
+__global__ void boundary_flags_kernel(const DeviceTypeBatch* __restrict__ tbs, const WorkItem* __restrict__ work, int work_count, long long peer_delta,
+                                      uint8_t* __restrict__ flags) {
     const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-    if (warp >= count) return;
-    const WorkRecord r = records[warp];
+    if (warp >= work_count) return;
+    const WorkItem w = work[warp];
+    const DeviceTypeBatch tb = tbs[w.type_batch];
+    const int32_t* refs = tb.refs + (size_t)w.bundle * tb.bodies * 32 + lane;
     uint32_t m = 0;
-    for (int s = 0; s < bodies_per_type[r.type_id]; ++s) m |= (uint32_t)r.refs[peer_delta + s * 32 + lane];
+    for (int s = 0; s < tb.bodies; ++s) m |= (uint32_t)refs[peer_delta + s * 32];
     const bool any = __any_sync(0xFFFFFFFFu, m != 0);
     if (lane == 0) flags[warp] = any ? 1 : 0;
 }
@@ -402,28 +405,28 @@ void launch_pack_ref_rows(const WorkRecord* records, int count, int32_t* rows, c
     if (count <= 0) return;
     pack_ref_rows_kernel<<<blocks_for((size_t)count * 64, 256), 256, 0, s>>>(records, count, rows);
 }
-void launch_boundary_flags(const WorkRecord* records, int count, const int32_t* bodies_per_type, long long peer_delta, uint8_t* flags, cudaStream_t s) {
-    if (count <= 0) return;
-    boundary_flags_kernel<<<blocks_for((size_t)count * 32, 128), 128, 0, s>>>(records, count, bodies_per_type, peer_delta, flags);
+void launch_boundary_flags(const DeviceTypeBatch* tbs, const WorkItem* work, int work_count, long long peer_delta, uint8_t* flags, cudaStream_t s) {
+    if (work_count <= 0) return;
+    boundary_flags_kernel<<<blocks_for((size_t)work_count * 32, 128), 128, 0, s>>>(tbs, work, work_count, peer_delta, flags);
 }
 void launch_fill_i32(int32_t* p, size_t n, int32_t v, cudaStream_t s) {
     if (n == 0) return;
     fill_i32_kernel<<<blocks_for(n, 256), 256, 0, s>>>(p, n, v);
 }
-void launch_ownership_pass1(const DeviceTypeBatch* tbs, const WorkItem* work, int work_count, const int32_t* bodies_per_type, int sync_batch_count, int body_count,
+void launch_ownership_pass1(const DeviceTypeBatch* tbs, const WorkItem* work, int work_count, int sync_batch_count, int body_count,
                             int32_t* first_batch, int32_t* sync_refcount, unsigned long long* sync_mask, int32_t* error_flag, cudaStream_t s) {
     if (work_count > 0)
-        ownership_pass1_kernel<<<blocks_for((size_t)work_count * 32, 128), 128, 0, s>>>(tbs, work, work_count, bodies_per_type, sync_batch_count, body_count, first_batch,
+        ownership_pass1_kernel<<<blocks_for((size_t)work_count * 32, 128), 128, 0, s>>>(tbs, work, work_count, sync_batch_count, body_count, first_batch,
                                                                                          sync_refcount, sync_mask, error_flag);
 }
 void launch_merge_first_batch(int32_t* first_batch, const int32_t* global_first_batch, int body_count, int fallback_threshold, cudaStream_t s) {
     if (body_count > 0) merge_first_batch_kernel<<<blocks_for(body_count, 256), 256, 0, s>>>(first_batch, global_first_batch, body_count, fallback_threshold);
 }
-void launch_ownership_rest(const DeviceTypeBatch* tbs, const WorkItem* work, int work_count, const int32_t* bodies_per_type, int body_count, const int32_t* first_batch,
+void launch_ownership_rest(const DeviceTypeBatch* tbs, const WorkItem* work, int work_count, int body_count, const int32_t* first_batch,
                            const int32_t* sync_refcount, const unsigned long long* sync_mask, uint8_t* constrained, const int32_t* kinematics, int kinematic_count,
                            int32_t* error_flag, const TransposeDesc* descs, int W, int32_t* source_bundle_flags, cudaStream_t s) {
     if (work_count > 0) {
-        ownership_pass2_kernel<<<blocks_for((size_t)work_count * 32, 128), 128, 0, s>>>(tbs, work, work_count, bodies_per_type, body_count, first_batch, constrained);
+        ownership_pass2_kernel<<<blocks_for((size_t)work_count * 32, 128), 128, 0, s>>>(tbs, work, work_count, body_count, first_batch, constrained);
         bundle_flags_pass_kernel<<<blocks_for((size_t)work_count * 32, 128), 128, 0, s>>>(tbs, descs, work, work_count, W, source_bundle_flags, 0);
         bundle_flags_pass_kernel<<<blocks_for((size_t)work_count * 32, 128), 128, 0, s>>>(tbs, descs, work, work_count, W, source_bundle_flags, 1);
     }

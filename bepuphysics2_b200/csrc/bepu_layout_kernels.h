@@ -1,6 +1,7 @@
 // Launchers of the layout / topology kernels (bepu_layout_kernels.cu).
 #pragma once
 #include "bepu_device_types.h"
+#include "bepu_type_table.h"
 
 namespace bepucuda {
 
@@ -16,6 +17,7 @@ struct TransposeDesc {
     int32_t bodies, prestep_rows, impulse_rows;
     int32_t src_bundle_base;  // index of the source type batch's first host-width bundle in the per-bundle flag array
     int32_t flags;            // kTransposePrestep / kTransposeImpulses: rows uploaded since the last transposition; kDescRedistribute
+    int32_t contacts;         // per manifold; 0 for joints
     const int32_t* features_old;  // contact feature ids the resident impulses belong to / the frame's new ids ([constraint][contact]); null = none
     const int32_t* features_new;
 };
@@ -39,9 +41,12 @@ struct ReadRequest {
 void launch_read_constraints(const DeviceTypeBatch* tbs, const TransposeDesc* descs, const DeviceSlot* inverse, const ReadRequest* requests, int count, int32_t* records,
                              cudaStream_t s);
 // Words of the 64-word record of bepucuda_read_constraints / bepucuda_write_constraints (include/bepucuda.h): 0 type id, 1 live, 2-5 body references,
-// 6-17 accumulated impulses, 18-52 prestep (as many rows as the largest type has), 53-63 zero.
+// 6-17 accumulated impulses, 18-52 prestep, 53-63 zero.
 constexpr int kRecordRefs = 2, kRecordImpulses = 6, kRecordPrestep = 18, kRecordEnd = 53;
 constexpr int kRecordPrestepWords = kRecordEnd - kRecordPrestep;
+static_assert(kRecordImpulses - kRecordRefs >= max_over_types([](const TypeRow& r) { return r.bodies; }), "record: body references of every type");
+static_assert(kRecordPrestep - kRecordImpulses >= max_over_types([](const TypeRow& r) { return r.impulse_rows; }), "record: impulse rows of every type");
+static_assert(kRecordPrestepWords >= max_over_types([](const TypeRow& r) { return r.prestep_rows; }), "record: prestep rows of every type");
 // One queued write of bepucuda_write_constraints: the constraint at `at` takes the prestep rows rows[row0 .. row0 + its type's prestep_rows).
 struct PrestepWrite {
     DeviceSlot at;
@@ -62,12 +67,12 @@ struct CopyChunk {
     size_t bytes;
 };
 void launch_batched_copy(const CopyChunk* chunks, int chunk_count, cudaStream_t s);
-void launch_ownership_pass1(const DeviceTypeBatch* tbs, const WorkItem* work, int work_count, const int32_t* bodies_per_type, int sync_batch_count, int body_count,
+void launch_ownership_pass1(const DeviceTypeBatch* tbs, const WorkItem* work, int work_count, int sync_batch_count, int body_count,
                             int32_t* first_batch, int32_t* sync_refcount, unsigned long long* sync_mask, int32_t* error_flag, cudaStream_t s);
 // Peer sharding, between the ownership passes: first_batch[i] = global_first_batch[i] (host batch indices, lowest over every rank) unless that is
 // at or above fallback_threshold, where the device batch of pass 1 (a fallback level of the fallback rank) stays.
 void launch_merge_first_batch(int32_t* first_batch, const int32_t* global_first_batch, int body_count, int fallback_threshold, cudaStream_t s);
-void launch_ownership_rest(const DeviceTypeBatch* tbs, const WorkItem* work, int work_count, const int32_t* bodies_per_type, int body_count, const int32_t* first_batch,
+void launch_ownership_rest(const DeviceTypeBatch* tbs, const WorkItem* work, int work_count, int body_count, const int32_t* first_batch,
                            const int32_t* sync_refcount, const unsigned long long* sync_mask, uint8_t* constrained, const int32_t* kinematics, int kinematic_count,
                            int32_t* error_flag, const TransposeDesc* descs, int W, int32_t* source_bundle_flags, cudaStream_t s);
 // Peer sharding, rank barrier: one CTA signals every peer and waits for every peer's signal of the same exchange point (flag barrier in peer
@@ -77,8 +82,8 @@ void launch_shard_barrier(const ShardPeers& peers, const FrameParams* fp, uint32
 // Peer sharding: peer_masks[i] = ranks other than `rank` that reference the dynamic body of device reference refs[i] (0 for empty and
 // kinematic slots); body_masks[b] has bit r set when rank r references body b.
 void launch_fill_peer_masks(const int32_t* refs, uint32_t* peer_masks, size_t count, const uint8_t* body_masks, int rank, cudaStream_t s);
-// flags[i] = 1 when any lane of work record i has a non-empty destination mask (a "boundary" bundle, see ShardStage).
-void launch_boundary_flags(const WorkRecord* records, int count, const int32_t* bodies_per_type, long long peer_delta, uint8_t* flags, cudaStream_t s);
+// flags[i] = 1 when any lane of work item i has a non-empty destination mask (a "boundary" bundle, see ShardStage).
+void launch_boundary_flags(const DeviceTypeBatch* tbs, const WorkItem* work, int work_count, long long peer_delta, uint8_t* flags, cudaStream_t s);
 
 // Reference rows next to the work list: rows[i][0..1][lane] = the first two body-reference rows of work record i (64 words per record), so that a
 // solver warp fetches its work record and its body references with independent loads (one DRAM round trip instead of two).

@@ -5,14 +5,6 @@
 
 namespace bepucuda {
 
-// Contacts of a contact constraint type: ids 0-7 (convex) 1-4, ids 8-10 / 15-17 (nonconvex) 2-4; 0 for any other type.
-__host__ __device__ __forceinline__ int contact_count_of_type(int type_id) {
-    if (type_id >= 0 && type_id <= 7) return (type_id & 3) + 1;
-    if (type_id >= 8 && type_id <= 10) return type_id - 6;
-    if (type_id >= 15 && type_id <= 17) return type_id - 13;
-    return 0;
-}
-
 // Row of contact i's penetration impulse among a contact constraint's accumulated impulses: convex types [2 + i] (after the two tangent rows,
 // ContactConstraintAccessor.cs:L58-66), nonconvex types [3 i + 2] (L70-76).
 __host__ __device__ __forceinline__ int penetration_impulse_row(int type_id, int i) { return type_id < 8 ? 2 + i : 3 * i + 2; }

@@ -348,7 +348,9 @@ __host__ __device__ constexpr StageRowCounts make_stage_row_counts() {
     return c;
 }
 __constant__ StageRowCounts kStageRowCounts = make_stage_row_counts();
-constexpr int kStageSlabRows = 48;  // >= max(prestep rows + impulse rows) over all types (Contact4Nonconvex: 35 + 12)
+constexpr int kStageSlabRows = 48;
+static_assert(kStageSlabRows >= bepucuda::max_over_types([](const bepucuda::TypeRow& r) { return r.prestep_rows + r.impulse_rows; }),
+              "a warp's stage slab must hold the prestep and impulse rows of every type");
 constexpr int kStageSlabBytes = kStageSlabRows * kLanes * 4;
 
 BEPU_DI uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }

@@ -72,4 +72,18 @@ constexpr const TypeRow* type_row(int type_id) {
     return nullptr;
 }
 
+// Contacts per constraint of a type id; 0 for joints and ids without a type.
+constexpr int32_t contact_count_of_type(int type_id) {
+    const TypeRow* r = type_row(type_id);
+    return r ? r->contacts : 0;
+}
+
+// The largest f(row) over the table: what a buffer sized for every type must hold.
+template <class F>
+constexpr int32_t max_over_types(F f) {
+    int32_t m = 0;
+    for (const TypeRow& r : kTypeTable) m = f(r) > m ? f(r) : m;
+    return m;
+}
+
 }  // namespace bepucuda

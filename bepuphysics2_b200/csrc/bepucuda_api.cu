@@ -137,7 +137,7 @@ struct bepucuda_ctx {
     bool constraints_open = false, constraints_ready = false, data_dirty = false;
     std::vector<SourceTypeBatch> sources;
     ChunkArena raw_arena, pinned_arena;
-    DeviceBuffer record_table, ref_rows, source_bundle_flags, refs32, prestep32, impulses32, tb_table, tdesc_table, work_table, map_table, bodies_per_type, kinematics_dev, frame_params_dev, error_dev;
+    DeviceBuffer record_table, ref_rows, source_bundle_flags, refs32, prestep32, impulses32, tb_table, tdesc_table, work_table, map_table, kinematics_dev, frame_params_dev, error_dev;
     TopologyPlan topo;                          // device batches and work list of the last successful end_constraints
     std::vector<TransposeDesc> tdescs;          // per planned type batch
     std::vector<WorkRecord> records;            // what the solver kernels read (parallel to topo.work)
@@ -790,21 +790,18 @@ int32_t bepucuda_end_constraints(bepucuda_ctx* ctx) {
         const PlannedTypeBatch& p = topo.tbs[i];
         const SourceTypeBatch& s = ctx->sources[(size_t)p.source];
         const TypeInfo* t = get_type_info(p.type_id);
-        tbs[i] = {p.type_id, p.bundle_count, p.device_batch, 0, ctx->refs32.as<int32_t>() + p.refs_offset, ctx->prestep32.as<float>() + p.prestep_offset,
+        tbs[i] = {p.type_id, p.bundle_count, p.device_batch, t->bodies, ctx->refs32.as<int32_t>() + p.refs_offset, ctx->prestep32.as<float>() + p.prestep_offset,
                   ctx->impulses32.as<float>() + p.impulse_offset};
         ctx->tdescs[i] = {s.raw_refs, s.raw_prestep, s.raw_impulses, p.map_offset < 0 ? nullptr : ctx->map_table.as<int32_t>() + p.map_offset, s.count, t->bodies, t->prestep_rows,
-                          t->impulse_rows, topo.source_bundle_base[(size_t)p.source], kTransposePrestep | kTransposeImpulses, nullptr, nullptr};
+                          t->impulse_rows, topo.source_bundle_base[(size_t)p.source], kTransposePrestep | kTransposeImpulses, t->contacts, nullptr, nullptr};
     }
     ctx->records = work_records(topo, ctx->refs32.as<int32_t>(), ctx->prestep32.as<float>(), ctx->impulses32.as<float>());
 
     // ---- upload tables ----
-    int32_t bodies_per_type[64];
-    for (int i = 0; i < 64; ++i) bodies_per_type[i] = get_type_info(i) ? get_type_info(i)->bodies : 0;
     CK(ctx->tb_table.reserve(tbs.size() * sizeof(DeviceTypeBatch) + 16));
     CK(ctx->tdesc_table.reserve(ctx->tdescs.size() * sizeof(TransposeDesc) + 16));
     CK(ctx->work_table.reserve(topo.work.size() * sizeof(WorkItem) + 16));
     CK(ctx->record_table.reserve(ctx->records.size() * sizeof(WorkRecord) + 64));
-    CK(ctx->bodies_per_type.reserve(sizeof(bodies_per_type)));
     CK(ctx->kinematics_dev.reserve(ctx->kinematics.size() * 4 + 4));
     if (!tbs.empty()) CK(cudaMemcpyAsync(ctx->tb_table.ptr, tbs.data(), tbs.size() * sizeof(DeviceTypeBatch), cudaMemcpyHostToDevice, ctx->stream));
     if (!ctx->tdescs.empty()) CK(cudaMemcpyAsync(ctx->tdesc_table.ptr, ctx->tdescs.data(), ctx->tdescs.size() * sizeof(TransposeDesc), cudaMemcpyHostToDevice, ctx->stream));
@@ -813,7 +810,6 @@ int32_t bepucuda_end_constraints(bepucuda_ctx* ctx) {
     if (!topo.maps.empty()) CK(cudaMemcpyAsync(ctx->map_table.ptr, topo.maps.data(), topo.maps.size() * 4, cudaMemcpyHostToDevice, ctx->stream));
     if (!topo.inverse.empty())
         CK(cudaMemcpyAsync(ctx->inverse_table.ptr, topo.inverse.data(), topo.inverse.size() * sizeof(DeviceSlot), cudaMemcpyHostToDevice, ctx->stream));
-    CK(cudaMemcpyAsync(ctx->bodies_per_type.ptr, bodies_per_type, sizeof(bodies_per_type), cudaMemcpyHostToDevice, ctx->stream));
     if (!ctx->kinematics.empty()) CK(cudaMemcpyAsync(ctx->kinematics_dev.ptr, ctx->kinematics.data(), ctx->kinematics.size() * 4, cudaMemcpyHostToDevice, ctx->stream));
 
     // ---- transposition into AOSOA-32 + ownership analysis ----
@@ -832,7 +828,7 @@ int32_t bepucuda_end_constraints(bepucuda_ctx* ctx) {
     CK(cudaMemsetAsync(ctx->error_dev.ptr, 0, 32, ctx->stream));
     CK(ctx->source_bundle_flags.reserve((size_t)std::max(topo.source_bundles, 1) * 16));
     CK(cudaMemsetAsync(ctx->source_bundle_flags.ptr, 0, (size_t)std::max(topo.source_bundles, 1) * 16, ctx->stream));
-    launch_ownership_pass1(ctx->tb_table.as<DeviceTypeBatch>(), ctx->work_table.as<WorkItem>(), topo.all_work_count, ctx->bodies_per_type.as<int32_t>(), topo.sync_batch_count,
+    launch_ownership_pass1(ctx->tb_table.as<DeviceTypeBatch>(), ctx->work_table.as<WorkItem>(), topo.all_work_count, topo.sync_batch_count,
                            ctx->body_count, ctx->first_batch.as<int32_t>(), ctx->sync_refcount.as<int32_t>(), (unsigned long long*)ctx->sync_mask.ptr, ctx->error_dev.as<int32_t>(),
                            ctx->stream);
     if (ctx->peer_mode && nb > 0) {
@@ -843,7 +839,7 @@ int32_t bepucuda_end_constraints(bepucuda_ctx* ctx) {
         CK(cudaMemcpyAsync(ctx->global_first_batch_dev.ptr, ctx->global_first_batch.data(), (size_t)ctx->body_count * 4, cudaMemcpyHostToDevice, ctx->stream));
         launch_merge_first_batch(ctx->first_batch.as<int32_t>(), ctx->global_first_batch_dev.as<int32_t>(), ctx->body_count, ctx->fallback_threshold, ctx->stream);
     }
-    launch_ownership_rest(ctx->tb_table.as<DeviceTypeBatch>(), ctx->work_table.as<WorkItem>(), topo.all_work_count, ctx->bodies_per_type.as<int32_t>(), ctx->body_count,
+    launch_ownership_rest(ctx->tb_table.as<DeviceTypeBatch>(), ctx->work_table.as<WorkItem>(), topo.all_work_count, ctx->body_count,
                           ctx->first_batch.as<int32_t>(), ctx->sync_refcount.as<int32_t>(), (const unsigned long long*)ctx->sync_mask.ptr, ctx->constrained.as<uint8_t>(),
                           ctx->kinematics_dev.as<int32_t>(), (int)ctx->kinematics.size(), ctx->error_dev.as<int32_t>(), ctx->tdesc_table.as<TransposeDesc>(), W,
                           ctx->source_bundle_flags.as<int32_t>(), ctx->stream);
@@ -859,7 +855,7 @@ int32_t bepucuda_end_constraints(bepucuda_ctx* ctx) {
         // the flag barrier of the stage involves only them (ShardStage)
         const int n_rec = topo.all_work_count;
         CK(ctx->boundary_flags_dev.reserve((size_t)n_rec + 16));
-        launch_boundary_flags(ctx->record_table.as<WorkRecord>(), n_rec, ctx->bodies_per_type.as<int32_t>(), (long long)(ctx->peer32.as<int32_t>() - ctx->refs32.as<int32_t>()),
+        launch_boundary_flags(ctx->tb_table.as<DeviceTypeBatch>(), ctx->work_table.as<WorkItem>(), n_rec, (long long)(ctx->peer32.as<int32_t>() - ctx->refs32.as<int32_t>()),
                               ctx->boundary_flags_dev.as<uint8_t>(), ctx->stream);
         std::vector<uint8_t> is_boundary((size_t)n_rec);
         if (n_rec > 0) CK(cudaMemcpyAsync(is_boundary.data(), ctx->boundary_flags_dev.ptr, (size_t)n_rec, cudaMemcpyDeviceToHost, ctx->stream));
@@ -1354,7 +1350,6 @@ int32_t bepucuda_find_sleepable_islands(bepucuda_ctx* ctx, const bepucuda_body_a
     ib.tbs = ctx->tb_table.as<DeviceTypeBatch>();
     ib.work = ctx->work_table.as<WorkItem>();
     ib.work_count = ctx->topo.all_work_count;
-    ib.bodies_per_type = ctx->bodies_per_type.as<int32_t>();
     ib.activities = ctx->island_activities.as<uint8_t>();
     ib.label = ctx->island_label.as<int32_t>();
     ib.blocked = ctx->island_blocked.as<int32_t>();

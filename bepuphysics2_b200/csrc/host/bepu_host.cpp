@@ -297,6 +297,8 @@ void* bepuhost_create(int32_t bundle_width, int32_t fallback_batch_threshold) {
     return s;
 }
 void bepuhost_destroy(void* sim) { delete (Simulation*)sim; }
+// Contacts per constraint of a type id (bepu_type_table.h); 0 for joints and ids without a type.
+int32_t bepuhost_contact_count(int32_t type_id) { return bepucuda::contact_count_of_type(type_id); }
 const char* bepuhost_last_error(void* sim) { return ((Simulation*)sim)->error.c_str(); }
 
 // SolveDescription(velocityIterationCount, substepCount) with an optional per-substep schedule (SolveDescription.cs:L21-38).

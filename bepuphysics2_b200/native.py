@@ -94,15 +94,9 @@ ERR_INVALID_ARGUMENT, ERR_NO_DEVICE, ERR_CUDA, ERR_UNSUPPORTED_TYPE, ERR_BATCH_I
 
 
 def contact_count(type_id):
-    """Contacts per constraint of a contact constraint type id: 1-4 for the convex ids 0-7, 2-4 for the nonconvex ids 8-10 and 15-17; 0 for every
-    other type (joints)."""
-    if 0 <= type_id <= 7:
-        return (type_id & 3) + 1
-    if 8 <= type_id <= 10:
-        return type_id - 6
-    if 15 <= type_id <= 17:
-        return type_id - 13
-    return 0
+    """Contacts per constraint of a constraint type id, from the library's type table: 1-4 for contact manifolds, 0 for joints and ids without a
+    type."""
+    return load_libraries()[1].bepuhost_contact_count(type_id)
 
 # Every symbol include/bepucuda.h declares (checked by the CPU test-suite).
 C_ABI_SYMBOLS = [
@@ -189,6 +183,7 @@ def load_libraries():
     host.bepuhost_create.restype = vp
     host.bepuhost_create.argtypes = [i32, i32]
     host.bepuhost_destroy.argtypes = [vp]
+    host.bepuhost_contact_count.argtypes = [i32]
     host.bepuhost_last_error.argtypes = [vp]
     host.bepuhost_last_error.restype = C.c_char_p
     host.bepuhost_set_solve_description.argtypes = [vp, i32, C.POINTER(i32)]

@@ -130,7 +130,7 @@ extern "C" int32_t device_on_host_update_contact_impulses(int32_t type_id, int32
                                                           const int32_t* new_feature_ids) {
     const int n = bepucuda::contact_count_of_type(type_id);
     if (n == 0) return -1;
-    const int rows = type_id < 8 ? n + 3 : 3 * n;
+    const int rows = bepucuda::type_row(type_id)->impulse_rows;
     for (int c = 0; c < constraint_count; ++c) {
         float* bundle = accumulated_impulses + (size_t)(c / W) * rows * W + (c % W);
         float oldImpulses[4], newImpulses[4];
@@ -140,6 +140,8 @@ extern "C" int32_t device_on_host_update_contact_impulses(int32_t type_id, int32
     }
     return 0;
 }
+// The row of contact i's penetration impulse that redistribute_impulses_kernel reads and writes.
+extern "C" int32_t device_on_host_penetration_impulse_row(int32_t type_id, int32_t i) { return bepucuda::penetration_impulse_row(type_id, i); }
 
 // PredictBoundingBoxes arithmetic of csrc/bepu_bounds_math.cuh (same operand layout as ref_convex_bounds of the transpiled reference's harness).
 #include "bepu_bounds_math.cuh"

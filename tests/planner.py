@@ -2,6 +2,7 @@
 program and how each of its stages is launched) compiled for the host with g++ behind tests/topology/topology_shim.cpp, and what the planner tests
 share: its constants, the plan and program readers, the launch rules and the scenes. TEST INFRASTRUCTURE: the product never loads the shim."""
 import ctypes as C
+import json
 import os
 import re
 
@@ -13,8 +14,28 @@ from tests import harness
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CSRC = os.path.join(ROOT, "bepuphysics2_b200", "csrc")
 
-# BatchTypeId of the reference's contact constraints: convex manifolds 0-7, nonconvex 8-10 and 15-17
-CONTACT_TYPES = set(range(11)) | {15, 16, 17}
+# The reference's constraint layouts by BatchTypeId (tests/golden/type_layouts.json, generated from its C# sources): bodies and the names of the
+# prestep and accumulated-impulse rows. The contact facts below are read from the row names.
+with open(os.path.join(ROOT, "tests", "golden", "type_layouts.json")) as f:
+    TYPE_LAYOUTS = {int(k): v for k, v in json.load(f)["types"].items()}
+
+
+def depth_rows(type_id):
+    """Prestep rows of a type's contact depths (Contact<i>.Depth) in contact order; [] for joints."""
+    return [r for r, name in enumerate(TYPE_LAYOUTS[type_id]["prestep_rows"]) if re.fullmatch(r"Contact\d\.Depth", name)]
+
+
+def penetration_rows(type_id):
+    """Accumulated-impulse rows of a type's penetration impulses (Penetration<i>, Contact<i>.Penetration) in contact order; [] for joints."""
+    return [r for r, name in enumerate(TYPE_LAYOUTS[type_id]["impulse_rows"]) if re.fullmatch(r"Penetration\d|Contact\d\.Penetration", name)]
+
+
+def contacts(type_id):
+    """Contacts per constraint of a type id; 0 for joints and ids without a type."""
+    return len(depth_rows(type_id)) if type_id in TYPE_LAYOUTS else 0
+
+
+CONTACT_TYPES = {t for t in TYPE_LAYOUTS if contacts(t)}
 WS_FIRST, WS, SOLVE, INCREMENTAL, KIN_FIRST, KIN, FINAL = range(7)
 NO_EXCHANGE, RANK_BARRIER = -1, -2
 ROWS_FREE, CONTACTS_ONLY, BODIES_FREE, INTEGRABLE = 2, 8, 16, 32  # facts of a program op (kOp*)

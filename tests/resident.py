@@ -5,7 +5,7 @@ import numpy as np
 import bepuphysics2_b200 as bp
 from bepuphysics2_b200.native import EXEC_GRAPH, contact_count
 from oracle import binding as ob
-from tests import util
+from tests import planner, util
 
 DT = 1.0 / 60.0
 
@@ -31,11 +31,7 @@ def narrow_phase_like_update(sim, features, rng):
         if n > 1:
             ids[swap] = ids[swap][:, ::-1]
         new[key] = ids
-        # depth rows: convex prestep rows 4 i + 3; nonconvex: after MaterialProperties (4 rows) [+ OffsetB (3 rows) for two bodies], contact i = 7 rows
-        # (Offset xyz, Depth, Normal xyz) with the depth at + 3 (tests/golden/type_layouts.json)
-        base = 4 if tb.type_id <= 10 else 7
-        rows = [4 * i + 3 for i in range(n)] if tb.type_id <= 7 else [base + 7 * i + 3 for i in range(n)]
-        for r in rows:  # the narrow phase writes fresh depths every frame (whatever the solver's incremental updates left in the row)
+        for r in planner.depth_rows(tb.type_id):  # the narrow phase writes fresh depths every frame (whatever the solver's incremental updates left in the row)
             tb.prestep[:, r, :] = rng.uniform(-0.02, 0.05, size=tb.prestep[:, r, :].shape).astype(np.float32)
     return new
 

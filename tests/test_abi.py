@@ -9,6 +9,7 @@ import pytest
 import bepuphysics2_b200 as bp
 from bepuphysics2_b200 import native
 from oracle import binding as ob
+from tests import planner
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
@@ -52,15 +53,18 @@ def test_error_codes_match_the_header():
 
 
 def test_contact_count_matches_the_type_registry(libs):
-    """native.contact_count (the feature-id layout of bepucuda_set_contact_features / bepucuda_update_contacts) against the registered layouts:
-    contacts only for the contact type ids, and the accumulated impulses hold their penetration rows (convex: 2 tangent + n + 1 twist,
-    nonconvex: 3 per contact)."""
+    """native.contact_count (the feature-id layout of bepucuda_set_contact_features / bepucuda_update_contacts) and bp.type_info against the
+    reference's layouts (tests/golden/type_layouts.json): one contact per depth row and one penetration impulse per contact, 0 for joints and ids
+    without a type, and the bodies and row counts of every type."""
     for type_id in range(64):
         info, n = bp.type_info(type_id), native.contact_count(type_id)
-        if info is None or type_id >= 22:
-            assert n == 0, type_id
+        assert n == planner.contacts(type_id), type_id
+        if type_id not in planner.TYPE_LAYOUTS:
+            assert info is None, type_id
             continue
-        assert n > 0 and info[2] == (n + 3 if type_id < 8 else 3 * n), type_id
+        ref = planner.TYPE_LAYOUTS[type_id]
+        assert info == (ref["bodies"], len(ref["prestep_rows"]), len(ref["impulse_rows"])), type_id
+        assert len(planner.penetration_rows(type_id)) == n, type_id
 
 
 def test_no_cpu_fallback_without_a_device(libs):

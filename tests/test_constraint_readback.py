@@ -9,12 +9,13 @@ import pytest
 import bepuphysics2_b200 as bp
 from bepuphysics2_b200 import scenes, sharding
 from bepuphysics2_b200.native import ERR_BAD_STATE, ERR_INVALID_ARGUMENT, EXEC_GRAPH, EXEC_STREAM
-from tests import util
+from tests import planner, util
 from tests.planner import constraints_of, inverse_of, plan, sim_sources
 from tests.resident import initial_features, narrow_phase_like_update, push_bodies
 
 DT = 1.0 / 60.0
-CONVEX, NONCONVEX = set(range(8)), {8, 9, 10, 15, 16, 17}
+CONVEX = {t for t in planner.CONTACT_TYPES if "Normal.X" in planner.TYPE_LAYOUTS[t]["prestep_rows"]}  # one normal per manifold
+NONCONVEX = planner.CONTACT_TYPES - CONVEX
 
 
 # ---- CPU: the inverse slot map -------------------------------------------------------------------------------------------------------------

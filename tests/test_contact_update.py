@@ -11,7 +11,7 @@ import bepuphysics2_b200 as bp
 from bepuphysics2_b200 import scenes
 from bepuphysics2_b200.native import ERR_BAD_STATE, ERR_INVALID_ARGUMENT, EXEC_STREAM, contact_count
 from oracle import binding as ob
-from tests import resident, util
+from tests import planner, resident, util
 
 DT = 1.0 / 60.0
 
@@ -42,12 +42,6 @@ def test_redistribute_impulses_known_answers(libs):
     assert np.array_equal(_redistribute([1, 2, 3], [3, 5, 7], [2]), np.array([5], dtype=np.float32))
     # duplicate ids: the inner loop always stops at the FIRST old contact with the id (only its impulse is zeroed, L96-101), so the second new contact matches it again and gets 0
     assert np.array_equal(_redistribute([5, 5], [2, 6], [5, 5]), np.array([2, 0], dtype=np.float32))
-
-
-def _penetration_rows(type_id):
-    """Rows of the penetration impulses among a contact constraint's accumulated impulses (ContactConstraintAccessor.cs:L58-76)."""
-    n = contact_count(type_id)
-    return [2 + i for i in range(n)] if type_id < 8 else [3 * i + 2 for i in range(n)]
 
 
 def _pile(nonconvex=0.0):
@@ -113,7 +107,7 @@ def _all_contact_types_scene(seed=3):
     batch sits whole in batch 0). Bodies and prestep rows come from the seeded pile."""
     pile = scenes.shape_pile(3000, seed=seed, nonconvex_fraction=0.5)
     by_type = {int(t): (h, p) for t, h, p in pile["constraints"]}
-    types = [0, 1, 2, 3, 4, 5, 6, 7, 8, 9, 10, 15, 16, 17]
+    types = sorted(planner.CONTACT_TYPES)
     assert all(t in by_type for t in types)
     constraints, next_body = [], 0
     for i, t in enumerate(types):
@@ -176,12 +170,12 @@ def test_redistribution_edges_through_the_kernel(libs):
         assert n and th.batch_index == 0
         counts.add(th.constraint_count)
         acc = rng.uniform(-1, 1, size=th.accumulated_impulses.shape).astype(np.float32)  # friction / twist rows: ordinary values, both signs
-        for r in _penetration_rows(th.type_id):
+        for r in planner.penetration_rows(th.type_id):
             acc[:, r, :] = values[rng.integers(0, values.size, size=acc[:, r, :].shape)]
         th.accumulated_impulses[:] = acc
         td.accumulated_impulses[:] = acc
         old_ids[key], new_ids[key] = _crafted_ids(rng, th.constraint_count, n)
-    assert sorted({tb.type_id for tb in host.type_batches()}) == [0, 1, 2, 3, 4, 5, 6, 7, 8, 9, 10, 15, 16, 17] and counts == {1, 33}
+    assert {tb.type_id for tb in host.type_batches()} == planner.CONTACT_TYPES and counts == {1, 33}
     ts = bp.CudaTimestepper(dev, strict_fp=True)
     try:
         ts.describe()
@@ -196,7 +190,7 @@ def test_redistribution_edges_through_the_kernel(libs):
         key = (tb.batch_index, tb.type_batch_index)
         ob.update_contact_impulses(tb, old_ids[key], new_ids[key])
     util.compare(util.snapshot(host), util.snapshot(dev) | {"bodies": host.bodies}, exact=True)
-    pen = np.concatenate([tb.accumulated_impulses[:, _penetration_rows(tb.type_id), :].ravel() for tb in host.type_batches()])
+    pen = np.concatenate([tb.accumulated_impulses[:, planner.penetration_rows(tb.type_id), :].ravel() for tb in host.type_batches()])
     assert np.isinf(pen).any() and (pen == 0).any() and ((pen > 0) & (pen < np.finfo(np.float32).tiny)).any()
 
 

@@ -11,7 +11,7 @@ import os
 import numpy as np
 
 from oracle import binding as ob
-from tests import device_source, util
+from tests import device_source, planner, util
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 DT = 1.0 / 240.0  # a substep of the 8 x 2 configuration at 1/30 s
@@ -163,9 +163,13 @@ def test_redistribution_source_matches_the_oracle_on_every_id_pattern(libs):
     """csrc/bepu_redistribute.cuh (the per-constraint body of redistribute_impulses_kernel) against oracle_update_contact_impulses bit for bit, for
     every id-equality pattern at n = 1-4 contacts (duplicates in old, in new and in both, nothing matched, all matched and permuted), with impulses
     of 0, subnormals, ordinary values and values near FLT_MAX (remainders that overflow to inf). Then against float64: a matched contact carries
-    its old impulse exactly (0 included: it stays matched), an unmatched one the remainder / unmatched count to within fp32 rounding."""
+    its old impulse exactly (0 included: it stays matched), an unmatched one the remainder / unmatched count to within fp32 rounding. The rows the
+    source redistributes are the reference's penetration impulses of every contact type."""
     dev, orc = device_source.load()
     i32p = C.POINTER(C.c_int32)
+    for type_id in sorted(planner.CONTACT_TYPES):
+        rows = [dev.device_on_host_penetration_impulse_row(type_id, i) for i in range(planner.contacts(type_id))]
+        assert rows == planner.penetration_rows(type_id), "type %d: penetration_impulse_row %s" % (type_id, rows)
     for lib, name in ((dev, "device_on_host_update_contact_impulses"), (orc, "oracle_update_contact_impulses")):
         getattr(lib, name).argtypes = [C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
     fmax = np.finfo(np.float32).max
@@ -177,7 +181,7 @@ def test_redistribution_source_matches_the_oracle_on_every_id_pattern(libs):
         cases = old_ids.shape[0]
         assert cases == (n + 1) ** (2 * n)
         # the type ids with n contacts: convex one- and two-body, nonconvex (2-4 contacts) one- and two-body
-        types = [n - 1, n + 3] + ([n + 6, n + 13] if n >= 2 else [])
+        types = [t for t in sorted(planner.CONTACT_TYPES) if planner.contacts(t) == n]
         for trial, type_id in enumerate(types):
             bodies, _, impulse_rows = ob.type_info(type_id)
             W = (1, 8, 16, 4)[trial]
@@ -188,7 +192,7 @@ def test_redistribution_source_matches_the_oracle_on_every_id_pattern(libs):
             else:
                 old_imp[::3] = pool[rng.integers(pool.size - 3, pool.size, size=old_imp[::3].shape)]  # near FLT_MAX only: remainders overflow
             acc = rng.normal(0, 1, size=(bundles, impulse_rows, W)).astype(np.float32)  # tangent / twist rows: must come out untouched
-            penetration = [2 + i for i in range(n)] if type_id < 8 else [3 * i + 2 for i in range(n)]
+            penetration = planner.penetration_rows(type_id)
             c = np.arange(cases)
             for i, r in enumerate(penetration):
                 acc[c // W, r, c % W] = old_imp[:, i]

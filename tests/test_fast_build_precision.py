@@ -21,14 +21,13 @@ from bepuphysics2_b200 import native, scenes
 from bepuphysics2_b200.native import EXEC_GRAPH
 from oracle import binding as ob
 from tests import harness, planner, util
-from tests.planner import DEEP_BUNDLES
+from tests.planner import CONTACT_TYPES, DEEP_BUNDLES
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 DRIVER = os.path.join(ROOT, "tests", "precision", "isolated_solve.cpp")
 DT = 1.0 / 60.0
 LANES = 32  # device bundle width
 REFERENCE_MASK = 0x3FFFFFFF  # body index of an encoded body reference
-CONTACT_TYPES = {0, 1, 2, 3, 4, 5, 6, 7, 8, 9, 10, 15, 16, 17}
 RAGDOLL_TYPES = {22, 25, 26, 27, 29, 30, 46, 47}
 ALL_TYPES = CONTACT_TYPES | RAGDOLL_TYPES | set(scenes.JOINT_ZOO_TYPES)
 BODY_QUANTITIES = {"position": np.r_[4:7], "orientation": np.r_[0:4], "linear velocity": np.r_[8:11], "angular velocity": np.r_[12:15]}

@@ -7,7 +7,7 @@ import pytest
 
 import bepuphysics2_b200 as bp
 from bepuphysics2_b200 import scenes
-from tests import util
+from tests import planner, util
 
 DT = 1.0 / 60.0
 
@@ -174,10 +174,9 @@ def _inactive(scene):
     out = {"bodies": scene["bodies"].copy(), "constraints": [], "description": scene.get("description", "")}
     for type_id, handles, pre in scene["constraints"]:
         pre = pre.copy()
-        assert type_id <= 7  # convex manifolds: depth rows are 4 i + 3
-        contacts = type_id % 4 + 1
-        for i in range(contacts):
-            pre[:, 4 * i + 3] = -100.0
+        rows = planner.depth_rows(type_id)
+        assert rows  # contacts only: a joint would still apply impulses
+        pre[:, rows] = -100.0
         out["constraints"].append((type_id, handles, pre))
     return out
 

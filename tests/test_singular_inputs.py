@@ -32,8 +32,8 @@ GOLDEN = os.path.join(ROOT, "tests", "golden", "reference_singular_vectors.npz")
 DT_LANE = 1.0 / 240.0  # the generator's dt
 DT = 1.0 / 60.0
 HEADERS = ("bepu_device_math.cuh", "bepu_contacts.cuh", "bepu_joints.cuh", "bepu_joints_more.cuh", "bepu_integration.cuh")
-CONTACT_TYPES = (0, 1, 2, 3, 4, 5, 6, 7, 8, 9, 10, 15, 16, 17)
-ONE_BODY_CONTACTS, TWO_BODY_CONTACTS = (0, 1, 2, 3, 8, 9, 10), (4, 5, 6, 7, 15, 16, 17)
+CONTACT_TYPES = tuple(sorted(planner.CONTACT_TYPES))
+ONE_BODY_CONTACTS, TWO_BODY_CONTACTS = ([t for t in CONTACT_TYPES if planner.TYPE_LAYOUTS[t]["bodies"] == n] for n in (1, 2))
 
 
 @pytest.fixture(scope="module")

@@ -14,8 +14,7 @@ from oracle import binding as ob
 from tests import planner
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-with open(os.path.join(ROOT, "tests", "golden", "type_layouts.json")) as f:
-    FIXTURE = {int(k): v for k, v in json.load(f)["types"].items()}
+FIXTURE = planner.TYPE_LAYOUTS
 
 
 def _compact(rows):

@@ -8,17 +8,17 @@ import numpy as np
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))))
 import bepuphysics2_b200 as bp
 from bepuphysics2_b200 import scenes
+from bepuphysics2_b200.native import contact_count
 
 sim = bp.Simulation(bundle_width=8, substeps=8, velocity_iterations=2)
 scenes.build(scenes.shape_pile(100_000, seed=5), sim)
 ts = bp.CudaTimestepper(sim)
 ts.register_host_buffers()
-count = lambda tid: (tid & 3) + 1 if tid <= 7 else (tid - 6 if tid <= 10 else tid - 13)
-tbs = [tb for tb in sim.type_batches() if tb.type_id <= 17]
-pool = np.random.default_rng(1).integers(0, 1 << 20, size=sum(tb.constraint_count * count(tb.type_id) for tb in tbs), dtype=np.int32)
+tbs = [tb for tb in sim.type_batches() if contact_count(tb.type_id)]
+pool = np.random.default_rng(1).integers(0, 1 << 20, size=sum(tb.constraint_count * contact_count(tb.type_id) for tb in tbs), dtype=np.int32)
 feats, at = {}, 0
 for tb in tbs:
-    n = tb.constraint_count * count(tb.type_id)
+    n = tb.constraint_count * contact_count(tb.type_id)
     feats[(tb.batch_index, tb.type_batch_index)] = pool[at:at + n].reshape(tb.constraint_count, -1)
     at += n
 ts.register_array(pool)
