@@ -115,4 +115,50 @@ void launch_color_round(const ColoringBuffers& cb, int round, cudaStream_t s) {
     color_assign_kernel<<<grid, 256, 0, s>>>(cb, round);
 }
 
+// Stages the references (and the priorities, given for order 2 only), runs rounds in chunks until every constraint has a batch, and copies the batch
+// indices to batch_indices_out (host). *rounds: the rounds run, or -1 if a round assigned nothing (an internal error). A failing CUDA call
+// returns its error, and its text in *failed.
+#define CHECK(call) do { const cudaError_t _e = (call); if (_e != cudaSuccess) { *failed = #call; return _e; } } while (0)
+cudaError_t color_constraints(ColoringScratch& scratch, int32_t constraint_count, int32_t bodies_per_constraint, const int32_t* encoded_body_references, int32_t body_count,
+                              int32_t fallback_threshold, int32_t order, const uint32_t* priorities, int32_t* batch_indices_out, int64_t* rounds, const char** failed, cudaStream_t s) {
+    constexpr int kRoundsPerChunk = 32;  // even: the ping-pong lists return to their starting roles after every chunk
+    const size_t words = (size_t)constraint_count * bodies_per_constraint, nb = (size_t)std::max(body_count, 1), nc = (size_t)constraint_count;
+    CHECK(scratch.refs.reserve(words * 4));
+    CHECK(scratch.priorities.reserve(nc * 4));
+    CHECK(scratch.body_min.reserve(nb * 8));
+    CHECK(scratch.body_mask.reserve(nb * 8));
+    CHECK(scratch.out.reserve(nc * 4));
+    CHECK(scratch.lists.reserve(nc * 8));
+    CHECK(scratch.counts.reserve((kRoundsPerChunk + 1) * 4));
+    CHECK(cudaMemcpyAsync(scratch.refs.ptr, encoded_body_references, words * 4, cudaMemcpyHostToDevice, s));
+    if (priorities) CHECK(cudaMemcpyAsync(scratch.priorities.ptr, priorities, nc * 4, cudaMemcpyHostToDevice, s));
+    const ColoringBuffers cb{scratch.refs.as<int32_t>(), scratch.priorities.as<uint32_t>(), scratch.body_min.as<unsigned long long>(), scratch.body_mask.as<unsigned long long>(),
+                             scratch.out.as<int32_t>(), {scratch.lists.as<int32_t>(), scratch.lists.as<int32_t>() + nc}, scratch.counts.as<unsigned int>(), constraint_count,
+                             bodies_per_constraint, body_count, fallback_threshold, order};
+    CHECK(cudaMemsetAsync(scratch.counts.ptr, 0, (kRoundsPerChunk + 1) * 4, s));
+    launch_color_init(cb, s);
+    unsigned int counts[kRoundsPerChunk + 1];
+    *rounds = 0;
+    for (;;) {
+        for (int r = 0; r < kRoundsPerChunk; ++r) launch_color_round(cb, r, s);
+        CHECK(cudaMemcpyAsync(counts, scratch.counts.ptr, sizeof(counts), cudaMemcpyDeviceToHost, s));
+        CHECK(cudaStreamSynchronize(s));
+        CHECK(cudaGetLastError());
+        int used = kRoundsPerChunk;
+        for (int r = 0; r < kRoundsPerChunk; ++r)
+            if (counts[r + 1] == 0) { used = r + 1; break; }
+        *rounds += used;
+        if (counts[used] == 0) break;
+        // every round assigns at least the constraint with the globally lowest key, so the list shrinks: the loop ends after at most constraint_count rounds
+        if (counts[kRoundsPerChunk] >= counts[0]) { *rounds = -1; return cudaSuccess; }
+        counts[0] = counts[kRoundsPerChunk];
+        for (int r = 1; r <= kRoundsPerChunk; ++r) counts[r] = 0;
+        CHECK(cudaMemcpyAsync(scratch.counts.ptr, counts, sizeof(counts), cudaMemcpyHostToDevice, s));
+        CHECK(cudaStreamSynchronize(s));  // `counts` is a stack array: the copy must have read it before the next chunk's download overwrites it
+    }
+    CHECK(cudaMemcpyAsync(batch_indices_out, scratch.out.ptr, nc * 4, cudaMemcpyDeviceToHost, s));
+    CHECK(cudaStreamSynchronize(s));
+    return cudaSuccess;
+}
+
 }  // namespace bepucuda

@@ -4,6 +4,8 @@
 #include <cuda_runtime.h>
 #include <cstdint>
 
+#include "bepu_cuda_handles.h"
+
 namespace bepucuda {
 
 // Priority key of constraint c: constraints are assigned in ascending key order; ties cannot occur (the low word is the constraint index).
@@ -35,5 +37,10 @@ struct ColoringBuffers {
 // entries), appends the rest to list[(round + 1) & 1] / counts[round + 1], which must be zero beforehand.
 void launch_color_init(const ColoringBuffers& cb, cudaStream_t s);
 void launch_color_round(const ColoringBuffers& cb, int round, cudaStream_t s);
+
+// bepucuda_color_constraints for checked arguments (bepu_coloring.cu). `scratch` keeps its device buffers from call to call.
+struct ColoringScratch { DeviceBuffer refs, priorities, body_min, body_mask, out, lists, counts; };
+cudaError_t color_constraints(ColoringScratch& scratch, int32_t constraint_count, int32_t bodies_per_constraint, const int32_t* encoded_body_references, int32_t body_count,
+                              int32_t fallback_threshold, int32_t order, const uint32_t* priorities, int32_t* batch_indices_out, int64_t* rounds, const char** failed, cudaStream_t s);
 
 }  // namespace bepucuda

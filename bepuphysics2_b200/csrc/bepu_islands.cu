@@ -125,4 +125,59 @@ cudaError_t launch_island_select(const IslandBuffers& ib, uint8_t* flags, int32_
     return cudaGetLastError();
 }
 
+// Stages the activities (8 bytes per body), runs rounds until one changes nothing, and copies the island of every body to island_of_body_out
+// (host, optional), the sleepable roots and their body counts to roots_out / counts_out (host) and their number to *sleepable_count. *rounds: the
+// rounds run, or -1 if they outnumbered the bodies (an internal error). A failing CUDA call returns its error, and its text in *failed.
+#define CHECK(call) do { const cudaError_t _e = (call); if (_e != cudaSuccess) { *failed = #call; return _e; } } while (0)
+cudaError_t find_sleepable_islands(IslandScratch& scratch, const DeviceTypeBatch* tbs, const WorkItem* work, int32_t work_count, const void* activities, int32_t body_count,
+                                   int32_t* island_of_body_out, int32_t* roots_out, int32_t* counts_out, int32_t* sleepable_count, int64_t* rounds, const char** failed, cudaStream_t s) {
+    const size_t n = (size_t)body_count;
+    CHECK(scratch.activities.reserve(n * 8));
+    CHECK(scratch.label.reserve(n * 4));
+    CHECK(scratch.blocked.reserve(n * 4));
+    CHECK(scratch.count.reserve(n * 4));
+    CHECK(scratch.flags.reserve(n));
+    CHECK(scratch.roots.reserve(n * 4));
+    CHECK(scratch.counts.reserve(n * 4));
+    CHECK(scratch.scalars.reserve(8));  // [0]: hook pass changed something, [1]: number of sleepable roots
+    const IslandBuffers ib{tbs, work, work_count, scratch.activities.as<uint8_t>(), scratch.label.as<int32_t>(), scratch.blocked.as<int32_t>(), scratch.count.as<int32_t>(),
+                           scratch.scalars.as<unsigned int>(), body_count};
+    int32_t* selected = scratch.scalars.as<int32_t>() + 1;
+    size_t temp_bytes = 0;
+    CHECK(launch_island_select(ib, nullptr, nullptr, nullptr, selected, nullptr, &temp_bytes, s));
+    CHECK(scratch.temp.reserve(std::max(temp_bytes, (size_t)16)));
+    temp_bytes = scratch.temp.capacity;
+    CHECK(cudaMemcpyAsync(scratch.activities.ptr, activities, n * 8, cudaMemcpyHostToDevice, s));
+    launch_island_init(ib, s);
+    CHECK(cudaGetLastError());
+    // every round that changes something joins at least two trees, so there are at most body_count of them; in practice O(log n)
+    *rounds = 0;
+    if (work_count > 0) {
+        for (;;) {
+            CHECK(cudaMemsetAsync(ib.changed, 0, 4, s));
+            launch_island_round(ib, s);
+            unsigned int changed = 0;
+            CHECK(cudaMemcpyAsync(&changed, ib.changed, 4, cudaMemcpyDeviceToHost, s));
+            CHECK(cudaStreamSynchronize(s));
+            CHECK(cudaGetLastError());
+            ++*rounds;
+            if (!changed) break;
+            if (*rounds > (int64_t)body_count) { *rounds = -1; return cudaSuccess; }
+        }
+    }
+    launch_island_verdict(ib, s);
+    CHECK(launch_island_select(ib, scratch.flags.as<uint8_t>(), scratch.roots.as<int32_t>(), scratch.counts.as<int32_t>(), selected, scratch.temp.ptr, &temp_bytes, s));
+    int32_t count = 0;
+    CHECK(cudaMemcpyAsync(&count, selected, 4, cudaMemcpyDeviceToHost, s));
+    if (island_of_body_out) CHECK(cudaMemcpyAsync(island_of_body_out, ib.label, n * 4, cudaMemcpyDeviceToHost, s));
+    CHECK(cudaStreamSynchronize(s));
+    if (count > 0) {
+        CHECK(cudaMemcpyAsync(roots_out, scratch.roots.ptr, (size_t)count * 4, cudaMemcpyDeviceToHost, s));
+        CHECK(cudaMemcpyAsync(counts_out, scratch.counts.ptr, (size_t)count * 4, cudaMemcpyDeviceToHost, s));
+        CHECK(cudaStreamSynchronize(s));
+    }
+    *sleepable_count = count;
+    return cudaSuccess;
+}
+
 }  // namespace bepucuda

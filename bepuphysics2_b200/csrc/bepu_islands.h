@@ -6,6 +6,7 @@
 #include <cuda_runtime.h>
 #include <cstdint>
 
+#include "bepu_cuda_handles.h"
 #include "bepu_device_types.h"
 #include "bepu_layout_kernels.h"
 
@@ -34,5 +35,10 @@ void launch_island_verdict(const IslandBuffers& ib, cudaStream_t s);
 // scratch (temp == nullptr: *temp_bytes receives the size needed and nothing is launched). flags: body_count bytes of scratch.
 cudaError_t launch_island_select(const IslandBuffers& ib, uint8_t* flags, int32_t* roots_out, int32_t* counts_out, int32_t* selected, void* temp, size_t* temp_bytes,
                                  cudaStream_t s);
+
+// bepucuda_find_sleepable_islands for checked arguments (bepu_islands.cu). `scratch` keeps its device buffers from call to call.
+struct IslandScratch { DeviceBuffer activities, label, blocked, count, flags, roots, counts, scalars, temp; };
+cudaError_t find_sleepable_islands(IslandScratch& scratch, const DeviceTypeBatch* tbs, const WorkItem* work, int32_t work_count, const void* activities, int32_t body_count,
+                                   int32_t* island_of_body_out, int32_t* roots_out, int32_t* counts_out, int32_t* sleepable_count, int64_t* rounds, const char** failed, cudaStream_t s);
 
 }  // namespace bepucuda

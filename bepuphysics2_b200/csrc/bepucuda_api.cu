@@ -12,76 +12,12 @@
 #include "bepu_coloring.h"
 #include "bepu_islands.h"
 #include "bepu_bounds.h"
+#include "bepu_cuda_handles.h"
 #include "bepu_topology.h"
 
 using namespace bepucuda;
 
 namespace bepucuda {
-
-// ---- small RAII helpers ------------------------------------------------------------------------------------------------------
-// Memory that grows on demand (contents are not kept) and is freed with its owner: device memory, or page-locked host memory.
-template <bool kPinnedHost> struct GrowBuffer {
-    void* ptr = nullptr;
-    size_t capacity = 0;
-    GrowBuffer() = default;
-    GrowBuffer(const GrowBuffer&) = delete;
-    GrowBuffer& operator=(const GrowBuffer&) = delete;
-    ~GrowBuffer() { release(); }
-    cudaError_t reserve(size_t bytes) {
-        if (bytes <= capacity) return cudaSuccess;
-        release();
-        size_t want = bytes + bytes / 4 + 256;
-        cudaError_t e = kPinnedHost ? cudaMallocHost(&ptr, want) : cudaMalloc(&ptr, want);
-        if (e == cudaSuccess) capacity = want;
-        else ptr = nullptr;
-        return e;
-    }
-    void release() {
-        if (ptr) kPinnedHost ? cudaFreeHost(ptr) : cudaFree(ptr);
-        ptr = nullptr;
-        capacity = 0;
-    }
-    template <class T> T* as() const { return (T*)ptr; }
-};
-using DeviceBuffer = GrowBuffer<false>;
-using PinnedBuffer = GrowBuffer<true>;
-
-// Bump allocator over chunks that are never reallocated (uploads are enqueued against their addresses).
-struct ChunkArena {
-    struct Chunk { char* base; size_t size, used; };
-    std::vector<Chunk> chunks;
-    bool pinned_host = false;
-    size_t min_chunk = (size_t)64 << 20;
-    ChunkArena() = default;
-    ChunkArena(const ChunkArena&) = delete;
-    ChunkArena& operator=(const ChunkArena&) = delete;
-    ~ChunkArena() {
-        for (auto& c : chunks) { if (pinned_host) cudaFreeHost(c.base); else cudaFree(c.base); }
-    }
-    void reset() { for (auto& c : chunks) c.used = 0; }
-    void* alloc(size_t bytes, cudaError_t* err) {
-        bytes = (bytes + 255) & ~(size_t)255;
-        for (auto& c : chunks)
-            if (c.size - c.used >= bytes) {
-                void* p = c.base + c.used;
-                c.used += bytes;
-                return p;
-            }
-        Chunk c{};
-        c.size = std::max(bytes, min_chunk);
-        cudaError_t e = pinned_host ? cudaMallocHost((void**)&c.base, c.size) : cudaMalloc((void**)&c.base, c.size);
-        if (e != cudaSuccess) { if (err) *err = e; return nullptr; }
-        c.used = bytes;
-        chunks.push_back(c);
-        return chunks.back().base;
-    }
-};
-
-// Pinned copy of a host buffer that the caller may reuse as soon as the upload is enqueued, and the event after which the copy has read it.
-struct StagedUpload {
-    PinnedBuffer host;
-    cudaEvent_t done = nullptr;
-};
 
 struct SourceTypeBatch {
     int batch_index, type_batch_index, type_id, count;
@@ -101,14 +37,27 @@ struct SourceTypeBatch {
     bool redistribute = false;
 };
 
+// The stage sequence of the program captured as a graph (dropped when the program is replaced), and the body buffers and launch context its
+// launches bake in besides the program: matches() says whether a frame can replay it.
+struct StageGraph {
+    Graph graph;
+    GraphExec exec;  // destroyed before the graph it was instantiated from
+    BodyBuffers bodies{};
+    LaunchContext launch{};
+    void reset() { exec.reset(); graph.reset(); }
+    bool matches(const BodyBuffers& b, const LaunchContext& lc) const {
+        return exec && bodies.pose == b.pose && bodies.velocity == b.velocity && bodies.inertia_local == b.inertia_local && bodies.inertia_world == b.inertia_world &&
+               bodies.constrained == b.constrained && bodies.first_batch == b.first_batch && bodies.count == b.count && same_launches(launch, lc);
+    }
+};
+
 }  // namespace bepucuda
 
 struct bepucuda_ctx {
     bepucuda_config cfg{};
     int device = 0;
-    cudaStream_t stream = nullptr;
-    cudaEvent_t ev_solve_begin = nullptr, ev_solve_end = nullptr, ev_up_begin = nullptr, ev_up_end = nullptr, ev_down_begin = nullptr, ev_down_end = nullptr;
-    bool up_open = false, have_solve = false, have_down = false, have_up = false;
+    Stream stream;  // declared before every other handle, so that it is destroyed after them
+    TimingWindow solve_window, upload_window, download_window;
     std::string error;
     const SolverLaunchers* launchers = nullptr;
 
@@ -148,7 +97,7 @@ struct bepucuda_ctx {
     uint32_t shard_solve_index = 0;                                 // solves since the arrival targets were last published
     std::vector<int> boundary_count;                                // per device batch: bundles that touch a body another rank references
     std::vector<uint8_t> body_masks;                                // bepucuda_shard_set_body_masks: per body, the ranks that reference it
-    std::vector<void*> opened_ipc;
+    std::vector<IpcMapping> opened_ipc;
     std::vector<int32_t> global_first_batch;
     DeviceBuffer global_first_batch_dev;
     std::vector<uint8_t> global_constrained;
@@ -161,11 +110,7 @@ struct bepucuda_ctx {
     int32_t hazard_canary = 0, hazard_delay_us = 0;  // BEPUCUDA_HAZARD at bepucuda_create (hazard build only, see hazard_launch_bits)
 #endif
 
-    // the captured stage sequence of the program (dropped when the program is replaced), and what its launches bake in besides the program
-    cudaGraph_t graph = nullptr;
-    cudaGraphExec_t graph_exec = nullptr;
-    BodyBuffers graph_bodies{};
-    LaunchContext graph_launch{};
+    StageGraph stage_graph;
 
     bepucuda_timings timings{};
     int64_t h2d_accum = 0;
@@ -175,16 +120,16 @@ struct bepucuda_ctx {
     DeviceBuffer chunk_table;
     StagedUpload chunk_stage[4];           // pinned ring for chunk tables
     int chunk_stage_next = 0;
-    cudaEvent_t user_events[16] = {};
+    Event user_events[16];
     DeviceBuffer body_shapes, body_activities, body_bounds;  // bepucuda_set_body_shapes / bepucuda_predict_bounding_boxes
     int shape_count = -1;
-    DeviceBuffer color_refs, color_priorities, color_body_min, color_body_mask, color_out, color_lists, color_counts;  // bepucuda_color_constraints
-    DeviceBuffer island_activities, island_label, island_blocked, island_count, island_flags, island_roots, island_counts, island_scalars, island_temp;  // bepucuda_find_sleepable_islands
+    ColoringScratch coloring;  // bepucuda_color_constraints
+    IslandScratch islands;     // bepucuda_find_sleepable_islands
     DeviceBuffer inverse_table, read_requests, read_records;  // bepucuda_read_constraints: the plan's inverse slot map, one call's requests and records
     PrestepWriteQueue prestep_writes;  // bepucuda_write_constraints since the last solve, applied by refresh_device_rows
     DeviceBuffer write_table, write_rows;
     StagedUpload write_stage, write_rows_stage;
-    std::vector<cudaEvent_t> profile_events;
+    std::vector<Event> profile_events;
 };
 
 namespace {
@@ -201,13 +146,12 @@ int cuda_fail(bepucuda_ctx* c, cudaError_t e, const char* what) {
         cudaError_t _e = (call);                                  \
         if (_e != cudaSuccess) return cuda_fail(ctx, _e, #call);  \
     } while (0)
-
-void open_upload_window(bepucuda_ctx* ctx) {
-    if (!ctx->up_open) {
-        cudaEventRecord(ctx->ev_up_begin, ctx->stream);
-        ctx->up_open = true;
-    }
-}
+// Returns a status other than BEPUCUDA_OK to the caller.
+#define TRY(expr)                                \
+    do {                                         \
+        const int _rc = (expr);                  \
+        if (_rc != BEPUCUDA_OK) return _rc;      \
+    } while (0)
 
 // Device alias of a host pointer if [ptr, ptr + bytes) lies inside a registered (mapped) range, else nullptr.
 char* map_host(bepucuda_ctx* ctx, const void* ptr, size_t bytes) {
@@ -222,7 +166,7 @@ void queue_chunks(std::vector<CopyChunk>& list, void* dst, const void* src, size
 }
 // H2D copy of `bytes` at `src` through the pinned staging buffer of `st`.
 int upload_staged(bepucuda_ctx* ctx, StagedUpload& st, void* dst, const void* src, size_t bytes) {
-    if (!st.done) CK(cudaEventCreateWithFlags(&st.done, cudaEventDisableTiming));
+    CK(st.done.create(cudaEventDisableTiming));
     CK(cudaEventSynchronize(st.done));  // the previous upload has left the staging buffer
     CK(st.host.reserve(bytes));
     std::memcpy(st.host.ptr, src, bytes);
@@ -239,7 +183,7 @@ int flush_chunks(bepucuda_ctx* ctx, std::vector<CopyChunk>& list) {
     StagedUpload& st = ctx->chunk_stage[ctx->chunk_stage_next];
     ctx->chunk_stage_next = (ctx->chunk_stage_next + 1) & 3;
     // The device-side table is reused by every flush: stream order keeps the previous batched copy ahead of this overwrite.
-    { int rc = upload_staged(ctx, st, ctx->chunk_table.ptr, list.data(), bytes); if (rc != BEPUCUDA_OK) return rc; }
+    TRY(upload_staged(ctx, st, ctx->chunk_table.ptr, list.data(), bytes));
     launch_batched_copy(ctx->chunk_table.as<CopyChunk>(), (int)list.size(), ctx->stream);
     CK(cudaGetLastError());
     list.clear();
@@ -266,17 +210,17 @@ int copy_in(bepucuda_ctx* ctx, void* dst, const void* src, size_t bytes) {
     return BEPUCUDA_OK;
 }
 
+// Reserves the device table `name` for the elements of `v` plus `slack` bytes, and queues their copy if there are any.
+template <class T> int upload_table(bepucuda_ctx* ctx, const char* name, DeviceBuffer& table, const std::vector<T>& v, size_t slack) {
+    cudaError_t e = table.reserve(v.size() * sizeof(T) + slack);
+    if (e == cudaSuccess && !v.empty()) e = cudaMemcpyAsync(table.ptr, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice, ctx->stream);
+    return e == cudaSuccess ? BEPUCUDA_OK : cuda_fail(ctx, e, name);
+}
+
 SourceTypeBatch* find_source(bepucuda_ctx* ctx, int32_t batch_index, int32_t type_batch_index) {
     for (auto& s : ctx->sources)
         if (s.batch_index == batch_index && s.type_batch_index == type_batch_index) return &s;
     return nullptr;
-}
-
-void invalidate_graph(bepucuda_ctx* ctx) {
-    if (ctx->graph_exec) cudaGraphExecDestroy(ctx->graph_exec);
-    if (ctx->graph) cudaGraphDestroy(ctx->graph);
-    ctx->graph_exec = nullptr;
-    ctx->graph = nullptr;
 }
 
 // The optional velocity terms that are set (bepucuda_set_body_accelerations / bepucuda_set_point_gravity): kIntegrateAccelerations |
@@ -302,14 +246,10 @@ void read_hazard_environment(bepucuda_ctx* ctx) {
 }
 #endif
 LaunchContext launch_context(const bepucuda_ctx* ctx, bool profile) { return {integrate_extensions(ctx) != 0, ctx->integ.angular_integration_mode, profile}; }
-bool same_bodies(const BodyBuffers& a, const BodyBuffers& b) {
-    return a.pose == b.pose && a.velocity == b.velocity && a.inertia_local == b.inertia_local && a.inertia_world == b.inertia_world && a.constrained == b.constrained &&
-           a.first_batch == b.first_batch && a.count == b.count;
-}
 
 // Profiling sink of issue_stage_sequence: the launch of program op i sets launched[i] and is bracketed by events[2i] and events[2i + 1].
 struct StageEvents {
-    const std::vector<cudaEvent_t>& events;
+    const std::vector<Event>& events;
     std::vector<int>& launched;
 };
 
@@ -368,7 +308,7 @@ int upload_program(bepucuda_ctx* ctx) {
     ctx->constraints_ready = false;
     // work issued under the previous program completes before that program and its graph are replaced
     CK(cudaStreamSynchronize(ctx->stream));
-    invalidate_graph(ctx);
+    ctx->stage_graph.reset();
     ctx->program = build_stage_program(ctx->topo, ctx->iterations, (int)ctx->kinematics.size(), ctx->integ.integrate_velocity_for_kinematics != 0, ctx->peer_mode,
                                        ctx->body_count);
     if (ctx->peer_mode) {
@@ -438,6 +378,26 @@ std::string no_constraint_at(int32_t i, const bepucuda_constraint_location& l) {
            ", index " + std::to_string(l.index_in_type_batch) + ") names no constraint of the active set";
 }
 
+// The prologue of bepucuda_read_constraints / bepucuda_write_constraints (`name`, `write`): the state and argument checks, then every location
+// resolved and, for a write, checked against its record. All of it runs before any device work or queueing, so a failing call changes nothing.
+int resolve_locations(bepucuda_ctx* ctx, const std::string& name, int32_t count, const bepucuda_constraint_location* locations, const int32_t* records, bool write,
+                      std::vector<ResolvedLocation>* resolved) {
+    if (ctx->peer_mode) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, name + " in peer mode: a rank holds its constraints compacted, so host locations do not address them");
+    if (!ctx->constraints_ready) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, name + " before end_constraints");
+    if (count < 0 || (count > 0 && (!locations || !records))) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, name + ": bad arguments");
+    resolved->resize((size_t)count);
+    for (int32_t i = 0; i < count; ++i) {
+        const bepucuda_constraint_location& l = locations[i];
+        ResolvedLocation& r = (*resolved)[(size_t)i];
+        if (resolve_location(ctx->topo, l, &r) != BEPUCUDA_OK) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, name + ": " + no_constraint_at(i, l));
+        if (write && r.at.type_batch < 0) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, name + ": " + no_constraint_at(i, l) + " (a hole of the fallback batch)");
+        if (write && records[(size_t)i * 64] != l.type_id)
+            return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, name + ": record " + std::to_string(i) + " has type id " + std::to_string(records[(size_t)i * 64]) +
+                                                                ", its location type id " + std::to_string(l.type_id));
+    }
+    return BEPUCUDA_OK;
+}
+
 // Accelerations set for another body count than the current one index the wrong bodies: solve, profile_stages and predict_bounding_boxes refuse
 // to run before any device work.
 int check_accelerations(bepucuda_ctx* ctx, const char* what) {
@@ -453,7 +413,7 @@ int check_accelerations(bepucuda_ctx* ctx, const char* what) {
 // of the same frame. A frame that refreshes every type batch in full (bepuhost_cuda_refresh) leaves the descriptors as end_constraints uploaded them.
 int refresh_device_rows(bepucuda_ctx* ctx) {
     if (!ctx->data_dirty) return BEPUCUDA_OK;
-    { int rc = flush_chunks(ctx, ctx->pending_h2d); if (rc != BEPUCUDA_OK) return rc; }
+    TRY(flush_chunks(ctx, ctx->pending_h2d));
     bool any_pending = false, any_redistribute = false, descs_changed = false;
     for (size_t tb = 0; tb < ctx->topo.tbs.size(); ++tb) {
         const SourceTypeBatch& s = ctx->sources[(size_t)ctx->topo.tbs[tb].source];
@@ -480,8 +440,8 @@ int refresh_device_rows(bepucuda_ctx* ctx) {
         const size_t bytes = q.writes.size() * sizeof(PrestepWrite), row_bytes = q.rows.size() * sizeof(float);
         CK(ctx->write_table.reserve(bytes));
         CK(ctx->write_rows.reserve(row_bytes));
-        { int rc = upload_staged(ctx, ctx->write_stage, ctx->write_table.ptr, q.writes.data(), bytes); if (rc != BEPUCUDA_OK) return rc; }
-        { int rc = upload_staged(ctx, ctx->write_rows_stage, ctx->write_rows.ptr, q.rows.data(), row_bytes); if (rc != BEPUCUDA_OK) return rc; }
+        TRY(upload_staged(ctx, ctx->write_stage, ctx->write_table.ptr, q.writes.data(), bytes));
+        TRY(upload_staged(ctx, ctx->write_rows_stage, ctx->write_rows.ptr, q.rows.data(), row_bytes));
         ctx->h2d_accum += (int64_t)(bytes + row_bytes);
         launch_write_constraints(ctx->tb_table.as<DeviceTypeBatch>(), ctx->tdesc_table.as<TransposeDesc>(), ctx->write_table.as<PrestepWrite>(), ctx->write_rows.as<float>(),
                                  (int)q.writes.size(), ctx->stream);
@@ -500,17 +460,13 @@ int refresh_device_rows(bepucuda_ctx* ctx) {
 // What a frame of length dt needs on the device before its first stage: the refreshed rows, the end of the upload window (bepucuda_timings
 // upload_ms / h2d_bytes) and the frame parameters.
 int prepare_frame(bepucuda_ctx* ctx, float dt) {
-    { int rc = refresh_device_rows(ctx); if (rc != BEPUCUDA_OK) return rc; }
-    if (ctx->up_open) {
-        cudaEventRecord(ctx->ev_up_end, ctx->stream);
-        ctx->up_open = false;
-        ctx->have_up = true;
-    }
+    TRY(refresh_device_rows(ctx));
+    if (ctx->upload_window.open) ctx->upload_window.stop(ctx->stream);
     ctx->timings.h2d_bytes = ctx->h2d_accum;
     ctx->h2d_accum = 0;
     // frame parameters (previous solve's copy has completed by stream order only after its graph, a stage profile's before it returned; wait for
     // it before reusing the pinned struct)
-    CK(cudaEventSynchronize(ctx->ev_solve_end));
+    CK(cudaEventSynchronize(ctx->solve_window.end));
     FrameParams* fp = ctx->frame_params_host.as<FrameParams>();
     compute_frame_params(ctx, dt, fp);
     fp->exchange_base = ctx->exchange_counter;
@@ -549,10 +505,9 @@ int32_t bepucuda_create(const bepucuda_config* cfg, bepucuda_ctx** out) {
     read_hazard_environment(ctx);
 #endif
     cudaError_t e = cudaSetDevice(ctx->device);
-    if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking);
-    cudaEvent_t* evs[] = {&ctx->ev_solve_begin, &ctx->ev_solve_end, &ctx->ev_up_begin, &ctx->ev_up_end, &ctx->ev_down_begin, &ctx->ev_down_end};
-    for (auto ev : evs)
-        if (e == cudaSuccess) e = cudaEventCreate(ev);
+    if (e == cudaSuccess) e = cudaStreamCreateWithFlags(ctx->stream.put(), cudaStreamNonBlocking);
+    for (TimingWindow* w : {&ctx->solve_window, &ctx->upload_window, &ctx->download_window})
+        for (Event* ev : {&w->begin, &w->end}) e = e == cudaSuccess ? ev->create() : e;
     if (e == cudaSuccess) e = ctx->frame_params_host.reserve(sizeof(FrameParams));
     if (e == cudaSuccess) e = ctx->frame_params_dev.reserve(sizeof(FrameParams));
     if (e == cudaSuccess) e = ctx->error_dev.reserve(8 * sizeof(int32_t));
@@ -572,18 +527,7 @@ int32_t bepucuda_destroy(bepucuda_ctx* ctx) {
     if (!ctx) return BEPUCUDA_OK;
     cudaSetDevice(ctx->device);
     if (ctx->stream) cudaStreamSynchronize(ctx->stream);
-    invalidate_graph(ctx);
-    for (void* p : ctx->opened_ipc) cudaIpcCloseMemHandle(p);
-    cudaEvent_t evs[] = {ctx->ev_solve_begin, ctx->ev_solve_end, ctx->ev_up_begin, ctx->ev_up_end, ctx->ev_down_begin, ctx->ev_down_end, ctx->accelerations_stage.done};
-    for (auto ev : evs)
-        if (ev) cudaEventDestroy(ev);
-    for (auto ev : ctx->user_events)
-        if (ev) cudaEventDestroy(ev);
-    for (auto& st : ctx->chunk_stage)
-        if (st.done) cudaEventDestroy(st.done);
-    for (auto ev : ctx->profile_events) cudaEventDestroy(ev);
-    if (ctx->stream) cudaStreamDestroy(ctx->stream);
-    delete ctx;  // the device and pinned buffers free themselves, on the device set above
+    delete ctx;  // every handle and buffer frees itself, on the device set above, the stream last among the handles
     return BEPUCUDA_OK;
 }
 
@@ -617,7 +561,7 @@ int32_t bepucuda_set_solve_description(bepucuda_ctx* ctx, int32_t substep_count,
     const bool changed = v != ctx->iterations || threshold_changed;
     ctx->iterations = v;
     ctx->fallback_threshold = fallback_batch_threshold;
-    if (threshold_changed && ctx->constraints_ready) ctx->constraints_ready = false;  // fallback split must be redone
+    if (threshold_changed) ctx->constraints_ready = false;  // fallback split must be redone
     if (changed && ctx->constraints_ready) {
         CK(cudaSetDevice(ctx->device));
         return upload_program(ctx);
@@ -646,13 +590,12 @@ int32_t bepucuda_set_body_accelerations(bepucuda_ctx* ctx, const float* accelera
     }
     if (body_count != ctx->body_count) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "set_body_accelerations: the body count must match the last upload_bodies");
     CK(cudaSetDevice(ctx->device));
-    open_upload_window(ctx);
+    ctx->upload_window.start_once(ctx->stream);
     const size_t bytes = (size_t)body_count * 32;
     CK(ctx->accelerations.reserve(std::max(bytes, (size_t)32)));
     if (bytes > 0) {
         // through a pinned staging copy, so that the caller's buffer is free when the call returns without waiting for the device
-        int rc = upload_staged(ctx, ctx->accelerations_stage, ctx->accelerations.ptr, accelerations, bytes);
-        if (rc != BEPUCUDA_OK) return rc;
+        TRY(upload_staged(ctx, ctx->accelerations_stage, ctx->accelerations.ptr, accelerations, bytes));
         ctx->h2d_accum += (int64_t)bytes;
     }
     ctx->accelerations_count = body_count;
@@ -671,7 +614,7 @@ int32_t bepucuda_upload_bodies(bepucuda_ctx* ctx, const void* body_dynamics, int
     if (!ctx || body_count < 0 || (body_count > 0 && !body_dynamics)) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "upload_bodies: bad arguments");
     if ((uint32_t)body_count > kRefIndexMask) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "upload_bodies: too many bodies");
     CK(cudaSetDevice(ctx->device));
-    open_upload_window(ctx);
+    ctx->upload_window.start_once(ctx->stream);
     const size_t n = (size_t)body_count;
     // constrained flags / ownership depend on the body count; force a rebuild of topology products.
     if (body_count != ctx->body_count) ctx->constraints_ready = false;
@@ -684,15 +627,8 @@ int32_t bepucuda_upload_bodies(bepucuda_ctx* ctx, const void* body_dynamics, int
     CK(ctx->constrained.reserve(n + 1));
     if (ctx->constrained.capacity != old_constrained_cap) CK(cudaMemsetAsync(ctx->constrained.ptr, 0, ctx->constrained.capacity, ctx->stream));
     ctx->body_count = body_count;
-    BodyBuffers B{};
-    B.pose = ctx->pose.as<float4>();
-    B.velocity = ctx->velocity.as<float4>();
-    B.inertia_local = ctx->inertia_local.as<float4>();
-    B.inertia_world = ctx->inertia_world.as<float4>();
-    B.constrained = ctx->constrained.as<uint8_t>();
-    B.first_batch = ctx->first_batch.as<int32_t>();
-    B.count = body_count;
-    ctx->B = B;
+    ctx->B = {ctx->pose.as<float4>(), ctx->velocity.as<float4>(), ctx->inertia_local.as<float4>(), ctx->inertia_world.as<float4>(), ctx->constrained.as<uint8_t>(),
+              ctx->first_batch.as<int32_t>(), body_count};
     if (body_count > 0) {
         CK(cudaMemcpyAsync(ctx->raw_bodies.ptr, body_dynamics, n * 128, cudaMemcpyHostToDevice, ctx->stream));
         ctx->h2d_accum += (int64_t)n * 128;
@@ -706,7 +642,7 @@ int32_t bepucuda_begin_constraints(bepucuda_ctx* ctx, int32_t source_bundle_widt
     if (!ctx || source_bundle_width < 1 || source_bundle_width > 64 || batch_count < 0) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "begin_constraints: bad arguments");
     CK(cudaSetDevice(ctx->device));
     CK(cudaStreamSynchronize(ctx->stream));  // staging arenas are recycled below
-    open_upload_window(ctx);
+    ctx->upload_window.start_once(ctx->stream);
     ctx->W = source_bundle_width;
     ctx->batch_count = batch_count;
     ctx->sources.clear();
@@ -743,10 +679,9 @@ int32_t bepucuda_upload_type_batch(bepucuda_ctx* ctx, int32_t batch_index, int32
     s.raw_prestep = (float*)ctx->raw_arena.alloc(s.prestep_bytes, &e);
     s.raw_impulses = (float*)ctx->raw_arena.alloc(s.impulse_bytes, &e);
     if (!s.raw_refs || !s.raw_prestep || !s.raw_impulses) return cuda_fail(ctx, e, "raw arena");
-    int rc;
-    if ((rc = copy_in(ctx, s.raw_refs, body_references, s.refs_bytes)) != BEPUCUDA_OK) return rc;
-    if ((rc = copy_in(ctx, s.raw_prestep, prestep, s.prestep_bytes)) != BEPUCUDA_OK) return rc;
-    if ((rc = copy_in(ctx, s.raw_impulses, accumulated_impulses, s.impulse_bytes)) != BEPUCUDA_OK) return rc;
+    TRY(copy_in(ctx, s.raw_refs, body_references, s.refs_bytes));
+    TRY(copy_in(ctx, s.raw_prestep, prestep, s.prestep_bytes));
+    TRY(copy_in(ctx, s.raw_impulses, accumulated_impulses, s.impulse_bytes));
     if (batch_index >= ctx->fallback_threshold) s.host_refs.assign(body_references, body_references + s.refs_bytes / 4);
     ctx->sources.push_back(std::move(s));
     return BEPUCUDA_OK;
@@ -755,7 +690,7 @@ int32_t bepucuda_upload_type_batch(bepucuda_ctx* ctx, int32_t batch_index, int32
 int32_t bepucuda_set_constrained_kinematics(bepucuda_ctx* ctx, const int32_t* body_indices, int32_t count) {
     if (!ctx || count < 0 || (count > 0 && !body_indices)) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "set_constrained_kinematics: bad arguments");
     ctx->kinematics.assign(body_indices, body_indices + count);
-    if (ctx->constraints_ready) ctx->constraints_ready = false;
+    ctx->constraints_ready = false;
     return BEPUCUDA_OK;
 }
 
@@ -782,8 +717,8 @@ int32_t bepucuda_end_constraints(bepucuda_ctx* ctx) {
     CK(ctx->refs32.reserve(topo.refs_words * 4 + 1024));  // slack: solver warps always read two body-reference rows
     CK(ctx->prestep32.reserve(topo.prestep_words * 4 + 4));
     CK(ctx->impulses32.reserve(topo.impulse_words * 4 + 4));
-    CK(ctx->map_table.reserve(topo.maps.size() * 4 + 4));
-    CK(ctx->inverse_table.reserve(topo.inverse.size() * sizeof(DeviceSlot) + 8));
+    TRY(upload_table(ctx, "map_table", ctx->map_table, topo.maps, 4));
+    TRY(upload_table(ctx, "inverse_table", ctx->inverse_table, topo.inverse, 8));
     std::vector<DeviceTypeBatch> tbs(topo.tbs.size());
     ctx->tdescs.resize(topo.tbs.size());
     for (size_t i = 0; i < topo.tbs.size(); ++i) {
@@ -798,22 +733,14 @@ int32_t bepucuda_end_constraints(bepucuda_ctx* ctx) {
     ctx->records = work_records(topo, ctx->refs32.as<int32_t>(), ctx->prestep32.as<float>(), ctx->impulses32.as<float>());
 
     // ---- upload tables ----
-    CK(ctx->tb_table.reserve(tbs.size() * sizeof(DeviceTypeBatch) + 16));
-    CK(ctx->tdesc_table.reserve(ctx->tdescs.size() * sizeof(TransposeDesc) + 16));
-    CK(ctx->work_table.reserve(topo.work.size() * sizeof(WorkItem) + 16));
-    CK(ctx->record_table.reserve(ctx->records.size() * sizeof(WorkRecord) + 64));
-    CK(ctx->kinematics_dev.reserve(ctx->kinematics.size() * 4 + 4));
-    if (!tbs.empty()) CK(cudaMemcpyAsync(ctx->tb_table.ptr, tbs.data(), tbs.size() * sizeof(DeviceTypeBatch), cudaMemcpyHostToDevice, ctx->stream));
-    if (!ctx->tdescs.empty()) CK(cudaMemcpyAsync(ctx->tdesc_table.ptr, ctx->tdescs.data(), ctx->tdescs.size() * sizeof(TransposeDesc), cudaMemcpyHostToDevice, ctx->stream));
-    if (!topo.work.empty()) CK(cudaMemcpyAsync(ctx->work_table.ptr, topo.work.data(), topo.work.size() * sizeof(WorkItem), cudaMemcpyHostToDevice, ctx->stream));
-    if (!ctx->records.empty()) CK(cudaMemcpyAsync(ctx->record_table.ptr, ctx->records.data(), ctx->records.size() * sizeof(WorkRecord), cudaMemcpyHostToDevice, ctx->stream));
-    if (!topo.maps.empty()) CK(cudaMemcpyAsync(ctx->map_table.ptr, topo.maps.data(), topo.maps.size() * 4, cudaMemcpyHostToDevice, ctx->stream));
-    if (!topo.inverse.empty())
-        CK(cudaMemcpyAsync(ctx->inverse_table.ptr, topo.inverse.data(), topo.inverse.size() * sizeof(DeviceSlot), cudaMemcpyHostToDevice, ctx->stream));
-    if (!ctx->kinematics.empty()) CK(cudaMemcpyAsync(ctx->kinematics_dev.ptr, ctx->kinematics.data(), ctx->kinematics.size() * 4, cudaMemcpyHostToDevice, ctx->stream));
+    TRY(upload_table(ctx, "tb_table", ctx->tb_table, tbs, 16));
+    TRY(upload_table(ctx, "tdesc_table", ctx->tdesc_table, ctx->tdescs, 16));
+    TRY(upload_table(ctx, "work_table", ctx->work_table, topo.work, 16));
+    TRY(upload_table(ctx, "record_table", ctx->record_table, ctx->records, 64));
+    TRY(upload_table(ctx, "kinematics_dev", ctx->kinematics_dev, ctx->kinematics, 4));
 
     // ---- transposition into AOSOA-32 + ownership analysis ----
-    { int rc = flush_chunks(ctx, ctx->pending_h2d); if (rc != BEPUCUDA_OK) return rc; }
+    TRY(flush_chunks(ctx, ctx->pending_h2d));
     launch_transpose_in_all(ctx->tb_table.as<DeviceTypeBatch>(), ctx->tdesc_table.as<TransposeDesc>(), ctx->work_table.as<WorkItem>(), topo.all_work_count, W,
                             kTransposeRefs | kTransposePrestep | kTransposeImpulses, ctx->stream);
     const size_t nb = (size_t)std::max(ctx->body_count, 1);
@@ -887,10 +814,9 @@ int32_t bepucuda_update_type_batch(bepucuda_ctx* ctx, int32_t batch_index, int32
     SourceTypeBatch* s = find_source(ctx, batch_index, type_batch_index);
     if (!s) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "update_type_batch: unknown type batch");
     CK(cudaSetDevice(ctx->device));
-    open_upload_window(ctx);
-    int rc;
-    if ((rc = copy_in(ctx, s->raw_prestep, prestep, s->prestep_bytes)) != BEPUCUDA_OK) return rc;
-    if ((rc = copy_in(ctx, s->raw_impulses, accumulated_impulses, s->impulse_bytes)) != BEPUCUDA_OK) return rc;
+    ctx->upload_window.start_once(ctx->stream);
+    TRY(copy_in(ctx, s->raw_prestep, prestep, s->prestep_bytes));
+    TRY(copy_in(ctx, s->raw_impulses, accumulated_impulses, s->impulse_bytes));
     s->host_impulses = accumulated_impulses;
     s->pending = kTransposePrestep | kTransposeImpulses;
     s->redistribute = false;  // the host took the impulses back
@@ -915,7 +841,7 @@ int32_t bepucuda_set_contact_features(bepucuda_ctx* ctx, int32_t batch_index, in
     if (!s) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "set_contact_features: unknown type batch");
     if (get_type_info(s->type_id)->contacts == 0) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "set_contact_features: not a contact constraint type");
     CK(cudaSetDevice(ctx->device));
-    { int rc = ensure_feature_arrays(ctx, *s); if (rc != BEPUCUDA_OK) return rc; }
+    TRY(ensure_feature_arrays(ctx, *s));
     // from a mapped buffer the ids are only queued: the next solve copies them, before the host writes the next frame's ids into the same buffer
     if (ctx->constraints_ready) ctx->data_dirty = true;
     return copy_in(ctx, s->raw_features_old, feature_ids, s->feature_bytes);
@@ -930,10 +856,9 @@ int32_t bepucuda_update_contacts(bepucuda_ctx* ctx, int32_t batch_index, int32_t
     if (!s->raw_features_old) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, "update_contacts: bepucuda_set_contact_features was never called for this type batch");
     if (s->redistribute) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, "update_contacts: called twice for the same type batch without a solve in between");
     CK(cudaSetDevice(ctx->device));
-    open_upload_window(ctx);
-    int rc;
-    if ((rc = copy_in(ctx, s->raw_prestep, prestep, s->prestep_bytes)) != BEPUCUDA_OK) return rc;
-    if ((rc = copy_in(ctx, s->raw_features_new, new_feature_ids, s->feature_bytes)) != BEPUCUDA_OK) return rc;
+    ctx->upload_window.start_once(ctx->stream);
+    TRY(copy_in(ctx, s->raw_prestep, prestep, s->prestep_bytes));
+    TRY(copy_in(ctx, s->raw_features_new, new_feature_ids, s->feature_bytes));
     s->pending |= kTransposePrestep;  // the accumulated impulses stay resident
     s->redistribute = true;
     ctx->data_dirty = true;
@@ -944,7 +869,7 @@ int32_t bepucuda_upload_body_motion(bepucuda_ctx* ctx, const void* body_dynamics
     if (!ctx || !body_dynamics || body_count != ctx->body_count) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "upload_body_motion: bad arguments (the body count must match the last upload_bodies)");
     if (body_count == 0) return BEPUCUDA_OK;
     CK(cudaSetDevice(ctx->device));
-    open_upload_window(ctx);
+    ctx->upload_window.start_once(ctx->stream);
     const size_t n = (size_t)body_count;
     if (char* alias = map_host(ctx, body_dynamics, n * 128)) {
         launch_scatter_body_motion(alias, body_count, ctx->B, ctx->stream);  // 64 of every 128 bytes read straight from the mapped host buffer
@@ -960,7 +885,7 @@ int32_t bepucuda_upload_body_motion(bepucuda_ctx* ctx, const void* body_dynamics
 int32_t bepucuda_download_body_motion(bepucuda_ctx* ctx, void* out, int32_t body_count) {
     if (!ctx || !out || body_count < 0 || body_count > ctx->body_count) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "download_body_motion: bad arguments");
     CK(cudaSetDevice(ctx->device));
-    CK(cudaEventRecord(ctx->ev_down_begin, ctx->stream));
+    CK(ctx->download_window.start(ctx->stream));
     const size_t n = (size_t)body_count;
     if (char* alias = map_host(ctx, out, n * 128)) {
         launch_gather_body_motion(alias, body_count, ctx->B, ctx->stream);
@@ -969,53 +894,51 @@ int32_t bepucuda_download_body_motion(bepucuda_ctx* ctx, void* out, int32_t body
         CK(cudaMemcpy2DAsync(out, 128, ctx->raw_bodies.ptr, 128, 64, n, cudaMemcpyDeviceToHost, ctx->stream));
     }
     CK(cudaGetLastError());
-    CK(cudaEventRecord(ctx->ev_down_end, ctx->stream));
+    CK(ctx->download_window.stop(ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
-    ctx->have_down = true;
     ctx->timings.d2h_bytes = (int64_t)n * 64;
     return BEPUCUDA_OK;
 }
 
 int32_t bepucuda_solve(bepucuda_ctx* ctx, float dt) {
     if (!ctx || !(dt > 0)) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "solve: bad arguments");
-    { int rc = check_accelerations(ctx, "solve"); if (rc != BEPUCUDA_OK) return rc; }
+    TRY(check_accelerations(ctx, "solve"));
     CK(cudaSetDevice(ctx->device));
     if (!ctx->constraints_ready) {
         // No constraints were ever described (or the description was invalidated): only legal when nothing was uploaded.
         if (ctx->constraints_open) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, "solve inside begin/end_constraints");
         if (!ctx->sources.empty()) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, "solve: constraint description is stale; re-run begin/upload/end_constraints");
-        int rc = bepucuda_begin_constraints(ctx, ctx->W, 0);
-        if (rc == BEPUCUDA_OK) rc = bepucuda_end_constraints(ctx);
-        if (rc != BEPUCUDA_OK) return rc;
+        TRY(bepucuda_begin_constraints(ctx, ctx->W, 0));
+        TRY(bepucuda_end_constraints(ctx));
     }
-    { int rc = prepare_frame(ctx, dt); if (rc != BEPUCUDA_OK) return rc; }
-    CK(cudaEventRecord(ctx->ev_solve_begin, ctx->stream));
+    TRY(prepare_frame(ctx, dt));
+    CK(ctx->solve_window.start(ctx->stream));
     int64_t launches = 0;
     if (ctx->cfg.execution_mode == BEPUCUDA_EXEC_GRAPH) {
         const LaunchContext lc = launch_context(ctx, false);
-        if (!ctx->graph_exec || !same_bodies(ctx->graph_bodies, ctx->B) || !same_launches(ctx->graph_launch, lc)) {
-            invalidate_graph(ctx);
+        StageGraph& g = ctx->stage_graph;
+        if (!g.matches(ctx->B, lc)) {
+            g.reset();
             CK(cudaStreamBeginCapture(ctx->stream, cudaStreamCaptureModeThreadLocal));
             int64_t n = 0;
             issue_stage_sequence(ctx, ctx->stream, &n);
-            cudaError_t e = cudaStreamEndCapture(ctx->stream, &ctx->graph);
-            if (e == cudaSuccess) e = cudaGraphInstantiate(&ctx->graph_exec, ctx->graph, 0);
+            cudaError_t e = cudaStreamEndCapture(ctx->stream, g.graph.put());
+            if (e == cudaSuccess) e = cudaGraphInstantiate(g.exec.put(), g.graph, 0);
             if (e != cudaSuccess) return cuda_fail(ctx, e, "graph capture");
-            ctx->graph_bodies = ctx->B;
-            ctx->graph_launch = lc;
+            g.bodies = ctx->B;
+            g.launch = lc;
             ctx->timings.kernel_launches = n;
             ++ctx->timings.graph_captures;
         }
-        CK(cudaGraphLaunch(ctx->graph_exec, ctx->stream));
+        CK(cudaGraphLaunch(g.exec, ctx->stream));
         launches = ctx->timings.kernel_launches;
     }
     if (ctx->cfg.execution_mode == BEPUCUDA_EXEC_STREAM) {
         issue_stage_sequence(ctx, ctx->stream, &launches);
         CK(cudaGetLastError());
     }
-    CK(cudaEventRecord(ctx->ev_solve_end, ctx->stream));
+    CK(ctx->solve_window.stop(ctx->stream));
     if (ctx->peer_mode) { ctx->exchange_counter += ctx->program.exchange_count; ++ctx->shard_solve_index; }  // the flag barrier and the arrival counters keep counting across solves
-    ctx->have_solve = true;
     ctx->timings.kernel_launches = launches;
 
     // metric bookkeeping (SURVEY.md §8d)
@@ -1046,13 +969,12 @@ int32_t bepucuda_synchronize(bepucuda_ctx* ctx) {
 int32_t bepucuda_download_bodies(bepucuda_ctx* ctx, void* out, int32_t body_count) {
     if (!ctx || !out || body_count < 0 || body_count > ctx->body_count) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "download_bodies: bad arguments");
     CK(cudaSetDevice(ctx->device));
-    CK(cudaEventRecord(ctx->ev_down_begin, ctx->stream));
+    CK(ctx->download_window.start(ctx->stream));
     launch_merge_bodies(ctx->raw_bodies.ptr, body_count, ctx->B, ctx->stream);
     CK(cudaGetLastError());
     CK(cudaMemcpyAsync(out, ctx->raw_bodies.ptr, (size_t)body_count * 128, cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaEventRecord(ctx->ev_down_end, ctx->stream));
+    CK(ctx->download_window.stop(ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
-    ctx->have_down = true;
     ctx->timings.d2h_bytes = (int64_t)body_count * 128;
     return BEPUCUDA_OK;
 }
@@ -1071,7 +993,7 @@ int32_t bepucuda_download_impulses(bepucuda_ctx* ctx) {
         else CK(cudaMemcpyAsync(s.host_impulses, s.raw_impulses, s.impulse_bytes, cudaMemcpyDeviceToHost, ctx->stream));
         bytes += (int64_t)s.impulse_bytes;
     }
-    { int rc = flush_chunks(ctx, d2h); if (rc != BEPUCUDA_OK) return rc; }
+    TRY(flush_chunks(ctx, d2h));
     CK(cudaStreamSynchronize(ctx->stream));
     ctx->timings.d2h_bytes += bytes;
     return BEPUCUDA_OK;
@@ -1095,20 +1017,14 @@ static_assert(sizeof(bepucuda_constraint_location) == 16, "bepucuda_constraint_l
 
 int32_t bepucuda_read_constraints(bepucuda_ctx* ctx, int32_t count, const bepucuda_constraint_location* locations, int32_t* records_out) {
     if (!ctx) return BEPUCUDA_ERR_INVALID_ARGUMENT;
-    if (ctx->peer_mode) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, "read_constraints in peer mode: a rank holds its constraints compacted, so host locations do not address them");
-    if (!ctx->constraints_ready) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, "read_constraints before end_constraints");
-    if (count < 0 || (count > 0 && (!locations || !records_out))) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "read_constraints: bad arguments");
+    std::vector<ResolvedLocation> resolved;
+    TRY(resolve_locations(ctx, "read_constraints", count, locations, records_out, false, &resolved));
     if (count == 0) return BEPUCUDA_OK;
-    // every location is checked before any device work, so a bad one leaves records_out untouched
     std::vector<ReadRequest> requests((size_t)count);
     for (int32_t i = 0; i < count; ++i) {
-        const bepucuda_constraint_location& l = locations[i];
-        ResolvedLocation r;
-        if (resolve_location(ctx->topo, l, &r) != BEPUCUDA_OK) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "read_constraints: " + no_constraint_at(i, l));
-        ReadRequest& q = requests[(size_t)i];
-        q.type_id = l.type_id;
+        const ResolvedLocation& r = resolved[(size_t)i];
         // a fallback constraint, a hole included, is looked up on the device through its inverse entry
-        q.at = r.inverse_entry < 0 ? r.at : DeviceSlot{-1, (int32_t)r.inverse_entry};
+        requests[(size_t)i] = {locations[i].type_id, r.inverse_entry < 0 ? r.at : DeviceSlot{-1, (int32_t)r.inverse_entry}};
     }
     CK(cudaSetDevice(ctx->device));
     const size_t n = (size_t)count;
@@ -1125,26 +1041,13 @@ int32_t bepucuda_read_constraints(bepucuda_ctx* ctx, int32_t count, const bepucu
 
 int32_t bepucuda_write_constraints(bepucuda_ctx* ctx, int32_t count, const bepucuda_constraint_location* locations, const int32_t* records) {
     if (!ctx) return BEPUCUDA_ERR_INVALID_ARGUMENT;
-    if (ctx->peer_mode) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, "write_constraints in peer mode: a rank holds its constraints compacted, so host locations do not address them");
-    if (!ctx->constraints_ready) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, "write_constraints before end_constraints");
-    if (count < 0 || (count > 0 && (!locations || !records))) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "write_constraints: bad arguments");
+    std::vector<ResolvedLocation> resolved;
+    TRY(resolve_locations(ctx, "write_constraints", count, locations, records, true, &resolved));
     if (count == 0) return BEPUCUDA_OK;
-    // every location and record is checked before anything is queued, so a failing call changes nothing
-    std::vector<DeviceSlot> slots((size_t)count);
-    for (int32_t i = 0; i < count; ++i) {
-        const bepucuda_constraint_location& l = locations[i];
-        ResolvedLocation r;
-        if (resolve_location(ctx->topo, l, &r) != BEPUCUDA_OK) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "write_constraints: " + no_constraint_at(i, l));
-        if (r.at.type_batch < 0) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "write_constraints: " + no_constraint_at(i, l) + " (a hole of the fallback batch)");
-        if (records[(size_t)i * 64] != l.type_id)
-            return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "write_constraints: record " + std::to_string(i) + " has type id " + std::to_string(records[(size_t)i * 64]) +
-                                                                ", its location type id " + std::to_string(l.type_id));
-        slots[(size_t)i] = r.at;
-    }
     CK(cudaSetDevice(ctx->device));
-    open_upload_window(ctx);
+    ctx->upload_window.start_once(ctx->stream);
     for (int32_t i = 0; i < count; ++i)
-        ctx->prestep_writes.put(slots[(size_t)i], (const float*)(records + (size_t)i * 64 + kRecordPrestep), get_type_info(locations[i].type_id)->prestep_rows);
+        ctx->prestep_writes.put(resolved[(size_t)i].at, (const float*)(records + (size_t)i * 64 + kRecordPrestep), get_type_info(locations[i].type_id)->prestep_rows);
     ctx->data_dirty = true;
     return BEPUCUDA_OK;
 }
@@ -1153,10 +1056,10 @@ int32_t bepucuda_get_timings(bepucuda_ctx* ctx, bepucuda_timings* out) {
     if (!ctx || !out) return BEPUCUDA_ERR_INVALID_ARGUMENT;
     CK(cudaSetDevice(ctx->device));
     CK(cudaStreamSynchronize(ctx->stream));
-    { int rc = check_device_error_flag(ctx); if (rc != BEPUCUDA_OK) return rc; }
-    if (ctx->have_solve) cudaEventElapsedTime(&ctx->timings.solve_ms, ctx->ev_solve_begin, ctx->ev_solve_end);
-    if (ctx->have_up && !ctx->up_open) cudaEventElapsedTime(&ctx->timings.upload_ms, ctx->ev_up_begin, ctx->ev_up_end);
-    if (ctx->have_down) cudaEventElapsedTime(&ctx->timings.download_ms, ctx->ev_down_begin, ctx->ev_down_end);
+    TRY(check_device_error_flag(ctx));
+    ctx->solve_window.measure(&ctx->timings.solve_ms);
+    ctx->upload_window.measure(&ctx->timings.upload_ms);
+    ctx->download_window.measure(&ctx->timings.download_ms);
     *out = ctx->timings;
     return BEPUCUDA_OK;
 }
@@ -1164,7 +1067,7 @@ int32_t bepucuda_get_timings(bepucuda_ctx* ctx, bepucuda_timings* out) {
 int32_t bepucuda_event_record(bepucuda_ctx* ctx, int32_t slot) {
     if (!ctx || slot < 0 || slot >= 16) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "event_record: bad slot");
     CK(cudaSetDevice(ctx->device));
-    if (!ctx->user_events[slot]) CK(cudaEventCreate(&ctx->user_events[slot]));
+    CK(ctx->user_events[slot].create());
     CK(cudaEventRecord(ctx->user_events[slot], ctx->stream));
     return BEPUCUDA_OK;
 }
@@ -1180,16 +1083,12 @@ int32_t bepucuda_profile_stages(bepucuda_ctx* ctx, float dt, bepucuda_stage_prof
     if (!ctx || !out || !(dt > 0)) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "profile_stages: bad arguments");
     if (!ctx->constraints_ready) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, "profile_stages before end_constraints");
     if (ctx->peer_mode) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, "profile_stages in peer mode: one rank alone cannot meet its peers at the rank barriers");
-    { int rc = check_accelerations(ctx, "profile_stages"); if (rc != BEPUCUDA_OK) return rc; }
+    TRY(check_accelerations(ctx, "profile_stages"));
     CK(cudaSetDevice(ctx->device));
     std::memset(out, 0, sizeof(*out));
-    const size_t need = ctx->program.ops.size() * 2;
-    while (ctx->profile_events.size() < need) {
-        cudaEvent_t ev;
-        CK(cudaEventCreate(&ev));
-        ctx->profile_events.push_back(ev);
-    }
-    { int rc = prepare_frame(ctx, dt); if (rc != BEPUCUDA_OK) return rc; }
+    ctx->profile_events.resize(std::max(ctx->profile_events.size(), ctx->program.ops.size() * 2));
+    for (Event& ev : ctx->profile_events) CK(ev.create());
+    TRY(prepare_frame(ctx, dt));
     std::vector<int> launched(ctx->program.ops.size(), 0);
     const StageEvents sink{ctx->profile_events, launched};
     issue_stage_sequence(ctx, ctx->stream, nullptr, &sink);
@@ -1207,7 +1106,7 @@ int32_t bepucuda_profile_stages(bepucuda_ctx* ctx, float dt, bepucuda_stage_prof
     return BEPUCUDA_OK;
 }
 
-static_assert(sizeof(bepucuda_body_shape) == sizeof(BodyShape) && sizeof(bepucuda_body_activity) == sizeof(BodyActivityRecord), "ABI structs mirror the device records");
+static_assert(sizeof(bepucuda_body_shape) == sizeof(BodyShape) && sizeof(bepucuda_body_activity) == sizeof(BodyActivityRecord) && sizeof(BodyActivityRecord) == 8, "ABI structs mirror the device records");
 
 int32_t bepucuda_set_body_shapes(bepucuda_ctx* ctx, const bepucuda_body_shape* shapes, int32_t body_count) {
     if (!ctx || body_count < 0 || (body_count > 0 && !shapes)) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "set_body_shapes: bad arguments");
@@ -1222,7 +1121,7 @@ int32_t bepucuda_set_body_shapes(bepucuda_ctx* ctx, const bepucuda_body_shape* s
 int32_t bepucuda_predict_bounding_boxes(bepucuda_ctx* ctx, float dt, bepucuda_body_activity* activities, float* bounds_out) {
     if (!ctx || !(dt > 0) || !activities || !bounds_out) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "predict_bounding_boxes: bad arguments");
     if (ctx->shape_count != ctx->body_count) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, "predict_bounding_boxes: bepucuda_set_body_shapes was not called for the current body count");
-    { int rc = check_accelerations(ctx, "predict_bounding_boxes"); if (rc != BEPUCUDA_OK) return rc; }
+    TRY(check_accelerations(ctx, "predict_bounding_boxes"));
     const int n = ctx->body_count;
     if (n == 0) return BEPUCUDA_OK;
     CK(cudaSetDevice(ctx->device));
@@ -1270,56 +1169,14 @@ int32_t bepucuda_color_constraints(bepucuda_ctx* ctx, int32_t constraint_count, 
         const int32_t enc = encoded_body_references[i];
         if (enc >= 0 && (int32_t)((uint32_t)enc & ((1u << 30) - 1u)) >= body_count) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "color_constraints: body reference out of range");
     }
-    constexpr int kRoundsPerChunk = 32;  // even: the ping-pong lists return to their starting roles after every chunk
-    const size_t nb = (size_t)std::max(body_count, 1), nc = (size_t)constraint_count;
-    CK(ctx->color_refs.reserve(words * 4));
-    CK(ctx->color_priorities.reserve(nc * 4));
-    CK(ctx->color_body_min.reserve(nb * 8));
-    CK(ctx->color_body_mask.reserve(nb * 8));
-    CK(ctx->color_out.reserve(nc * 4));
-    CK(ctx->color_lists.reserve(nc * 8));
-    CK(ctx->color_counts.reserve((kRoundsPerChunk + 1) * 4));
-    CK(cudaMemcpyAsync(ctx->color_refs.ptr, encoded_body_references, words * 4, cudaMemcpyHostToDevice, ctx->stream));
-    if (order == BEPUCUDA_COLOR_BY_PRIORITY) CK(cudaMemcpyAsync(ctx->color_priorities.ptr, priorities, nc * 4, cudaMemcpyHostToDevice, ctx->stream));
-    ColoringBuffers cb{};
-    cb.refs = ctx->color_refs.as<int32_t>();
-    cb.priorities = ctx->color_priorities.as<uint32_t>();
-    cb.body_min = ctx->color_body_min.as<unsigned long long>();
-    cb.body_mask = ctx->color_body_mask.as<unsigned long long>();
-    cb.batch_out = ctx->color_out.as<int32_t>();
-    cb.list[0] = ctx->color_lists.as<int32_t>();
-    cb.list[1] = ctx->color_lists.as<int32_t>() + nc;
-    cb.counts = ctx->color_counts.as<unsigned int>();
-    cb.constraint_count = constraint_count;
-    cb.bodies_per_constraint = bodies_per_constraint;
-    cb.body_count = body_count;
-    cb.fallback_threshold = fallback_batch_threshold;
-    cb.order = order;
-    CK(cudaMemsetAsync(ctx->color_counts.ptr, 0, (kRoundsPerChunk + 1) * 4, ctx->stream));
-    launch_color_init(cb, ctx->stream);
-    unsigned int counts[kRoundsPerChunk + 1];
     int64_t rounds = 0;
-    for (;;) {
-        for (int r = 0; r < kRoundsPerChunk; ++r) launch_color_round(cb, r, ctx->stream);
-        CK(cudaMemcpyAsync(counts, ctx->color_counts.ptr, sizeof(counts), cudaMemcpyDeviceToHost, ctx->stream));
-        CK(cudaStreamSynchronize(ctx->stream));
-        CK(cudaGetLastError());
-        int used = kRoundsPerChunk;
-        for (int r = 0; r < kRoundsPerChunk; ++r)
-            if (counts[r + 1] == 0) { used = r + 1; break; }
-        rounds += used;
-        if (counts[used] == 0) break;
-        // every round assigns at least the constraint with the globally lowest key, so the list shrinks: the loop ends after at most constraint_count rounds
-        if (counts[kRoundsPerChunk] >= counts[0]) return fail(ctx, BEPUCUDA_ERR_CUDA, "color_constraints: no progress (internal error)");
-        counts[0] = counts[kRoundsPerChunk];
-        for (int r = 1; r <= kRoundsPerChunk; ++r) counts[r] = 0;
-        CK(cudaMemcpyAsync(ctx->color_counts.ptr, counts, sizeof(counts), cudaMemcpyHostToDevice, ctx->stream));
-        CK(cudaStreamSynchronize(ctx->stream));  // `counts` is a stack array: the copy must have read it before the next chunk's download overwrites it
-    }
-    CK(cudaMemcpyAsync(batch_indices_out, ctx->color_out.ptr, nc * 4, cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaStreamSynchronize(ctx->stream));
+    const char* failed = nullptr;
+    if (const cudaError_t e = color_constraints(ctx->coloring, constraint_count, bodies_per_constraint, encoded_body_references, body_count, fallback_batch_threshold, order,
+                                                order == BEPUCUDA_COLOR_BY_PRIORITY ? priorities : nullptr, batch_indices_out, &rounds, &failed, ctx->stream))
+        return cuda_fail(ctx, e, failed);
+    if (rounds < 0) return fail(ctx, BEPUCUDA_ERR_CUDA, "color_constraints: no progress (internal error)");
     int32_t highest = -1;
-    for (size_t i = 0; i < nc; ++i) highest = std::max(highest, batch_indices_out[i]);
+    for (int32_t i = 0; i < constraint_count; ++i) highest = std::max(highest, batch_indices_out[i]);
     if (batch_count_out) *batch_count_out = highest + 1;
     if (rounds_out) *rounds_out = (int32_t)std::min<int64_t>(rounds, 0x7fffffff);
     return BEPUCUDA_OK;
@@ -1337,61 +1194,12 @@ int32_t bepucuda_find_sleepable_islands(bepucuda_ctx* ctx, const bepucuda_body_a
     if (rounds_out) *rounds_out = 0;
     if (body_count == 0) return BEPUCUDA_OK;
     CK(cudaSetDevice(ctx->device));
-    const size_t n = (size_t)body_count;
-    CK(ctx->island_activities.reserve(n * sizeof(bepucuda_body_activity)));
-    CK(ctx->island_label.reserve(n * 4));
-    CK(ctx->island_blocked.reserve(n * 4));
-    CK(ctx->island_count.reserve(n * 4));
-    CK(ctx->island_flags.reserve(n));
-    CK(ctx->island_roots.reserve(n * 4));
-    CK(ctx->island_counts.reserve(n * 4));
-    CK(ctx->island_scalars.reserve(8));  // [0]: hook pass changed something, [1]: number of sleepable roots
-    IslandBuffers ib{};
-    ib.tbs = ctx->tb_table.as<DeviceTypeBatch>();
-    ib.work = ctx->work_table.as<WorkItem>();
-    ib.work_count = ctx->topo.all_work_count;
-    ib.activities = ctx->island_activities.as<uint8_t>();
-    ib.label = ctx->island_label.as<int32_t>();
-    ib.blocked = ctx->island_blocked.as<int32_t>();
-    ib.count = ctx->island_count.as<int32_t>();
-    ib.changed = ctx->island_scalars.as<unsigned int>();
-    ib.body_count = body_count;
-    int32_t* selected = ctx->island_scalars.as<int32_t>() + 1;
-    size_t temp_bytes = 0;
-    CK(launch_island_select(ib, nullptr, nullptr, nullptr, selected, nullptr, &temp_bytes, ctx->stream));
-    CK(ctx->island_temp.reserve(std::max(temp_bytes, (size_t)16)));
-    temp_bytes = ctx->island_temp.capacity;
-    CK(cudaMemcpyAsync(ctx->island_activities.ptr, activities, n * sizeof(bepucuda_body_activity), cudaMemcpyHostToDevice, ctx->stream));
-    launch_island_init(ib, ctx->stream);
-    CK(cudaGetLastError());
-    // every round that changes something joins at least two trees, so there are at most body_count of them; in practice O(log n)
     int64_t rounds = 0;
-    if (ib.work_count > 0) {
-        for (;;) {
-            CK(cudaMemsetAsync(ib.changed, 0, 4, ctx->stream));
-            launch_island_round(ib, ctx->stream);
-            unsigned int changed = 0;
-            CK(cudaMemcpyAsync(&changed, ib.changed, 4, cudaMemcpyDeviceToHost, ctx->stream));
-            CK(cudaStreamSynchronize(ctx->stream));
-            CK(cudaGetLastError());
-            ++rounds;
-            if (!changed) break;
-            if (rounds > (int64_t)body_count) return fail(ctx, BEPUCUDA_ERR_CUDA, "find_sleepable_islands: no convergence (internal error)");
-        }
-    }
-    launch_island_verdict(ib, ctx->stream);
-    CK(launch_island_select(ib, ctx->island_flags.as<uint8_t>(), ctx->island_roots.as<int32_t>(), ctx->island_counts.as<int32_t>(), selected, ctx->island_temp.ptr, &temp_bytes,
-                            ctx->stream));
-    int32_t count = 0;
-    CK(cudaMemcpyAsync(&count, selected, 4, cudaMemcpyDeviceToHost, ctx->stream));
-    if (island_of_body_out) CK(cudaMemcpyAsync(island_of_body_out, ib.label, n * 4, cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaStreamSynchronize(ctx->stream));
-    if (count > 0) {
-        CK(cudaMemcpyAsync(sleepable_roots_out, ctx->island_roots.ptr, (size_t)count * 4, cudaMemcpyDeviceToHost, ctx->stream));
-        CK(cudaMemcpyAsync(sleepable_body_counts_out, ctx->island_counts.ptr, (size_t)count * 4, cudaMemcpyDeviceToHost, ctx->stream));
-        CK(cudaStreamSynchronize(ctx->stream));
-    }
-    *sleepable_count_out = count;
+    const char* failed = nullptr;
+    if (const cudaError_t e = find_sleepable_islands(ctx->islands, ctx->tb_table.as<DeviceTypeBatch>(), ctx->work_table.as<WorkItem>(), ctx->topo.all_work_count, activities, body_count,
+                                                     island_of_body_out, sleepable_roots_out, sleepable_body_counts_out, sleepable_count_out, &rounds, &failed, ctx->stream))
+        return cuda_fail(ctx, e, failed);
+    if (rounds < 0) return fail(ctx, BEPUCUDA_ERR_CUDA, "find_sleepable_islands: no convergence (internal error)");
     if (rounds_out) *rounds_out = (int32_t)std::min<int64_t>(rounds, 0x7fffffff);
     return BEPUCUDA_OK;
 }
@@ -1412,6 +1220,15 @@ int32_t bepucuda_shard_export(bepucuda_ctx* ctx, bepucuda_ipc_handles* out) {
     return BEPUCUDA_OK;
 }
 
+// The end of both shard imports: the context runs as rank p.rank of p.rank_count from its next describe on.
+static int enter_peer_mode(bepucuda_ctx* ctx, const ShardPeers& p) {
+    ctx->peers = p;
+    ctx->peer_mode = true;
+    ctx->exchange_counter = 0;
+    ctx->constraints_ready = false;
+    return BEPUCUDA_OK;
+}
+
 int32_t bepucuda_shard_import(bepucuda_ctx* ctx, int32_t rank, int32_t rank_count, const bepucuda_ipc_handles* all) {
     if (!ctx || !all || rank_count < 1 || rank_count > kMaxShardRanks || rank < 0 || rank >= rank_count) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "shard_import: bad arguments");
     if (!ctx->shard_flags.ptr) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, "shard_import before shard_export");
@@ -1425,19 +1242,15 @@ int32_t bepucuda_shard_import(bepucuda_ctx* ctx, int32_t rank, int32_t rank_coun
             for (int i = 0; i < 4; ++i) {
                 cudaIpcMemHandle_t h;
                 std::memcpy(&h, all[r].bytes[i], 64);
-                CK(cudaIpcOpenMemHandle(&ptrs[i], h, cudaIpcMemLazyEnablePeerAccess));
-                ctx->opened_ipc.push_back(ptrs[i]);
+                CK(cudaIpcOpenMemHandle(ctx->opened_ipc.emplace_back().put(), h, cudaIpcMemLazyEnablePeerAccess));
+                ptrs[i] = ctx->opened_ipc.back();
             }
         p.pose[r] = (float4*)ptrs[0];
         p.velocity[r] = (float4*)ptrs[1];
         p.inertia_world[r] = (float4*)ptrs[2];
         p.flags[r] = (unsigned long long*)ptrs[3];
     }
-    ctx->peers = p;
-    ctx->peer_mode = true;
-    ctx->exchange_counter = 0;
-    if (ctx->constraints_ready) ctx->constraints_ready = false;
-    return BEPUCUDA_OK;
+    return enter_peer_mode(ctx, p);
 }
 
 int32_t bepucuda_shard_import_contexts(bepucuda_ctx* ctx, int32_t rank, int32_t rank_count, bepucuda_ctx* const* all) {
@@ -1463,25 +1276,21 @@ int32_t bepucuda_shard_import_contexts(bepucuda_ctx* ctx, int32_t rank, int32_t 
         p.inertia_world[r] = o->inertia_world.as<float4>();
         p.flags[r] = (unsigned long long*)o->shard_flags.ptr;
     }
-    ctx->peers = p;
-    ctx->peer_mode = true;
-    ctx->exchange_counter = 0;
-    if (ctx->constraints_ready) ctx->constraints_ready = false;
-    return BEPUCUDA_OK;
+    return enter_peer_mode(ctx, p);
 }
 
 int32_t bepucuda_shard_set_global(bepucuda_ctx* ctx, const int32_t* first_batch, const uint8_t* constrained) {
     if (!ctx || !first_batch || !constrained) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "shard_set_global: bad arguments");
     ctx->global_first_batch.assign(first_batch, first_batch + ctx->body_count);
     ctx->global_constrained.assign(constrained, constrained + ctx->body_count);
-    if (ctx->constraints_ready) ctx->constraints_ready = false;
+    ctx->constraints_ready = false;
     return BEPUCUDA_OK;
 }
 
 int32_t bepucuda_shard_set_body_masks(bepucuda_ctx* ctx, const uint8_t* rank_masks) {
     if (!ctx || !rank_masks) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "shard_set_body_masks: bad arguments");
     ctx->body_masks.assign(rank_masks, rank_masks + ctx->body_count);
-    if (ctx->constraints_ready) ctx->constraints_ready = false;
+    ctx->constraints_ready = false;
     return BEPUCUDA_OK;
 }
 
@@ -1490,7 +1299,7 @@ int32_t bepucuda_shard_set_fallback_rank(bepucuda_ctx* ctx, int32_t rank) {
     if (!ctx->peer_mode) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "shard_set_fallback_rank: the context is not in peer mode (bepucuda_shard_import*)");
     if (rank < -1 || rank >= ctx->peers.rank_count) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "shard_set_fallback_rank: rank out of range");
     ctx->fallback_rank = rank;
-    if (ctx->constraints_ready) ctx->constraints_ready = false;
+    ctx->constraints_ready = false;
     return BEPUCUDA_OK;
 }
 

@@ -170,3 +170,24 @@ def test_library_binary_matches_its_stamp(libs):
         assert _build.binary_matches_stamp(lib) is False
         os.remove(lib + ".stamp")
         assert _build.binary_matches_stamp(lib) is None
+
+
+def test_every_cuda_handle_is_released_by_its_owner():
+    """cudaEventCreate*, and the calls that release an event, the stream, a captured graph or an opened IPC mapping, appear in csrc/ only inside the
+    owner types of bepu_cuda_handles.h: a handle the context or a driver holds is freed by its owner's destructor, never by a hand-written list."""
+    csrc = os.path.join(ROOT, "bepuphysics2_b200", "csrc")
+    calls = re.compile(r"\b(cudaEventCreate\w*|cudaEventDestroy|cudaStreamDestroy|cudaGraphDestroy|cudaGraphExecDestroy|cudaIpcCloseMemHandle)\b")
+    hits = []
+    for dirpath, _, files in os.walk(csrc):
+        for name in sorted(f for f in files if f.endswith((".cu", ".cuh", ".h", ".cpp", ".inc"))):
+            with open(os.path.join(dirpath, name), errors="replace") as f:
+                for line in f:
+                    code = line.split("//", 1)[0]
+                    hits += [(name, call) for call in calls.findall(code)]
+    assert sorted(hits) == sorted([("bepu_cuda_handles.h", "cudaStreamDestroy"), ("bepu_cuda_handles.h", "cudaGraphDestroy"),
+                                   ("bepu_cuda_handles.h", "cudaGraphExecDestroy"), ("bepu_cuda_handles.h", "cudaIpcCloseMemHandle"),
+                                   ("bepu_cuda_handles.h", "cudaEventDestroy"), ("bepu_cuda_handles.h", "cudaEventCreateWithFlags")]), hits
+    with open(os.path.join(csrc, "bepu_cuda_handles.h")) as f:
+        header = f.read()
+    owners = header[header.index("struct Owned {"):header.index("\n};\n", header.index("struct Event :"))]
+    assert len(calls.findall(owners)) == len(hits), "a release or create call of bepu_cuda_handles.h lies outside Owned and Event"
