@@ -107,6 +107,18 @@ __global__ void scatter_body_motion_kernel(const float4* __restrict__ raw, int b
     if (part != 0) v.w = 0.0f;  // padding floats carry no meaning (and hold versions / stamps on the device)
     (part < 2 ? B.pose : B.velocity)[body * 2 + (part & 1)] = v;
 }
+// bepucuda_write_bodies: the same per-float4 scatter for the listed bodies only. List entry i reads whole record indices[i] of `src` (mapped host
+// memory), or the i-th 64-B motion half when `gathered` (the host's staging). Neither inertia array is written.
+__global__ void write_body_motion_kernel(const float4* __restrict__ src, const int32_t* __restrict__ indices, int count, int gathered, BodyBuffers B) {
+    const size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= (size_t)count * 4) return;
+    const size_t i = t >> 2;
+    const int part = (int)(t & 3);
+    const size_t body = (size_t)indices[i];
+    float4 v = src[gathered ? i * 4 + part : body * 8 + part];
+    if (part != 0) v.w = 0.0f;
+    (part < 2 ? B.pose : B.velocity)[body * 2 + (part & 1)] = v;
+}
 __global__ void gather_body_motion_kernel(float4* __restrict__ raw, int body_count, BodyBuffers B) {
     const size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= (size_t)body_count * 4) return;
@@ -332,6 +344,10 @@ void launch_redistribute_impulses(const DeviceTypeBatch* tbs, const TransposeDes
 void launch_scatter_body_motion(const void* raw, int body_count, const BodyBuffers& B, cudaStream_t s) {
     if (body_count <= 0) return;
     scatter_body_motion_kernel<<<blocks_for((size_t)body_count * 4, 256), 256, 0, s>>>((const float4*)raw, body_count, B);
+}
+void launch_write_body_motion(const void* src, const int32_t* indices, int count, bool gathered, const BodyBuffers& B, cudaStream_t s) {
+    if (count <= 0) return;
+    write_body_motion_kernel<<<blocks_for((size_t)count * 4, 256), 256, 0, s>>>((const float4*)src, indices, count, gathered ? 1 : 0, B);
 }
 void launch_gather_body_motion(void* raw, int body_count, const BodyBuffers& B, cudaStream_t s) {
     if (body_count <= 0) return;

@@ -60,6 +60,9 @@ void launch_redistribute_impulses(const DeviceTypeBatch* tbs, const TransposeDes
 // Motion half (floats 0-15) of 128-B BodyDynamics records <-> pose / velocity records. `raw` may be mapped host memory.
 void launch_scatter_body_motion(const void* raw, int body_count, const BodyBuffers& B, cudaStream_t s);
 void launch_gather_body_motion(void* raw, int body_count, const BodyBuffers& B, cudaStream_t s);
+// bepucuda_write_bodies: the motion half of the `count` listed bodies (indices: device, or mapped host memory). gathered = false: `src` is the whole
+// 128-B record array (mapped host memory), read at each listed index; true: `src` holds the listed motion halves back to back, 64 B each.
+void launch_write_body_motion(const void* src, const int32_t* indices, int count, bool gathered, const BodyBuffers& B, cudaStream_t s);
 // One chunk (<= 64 KiB, sizes multiple of 4 bytes) of a batched host<->device copy through mapped pinned memory.
 struct CopyChunk {
     void* dst;

@@ -258,6 +258,28 @@ void PrestepWriteQueue::clear() {
     rows.clear();
 }
 
+int check_body_write(bool bodies_uploaded, int32_t body_count, const void* body_dynamics, int32_t count, const int32_t* body_indices, const char** why) {
+    if (count < 0 || (count > 0 && (!body_dynamics || !body_indices))) {
+        *why = "bad arguments";
+        return BEPUCUDA_ERR_INVALID_ARGUMENT;
+    }
+    if (!bodies_uploaded) {
+        *why = "before upload_bodies";
+        return BEPUCUDA_ERR_BAD_STATE;
+    }
+    for (int32_t i = 0; i < count; ++i)
+        if (body_indices[i] < 0 || body_indices[i] >= body_count) {
+            *why = "a body index outside the bodies of the last upload_bodies";
+            return BEPUCUDA_ERR_INVALID_ARGUMENT;
+        }
+    return BEPUCUDA_OK;
+}
+
+void gather_motion_halves(const void* body_dynamics, const int32_t* body_indices, int32_t count, float* out) {
+    const char* records = (const char*)body_dynamics;
+    for (int32_t i = 0; i < count; ++i) std::memcpy(out + (size_t)i * 16, records + (size_t)body_indices[i] * 128, 64);
+}
+
 std::vector<WorkRecord> work_records(const TopologyPlan& plan, int32_t* refs, float* prestep, float* impulses) {
     std::vector<WorkRecord> records(plan.work.size());
     for (size_t i = 0; i < plan.work.size(); ++i) {

@@ -98,6 +98,13 @@ struct PrestepWriteQueue {
     std::vector<int32_t> entry_of_slot_;  // per device slot: its entry of `writes`, -1 = none (allocated by the first write of a plan)
 };
 
+// bepucuda_write_bodies on the host. check_body_write: BEPUCUDA_ERR_INVALID_ARGUMENT for count < 0 or a NULL pointer with count > 0,
+// BEPUCUDA_ERR_BAD_STATE before the first bepucuda_upload_bodies, BEPUCUDA_ERR_INVALID_ARGUMENT for an index outside [0, body_count); *why names
+// the failure. Duplicates and count == 0 are OK.
+int check_body_write(bool bodies_uploaded, int32_t body_count, const void* body_dynamics, int32_t count, const int32_t* body_indices, const char** why);
+// The staging of an unregistered buffer: out[i][0 .. 16) = floats 0-15 (pose and velocity) of the 128-B record body_indices[i], in list order.
+void gather_motion_halves(const void* body_dynamics, const int32_t* body_indices, int32_t count, float* out);
+
 // What the solver kernels read per work item, with the plan's offsets applied to the arena bases.
 std::vector<WorkRecord> work_records(const TopologyPlan& plan, int32_t* refs, float* prestep, float* impulses);
 

@@ -77,6 +77,7 @@ struct bepucuda_ctx {
 
     // bodies
     int body_count = 0;
+    bool bodies_uploaded = false;  // a bepucuda_upload_bodies has succeeded
     DeviceBuffer raw_bodies, pose, velocity, inertia_local, inertia_world, constrained, first_batch, sync_refcount, sync_mask;
     BodyBuffers B{};
 
@@ -129,6 +130,8 @@ struct bepucuda_ctx {
     PrestepWriteQueue prestep_writes;  // bepucuda_write_constraints since the last solve, applied by refresh_device_rows
     DeviceBuffer write_table, write_rows;
     StagedUpload write_stage, write_rows_stage;
+    DeviceBuffer body_writes;         // bepucuda_write_bodies: one call's staged motion halves (unregistered buffers) and body indices
+    StagedUpload body_write_stage;
     std::vector<Event> profile_events;
 };
 
@@ -164,15 +167,24 @@ void queue_chunks(std::vector<CopyChunk>& list, void* dst, const void* src, size
     const size_t kChunk = (size_t)64 << 10;
     for (size_t off = 0; off < bytes; off += kChunk) list.push_back({(char*)dst + off, (const char*)src + off, std::min(kChunk, bytes - off)});
 }
-// H2D copy of `bytes` at `src` through the pinned staging buffer of `st`.
-int upload_staged(bepucuda_ctx* ctx, StagedUpload& st, void* dst, const void* src, size_t bytes) {
+// Room for `bytes` in the pinned staging buffer of `st`, once the previous upload has left it.
+int reserve_staging(bepucuda_ctx* ctx, StagedUpload& st, size_t bytes) {
     CK(st.done.create(cudaEventDisableTiming));
-    CK(cudaEventSynchronize(st.done));  // the previous upload has left the staging buffer
+    CK(cudaEventSynchronize(st.done));
     CK(st.host.reserve(bytes));
-    std::memcpy(st.host.ptr, src, bytes);
+    return BEPUCUDA_OK;
+}
+// H2D copy of the first `bytes` of the staging buffer of `st`.
+int send_staging(bepucuda_ctx* ctx, StagedUpload& st, void* dst, size_t bytes) {
     CK(cudaMemcpyAsync(dst, st.host.ptr, bytes, cudaMemcpyHostToDevice, ctx->stream));
     CK(cudaEventRecord(st.done, ctx->stream));
     return BEPUCUDA_OK;
+}
+// H2D copy of `bytes` at `src` through the pinned staging buffer of `st`.
+int upload_staged(bepucuda_ctx* ctx, StagedUpload& st, void* dst, const void* src, size_t bytes) {
+    TRY(reserve_staging(ctx, st, bytes));
+    std::memcpy(st.host.ptr, src, bytes);
+    return send_staging(ctx, st, dst, bytes);
 }
 
 // Runs the queued chunks as one kernel. The chunk table travels through a ring of pinned staging buffers.
@@ -627,6 +639,7 @@ int32_t bepucuda_upload_bodies(bepucuda_ctx* ctx, const void* body_dynamics, int
     CK(ctx->constrained.reserve(n + 1));
     if (ctx->constrained.capacity != old_constrained_cap) CK(cudaMemsetAsync(ctx->constrained.ptr, 0, ctx->constrained.capacity, ctx->stream));
     ctx->body_count = body_count;
+    ctx->bodies_uploaded = true;
     ctx->B = {ctx->pose.as<float4>(), ctx->velocity.as<float4>(), ctx->inertia_local.as<float4>(), ctx->inertia_world.as<float4>(), ctx->constrained.as<uint8_t>(),
               ctx->first_batch.as<int32_t>(), body_count};
     if (body_count > 0) {
@@ -879,6 +892,31 @@ int32_t bepucuda_upload_body_motion(bepucuda_ctx* ctx, const void* body_dynamics
     }
     CK(cudaGetLastError());
     ctx->h2d_accum += (int64_t)n * 64;
+    return BEPUCUDA_OK;
+}
+
+int32_t bepucuda_write_bodies(bepucuda_ctx* ctx, const void* body_dynamics, int32_t count, const int32_t* body_indices) {
+    if (!ctx) return BEPUCUDA_ERR_INVALID_ARGUMENT;
+    const char* why = "";
+    const int rc = check_body_write(ctx->bodies_uploaded, ctx->body_count, body_dynamics, count, body_indices, &why);
+    if (rc != BEPUCUDA_OK) return fail(ctx, rc, std::string("write_bodies: ") + why);
+    if (count == 0) return BEPUCUDA_OK;
+    CK(cudaSetDevice(ctx->device));
+    ctx->upload_window.start_once(ctx->stream);
+    const size_t n = (size_t)count, index_bytes = n * sizeof(int32_t);
+    // A registered buffer is read by the kernel when the stream reaches it; an unregistered one is gathered here, so it is free on return.
+    const char* alias = map_host(ctx, body_dynamics, (size_t)ctx->body_count * 128);
+    const size_t motion_bytes = alias ? 0 : n * 64;
+    StagedUpload& st = ctx->body_write_stage;
+    TRY(reserve_staging(ctx, st, motion_bytes + index_bytes));
+    CK(ctx->body_writes.reserve(motion_bytes + index_bytes));
+    if (!alias) gather_motion_halves(body_dynamics, body_indices, count, st.host.as<float>());
+    std::memcpy(st.host.as<char>() + motion_bytes, body_indices, index_bytes);
+    TRY(send_staging(ctx, st, ctx->body_writes.ptr, motion_bytes + index_bytes));
+    const int32_t* indices = (const int32_t*)(ctx->body_writes.as<char>() + motion_bytes);
+    launch_write_body_motion(alias ? (const void*)alias : ctx->body_writes.ptr, indices, count, !alias, ctx->B, ctx->stream);
+    CK(cudaGetLastError());
+    ctx->h2d_accum += (int64_t)n * (64 + 4);
     return BEPUCUDA_OK;
 }
 

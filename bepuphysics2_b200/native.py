@@ -110,7 +110,7 @@ C_ABI_SYMBOLS = [
     "bepucuda_shard_set_fallback_rank",
     "bepucuda_color_constraints", "bepucuda_color_hash", "bepucuda_set_body_shapes", "bepucuda_predict_bounding_boxes",
     "bepucuda_set_body_accelerations", "bepucuda_set_point_gravity", "bepucuda_find_sleepable_islands", "bepucuda_read_constraints",
-    "bepucuda_write_constraints",
+    "bepucuda_write_constraints", "bepucuda_write_bodies",
 ]
 
 
@@ -161,6 +161,7 @@ def load_libraries():
     cuda.bepucuda_update_contacts.argtypes = [vp, i32, i32, vp, vp]
     cuda.bepucuda_upload_body_motion.argtypes = [vp, vp, i32]
     cuda.bepucuda_download_body_motion.argtypes = [vp, vp, i32]
+    cuda.bepucuda_write_bodies.argtypes = [vp, vp, i32, vp]
     cuda.bepucuda_download_bodies.argtypes = [vp, vp, i32]
     cuda.bepucuda_download_impulses.argtypes = [vp]
     cuda.bepucuda_download_prestep.argtypes = [vp, i32, i32, vp]
@@ -549,6 +550,12 @@ class CudaTimestepper:
     def upload_body_motion(self):
         """Pose + velocity halves of every BodyDynamics record only (64 of 128 bytes per body)."""
         self._check(self._cuda.bepucuda_upload_body_motion(self._ctx, self.sim.bodies.ctypes.data, self.sim.body_count))
+
+    def write_bodies(self, indices):
+        """bepucuda_write_bodies from the simulation's bodies: the pose + velocity halves of the listed active-set records only (an impulse, a new
+        velocity, a teleport the host applied). Duplicates are allowed; inertia is not written."""
+        idx = np.ascontiguousarray(indices, dtype=np.int32).reshape(-1)
+        self._check(self._cuda.bepucuda_write_bodies(self._ctx, self.sim.bodies.ctypes.data, idx.shape[0], idx.ctypes.data if idx.size else None))
 
     def download_bodies(self):
         """Full 128-B records: pose, velocity and world inertia."""

@@ -190,6 +190,24 @@ int32_t bepucuda_update_contacts(bepucuda_ctx* ctx, int32_t batch_index, int32_t
  * count must equal the one of the last bepucuda_upload_bodies. */
 int32_t bepucuda_upload_body_motion(bepucuda_ctx* ctx, const void* body_dynamics, int32_t body_count);
 int32_t bepucuda_download_body_motion(bepucuda_ctx* ctx, void* body_dynamics_out, int32_t body_count);
+/* Write the motion of listed bodies straight into the device's body state: what the host changed through BodyReference between frames (an
+ * ApplyImpulse, a new velocity, a teleport, a kinematic mover's pose) without sending the motion of every body. The host mutates its own
+ * Bodies.ActiveSet.DynamicsState as before (after bepucuda_download_body_motion it is current) and names the active-set indices it touched.
+ *   body_dynamics: the whole DynamicsState buffer, 128-B records as for bepucuda_upload_body_motion; body_indices: count active-set indices.
+ *   For each listed index, floats 0-15 of its record (pose and velocity) replace the device's pose and velocity. Local and world inertia are never
+ *   written: the stage kernels load local inertia before their grid-dependency wait, and a kinematic <-> dynamic change also changes the constraints'
+ *   kinematic bits, so an inertia change goes through bepucuda_upload_bodies and a describe (begin/upload/end_constraints).
+ *   Duplicates are allowed and write the same record; count == 0 is OK and changes nothing.
+ * Stream-ordered with bepucuda_upload_bodies and bepucuda_upload_body_motion (whichever is called last wins for a body), and seen by the next
+ * bepucuda_solve / bepucuda_profile_stages, by bepucuda_predict_bounding_boxes and by bepucuda_download_body_motion / bepucuda_download_bodies, before
+ * any solve too. From a buffer registered with bepucuda_host_register one kernel reads the listed records straight from mapped memory when the stream
+ * reaches the write: keep them unchanged until then (the next download or synchronize). From any other buffer the listed 64-B halves are gathered
+ * into a context-owned pinned staging buffer during the call, and the caller's buffers are free when it returns. The index list is always copied.
+ * Adds count * (64 + 4) bytes to h2d_bytes, inside upload_ms; never re-captures the graph. A peer-sharded rank is given the same list as every
+ * other rank, as it is given all bodies.
+ * BEPUCUDA_ERR_INVALID_ARGUMENT for count < 0, a NULL pointer with count > 0, or an index outside [0, body_count of the last bepucuda_upload_bodies);
+ * BEPUCUDA_ERR_BAD_STATE before the first bepucuda_upload_bodies. All are checked before any device work, and a failing call writes nothing. */
+int32_t bepucuda_write_bodies(bepucuda_ctx* ctx, const void* body_dynamics, int32_t count, const int32_t* body_indices);
 
 /* Replaces: Solver.Solve (Solver_Solve.cs:L1415-1484) + PoseIntegrator.IntegrateAfterSubstepping
  * (PoseIntegrator.cs:L707-726). Asynchronous on the context stream. */

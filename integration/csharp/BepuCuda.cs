@@ -63,6 +63,8 @@ namespace BepuCuda
         [DllImport(Lib)] public static extern int bepucuda_update_contacts(IntPtr ctx, int batchIndex, int typeBatchIndex, void* prestep, int* newFeatureIds);
         [DllImport(Lib)] public static extern int bepucuda_upload_body_motion(IntPtr ctx, void* bodyDynamics, int bodyCount);
         [DllImport(Lib)] public static extern int bepucuda_download_body_motion(IntPtr ctx, void* bodyDynamicsOut, int bodyCount);
+        /// <summary>Pose and velocity (floats 0-15) of the listed active-set records of DynamicsState into the device's body state; inertia is never written.</summary>
+        [DllImport(Lib)] public static extern int bepucuda_write_bodies(IntPtr ctx, void* bodyDynamics, int count, int* bodyIndices);
         [DllImport(Lib)] public static extern int bepucuda_solve(IntPtr ctx, float dt);
         [DllImport(Lib)] public static extern int bepucuda_synchronize(IntPtr ctx);
         [DllImport(Lib)] public static extern int bepucuda_download_bodies(IntPtr ctx, void* bodyDynamicsOut, int bodyCount);

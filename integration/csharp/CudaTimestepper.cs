@@ -160,6 +160,24 @@ public unsafe class CudaTimestepper<TCallbacks> : ITimestepper, IDisposable wher
             Check(Native.bepucuda_read_constraints(ctx, handles.Length, l, r));
     }
 
+    /// <summary>Sends the motion (pose and velocity) of the listed bodies, as the host's BodyReferences left them in the active set's DynamicsState,
+    /// into the device's body state (bepucuda_write_bodies): an ApplyImpulse, a new velocity, a teleport or a kinematic mover's pose, without the
+    /// motion of every other body. The handles must name awake bodies; a body count change or an inertia change still needs bepucuda_upload_bodies and
+    /// a describe. Every host change to a body's motion must be written before the next solve, or that solve starts from the device's old motion.</summary>
+    public void WriteBodies(Simulation simulation, ReadOnlySpan<BodyHandle> handles)
+    {
+        ref var bodies = ref simulation.Bodies.ActiveSet;
+        var indices = new int[handles.Length];
+        for (int i = 0; i < handles.Length; ++i)
+        {
+            ref var l = ref simulation.Bodies.HandleToLocation[handles[i].Value];                                      // BodyMemoryLocation
+            if (l.SetIndex != 0) throw new ArgumentException("WriteBodies: a sleeping body is not on the device");
+            indices[i] = l.Index;
+        }
+        fixed (int* p = indices)
+            Check(Native.bepucuda_write_bodies(ctx, bodies.DynamicsState.Memory, handles.Length, p));
+    }
+
     // FNV-1a over everything bepucuda_end_constraints analyses: batch / type batch shape, every body reference, the constrained kinematics.
     // (~8 bytes per constraint body: a few hundred microseconds for 300 k contacts, against a graph re-capture per frame.)
     static ulong TopologySignature(Simulation simulation)
