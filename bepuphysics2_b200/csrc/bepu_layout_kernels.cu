@@ -196,6 +196,48 @@ __global__ void write_constraints_kernel(const DeviceTypeBatch* __restrict__ tbs
     for (int r = lane; r < n; r += 32) dst[r * 32] = rows[q.row0 + r];
 }
 
+// Word w of a source lane's record (kRecord* layout): its address in the AOSOA-W rows of `r`, or null for a word no row holds.
+__device__ __forceinline__ int32_t* source_word(const SourceRows& r, int W, int index, int w) {
+    const size_t bundle = (size_t)(index / W), lane = (size_t)(index % W);
+    if (w >= kRecordRefs && w < kRecordRefs + r.bodies) return r.refs + (bundle * r.bodies + (w - kRecordRefs)) * W + lane;
+    if (w >= kRecordImpulses && w < kRecordImpulses + r.impulse_rows) return (int32_t*)r.impulses + (bundle * r.impulse_rows + (w - kRecordImpulses)) * W + lane;
+    if (w >= kRecordPrestep && w < kRecordPrestep + r.prestep_rows) return (int32_t*)r.prestep + (bundle * r.prestep_rows + (w - kRecordPrestep)) * W + lane;
+    return nullptr;
+}
+// bepucuda_remove_constraints: one warp per copy; lane l stages words l and l + 32 of the source lane's record, and lanes 0-3 its feature ids.
+__global__ void gather_lanes_kernel(const SourceRows* __restrict__ sources, const LaneCopy* __restrict__ copies, int count, int W, int32_t* __restrict__ records,
+                                    int32_t* __restrict__ features) {
+    const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+    if (warp >= count) return;
+    const LaneCopy c = copies[warp];
+    if (c.src_source < 0) return;
+    const SourceRows r = sources[c.src_source];
+    for (int k = 0; k < 2; ++k) {
+        const int32_t* p = source_word(r, W, c.src_index, lane + 32 * k);
+        records[(size_t)warp * 64 + lane + 32 * k] = p ? *p : 0;
+    }
+    if (lane < 4 && r.features && lane < r.contacts) features[(size_t)warp * 4 + lane] = r.features[(size_t)c.src_index * r.contacts + lane];
+}
+// bepucuda_add_constraints / bepucuda_remove_constraints: one warp per copy, the gather's word assignment.
+__global__ void scatter_lanes_kernel(const SourceRows* __restrict__ sources, const LaneCopy* __restrict__ copies, int count, int W, const int32_t* __restrict__ records,
+                                     const int32_t* __restrict__ features) {
+    const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+    if (warp >= count) return;
+    const LaneCopy c = copies[warp];
+    const SourceRows r = sources[c.dst_source];
+    for (int k = 0; k < 2; ++k) {
+        const int w = lane + 32 * k;
+        int32_t* p = source_word(r, W, c.dst_index, w);
+        if (!p) continue;
+        if (c.src_source == kLaneClear) {
+            if (w < kRecordImpulses) *p = -1;
+        } else {
+            *p = records[(size_t)warp * 64 + w];
+        }
+    }
+    if (c.src_source != kLaneClear && features && r.features && lane < r.contacts) r.features[(size_t)c.dst_index * r.contacts + lane] = features[(size_t)warp * 4 + lane];
+}
+
 // Pass 1 over every (constraint, body slot): first_batch[body] = min device batch referencing it as a dynamic body;
 // per-body reference count and bitmask of synchronized batches for the batch-invariant check.
 __global__ void ownership_pass1_kernel(const DeviceTypeBatch* __restrict__ tbs, const WorkItem* __restrict__ work, int work_count, int sync_batch_count, int body_count,
@@ -336,6 +378,14 @@ void launch_read_constraints(const DeviceTypeBatch* tbs, const TransposeDesc* de
 void launch_write_constraints(const DeviceTypeBatch* tbs, const TransposeDesc* descs, const PrestepWrite* writes, const float* rows, int count, cudaStream_t s) {
     if (count <= 0) return;
     write_constraints_kernel<<<blocks_for((size_t)count * 32, 128), 128, 0, s>>>(tbs, descs, writes, rows, count);
+}
+void launch_gather_lanes(const SourceRows* sources, const LaneCopy* copies, int count, int W, int32_t* records, int32_t* features, cudaStream_t s) {
+    if (count <= 0) return;
+    gather_lanes_kernel<<<blocks_for((size_t)count * 32, 128), 128, 0, s>>>(sources, copies, count, W, records, features);
+}
+void launch_scatter_lanes(const SourceRows* sources, const LaneCopy* copies, int count, int W, const int32_t* records, const int32_t* features, cudaStream_t s) {
+    if (count <= 0) return;
+    scatter_lanes_kernel<<<blocks_for((size_t)count * 32, 128), 128, 0, s>>>(sources, copies, count, W, records, features);
 }
 void launch_redistribute_impulses(const DeviceTypeBatch* tbs, const TransposeDesc* descs, const WorkItem* work, int work_count, cudaStream_t s) {
     if (work_count <= 0) return;

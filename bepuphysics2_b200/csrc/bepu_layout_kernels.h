@@ -54,6 +54,27 @@ struct PrestepWrite {
 };
 // bepucuda_write_constraints: the prestep rows of every write into the AOSOA-32 rows of its slot (impulses and body references untouched).
 void launch_write_constraints(const DeviceTypeBatch* tbs, const TransposeDesc* descs, const PrestepWrite* writes, const float* rows, int count, cudaStream_t s);
+// The raw reference-layout (AOSOA-W) rows of one source type batch, for the lane copies of bepucuda_add_constraints / bepucuda_remove_constraints.
+// features: the feature ids of its resident impulses ([constraint][contacts]), or null.
+struct SourceRows {
+    int32_t* refs;
+    float* prestep;
+    float* impulses;
+    int32_t* features;
+    int32_t bodies, prestep_rows, impulse_rows, contacts;
+};
+// One lane of a source written: the lane (dst_source, dst_index) takes every row of the lane (src_source, src_index); src_source == kLaneClear: its
+// body references become -1 (RemoveBodyReferencesLane; its other rows stay); kLaneNew: it takes the rows of add entry src_index.
+struct LaneCopy {
+    int32_t dst_source, dst_index, src_source, src_index;
+};
+constexpr int32_t kLaneClear = -1, kLaneNew = -2;
+// Stages the rows of every copy (after compose_lane_ops, bepu_topology.h) whose src_source >= 0 from its source lane: records[i][64] in the record layout of bepucuda_read_constraints
+// (words kRecord*), features[i][4] when the source has feature ids.
+void launch_gather_lanes(const SourceRows* sources, const LaneCopy* copies, int count, int W, int32_t* records, int32_t* features, cudaStream_t s);
+// Writes records[i] (and features[i], when `features` is not null and the destination has feature ids) into the destination lane of every copy.
+// The copies of one launch write distinct lanes and read only the staging, so they run in parallel.
+void launch_scatter_lanes(const SourceRows* sources, const LaneCopy* copies, int count, int W, const int32_t* records, const int32_t* features, cudaStream_t s);
 void launch_fill_i32(int32_t* p, size_t n, int32_t v, cudaStream_t s);
 // RedistributeImpulses (NarrowPhaseConstraintUpdate.cs:L81-135) for every device type batch whose descriptor has kDescRedistribute, on the AOSOA-32 impulses.
 void launch_redistribute_impulses(const DeviceTypeBatch* tbs, const TransposeDesc* descs, const WorkItem* work, int work_count, cudaStream_t s);

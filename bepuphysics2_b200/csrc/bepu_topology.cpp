@@ -6,6 +6,7 @@
 #include <array>
 #include <cstring>
 #include <numeric>
+#include <unordered_map>
 
 #include "../../include/bepucuda.h"
 #include "bepu_type_table.h"
@@ -278,6 +279,150 @@ int check_body_write(bool bodies_uploaded, int32_t body_count, const void* body_
 void gather_motion_halves(const void* body_dynamics, const int32_t* body_indices, int32_t count, float* out) {
     const char* records = (const char*)body_dynamics;
     for (int32_t i = 0; i < count; ++i) std::memcpy(out + (size_t)i * 16, records + (size_t)body_indices[i] * 128, 64);
+}
+
+// ---- constraint adds and removes ---------------------------------------------------------------------------------------------------------
+namespace {
+struct Replay {
+    ChangeState& st;
+    int W, threshold, body_count;
+    std::vector<LaneCopy>& ops;
+    std::string& error;
+    std::vector<int32_t> tb_count;  // per batch: its type batches
+
+    int fail(int32_t i, const std::string& why) {
+        error = "entry " + std::to_string(i) + ": " + why;
+        return BEPUCUDA_ERR_INVALID_ARGUMENT;
+    }
+    int find(int32_t batch, int32_t type_id) const {
+        for (size_t s = 0; s < st.sources.size(); ++s)
+            if (st.sources[s].type_batch_index >= 0 && st.sources[s].batch_index == batch && st.sources[s].type_id == type_id) return (int)s;
+        return -1;
+    }
+    // the first body reference of lane `index` (fallback sources), -1 beyond the bundles
+    int32_t first_ref(const ChangeSource& s, int nb, int32_t index) const {
+        const size_t at = (size_t)(index / W) * nb * W + (size_t)(index % W);
+        return at < s.refs.size() ? s.refs[at] : -1;
+    }
+    void set_lane_refs(ChangeSource& s, int nb, int32_t index, const int32_t* v) {
+        for (int b = 0; b < nb; ++b) s.refs[((size_t)(index / W) * nb + b) * W + (size_t)(index % W)] = v ? v[b] : -1;
+    }
+    int add(int32_t i, const bepucuda_constraint_location& l, const int32_t* record) {
+        const TypeInfo* t = get_type_info(l.type_id);
+        if (l.set_index != 0 || !t) return fail(i, "not a location of the active set with a supported type id");
+        if (record[0] != l.type_id) return fail(i, "record type id " + std::to_string(record[0]) + ", location type id " + std::to_string(l.type_id));
+        for (int b = 0; b < t->bodies; ++b) {
+            const int32_t v = record[kRecordRefs + b];
+            if (v < 0 || (int64_t)((uint32_t)v & ~kRefKinematicBit) >= (int64_t)body_count) return fail(i, "body reference out of range");
+        }
+        if (l.batch_index < 0 || l.batch_index > st.batch_count) return fail(i, "batch index out of range");
+        if (l.batch_index == st.batch_count) {
+            ++st.batch_count;
+            tb_count.push_back(0);
+        }
+        const bool fallback = l.batch_index >= threshold;
+        int s = find(l.batch_index, l.type_id);
+        if (s < 0) {
+            if (l.index_in_type_batch != 0) return fail(i, "a new type batch starts at index 0");
+            st.sources.push_back({l.batch_index, tb_count[(size_t)l.batch_index]++, l.type_id, 0, {}});
+            s = (int)st.sources.size() - 1;
+        }
+        ChangeSource& src = st.sources[(size_t)s];
+        const int32_t index = l.index_in_type_batch, bundles = (src.count + W - 1) / W;
+        if (!fallback) {
+            if (index != src.count) return fail(i, "a synchronized add goes to index ConstraintCount = " + std::to_string(src.count));
+        } else if (index == bundles * W) {
+            src.refs.resize((size_t)(bundles + 1) * t->bodies * W, -1);  // a new bundle: every lane empty
+        } else if (index < 0 || index > bundles * W || first_ref(src, t->bodies, index) >= 0) {
+            return fail(i, "a fallback add goes to an empty lane or to the first lane of a new bundle");
+        }
+        if (fallback) set_lane_refs(src, t->bodies, index, record + kRecordRefs);
+        src.count = std::max(src.count, index + 1);
+        ops.push_back({s, index, kLaneNew, i});
+        return BEPUCUDA_OK;
+    }
+    int remove(int32_t i, const bepucuda_constraint_location& l) {
+        const int s = l.set_index == 0 && l.type_id >= 0 && l.type_id < 64 ? find(l.batch_index, l.type_id) : -1;
+        if (s < 0 || l.index_in_type_batch < 0 || l.index_in_type_batch >= st.sources[(size_t)s].count) return fail(i, "names no constraint of the active set");
+        ChangeSource& src = st.sources[(size_t)s];
+        const int nb = get_type_info(src.type_id)->bodies;
+        const int32_t index = l.index_in_type_batch;
+        if (src.batch_index >= threshold) {
+            if (first_ref(src, nb, index) < 0) return fail(i, "a hole of the fallback batch");
+            ops.push_back({s, index, kLaneClear, 0});
+            set_lane_refs(src, nb, index, nullptr);
+            const int32_t removed_bundle = index / W;
+            bool empty = true;
+            for (int l2 = 0; l2 < W; ++l2) empty = empty && first_ref(src, nb, removed_bundle * W + l2) < 0;
+            if (empty) {
+                int32_t last = (src.count + W - 1) / W - 1;
+                if (removed_bundle != last) {
+                    for (int l2 = 0; l2 < W; ++l2) {
+                        ops.push_back({s, removed_bundle * W + l2, s, last * W + l2});
+                        for (int b = 0; b < nb; ++b) src.refs[((size_t)removed_bundle * nb + b) * W + l2] = src.refs[((size_t)last * nb + b) * W + l2];
+                    }
+                    --last;
+                }
+                int32_t lanes = 0;
+                for (int l2 = 0; l2 < W; ++l2)
+                    if (first_ref(src, nb, last * W + l2) >= 0) lanes = l2 + 1;
+                src.count = last * W + lanes;
+                src.refs.resize((size_t)((src.count + W - 1) / W) * nb * W);
+            }
+        } else {
+            const int32_t last = src.count - 1;
+            if (index < last) ops.push_back({s, index, s, last});
+            src.count = last;
+        }
+        if (src.count == 0) {
+            // ConstraintBatch.RemoveTypeBatchIfEmpty: the batch's last type batch takes the removed one's index
+            const int32_t batch = src.batch_index, removed = src.type_batch_index;
+            src.type_batch_index = -1;
+            for (ChangeSource& o : st.sources)
+                if (o.type_batch_index == tb_count[(size_t)batch] - 1 && o.batch_index == batch) o.type_batch_index = removed;
+            --tb_count[(size_t)batch];
+            // Solver.RemoveBatchIfEmpty: only the last batch goes, and with it the empty batches it reveals
+            if (batch == st.batch_count - 1)
+                while (st.batch_count > 0 && tb_count[(size_t)st.batch_count - 1] == 0) {
+                    --st.batch_count;
+                    tb_count.pop_back();
+                }
+        }
+        return BEPUCUDA_OK;
+    }
+};
+}  // namespace
+
+int replay_changes(ChangeState* state, bool remove, int W, int fallback_threshold, int body_count, int32_t count, const bepucuda_constraint_location* locations,
+                   const int32_t* records, std::vector<LaneCopy>* ops, std::string* error) {
+    Replay r{*state, W, fallback_threshold, body_count, *ops, *error, std::vector<int32_t>((size_t)std::max(state->batch_count, 0), 0)};
+    for (const ChangeSource& s : state->sources)
+        if (s.type_batch_index >= 0 && s.batch_index >= 0 && s.batch_index < state->batch_count) ++r.tb_count[(size_t)s.batch_index];
+    for (int32_t i = 0; i < count; ++i) {
+        const int rc = remove ? r.remove(i, locations[i]) : r.add(i, locations[i], records + (size_t)i * 64);
+        if (rc != BEPUCUDA_OK) return rc;
+    }
+    return BEPUCUDA_OK;
+}
+
+std::vector<LaneCopy> compose_lane_ops(const std::vector<LaneCopy>& ops) {
+    std::vector<LaneCopy> out;
+    std::unordered_map<int64_t, size_t> written;  // lane -> its entry of `out`
+    written.reserve(ops.size() * 2);
+    auto key = [](int32_t source, int32_t index) { return ((int64_t)source << 32) | (uint32_t)index; };
+    for (const LaneCopy& op : ops) {
+        LaneCopy origin = op;
+        if (op.src_source >= 0) {
+            const auto from = written.find(key(op.src_source, op.src_index));
+            if (from != written.end()) origin = {op.dst_source, op.dst_index, out[from->second].src_source, out[from->second].src_index};
+        }
+        const auto [at, inserted] = written.try_emplace(key(op.dst_source, op.dst_index), out.size());
+        if (inserted) out.push_back(origin);
+        else out[at->second] = origin;
+    }
+    // a lane that ends with its own rows needs no copy
+    out.erase(std::remove_if(out.begin(), out.end(), [](const LaneCopy& o) { return o.src_source == o.dst_source && o.src_index == o.dst_index; }), out.end());
+    return out;
 }
 
 std::vector<WorkRecord> work_records(const TopologyPlan& plan, int32_t* refs, float* prestep, float* impulses) {

@@ -105,6 +105,33 @@ int check_body_write(bool bodies_uploaded, int32_t body_count, const void* body_
 // The staging of an unregistered buffer: out[i][0 .. 16) = floats 0-15 (pose and velocity) of the 128-B record body_indices[i], in list order.
 void gather_motion_halves(const void* body_dynamics, const int32_t* body_indices, int32_t count, float* out);
 
+// bepucuda_add_constraints / bepucuda_remove_constraints on the host: Solver.Add's placement checked and Solver.Remove's lane moves replayed on the
+// context's type batches (its sources), without the rows. A fallback source keeps its AOSOA-W body references (W lanes per row, `count`'s bundles),
+// which tell holes from constraints; a synchronized one needs none. A source removed by the replay keeps its place with type_batch_index -1, and
+// a new one is appended, so that the lane ops of one call index the sources of the state before it and after it alike.
+struct ChangeSource {
+    int32_t batch_index, type_batch_index, type_id, count;
+    std::vector<int32_t> refs;
+};
+struct ChangeState {
+    std::vector<ChangeSource> sources;
+    int32_t batch_count = 0;
+};
+// Applies `count` entries in list order to *state and appends their lane copies (LaneCopy, in the order the reference writes the lanes) to *ops. Adds (remove = false; records: the 64-word records of the
+// entries): a synchronized location must be the end of its type batch, a type id without a type batch in the batch opens one at index 0, batch
+// batch_count opens a new batch, and a fallback location must be an empty lane of an existing bundle or the first lane of a new one at the end;
+// word 0 must be the location's type id and every body reference must name a body below body_count (bit 30: kinematic). Removes
+// (TypeProcessor.Remove, TypeProcessor.cs:L634-720): a synchronized one pulls the last constraint into the hole; a fallback one clears its lane
+// and, when that empties the bundle, pulls the last bundle into it and recomputes ConstraintCount from the new last bundle (L647-693). An emptied
+// type batch is swap-removed from its batch (ConstraintBatch.RemoveTypeBatchIfEmpty, ConstraintBatch.cs:L170-185), and trailing empty batches are
+// dropped (Solver.RemoveBatchIfEmpty, Solver.cs:L1294-1336). BEPUCUDA_ERR_INVALID_ARGUMENT with *error set for the first entry that breaks a rule;
+// *state is then partly changed, so callers replay on a copy.
+int replay_changes(ChangeState* state, bool remove, int W, int fallback_threshold, int body_count, int32_t count, const bepucuda_constraint_location* locations,
+                   const int32_t* records, std::vector<LaneCopy>* ops, std::string* error);
+// The lane ops of one call as one parallel step: per written lane, in the order lanes were first written, the lane of the state BEFORE the call
+// whose rows it ends with (or kLaneClear / kLaneNew). A lane cleared and later copied elsewhere carries only its cleared body references there.
+std::vector<LaneCopy> compose_lane_ops(const std::vector<LaneCopy>& ops);
+
 // What the solver kernels read per work item, with the plan's offsets applied to the arena bases.
 std::vector<WorkRecord> work_records(const TopologyPlan& plan, int32_t* refs, float* prestep, float* impulses);
 

@@ -21,13 +21,15 @@ namespace bepucuda {
 
 struct SourceTypeBatch {
     int batch_index, type_batch_index, type_id, count;
-    float* host_impulses;
+    int capacity;          // constraints the raw arrays hold (whole bundles); bepucuda_add_constraints grows them
+    float* host_impulses;  // the host's AccumulatedImpulses (bepucuda_download_impulses); null after an add until the host passes it again
     int32_t* raw_refs;     // device, reference AOSOA-W layout
     float* raw_prestep;
     float* raw_impulses;
     size_t refs_bytes, prestep_bytes, impulse_bytes;
     std::vector<int32_t> host_refs;  // retained only for fallback batches (levelisation)
-    // device-side contact update (bepucuda_update_contacts): feature ids of the resident impulses / of the frame being uploaded
+    // device-side contact update (bepucuda_update_contacts): feature ids of the resident impulses / of the frame being uploaded, `capacity`
+    // constraints each
     int32_t* raw_features_old = nullptr;
     int32_t* raw_features_new = nullptr;
     size_t feature_bytes = 0;
@@ -133,6 +135,8 @@ struct bepucuda_ctx {
     DeviceBuffer body_writes;         // bepucuda_write_bodies: one call's staged motion halves (unregistered buffers) and body indices
     StagedUpload body_write_stage;
     std::vector<Event> profile_events;
+    DeviceBuffer change_sources, change_copies, change_records, change_features;  // bepucuda_add_constraints / bepucuda_remove_constraints
+    std::vector<std::pair<void*, size_t>> spare_rows;  // raw-arena blocks of grown and removed sources, taken again by later growth (until a describe)
 };
 
 namespace {
@@ -489,6 +493,8 @@ int prepare_frame(bepucuda_ctx* ctx, float dt) {
 
 }  // namespace
 
+static int plan_device_rows(bepucuda_ctx* ctx);
+
 extern "C" {
 
 int32_t bepucuda_type_info(int32_t type_id, int32_t* bodies_per_constraint, int32_t* prestep_floats, int32_t* impulse_floats) {
@@ -662,6 +668,7 @@ int32_t bepucuda_begin_constraints(bepucuda_ctx* ctx, int32_t source_bundle_widt
     ctx->pending_h2d.clear();  // queued refreshes target raw-arena addresses that are recycled below; a re-describe uploads everything anyway
     ctx->prestep_writes.clear();  // slots of the old plan; the describe uploads the host's prestep, which ApplyDescription already wrote
     ctx->raw_arena.reset();
+    ctx->spare_rows.clear();
     ctx->pinned_arena.reset();
     ctx->constraints_open = true;
     ctx->constraints_ready = false;
@@ -682,7 +689,7 @@ int32_t bepucuda_upload_type_batch(bepucuda_ctx* ctx, int32_t batch_index, int32
     const int W = ctx->W;
     const size_t bundles = ((size_t)constraint_count + W - 1) / W;
     SourceTypeBatch s{};
-    s.batch_index = batch_index; s.type_batch_index = type_batch_index; s.type_id = type_id; s.count = constraint_count;
+    s.batch_index = batch_index; s.type_batch_index = type_batch_index; s.type_id = type_id; s.count = constraint_count; s.capacity = (int)bundles * W;
     s.host_impulses = accumulated_impulses;
     s.refs_bytes = bundles * t->bodies * W * 4;
     s.prestep_bytes = bundles * t->prestep_rows * W * 4;
@@ -713,6 +720,14 @@ int32_t bepucuda_end_constraints(bepucuda_ctx* ctx) {
     if (ctx->peer_mode && (int)ctx->body_masks.size() != ctx->body_count)
         return fail(ctx, BEPUCUDA_ERR_BAD_STATE, "end_constraints: peer sharding needs bepucuda_shard_set_body_masks for the current body count");
     CK(cudaSetDevice(ctx->device));
+    return plan_device_rows(ctx);
+}
+
+}  // extern "C"
+
+// The body of bepucuda_end_constraints, shared with bepucuda_add_constraints / bepucuda_remove_constraints: plans the sources' rows as they are on
+// the device (raw arrays), builds the tables, transposes every row in, runs the ownership passes and replaces the stage program.
+static int plan_device_rows(bepucuda_ctx* ctx) {
     const int W = ctx->W;
     {
         std::vector<SourceView> views;
@@ -821,6 +836,8 @@ int32_t bepucuda_end_constraints(bepucuda_ctx* ctx) {
     return upload_program(ctx);
 }
 
+extern "C" {
+
 int32_t bepucuda_update_type_batch(bepucuda_ctx* ctx, int32_t batch_index, int32_t type_batch_index, const float* prestep, float* accumulated_impulses) {
     if (!ctx || !prestep || !accumulated_impulses) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "update_type_batch: bad arguments");
     if (!ctx->constraints_ready) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, "update_type_batch before end_constraints");
@@ -839,10 +856,11 @@ int32_t bepucuda_update_type_batch(bepucuda_ctx* ctx, int32_t batch_index, int32
 
 static int ensure_feature_arrays(bepucuda_ctx* ctx, SourceTypeBatch& s) {
     if (s.raw_features_old) return BEPUCUDA_OK;
-    s.feature_bytes = (size_t)s.count * get_type_info(s.type_id)->contacts * sizeof(int32_t);
+    const size_t contacts = (size_t)get_type_info(s.type_id)->contacts;
+    s.feature_bytes = (size_t)s.count * contacts * sizeof(int32_t);
     cudaError_t e = cudaSuccess;
-    s.raw_features_old = (int32_t*)ctx->raw_arena.alloc(s.feature_bytes, &e);
-    s.raw_features_new = (int32_t*)ctx->raw_arena.alloc(s.feature_bytes, &e);
+    s.raw_features_old = (int32_t*)ctx->raw_arena.alloc((size_t)s.capacity * contacts * sizeof(int32_t), &e);
+    s.raw_features_new = (int32_t*)ctx->raw_arena.alloc((size_t)s.capacity * contacts * sizeof(int32_t), &e);
     if (!s.raw_features_old || !s.raw_features_new) return cuda_fail(ctx, e, "raw arena (contact feature ids)");
     return BEPUCUDA_OK;
 }
@@ -1020,6 +1038,10 @@ int32_t bepucuda_download_bodies(bepucuda_ctx* ctx, void* out, int32_t body_coun
 int32_t bepucuda_download_impulses(bepucuda_ctx* ctx) {
     if (!ctx) return BEPUCUDA_ERR_INVALID_ARGUMENT;
     if (!ctx->constraints_ready) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, "download_impulses before end_constraints");
+    for (const SourceTypeBatch& s : ctx->sources)
+        if (!s.host_impulses)
+            return fail(ctx, BEPUCUDA_ERR_BAD_STATE, "download_impulses: type batch (" + std::to_string(s.batch_index) + ", " + std::to_string(s.type_batch_index) +
+                                                         ") took constraints through bepucuda_add_constraints; pass its buffers again (update_type_batch or a describe)");
     CK(cudaSetDevice(ctx->device));
     launch_transpose_out_all(ctx->tb_table.as<DeviceTypeBatch>(), ctx->tdesc_table.as<TransposeDesc>(), ctx->work_table.as<WorkItem>(), ctx->topo.all_work_count, ctx->W,
                              kTransposeImpulses, ctx->stream);
@@ -1088,6 +1110,210 @@ int32_t bepucuda_write_constraints(bepucuda_ctx* ctx, int32_t count, const bepuc
         ctx->prestep_writes.put(resolved[(size_t)i].at, (const float*)(records + (size_t)i * 64 + kRecordPrestep), get_type_info(locations[i].type_id)->prestep_rows);
     ctx->data_dirty = true;
     return BEPUCUDA_OK;
+}
+
+// Raw rows of a source at `capacity` constraints: body references, prestep, impulses, and feature ids (old / new) when `contacts` > 0 and features
+// are kept.
+struct RawRows {
+    int32_t* refs = nullptr;
+    float* prestep = nullptr;
+    float* impulses = nullptr;
+    int32_t* features_old = nullptr;
+    int32_t* features_new = nullptr;
+};
+static size_t rows_bytes(const TypeInfo* t, int capacity, int k) {
+    const int per[5] = {t->bodies, t->prestep_rows, t->impulse_rows, t->contacts, t->contacts};
+    return (size_t)capacity * per[k] * 4;
+}
+// A block of `bytes` for source rows: a spare block of the arena between `bytes` and twice that, or a new one. Spare blocks are what grown and
+// removed sources left, so a run that stays on the change calls reuses them instead of growing the arena with every re-created type batch.
+static void* take_rows(bepucuda_ctx* ctx, size_t bytes, cudaError_t* e) {
+    size_t best = ctx->spare_rows.size();
+    for (size_t i = 0; i < ctx->spare_rows.size(); ++i) {
+        const size_t have = ctx->spare_rows[i].second;
+        if (have >= bytes && have <= 2 * bytes && (best == ctx->spare_rows.size() || have < ctx->spare_rows[best].second)) best = i;
+    }
+    if (best == ctx->spare_rows.size()) return ctx->raw_arena.alloc(bytes, e);
+    void* p = ctx->spare_rows[best].first;
+    ctx->spare_rows[best] = ctx->spare_rows.back();
+    ctx->spare_rows.pop_back();
+    return p;
+}
+static void give_rows(bepucuda_ctx* ctx, void* p, size_t bytes) {
+    if (p && bytes) ctx->spare_rows.push_back({p, bytes});
+}
+static void give_source_rows(bepucuda_ctx* ctx, const RawRows& r, const TypeInfo* t, int capacity) {
+    void* p[5] = {r.refs, r.prestep, r.impulses, r.features_old, r.features_new};
+    for (int k = 0; k < 5; ++k) give_rows(ctx, p[k], rows_bytes(t, capacity, k));
+}
+// The rows of `capacity` constraints, with feature arrays when `features`; on failure every block taken goes back and the error is returned.
+static cudaError_t take_source_rows(bepucuda_ctx* ctx, const TypeInfo* t, int capacity, bool features, RawRows* out) {
+    cudaError_t e = cudaSuccess;
+    RawRows r;
+    r.refs = (int32_t*)take_rows(ctx, rows_bytes(t, capacity, 0), &e);
+    if (r.refs) r.prestep = (float*)take_rows(ctx, rows_bytes(t, capacity, 1), &e);
+    if (r.prestep) r.impulses = (float*)take_rows(ctx, rows_bytes(t, capacity, 2), &e);
+    bool ok = r.impulses != nullptr;
+    if (ok && features && t->contacts > 0) {
+        r.features_old = (int32_t*)take_rows(ctx, rows_bytes(t, capacity, 3), &e);
+        if (r.features_old) r.features_new = (int32_t*)take_rows(ctx, rows_bytes(t, capacity, 4), &e);
+        ok = r.features_new != nullptr;
+    }
+    if (!ok) {
+        give_source_rows(ctx, r, t, capacity);
+        return e == cudaSuccess ? cudaErrorMemoryAllocation : e;
+    }
+    *out = r;
+    return cudaSuccess;
+}
+
+// bepucuda_add_constraints (remove = false) and bepucuda_remove_constraints: the dry run of the whole list on the host (replay_changes), then the
+// rows brought back to the sources, the lane copies, the new sources and counts, and the plan of the describe over the device rows.
+static int change_constraints(bepucuda_ctx* ctx, const std::string& name, bool remove, int32_t count, const bepucuda_constraint_location* locations, const int32_t* records,
+                              const int32_t* feature_ids, const int32_t* kinematics, int32_t kinematic_count) {
+    if (ctx->peer_mode) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, name + " in peer mode");
+    if (!ctx->constraints_ready) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, name + " before end_constraints");
+    if (ctx->data_dirty) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, name + ": rows are pending (uploads or writes since the last solve); change the constraints before them");
+    if (count < 0 || (count > 0 && (!locations || (!remove && !records))) || kinematic_count < 0 || (kinematic_count > 0 && !kinematics))
+        return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, name + ": bad arguments");
+    for (int32_t i = 0; i < kinematic_count; ++i)
+        if (kinematics[i] < 0 || kinematics[i] >= ctx->body_count) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, name + ": constrained kinematic index out of range");
+    if (!remove && !feature_ids)
+        for (int32_t i = 0; i < count; ++i)
+            if (contact_count_of_type(locations[i].type_id) > 0) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, name + ": feature_ids is NULL and entry " + std::to_string(i) + " is a contact");
+    const int W = ctx->W;
+    ChangeState next;
+    next.batch_count = ctx->batch_count;
+    for (const SourceTypeBatch& s : ctx->sources) next.sources.push_back({s.batch_index, s.type_batch_index, s.type_id, s.count, s.host_refs});
+    std::vector<LaneCopy> ops;
+    std::string error;
+    if (replay_changes(&next, remove, W, ctx->fallback_threshold, ctx->body_count, count, locations, records, &ops, &error) != BEPUCUDA_OK)
+        return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, name + ": " + error);
+    const std::vector<LaneCopy> copies = compose_lane_ops(ops);
+    std::vector<char> took_add(next.sources.size(), 0);
+    for (const LaneCopy& c : copies) took_add[(size_t)c.dst_source] |= c.src_source == kLaneNew;
+
+    CK(cudaSetDevice(ctx->device));
+    // Rows for every source that outgrows its arrays (new sources included), taken before any device work: a failure returns every block taken
+    // and leaves the context as it was. A new contact source keeps feature ids when the adds bring them; an existing one keeps them if it had them
+    // (one that never had bepucuda_set_contact_features still refuses bepucuda_update_contacts).
+    struct Growth { size_t source; int capacity; RawRows rows; };
+    std::vector<Growth> growth;
+    for (size_t i = 0; i < next.sources.size(); ++i) {
+        const ChangeSource& n = next.sources[i];
+        const int capacity = i < ctx->sources.size() ? ctx->sources[i].capacity : 0;
+        const int needed = (n.count + W - 1) / W * W;
+        if (needed <= capacity) continue;
+        const bool features = i < ctx->sources.size() ? ctx->sources[i].raw_features_old != nullptr : feature_ids != nullptr;
+        Growth g{i, std::max(needed, 2 * capacity), {}};
+        if (const cudaError_t e = take_source_rows(ctx, get_type_info(n.type_id), g.capacity, features, &g.rows)) {
+            for (const Growth& h : growth) give_source_rows(ctx, h.rows, get_type_info(next.sources[h.source].type_id), h.capacity);
+            return cuda_fail(ctx, e, (name + ": raw arena").c_str());
+        }
+        growth.push_back(g);
+    }
+    ctx->upload_window.start_once(ctx->stream);
+    // the device's rows of every constraint back into the sources, where the copies and the plan below read them
+    launch_transpose_out_all(ctx->tb_table.as<DeviceTypeBatch>(), ctx->tdesc_table.as<TransposeDesc>(), ctx->work_table.as<WorkItem>(), ctx->topo.all_work_count, W,
+                             kTransposePrestep | kTransposeImpulses, ctx->stream);
+    CK(cudaGetLastError());
+    ctx->constraints_ready = false;  // from here on a failure leaves a context that needs a describe
+    std::vector<SourceTypeBatch> old = std::move(ctx->sources);
+    std::vector<SourceTypeBatch> all(next.sources.size());
+    for (size_t i = 0; i < next.sources.size(); ++i) {
+        if (i < old.size()) all[i] = std::move(old[i]);
+        else all[i].type_id = next.sources[i].type_id;
+    }
+    // grown sources: the rows of their old constraints (as transposed out above) into the new arrays; the old arrays become spare
+    for (const Growth& g : growth) {
+        SourceTypeBatch& s = all[g.source];
+        const TypeInfo* t = get_type_info(s.type_id);
+        const size_t kept = ((size_t)s.count + W - 1) / W * W;  // whole bundles of the old count (0 for a new source)
+        CK(cudaMemsetAsync(g.rows.refs, 0xff, rows_bytes(t, g.capacity, 0), ctx->stream));
+        if (g.rows.features_old) CK(cudaMemsetAsync(g.rows.features_old, 0, rows_bytes(t, g.capacity, 3), ctx->stream));
+        if (kept > 0) {
+            CK(cudaMemcpyAsync(g.rows.refs, s.raw_refs, kept * t->bodies * 4, cudaMemcpyDeviceToDevice, ctx->stream));
+            CK(cudaMemcpyAsync(g.rows.prestep, s.raw_prestep, kept * t->prestep_rows * 4, cudaMemcpyDeviceToDevice, ctx->stream));
+            CK(cudaMemcpyAsync(g.rows.impulses, s.raw_impulses, kept * t->impulse_rows * 4, cudaMemcpyDeviceToDevice, ctx->stream));
+            if (s.raw_features_old) CK(cudaMemcpyAsync(g.rows.features_old, s.raw_features_old, (size_t)s.count * t->contacts * 4, cudaMemcpyDeviceToDevice, ctx->stream));
+        }
+        if (s.capacity > 0) give_source_rows(ctx, {s.raw_refs, s.raw_prestep, s.raw_impulses, s.raw_features_old, s.raw_features_new}, t, s.capacity);
+        s.raw_refs = g.rows.refs;
+        s.raw_prestep = g.rows.prestep;
+        s.raw_impulses = g.rows.impulses;
+        s.raw_features_old = g.rows.features_old;
+        s.raw_features_new = g.rows.features_new;
+        s.capacity = g.capacity;
+    }
+    for (size_t i = 0; i < next.sources.size(); ++i) {
+        const ChangeSource& n = next.sources[i];
+        SourceTypeBatch& s = all[i];
+        const TypeInfo* t = get_type_info(n.type_id);
+        s.batch_index = n.batch_index;
+        s.type_batch_index = n.type_batch_index;
+        s.count = n.count;
+        const size_t bundles = ((size_t)n.count + W - 1) / W;
+        s.refs_bytes = bundles * t->bodies * W * 4;
+        s.prestep_bytes = bundles * t->prestep_rows * W * 4;
+        s.impulse_bytes = bundles * t->impulse_rows * W * 4;
+        s.feature_bytes = (size_t)n.count * t->contacts * 4;
+        if (n.batch_index >= ctx->fallback_threshold) s.host_refs = n.refs;
+        if (took_add[i]) s.host_impulses = nullptr;
+    }
+    if (!copies.empty()) {
+        std::vector<SourceRows> rows(all.size());
+        for (size_t i = 0; i < all.size(); ++i) {
+            const TypeInfo* t = get_type_info(all[i].type_id);
+            rows[i] = {all[i].raw_refs, all[i].raw_prestep, all[i].raw_impulses, all[i].raw_features_old, t->bodies, t->prestep_rows, t->impulse_rows, t->contacts};
+        }
+        const size_t n = copies.size();
+        TRY(upload_table(ctx, "change_sources", ctx->change_sources, rows, 0));
+        TRY(upload_table(ctx, "change_copies", ctx->change_copies, copies, 0));
+        CK(ctx->change_records.reserve(n * 256));
+        CK(ctx->change_features.reserve(n * 16));
+        int64_t bytes = (int64_t)(n * sizeof(LaneCopy));
+        const bool features = remove || feature_ids;
+        if (remove) {
+            launch_gather_lanes(ctx->change_sources.as<SourceRows>(), ctx->change_copies.as<LaneCopy>(), (int)n, W, ctx->change_records.as<int32_t>(),
+                                ctx->change_features.as<int32_t>(), ctx->stream);
+        } else {
+            // an add entry writes one new lane, so copy i is entry copies[i].src_index
+            std::vector<int32_t> staged(n * 64), staged_features(feature_ids ? n * 4 : 0);
+            for (size_t i = 0; i < n; ++i) {
+                const size_t entry = (size_t)copies[i].src_index;
+                std::memcpy(staged.data() + i * 64, records + entry * 64, 256);
+                if (feature_ids) std::memcpy(staged_features.data() + i * 4, feature_ids + entry * 4, 16);
+            }
+            CK(cudaMemcpyAsync(ctx->change_records.ptr, staged.data(), n * 256, cudaMemcpyHostToDevice, ctx->stream));
+            if (feature_ids) CK(cudaMemcpyAsync(ctx->change_features.ptr, staged_features.data(), n * 16, cudaMemcpyHostToDevice, ctx->stream));
+            bytes += (int64_t)n * (256 + (feature_ids ? 16 : 0));
+        }
+        launch_scatter_lanes(ctx->change_sources.as<SourceRows>(), ctx->change_copies.as<LaneCopy>(), (int)n, W, ctx->change_records.as<int32_t>(),
+                             features ? ctx->change_features.as<int32_t>() : nullptr, ctx->stream);
+        CK(cudaGetLastError());
+        ctx->h2d_accum += bytes;
+    }
+    for (size_t i = 0; i < all.size(); ++i) {
+        if (next.sources[i].type_batch_index >= 0) ctx->sources.push_back(std::move(all[i]));
+        else give_source_rows(ctx, {all[i].raw_refs, all[i].raw_prestep, all[i].raw_impulses, all[i].raw_features_old, all[i].raw_features_new},
+                              get_type_info(all[i].type_id), all[i].capacity);  // stream order keeps this call's copies ahead of any reuse
+    }
+    ctx->batch_count = next.batch_count;
+    ctx->kinematics.assign(kinematics, kinematics + kinematic_count);
+    ctx->prestep_writes.clear();
+    return plan_device_rows(ctx);
+}
+
+int32_t bepucuda_add_constraints(bepucuda_ctx* ctx, int32_t count, const bepucuda_constraint_location* locations, const int32_t* records, const int32_t* feature_ids,
+                                 const int32_t* constrained_kinematics, int32_t kinematic_count) {
+    if (!ctx) return BEPUCUDA_ERR_INVALID_ARGUMENT;
+    return change_constraints(ctx, "add_constraints", false, count, locations, records, feature_ids, constrained_kinematics, kinematic_count);
+}
+
+int32_t bepucuda_remove_constraints(bepucuda_ctx* ctx, int32_t count, const bepucuda_constraint_location* locations, const int32_t* constrained_kinematics,
+                                    int32_t kinematic_count) {
+    if (!ctx) return BEPUCUDA_ERR_INVALID_ARGUMENT;
+    return change_constraints(ctx, "remove_constraints", true, count, locations, nullptr, nullptr, constrained_kinematics, kinematic_count);
 }
 
 int32_t bepucuda_get_timings(bepucuda_ctx* ctx, bepucuda_timings* out) {

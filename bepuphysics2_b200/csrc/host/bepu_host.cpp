@@ -5,8 +5,10 @@
 //
 // Mirrored (names kept): Bodies.Add (Bodies.cs), Solver.Add -> TryAllocateInBatch -> AllocateInTypeBatch[ForFallback]
 // (Solver.cs:L1093-1199, Constraints/TypeProcessor.cs:L314-334,L451-540), ConstrainedKinematicHandles (Solver.cs:L68),
-// SolveDescription (SolveDescription.cs:L16-137), ITimestepper.Timestep's Solve slot (DefaultTimestepper.cs:L28-43).
-// Not mirrored: removal, sleeping, batch compression, collision detection (out of scope, SURVEY.md §2).
+// SolveDescription (SolveDescription.cs:L16-137), ITimestepper.Timestep's Solve slot (DefaultTimestepper.cs:L28-43), Solver.Remove ->
+// RemoveFromBatch -> TypeProcessor.Remove, RemoveTypeBatchIfEmpty, RemoveBatchIfEmpty (Solver.cs:L1294-1405, TypeProcessor.cs:L634-720,
+// ConstraintBatch.cs:L170-185).
+// Not mirrored: sleeping, batch compression, collision detection (out of scope, SURVEY.md §2).
 #include <algorithm>
 #include <cstdint>
 #include <cstdlib>
@@ -70,9 +72,19 @@ struct IndexSet {  // BepuUtilities/Collections/IndexSet.cs
     std::vector<uint64_t> flags;
     bool contains(int i) const { size_t w = (size_t)i >> 6; return w < flags.size() && ((flags[w] >> (i & 63)) & 1); }
     void set(int i) { size_t w = (size_t)i >> 6; if (w >= flags.size()) flags.resize(w + 1, 0); flags[w] |= (uint64_t)1 << (i & 63); }
+    void unset(int i) { size_t w = (size_t)i >> 6; if (w < flags.size()) flags[w] &= ~((uint64_t)1 << (i & 63)); }
 };
 
-struct ConstraintLocation { int batch, type_id, index_in_type_batch; };
+struct ConstraintLocation { int batch, type_id, index_in_type_batch; };  // batch -1: a removed handle
+
+// One Solver.Add / Solver.Remove since the last describe or bepuhost_cuda_change, for bepuhost_cuda_change: the location the call produced or
+// consumed, and for an add its handle and encoded body references.
+struct ChangeEntry {
+    bool remove;
+    ConstraintLocation at;
+    int handle;
+    int32_t refs[4];
+};
 
 struct Simulation {
     int W;                       // Vector<float>.Count of the emulated host
@@ -86,6 +98,8 @@ struct Simulation {
     std::vector<int32_t> constrained_kinematic_handles;
     IndexSet constrained_kinematic_set;
     std::vector<ConstraintLocation> handle_to_constraint;
+    std::vector<int32_t> kinematic_constraint_count;  // per body: constraints referencing it as a kinematic (Bodies' constraint lists, kinematics only)
+    std::vector<ChangeEntry> changes;
     std::string error;
     ~Simulation() { for (auto b : batches) delete b; }
 };
@@ -226,6 +240,8 @@ int allocate_in_batch(Simulation& sim, int target, int type_id, int nb, const in
         if ((uint32_t)encoded[i] & kKinematicMask) {
             const int h = encoded[i] & ~(int32_t)kKinematicMask;
             if (!sim.constrained_kinematic_set.contains(h)) { sim.constrained_kinematic_set.set(h); sim.constrained_kinematic_handles.push_back(h); }
+            if ((int)sim.kinematic_constraint_count.size() <= h) sim.kinematic_constraint_count.resize((size_t)h + 1, 0);
+            ++sim.kinematic_constraint_count[(size_t)h];
         }
     TypeBatch* tb = get_or_create_type_batch(sim, *sim.batches[target], type_id);
     if (!tb) { sim.error = "unsupported constraint type"; return -1; }
@@ -233,7 +249,103 @@ int allocate_in_batch(Simulation& sim, int target, int type_id, int nb, const in
     write_lane(sim, *tb, index, encoded, prestep);
     for (int i = 0; i < blocking_count; ++i) sim.batch_referenced_handles[target].set(blocking[i]);
     sim.handle_to_constraint.push_back({target, type_id, index});
+    ChangeEntry e{false, {target, type_id, index}, handle, {-1, -1, -1, -1}};
+    for (int i = 0; i < nb; ++i) e.refs[i] = encoded[i];
+    sim.changes.push_back(e);
     return handle;
+}
+
+// Moves lane `from` of `t` into lane `to` (TypeProcessor.Move / whole-bundle pulls): body references, prestep, impulses, and the handle's location.
+void move_lane(Simulation& sim, TypeBatch& t, int from, int to) {
+    const int W = sim.W;
+    auto lane = [&](auto* data, int rows, int index, int r) -> auto& { return data[((size_t)(index / W) * rows + r) * W + index % W]; };
+    for (int r = 0; r < t.bodies; ++r) lane(t.body_references.data, t.bodies, to, r) = lane(t.body_references.data, t.bodies, from, r);
+    for (int r = 0; r < t.prestep_rows; ++r) lane(t.prestep.data, t.prestep_rows, to, r) = lane(t.prestep.data, t.prestep_rows, from, r);
+    for (int r = 0; r < t.impulse_rows; ++r) lane(t.impulses.data, t.impulse_rows, to, r) = lane(t.impulses.data, t.impulse_rows, from, r);
+    const int handle = t.index_to_handle[(size_t)from];
+    t.index_to_handle[(size_t)to] = handle;
+    t.index_to_handle[(size_t)from] = -1;
+    if (handle >= 0) sim.handle_to_constraint[(size_t)handle].index_in_type_batch = to;
+}
+void clear_lane_references(Simulation& sim, TypeBatch& t, int index) {  // RemoveBodyReferencesLane
+    for (int r = 0; r < t.bodies; ++r) t.body_references.data[((size_t)(index / sim.W) * t.bodies + r) * sim.W + index % sim.W] = -1;
+}
+
+// Solver.Remove (Solver.cs:L1385-1405): the bodies' kinematic bookkeeping, RemoveFromBatch (L1344-1358) with TypeProcessor.Remove (TypeProcessor.cs:
+// L634-720), RemoveTypeBatchIfEmpty (ConstraintBatch.cs:L170-185) and RemoveBatchIfEmpty (Solver.cs:L1294-1336).
+int solver_remove(Simulation& sim, int handle) {
+    if (handle < 0 || handle >= (int)sim.handle_to_constraint.size() || sim.handle_to_constraint[(size_t)handle].batch < 0) { sim.error = "no such constraint handle"; return -1; }
+    const ConstraintLocation at = sim.handle_to_constraint[(size_t)handle];
+    sim.changes.push_back({true, at, handle, {-1, -1, -1, -1}});
+    ConstraintBatch& batch = *sim.batches[(size_t)at.batch];
+    const int tb_index = batch.type_index_to_type_batch_index[at.type_id];
+    TypeBatch& t = *batch.type_batches[(size_t)tb_index];
+    const int W = sim.W, index = at.index_in_type_batch;
+    const int32_t* refs = t.body_references.data + (size_t)(index / W) * t.bodies * W + index % W;
+    for (int b = 0; b < t.bodies; ++b) {
+        const int32_t enc = refs[(size_t)b * W];
+        const int body = enc & ~(int32_t)kKinematicMask;
+        if ((uint32_t)enc & kKinematicMask) {
+            // RemoveConstraintReferencesFromBodiesEnumerator: the last constraint of a kinematic takes it out of ConstrainedKinematicHandles (FastRemove)
+            if (--sim.kinematic_constraint_count[(size_t)body] == 0) {
+                auto& list = sim.constrained_kinematic_handles;
+                const auto it = std::find(list.begin(), list.end(), body);
+                *it = list.back();
+                list.pop_back();
+                sim.constrained_kinematic_set.unset(body);
+            }
+        } else if (at.batch < sim.fallback_batch_threshold) {
+            sim.batch_referenced_handles[(size_t)at.batch].unset(body);  // RemoveBodyHandlesFromBatchForConstraint
+        }
+    }
+    if (at.batch == sim.fallback_batch_threshold) {
+        // The fallback batch's body set decides nothing here (it accepts every constraint), so it is not kept up to date.
+        t.index_to_handle[(size_t)index] = -1;
+        clear_lane_references(sim, t, index);
+        const int removed_bundle = index / W;
+        bool empty = true;
+        for (int l = 0; l < W; ++l) empty = empty && t.body_references.data[(size_t)removed_bundle * t.bodies * W + l] < 0;
+        if (empty) {
+            int last = t.bundle_count(W) - 1;
+            if (removed_bundle != last) {
+                for (int l = 0; l < W; ++l) {
+                    const int from = last * W + l;
+                    if (from < t.constraint_count && t.body_references.data[(size_t)last * t.bodies * W + l] >= 0) move_lane(sim, t, from, removed_bundle * W + l);
+                    else {  // a hole moves as it is: its body references
+                        for (int r = 0; r < t.bodies; ++r) t.body_references.data[((size_t)removed_bundle * t.bodies + r) * W + l] = t.body_references.data[((size_t)last * t.bodies + r) * W + l];
+                    }
+                }
+                --last;
+            }
+            int lanes = 0;
+            for (int l = 0; l < W; ++l)
+                if (last >= 0 && t.body_references.data[(size_t)last * t.bodies * W + l] >= 0) lanes = l + 1;
+            t.constraint_count = std::max(last, 0) * W + lanes;
+            t.index_to_handle.resize((size_t)t.constraint_count);
+        }
+    } else {
+        const int last = t.constraint_count - 1;
+        if (index < last) move_lane(sim, t, last, index);
+        else t.index_to_handle[(size_t)index] = -1;
+        clear_lane_references(sim, t, last);
+        t.constraint_count = last;
+        t.index_to_handle.resize((size_t)last);
+    }
+    sim.handle_to_constraint[(size_t)handle] = {-1, -1, -1};
+    if (t.constraint_count == 0) {
+        batch.type_index_to_type_batch_index[at.type_id] = -1;
+        delete batch.type_batches[(size_t)tb_index];
+        batch.type_batches[(size_t)tb_index] = batch.type_batches.back();
+        batch.type_batches.pop_back();
+        if (tb_index < (int)batch.type_batches.size()) batch.type_index_to_type_batch_index[batch.type_batches[(size_t)tb_index]->type_id] = tb_index;
+        if (at.batch == (int)sim.batches.size() - 1)
+            while (!sim.batches.empty() && sim.batches.back()->type_batches.empty()) {
+                delete sim.batches.back();
+                sim.batches.pop_back();
+                sim.batch_referenced_handles.pop_back();
+            }
+    }
+    return 0;
 }
 
 // Solver.Add (Solver.cs:L1182-1199): greedy first fit over batches; kinematics never block (GetBlockingBodyHandles L1058-1078);
@@ -352,12 +464,24 @@ int32_t bepuhost_add_constraints_in_batches(void* simp, int32_t type_id, int32_t
     }
     return first;
 }
-// In handle (= add) order: the encoded body references of every constraint, 4 slots each (-1 = unused), and its batch index.
+// Solver.Remove for `count` handles in order. Returns 0, or -1 at the first handle that names no constraint (the ones before it are removed).
+int32_t bepuhost_remove_constraints(void* simp, int32_t count, const int32_t* handles) {
+    Simulation& sim = *(Simulation*)simp;
+    for (int32_t i = 0; i < count; ++i)
+        if (solver_remove(sim, handles[i]) != 0) return -1;
+    return 0;
+}
+// In handle (= add) order (-1 for a removed handle): the encoded body references of every constraint, 4 slots each (-1 = unused), and its batch index.
 int32_t bepuhost_export_constraint_references(void* simp, int32_t* references_out, int32_t* batch_indices_out) {
     Simulation& sim = *(Simulation*)simp;
     const int W = sim.W;
     for (size_t h = 0; h < sim.handle_to_constraint.size(); ++h) {
         const ConstraintLocation& loc = sim.handle_to_constraint[h];
+        if (loc.batch < 0) {  // removed
+            for (int b = 0; b < 4; ++b) references_out[h * 4 + b] = -1;
+            if (batch_indices_out) batch_indices_out[h] = -1;
+            continue;
+        }
         ConstraintBatch& batch = *sim.batches[loc.batch];
         TypeBatch& t = *batch.type_batches[batch.type_index_to_type_batch_index[loc.type_id]];
         const int bundle = loc.index_in_type_batch / W, inner = loc.index_in_type_batch % W;
@@ -369,7 +493,7 @@ int32_t bepuhost_export_constraint_references(void* simp, int32_t* references_ou
 }
 int32_t bepuhost_constraint_location(void* simp, int32_t handle, int32_t* batch, int32_t* type_id, int32_t* index_in_type_batch) {
     Simulation& sim = *(Simulation*)simp;
-    if (handle < 0 || handle >= (int)sim.handle_to_constraint.size()) return -1;
+    if (handle < 0 || handle >= (int)sim.handle_to_constraint.size() || sim.handle_to_constraint[handle].batch < 0) return -1;
     *batch = sim.handle_to_constraint[handle].batch;
     *type_id = sim.handle_to_constraint[handle].type_id;
     *index_in_type_batch = sim.handle_to_constraint[handle].index_in_type_batch;
@@ -416,7 +540,56 @@ int32_t bepuhost_cuda_describe(void* simp, bepucuda_ctx* ctx) {
         }
     }
     if ((rc = bepucuda_set_constrained_kinematics(ctx, sim.constrained_kinematic_handles.data(), (int32_t)sim.constrained_kinematic_handles.size())) != 0) return rc;
+    sim.changes.clear();
     return bepucuda_end_constraints(ctx);
+}
+
+// The constraint adds and removes since the last describe or change on the resident rows: one bepucuda_add_constraints / bepucuda_remove_constraints
+// per run of adds or removes, in the order they were made, each with the constrained kinematics as they are now. An add's record is its lane as
+// the host holds it now (body references, impulses the host may have written since, prestep); a constraint added and removed again since sends its
+// body references and zero rows. add_feature_ids: 4 int32 per add in order, or NULL when no add is a contact. At a failing call the runs before it
+// leave the log and its code is returned; the failing run and those after it stay (add_feature_ids then starts at the first add still logged).
+int32_t bepuhost_cuda_change(void* simp, bepucuda_ctx* ctx, const int32_t* add_feature_ids) {
+    Simulation& sim = *(Simulation*)simp;
+    const int W = sim.W;
+    const int32_t* kin = sim.constrained_kinematic_handles.data();
+    const int32_t kin_count = (int32_t)sim.constrained_kinematic_handles.size();
+    size_t adds = 0;
+    for (size_t i = 0; i < sim.changes.size();) {
+        size_t j = i;
+        while (j < sim.changes.size() && sim.changes[j].remove == sim.changes[i].remove) ++j;
+        std::vector<bepucuda_constraint_location> locations;
+        std::vector<int32_t> records;
+        for (size_t k = i; k < j; ++k) {
+            const ChangeEntry& e = sim.changes[k];
+            locations.push_back({0, e.at.batch, e.at.type_id, e.at.index_in_type_batch});
+            if (e.remove) continue;
+            records.resize(records.size() + 64, 0);
+            int32_t* r = records.data() + records.size() - 64;
+            r[0] = e.at.type_id;
+            r[1] = 1;
+            const bepucuda::TypeRow* t = bepucuda::type_row(e.at.type_id);
+            for (int b = 0; b < t->bodies; ++b) r[2 + b] = e.refs[b];
+            const ConstraintLocation now = sim.handle_to_constraint[(size_t)e.handle];
+            if (now.batch < 0) continue;
+            ConstraintBatch& batch = *sim.batches[(size_t)now.batch];
+            const TypeBatch& tb = *batch.type_batches[(size_t)batch.type_index_to_type_batch_index[now.type_id]];
+            const size_t bundle = (size_t)(now.index_in_type_batch / W), lane = (size_t)(now.index_in_type_batch % W);
+            for (int q = 0; q < tb.impulse_rows; ++q) std::memcpy(r + 6 + q, tb.impulses.data + (bundle * tb.impulse_rows + q) * W + lane, 4);
+            for (int q = 0; q < tb.prestep_rows; ++q) std::memcpy(r + 18 + q, tb.prestep.data + (bundle * tb.prestep_rows + q) * W + lane, 4);
+        }
+        const int32_t n = (int32_t)(j - i);
+        const int32_t rc = sim.changes[i].remove ? bepucuda_remove_constraints(ctx, n, locations.data(), kin, kin_count)
+                                                 : bepucuda_add_constraints(ctx, n, locations.data(), records.data(), add_feature_ids ? add_feature_ids + adds * 4 : nullptr, kin, kin_count);
+        if (rc != 0) {
+            sim.changes.erase(sim.changes.begin(), sim.changes.begin() + (std::ptrdiff_t)i);  // the runs before it went through: not forwarded again
+            return rc;
+        }
+        if (!sim.changes[i].remove) adds += (size_t)n;
+        i = j;
+    }
+    sim.changes.clear();
+    return 0;
 }
 
 // Per-frame refresh with unchanged topology: body state + the prestep/impulse data the narrow phase rewrote.

@@ -110,7 +110,7 @@ C_ABI_SYMBOLS = [
     "bepucuda_shard_set_fallback_rank",
     "bepucuda_color_constraints", "bepucuda_color_hash", "bepucuda_set_body_shapes", "bepucuda_predict_bounding_boxes",
     "bepucuda_set_body_accelerations", "bepucuda_set_point_gravity", "bepucuda_find_sleepable_islands", "bepucuda_read_constraints",
-    "bepucuda_write_constraints", "bepucuda_write_bodies",
+    "bepucuda_write_constraints", "bepucuda_write_bodies", "bepucuda_add_constraints", "bepucuda_remove_constraints",
 ]
 
 
@@ -180,6 +180,8 @@ def load_libraries():
     cuda.bepucuda_find_sleepable_islands.argtypes = [vp, vp, i32, vp, vp, vp, C.POINTER(i32), C.POINTER(i32)]
     cuda.bepucuda_read_constraints.argtypes = [vp, i32, vp, vp]
     cuda.bepucuda_write_constraints.argtypes = [vp, i32, vp, vp]
+    cuda.bepucuda_add_constraints.argtypes = [vp, i32, vp, vp, vp, vp, i32]
+    cuda.bepucuda_remove_constraints.argtypes = [vp, i32, vp, vp, i32]
 
     host.bepuhost_create.restype = vp
     host.bepuhost_create.argtypes = [i32, i32]
@@ -195,6 +197,8 @@ def load_libraries():
     host.bepuhost_body_count.argtypes = [vp]
     host.bepuhost_add_constraints.argtypes = [vp, i32, i32, vp, vp]
     host.bepuhost_add_constraints_in_batches.argtypes = [vp, i32, i32, vp, vp, vp]
+    host.bepuhost_remove_constraints.argtypes = [vp, i32, vp]
+    host.bepuhost_cuda_change.argtypes = [vp, vp, vp]
     host.bepuhost_export_constraint_references.argtypes = [vp, vp, vp]
     host.bepuhost_constraint_location.argtypes = [vp, i32, C.POINTER(i32), C.POINTER(i32), C.POINTER(i32)]
     host.bepuhost_constraint_count.argtypes = [vp]
@@ -318,6 +322,13 @@ class Simulation:
         if first < 0:
             raise ValueError(self._host.bepuhost_last_error(self._sim).decode())
         return first
+
+    def remove_constraints(self, handles):
+        """Solver.Remove for each handle in order (Solver.cs:L1385-1405): swap-remove in a synchronized type batch, lane clear and bundle pull in the
+        fallback batch, then the emptied type batch and trailing empty batches go. Raises at a handle that names no constraint."""
+        h = np.ascontiguousarray(handles, dtype=np.int32).reshape(-1)
+        if self._host.bepuhost_remove_constraints(self._sim, h.shape[0], h.ctypes.data) != 0:
+            raise ValueError(self._host.bepuhost_last_error(self._sim).decode())
 
     def constraint_references(self):
         """(references[n, 4], batch[n]) in handle (= add) order: encoded body references (kinematic flag in bit 30, -1 = unused slot) and batch indices."""
@@ -482,6 +493,33 @@ class CudaTimestepper:
         rec = np.ascontiguousarray(records, dtype=np.int32).reshape(-1, 64)
         assert rec.shape[0] == loc.shape[0]
         self._check(self._cuda.bepucuda_write_constraints(self._ctx, loc.shape[0], loc.ctypes.data, rec.ctypes.data))
+
+    def _kinematics(self, kinematics):
+        k = np.ascontiguousarray(self.sim.constrained_kinematics if kinematics is None else kinematics, dtype=np.int32).reshape(-1)
+        return k, (k.ctypes.data if k.size else None)
+
+    def add_constraints(self, locations, records, feature_ids=None, kinematics=None):
+        """bepucuda_add_constraints: the constraints the host added, in order, at the locations its Solver.Add gave them (locations as for
+        read_constraints), with int32[n, 64] records in the read_constraints layout (impulses written as given) and optionally int32[n, 4] feature
+        ids. kinematics: the constrained kinematic indices after the changes (the simulation's by default)."""
+        loc = self._locations(locations)
+        rec = np.ascontiguousarray(records, dtype=np.int32).reshape(-1, 64)
+        assert rec.shape[0] == loc.shape[0]
+        feat = None if feature_ids is None else np.ascontiguousarray(feature_ids, dtype=np.int32).reshape(-1, 4)
+        k, kp = self._kinematics(kinematics)
+        self._check(self._cuda.bepucuda_add_constraints(self._ctx, loc.shape[0], loc.ctypes.data, rec.ctypes.data, None if feat is None else feat.ctypes.data, kp, k.shape[0]))
+
+    def remove_constraints(self, locations, kinematics=None):
+        """bepucuda_remove_constraints: the constraints the host removed, in order, at the locations its Solver.Remove found them."""
+        loc = self._locations(locations)
+        k, kp = self._kinematics(kinematics)
+        self._check(self._cuda.bepucuda_remove_constraints(self._ctx, loc.shape[0], loc.ctypes.data, kp, k.shape[0]))
+
+    def change(self, add_feature_ids=None):
+        """bepuhost_cuda_change: every constraint add and remove of the simulation since the last describe or change, forwarded to the device rows
+        run by run. add_feature_ids: int32[adds, 4] in add order, or None when no add is a contact."""
+        feat = None if add_feature_ids is None else np.ascontiguousarray(add_feature_ids, dtype=np.int32).reshape(-1, 4)
+        self._check(self._host.bepuhost_cuda_change(self.sim._sim, self._ctx, None if feat is None else feat.ctypes.data))
 
     def register_host_buffers(self):
         """Page-locks the simulation's buffers (a C# host would register its BufferPool blocks once)."""

@@ -277,6 +277,50 @@ int32_t bepucuda_read_constraints(bepucuda_ctx* ctx, int32_t count, const bepucu
  * is OK and changes nothing. */
 int32_t bepucuda_write_constraints(bepucuda_ctx* ctx, int32_t count, const bepucuda_constraint_location* locations, const int32_t* records);
 
+/* Add and remove listed constraints of the device rows: Solver.Add (Solver.cs:L1182-1199; TypeProcessor.AllocateInTypeBatch L314,
+ * AllocateInTypeBatchForFallback L451) and Solver.Remove (Solver.cs:L1385-1405 -> RemoveFromBatch L1344-1358, TypeProcessor.Remove L634-720,
+ * ConstraintBatch.RemoveTypeBatchIfEmpty ConstraintBatch.cs:L170-185, Solver.RemoveBatchIfEmpty L1294-1336) on the resident path, where a describe
+ * would first need every impulse downloaded and then send every type batch back up. The host runs Solver.Add / Solver.Remove on its own buffers as
+ * before and decides every location; the device replays the reference's lane moves (the swap-remove of a synchronized type batch, the lane clear and
+ * bundle pull of the fallback batch, the removal of emptied type batches and of trailing empty batches), so that afterwards every location the
+ * host holds names the same constraint on the device.
+ *   Entries apply in list order, each in the state the entries before it left. locations[i]: the Solver.HandleToConstraint entry the host's own
+ *   call produced (add) or consumed (remove). Make one call per run of adds or removes, in the order the host applied them; the reference's narrow
+ *   phase adds first (OnPreflush) and removes after (the ConstraintRemover jobs of NarrowPhase.Flush).
+ *   Add placement must be Solver.Add's: in a synchronized batch index_in_type_batch == the type batch's ConstraintCount; a type id without a type
+ *   batch in the batch opens one (index 0) at TypeBatches.Count; batch_index == the batch count opens a batch; in the fallback batch the index names
+ *   an empty lane or the first lane of a new bundle at the end.
+ *   records: count records of 64 int32 in the layout of bepucuda_read_constraints. Word 0 is the type id, words 2-5 the body references (bit 30:
+ *   kinematic), words 6.. the accumulated impulses and words 18.. the prestep, all written as given: zero impulses for a new pair; for a contact
+ *   whose type changed, the impulses the host redistributed from the old constraint it read with bepucuda_read_constraints before removing it
+ *   (NarrowPhase.UpdateConstraint gathers them before the remove).
+ *   feature_ids: 4 int32 per entry, the ids of the entry's impulses for the next bepucuda_update_contacts (words past its contact count ignored);
+ *   NULL is allowed when no entry is a contact type, and then no feature id is written.
+ *   constrained_kinematics: Solver.ConstrainedKinematicHandles after the host's changes, mapped to active-set indices, as for
+ *   bepucuda_set_constrained_kinematics.
+ * After a successful call the context is as if the host had described its current buffers, except that every row of a constraint that already
+ * existed comes from the device (its accumulated impulses, incrementally updated depths and resident feature ids) and only the listed entries
+ * crossed the bus: 16 B per lane copy plus, per add entry, its 256-B record and, with feature_ids, 16 B (bepucuda_timings h2d_bytes, inside
+ * upload_ms). An add entry is one lane copy; a synchronized remove is at most one, a fallback remove one lane clear and, when it pulls a bundle,
+ * W copies (the clear lane among them). Reads, writes, bepucuda_find_sleepable_islands and bepucuda_update_contacts take the new locations at once;
+ * the next solve re-captures the graph. The host buffers passed to bepucuda_upload_type_batch / bepucuda_update_type_batch of a type batch that
+ * took an add may since have been reallocated: until that type batch is passed again (bepucuda_update_type_batch or a describe),
+ * bepucuda_download_impulses returns BEPUCUDA_ERR_BAD_STATE; bepucuda_read_constraints reads its impulses. The device rows of grown and removed
+ * type batches are reused by later growth; a describe releases them all. A contact type batch that never had bepucuda_set_contact_features
+ * keeps refusing bepucuda_update_contacts after adds; a type batch the adds create keeps the feature ids they bring.
+ * BEPUCUDA_ERR_BAD_STATE before the first bepucuda_end_constraints, between begin and end, in peer mode, and while rows are pending
+ * (bepucuda_update_type_batch, bepucuda_update_contacts, bepucuda_set_contact_features or bepucuda_write_constraints since the last solve; a frame
+ * is solve, changes, then that frame's uploads and writes). BEPUCUDA_ERR_INVALID_ARGUMENT for count < 0, a NULL pointer with count > 0 (feature_ids
+ * aside), a placement other than the above, a word 0 other than the location's type id, a body reference out of range, a remove of a hole or at or
+ * beyond ConstraintCount, and a constrained kinematic index out of range. These are found by a dry run of the whole list on the host: a failing
+ * call does no device work and changes nothing. An add that breaks the batch invariant (a synchronized batch holding a dynamic body twice) is
+ * found by the ownership pass: BEPUCUDA_ERR_BATCH_INVARIANT, and the context needs a describe (bepucuda_solve returns BEPUCUDA_ERR_BAD_STATE until
+ * begin/end_constraints). count == 0 re-plans with the new constrained kinematics. */
+int32_t bepucuda_add_constraints(bepucuda_ctx* ctx, int32_t count, const bepucuda_constraint_location* locations, const int32_t* records, const int32_t* feature_ids,
+                                 const int32_t* constrained_kinematics, int32_t kinematic_count);
+int32_t bepucuda_remove_constraints(bepucuda_ctx* ctx, int32_t count, const bepucuda_constraint_location* locations, const int32_t* constrained_kinematics,
+                                    int32_t kinematic_count);
+
 int32_t bepucuda_get_timings(bepucuda_ctx* ctx, bepucuda_timings* out);
 
 /* Replaces SimulationProfiler.Start/End (SimulationProfiler.cs:L25-60): CUDA events on the context stream, 16 slots. */

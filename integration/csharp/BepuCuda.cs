@@ -92,6 +92,8 @@ namespace BepuCuda
         /// <summary>Device-side batch colouring: the batch Solver.Add's first-fit search would pick for every constraint of a list (order 0 = add order, 1 = hashed, 2 = priorities).</summary>
         [DllImport(Lib)] public static extern int bepucuda_color_constraints(IntPtr ctx, int constraintCount, int bodiesPerConstraint, int* encodedBodyReferences, int bodyCount, int fallbackBatchThreshold, int order, uint* priorities, int* batchIndicesOut, int* batchCountOut, int* roundsOut);
         [DllImport(Lib)] public static extern uint bepucuda_color_hash(uint constraintIndex);
+        [DllImport(Lib)] public static extern int bepucuda_add_constraints(IntPtr ctx, int count, CudaConstraintLocation* locations, int* records, int* featureIds, int* constrainedKinematics, int kinematicCount);
+        [DllImport(Lib)] public static extern int bepucuda_remove_constraints(IntPtr ctx, int count, CudaConstraintLocation* locations, int* constrainedKinematics, int kinematicCount);
         /// <summary>Sleepable islands on the device: per body the smallest body index of its island, and the islands whose bodies are all sleep candidates (ascending, with body counts).
         /// Call after bepucuda_solve and before IncrementallyOptimizeDataStructures; see INTEGRATION.md.</summary>
         [DllImport(Lib)] public static extern int bepucuda_find_sleepable_islands(IntPtr ctx, BodyActivity* activities, int bodyCount, int* islandOfBodyOut, int* sleepableRootsOut, int* sleepableBodyCountsOut, int* sleepableCountOut, int* roundsOut);

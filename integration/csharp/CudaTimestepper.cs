@@ -97,7 +97,9 @@ public unsafe class CudaTimestepper<TCallbacks> : ITimestepper, IDisposable wher
         else fixed (float* a = bodyAccelerations) Check(Native.bepucuda_set_body_accelerations(ctx, a, bodyAccelerations.Length / 8));
 
         // Frames whose constraint graph did not change (same type batches, same body references, same kinematics) only refresh what the
-        // narrow phase rewrote: the device keeps its batch analysis and the captured CUDA graph (INTEGRATION.md, performance notes).
+        // narrow phase rewrote: the device keeps its batch analysis and the captured CUDA graph (INTEGRATION.md, performance notes). A changed
+        // graph is described again: bepucuda_add_constraints / bepucuda_remove_constraints need every Solver.Add and Solver.Remove of the frame in
+        // the order they ran, and the simulation gives an ITimestepper no record of them, so only an application that logs them can forward them.
         ref var set = ref solver.ActiveSet;
         ulong topology = TopologySignature(simulation);
         if (topology == uploadedTopology)

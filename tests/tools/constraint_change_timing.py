@@ -1,0 +1,121 @@
+"""Measurement: a frame of C2 (the 100 k-body shape pile) whose collision detection removes and re-adds a fraction of the manifolds, sent to the
+device either as the change calls (bepuhost_cuda_change: bepucuda_remove_constraints + bepucuda_add_constraints on the resident rows) or as
+bepucuda_download_impulses before the host's changes and a full describe after them. Fast build, graph mode, pageable host buffers. Two twin
+simulations, one per route, alternate frame by frame; each frame is changes, solve (which re-captures the graph), download_body_motion.
+Per route and fraction: medians over the timed frames of the device time of the route's calls (CUDA events around them) and of their host wall
+clock, the wall clock of the whole frame, and the bytes up. Prints one JSON line per route with the card it ran on, and writes the lines to --out
+when given."""
+import argparse
+import json
+import os
+import subprocess
+import sys
+import time
+
+import numpy as np
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))))
+import bepuphysics2_b200 as bp  # noqa: E402
+from bepuphysics2_b200 import scenes  # noqa: E402
+
+DT = 1.0 / 60.0
+
+
+def card():
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True, check=True)
+    name, limit = [x.strip() for x in q.stdout.splitlines()[0].split(",")]
+    return {"gpu": name, "power_limit": limit}
+
+
+def host_changes(sim, rng, fraction, original):
+    """Solver.Remove of a fraction of the live constraints, then Solver.Add of the same pairs again, one bulk call per type. Returns the adds."""
+    _, batches = sim.constraint_references()
+    live = np.flatnonzero(batches >= 0)
+    pick = rng.choice(live, size=max(1, int(len(live) * fraction)), replace=False)
+    sim.remove_constraints(pick)
+    by_type = {}
+    for h in pick:
+        type_id, bodies, prestep = original[int(h)]
+        by_type.setdefault(type_id, []).append((bodies, prestep))
+    for type_id, items in sorted(by_type.items()):
+        first = sim.add_constraints(type_id, np.stack([b for b, _ in items]), np.stack([p for _, p in items]))
+        for k, (b, p) in enumerate(items):
+            original[first + k] = (type_id, b, p)
+    return len(pick)
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--bodies", type=int, default=100_000)
+    ap.add_argument("--frames", type=int, default=8, help="timed frames per route and fraction")
+    ap.add_argument("--warmup", type=int, default=2)
+    ap.add_argument("--fractions", default="0.01,0.1")
+    ap.add_argument("--out", default=None)
+    args = ap.parse_args()
+    scene = scenes.shape_pile(args.bodies, seed=5)
+    base = []
+    for type_id, handles, prestep in scene["constraints"]:
+        base += [(type_id, np.asarray(h, dtype=np.int32), np.asarray(p, dtype=np.float32)) for h, p in zip(handles, prestep)]
+    info = card()
+    lines = []
+    for fraction in [float(f) for f in args.fractions.split(",")]:
+        twins = {}
+        for route in ("change", "describe"):
+            sim = bp.Simulation(bundle_width=8, substeps=8, velocity_iterations=2)
+            scenes.build(scene, sim)
+            ts = bp.CudaTimestepper(sim, strict_fp=False)  # pageable buffers: Solver.Add reallocates the mirror's type batches
+            ts.describe()
+            ts.solve_device_only(DT)
+            twins[route] = (sim, ts, dict(enumerate(base)), np.random.default_rng(7))
+        samples = {r: {"device_ms": [], "wall_ms": [], "frame_wall_ms": [], "h2d_bytes": []} for r in twins}
+        for frame in range(args.warmup + args.frames):
+            for route, (sim, ts, original, rng) in twins.items():
+                start = time.perf_counter()
+                if route == "change":
+                    adds = host_changes(sim, rng, fraction, original)
+                    t0 = time.perf_counter()
+                    ts.event_record(0)
+                    ts.change(np.zeros((adds, 4), dtype=np.int32))
+                    ts.event_record(1)
+                    ts.synchronize()
+                    wall = time.perf_counter() - t0
+                    device = ts.event_elapsed_ms(0, 1)
+                else:
+                    t0 = time.perf_counter()
+                    ts.event_record(0)
+                    ts.download_impulses()
+                    ts.event_record(1)
+                    wall = time.perf_counter() - t0
+                    device = ts.event_elapsed_ms(0, 1)
+                    host_changes(sim, rng, fraction, original)
+                    t0 = time.perf_counter()
+                    ts.event_record(2)
+                    ts.describe()
+                    ts.event_record(3)
+                    ts.synchronize()
+                    wall += time.perf_counter() - t0
+                    device += ts.event_elapsed_ms(2, 3)
+                ts.solve_device_only(DT)
+                ts.download_body_motion()
+                t = ts.timings()
+                if frame >= args.warmup:
+                    s = samples[route]
+                    s["device_ms"].append(device)
+                    s["wall_ms"].append(wall * 1e3)
+                    s["frame_wall_ms"].append((time.perf_counter() - start) * 1e3)
+                    s["h2d_bytes"].append(t.h2d_bytes)
+        for route, (sim, ts, _, _) in twins.items():
+            s = samples[route]
+            line = dict(info, route=route, fraction=fraction, bodies=sim.body_count, constraints=int(sum(tb.constraint_count for tb in sim.type_batches())),
+                        frames=args.frames, **{"median_" + k: float(np.median(v)) for k, v in s.items()})
+            print(json.dumps(line), flush=True)
+            lines.append(line)
+            ts.close()
+    if args.out:
+        os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
+        with open(args.out, "w") as f:
+            f.write("\n".join(json.dumps(x) for x in lines) + "\n")
+
+
+if __name__ == "__main__":
+    main()
