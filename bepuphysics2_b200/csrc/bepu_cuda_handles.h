@@ -26,6 +26,24 @@ template <bool kPinnedHost> struct GrowBuffer {
         else ptr = nullptr;
         return e;
     }
+    // Device memory only: room for `bytes` with the first `keep` bytes kept (a stream-ordered device copy into a block of at least twice the
+    // capacity, so that repeated growth copies each byte a bounded number of times). On failure the buffer is as it was.
+    cudaError_t grow(size_t bytes, size_t keep, cudaStream_t s) {
+        static_assert(!kPinnedHost, "grow keeps device memory");
+        if (bytes <= capacity) return cudaSuccess;
+        const size_t want = std::max(bytes, 2 * capacity);
+        void* n = nullptr;
+        cudaError_t e = cudaMalloc(&n, want);
+        if (e == cudaSuccess && keep > 0) e = cudaMemcpyAsync(n, ptr, std::min(keep, capacity), cudaMemcpyDeviceToDevice, s);
+        if (e != cudaSuccess) {
+            if (n) cudaFree(n);
+            return e;
+        }
+        release();  // cudaFree waits for the copy
+        ptr = n;
+        capacity = want;
+        return cudaSuccess;
+    }
     void release() {
         if (ptr) kPinnedHost ? cudaFreeHost(ptr) : cudaFree(ptr);
         ptr = nullptr;

@@ -238,6 +238,56 @@ __global__ void scatter_lanes_kernel(const SourceRows* __restrict__ sources, con
     if (c.src_source != kLaneClear && features && r.features && lane < r.contacts) r.features[(size_t)c.dst_index * r.contacts + lane] = features[(size_t)warp * 4 + lane];
 }
 
+// ---- bepucuda_remove_bodies ----
+__global__ void mark_removed_bodies_kernel(const int32_t* __restrict__ moved_to, int count, int final_count, uint8_t* removed) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= count) return;
+    const int32_t to = moved_to[i];
+    removed[to >= 0 ? to : final_count + i] = 1;
+}
+// One warp per work item, as the ownership passes walk the rows.
+__global__ void check_removed_references_kernel(const DeviceTypeBatch* __restrict__ tbs, const WorkItem* __restrict__ work, int work_count,
+                                                const uint8_t* __restrict__ removed, int body_count, int32_t* flag) {
+    const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+    if (warp >= work_count) return;
+    const WorkItem w = work[warp];
+    const DeviceTypeBatch tb = tbs[w.type_batch];
+    for (int s = 0; s < tb.bodies; ++s) {
+        const int32_t enc = tb.refs[((size_t)w.bundle * tb.bodies + s) * 32 + lane];
+        if (enc < 0) continue;
+        const int idx = enc & kRefIndexMask;
+        if (idx < body_count && removed[idx]) *flag = 1;
+    }
+}
+// One thread per float4: 8 of the raw image, 2 each of pose, velocity, local and world inertia, accelerations and shape.
+__global__ void move_bodies_kernel(BodyRecords r, const int32_t* __restrict__ moved_to, int count, int final_count) {
+    const size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= (size_t)count * 20) return;
+    const int i = (int)(t / 20), part = (int)(t % 20);
+    const int32_t to = moved_to[i];
+    if (to < 0) return;
+    const size_t from = (size_t)final_count + i, dst = (size_t)to;
+    if (part < 8) {
+        r.raw[dst * 8 + part] = r.raw[from * 8 + part];
+        return;
+    }
+    const int k = (part - 8) >> 1, half = part & 1;
+    float4* a = k == 0 ? r.B.pose : k == 1 ? r.B.velocity : k == 2 ? r.B.inertia_local : k == 3 ? r.B.inertia_world : k == 4 ? r.accelerations : r.shapes;
+    if (a) a[dst * 2 + half] = a[from * 2 + half];
+}
+// One block row per span.
+__global__ void remap_body_references_kernel(const RefSpan* __restrict__ spans, const int32_t* __restrict__ moved_to, int count, int final_count) {
+    const RefSpan span = spans[blockIdx.y];
+    for (int64_t w = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; w < span.words; w += (int64_t)gridDim.x * blockDim.x) {
+        const int32_t enc = span.refs[w];
+        if (enc < 0) continue;
+        const int idx = enc & kRefIndexMask;
+        if (idx < final_count || idx >= final_count + count) continue;
+        const int32_t to = moved_to[idx - final_count];
+        if (to >= 0) span.refs[w] = (int32_t)(((uint32_t)enc & kRefKinematicBit) | (uint32_t)to);
+    }
+}
+
 // Pass 1 over every (constraint, body slot): first_batch[body] = min device batch referencing it as a dynamic body;
 // per-body reference count and bitmask of synchronized batches for the batch-invariant check.
 __global__ void ownership_pass1_kernel(const DeviceTypeBatch* __restrict__ tbs, const WorkItem* __restrict__ work, int work_count, int sync_batch_count, int body_count,
@@ -474,6 +524,24 @@ void launch_pack_ref_rows(const WorkRecord* records, int count, int32_t* rows, c
 void launch_boundary_flags(const DeviceTypeBatch* tbs, const WorkItem* work, int work_count, long long peer_delta, uint8_t* flags, cudaStream_t s) {
     if (work_count <= 0) return;
     boundary_flags_kernel<<<blocks_for((size_t)work_count * 32, 128), 128, 0, s>>>(tbs, work, work_count, peer_delta, flags);
+}
+void launch_mark_removed_bodies(const int32_t* moved_to, int count, int final_count, uint8_t* removed, cudaStream_t s) {
+    if (count <= 0) return;
+    mark_removed_bodies_kernel<<<blocks_for(count, 256), 256, 0, s>>>(moved_to, count, final_count, removed);
+}
+void launch_check_removed_references(const DeviceTypeBatch* tbs, const WorkItem* work, int work_count, const uint8_t* removed, int body_count, int32_t* flag,
+                                     cudaStream_t s) {
+    if (work_count <= 0) return;
+    check_removed_references_kernel<<<blocks_for((size_t)work_count * 32, 128), 128, 0, s>>>(tbs, work, work_count, removed, body_count, flag);
+}
+void launch_move_bodies(const BodyRecords& r, const int32_t* moved_to, int count, int final_count, cudaStream_t s) {
+    if (count <= 0) return;
+    move_bodies_kernel<<<blocks_for((size_t)count * 20, 256), 256, 0, s>>>(r, moved_to, count, final_count);
+}
+void launch_remap_body_references(const RefSpan* spans, int span_count, int64_t max_words, const int32_t* moved_to, int count, int final_count, cudaStream_t s) {
+    if (span_count <= 0 || max_words <= 0 || count <= 0) return;
+    const dim3 grid(std::min(blocks_for((size_t)max_words, 256), 1024u), (unsigned)span_count);
+    remap_body_references_kernel<<<grid, 256, 0, s>>>(spans, moved_to, count, final_count);
 }
 void launch_fill_i32(int32_t* p, size_t n, int32_t v, cudaStream_t s) {
     if (n == 0) return;

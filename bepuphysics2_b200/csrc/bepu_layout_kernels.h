@@ -76,6 +76,31 @@ void launch_gather_lanes(const SourceRows* sources, const LaneCopy* copies, int 
 // The copies of one launch write distinct lanes and read only the staging, so they run in parallel.
 void launch_scatter_lanes(const SourceRows* sources, const LaneCopy* copies, int count, int W, const int32_t* records, const int32_t* features, cudaStream_t s);
 void launch_fill_i32(int32_t* p, size_t n, int32_t v, cudaStream_t s);
+// bepucuda_remove_bodies. moved_to[i] (replay_body_removes, bepu_topology.h): the new index of the body at final_count + i, or -1 when it was removed.
+// removed[b] = 1 for every body index b < final_count + count that the list removes (the array is zeroed by the caller): the slot a moved body
+// takes, or final_count + i where moved_to[i] is -1.
+void launch_mark_removed_bodies(const int32_t* moved_to, int count, int final_count, uint8_t* removed, cudaStream_t s);
+// *flag = 1 when a constraint of the AOSOA-32 rows references a body marked in `removed` (body_count entries).
+void launch_check_removed_references(const DeviceTypeBatch* tbs, const WorkItem* work, int work_count, const uint8_t* removed, int body_count, int32_t* flag,
+                                     cudaStream_t s);
+// Per-body records that move with the bodies: `raw` (the 128-B BodyDynamics image), the four 32-B records of B, and the 32-B acceleration and shape
+// records when those are not null.
+struct BodyRecords {
+    float4* raw;
+    BodyBuffers B;
+    float4* accelerations;
+    float4* shapes;
+};
+// BodySet.RemoveAt's copies as one step: the body at final_count + i takes slot moved_to[i] (when >= 0) in every array of `r`.
+void launch_move_bodies(const BodyRecords& r, const int32_t* moved_to, int count, int final_count, cudaStream_t s);
+// The body references of one source type batch's raw (AOSOA-W) rows: `words` int32.
+struct RefSpan {
+    int32_t* refs;
+    int64_t words;
+};
+// TypeProcessor.UpdateForBodyMemoryMove (TypeProcessor.cs:L807-817) for every move of one step: a reference to index final_count + i with
+// moved_to[i] >= 0 becomes moved_to[i], its kinematic bit kept; -1 and every other reference stay.
+void launch_remap_body_references(const RefSpan* spans, int span_count, int64_t max_words, const int32_t* moved_to, int count, int final_count, cudaStream_t s);
 // RedistributeImpulses (NarrowPhaseConstraintUpdate.cs:L81-135) for every device type batch whose descriptor has kDescRedistribute, on the AOSOA-32 impulses.
 void launch_redistribute_impulses(const DeviceTypeBatch* tbs, const TransposeDesc* descs, const WorkItem* work, int work_count, cudaStream_t s);
 // Motion half (floats 0-15) of 128-B BodyDynamics records <-> pose / velocity records. `raw` may be mapped host memory.

@@ -425,6 +425,35 @@ std::vector<LaneCopy> compose_lane_ops(const std::vector<LaneCopy>& ops) {
     return out;
 }
 
+int replay_body_removes(int32_t body_count, int32_t count, const int32_t* body_indices, int32_t* final_count, std::vector<int32_t>* moved_to, std::string* error) {
+    if (count < 0 || body_count < 0 || (count > 0 && !body_indices)) {
+        *error = "bad arguments";
+        return BEPUCUDA_ERR_INVALID_ARGUMENT;
+    }
+    // slot -> the original index of the body it holds, for the slots whose body moved (every other slot holds its own)
+    std::unordered_map<int32_t, int32_t> at;
+    at.reserve((size_t)count * 2);
+    auto body_at = [&](int32_t slot) {
+        const auto it = at.find(slot);
+        return it == at.end() ? slot : it->second;
+    };
+    int32_t n = body_count;
+    for (int32_t i = 0; i < count; ++i) {
+        const int32_t index = body_indices[i];
+        if (index < 0 || index >= n) {
+            *error = "entry " + std::to_string(i) + ": body index " + std::to_string(index) + " outside the " + std::to_string(n) + " bodies at that entry";
+            return BEPUCUDA_ERR_INVALID_ARGUMENT;
+        }
+        --n;
+        if (index < n) at[index] = body_at(n);
+        at.erase(n);
+    }
+    *final_count = n;
+    moved_to->assign((size_t)count, -1);
+    for (const auto& [slot, original] : at) (*moved_to)[(size_t)(original - n)] = slot;
+    return BEPUCUDA_OK;
+}
+
 std::vector<WorkRecord> work_records(const TopologyPlan& plan, int32_t* refs, float* prestep, float* impulses) {
     std::vector<WorkRecord> records(plan.work.size());
     for (size_t i = 0; i < plan.work.size(); ++i) {

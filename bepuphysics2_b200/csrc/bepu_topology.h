@@ -132,6 +132,14 @@ int replay_changes(ChangeState* state, bool remove, int W, int fallback_threshol
 // whose rows it ends with (or kLaneClear / kLaneNew). A lane cleared and later copied elsewhere carries only its cleared body references there.
 std::vector<LaneCopy> compose_lane_ops(const std::vector<LaneCopy>& ops);
 
+// bepucuda_remove_bodies on the host: `count` BodySet.RemoveAt (BodySet.cs:L83-111) in list order on `body_count` bodies, each on the state the
+// entries before it left (the count drops by one and, when the index is below the new count, the last body moves into its slot), composed into
+// one parallel step. *final_count = body_count - count; moved_to[i] (count entries): the new index of the body that was at final_count + i, or -1
+// when it was removed. Every moved body comes from [final_count, body_count) and goes to a distinct slot below final_count, and that slot's body
+// was removed, so the moves of one step neither read nor write each other's records. BEPUCUDA_ERR_INVALID_ARGUMENT with *error set for count < 0,
+// a NULL list with count > 0, or the first index outside [0, count at that entry); nothing else is written then.
+int replay_body_removes(int32_t body_count, int32_t count, const int32_t* body_indices, int32_t* final_count, std::vector<int32_t>* moved_to, std::string* error);
+
 // What the solver kernels read per work item, with the plan's offsets applied to the arena bases.
 std::vector<WorkRecord> work_records(const TopologyPlan& plan, int32_t* refs, float* prestep, float* impulses);
 

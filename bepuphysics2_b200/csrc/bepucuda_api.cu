@@ -137,6 +137,7 @@ struct bepucuda_ctx {
     std::vector<Event> profile_events;
     DeviceBuffer change_sources, change_copies, change_records, change_features;  // bepucuda_add_constraints / bepucuda_remove_constraints
     std::vector<std::pair<void*, size_t>> spare_rows;  // raw-arena blocks of grown and removed sources, taken again by later growth (until a describe)
+    DeviceBuffer moved_to, removed_marks, ref_spans;  // bepucuda_remove_bodies
 };
 
 namespace {
@@ -1314,6 +1315,141 @@ int32_t bepucuda_remove_constraints(bepucuda_ctx* ctx, int32_t count, const bepu
                                     int32_t kinematic_count) {
     if (!ctx) return BEPUCUDA_ERR_INVALID_ARGUMENT;
     return change_constraints(ctx, "remove_constraints", true, count, locations, nullptr, nullptr, constrained_kinematics, kinematic_count);
+}
+
+// ---- body adds and removes on the resident state ----
+static void refresh_body_buffers(bepucuda_ctx* ctx) {
+    ctx->B = {ctx->pose.as<float4>(), ctx->velocity.as<float4>(), ctx->inertia_local.as<float4>(), ctx->inertia_world.as<float4>(), ctx->constrained.as<uint8_t>(),
+              ctx->first_batch.as<int32_t>(), ctx->body_count};
+}
+
+// The state rules bepucuda_add_bodies / bepucuda_remove_bodies share with the constraint change calls.
+static int check_body_change(bepucuda_ctx* ctx, const std::string& name) {
+    if (ctx->peer_mode) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, name + " in peer mode");
+    if (ctx->constraints_open) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, name + " between begin_constraints and end_constraints");
+    if (!ctx->constraints_ready) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, name + " before end_constraints");
+    if (ctx->data_dirty) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, name + ": rows are pending (uploads or writes since the last solve); change the bodies before them");
+    return BEPUCUDA_OK;
+}
+
+// Room for `n` bodies in every per-body array, the records of the first `keep` bodies kept. The per-body accelerations and shapes grow when they
+// are set for `keep` bodies. B is refreshed whether or not this succeeds: a failed growth leaves the arrays it grew, records and all.
+static cudaError_t grow_body_arrays(bepucuda_ctx* ctx, size_t n, size_t keep) {
+    cudaStream_t s = ctx->stream;
+    cudaError_t e = ctx->raw_bodies.grow(n * 128, keep * 128, s);
+    for (DeviceBuffer* b : {&ctx->pose, &ctx->velocity, &ctx->inertia_local, &ctx->inertia_world})
+        if (e == cudaSuccess) e = b->grow(n * 32, keep * 32, s);
+    if (e == cudaSuccess) e = ctx->constrained.grow(n + 1, keep, s);
+    if (e == cudaSuccess) e = ctx->first_batch.grow(n * 4, keep * 4, s);
+    if (e == cudaSuccess && ctx->accelerations_count == (int)keep) e = ctx->accelerations.grow(n * 32, keep * 32, s);
+    if (e == cudaSuccess && ctx->shape_count == (int)keep) e = ctx->body_shapes.grow(n * sizeof(BodyShape), keep * sizeof(BodyShape), s);
+    refresh_body_buffers(ctx);
+    return e;
+}
+
+int32_t bepucuda_add_bodies(bepucuda_ctx* ctx, const void* body_dynamics, int32_t count, const bepucuda_body_shape* shapes, const float* accelerations) {
+    if (!ctx) return BEPUCUDA_ERR_INVALID_ARGUMENT;
+    TRY(check_body_change(ctx, "add_bodies"));
+    if (count < 0 || (count > 0 && !body_dynamics)) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "add_bodies: bad arguments");
+    if ((int64_t)ctx->body_count + count > (int64_t)kRefIndexMask) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "add_bodies: too many bodies");
+    if (count == 0) return BEPUCUDA_OK;
+    CK(cudaSetDevice(ctx->device));
+    const int first = ctx->body_count;
+    const size_t n = (size_t)first + count, added = (size_t)count;
+    if (const cudaError_t e = grow_body_arrays(ctx, n, (size_t)first)) return cuda_fail(ctx, e, "add_bodies: body arrays");
+    ctx->upload_window.start_once(ctx->stream);
+    int64_t bytes = (int64_t)added * 128;
+    CK(cudaMemcpyAsync(ctx->raw_bodies.as<char>() + (size_t)first * 128, body_dynamics, added * 128, cudaMemcpyHostToDevice, ctx->stream));
+    // the appended range through the describe's split, and "unconstrained" until a plan says otherwise
+    BodyBuffers appended = ctx->B;
+    for (float4** p : {&appended.pose, &appended.velocity, &appended.inertia_local, &appended.inertia_world}) *p += (size_t)first * 2;
+    launch_split_bodies(ctx->raw_bodies.as<char>() + (size_t)first * 128, count, appended, ctx->stream);
+    launch_fill_i32(ctx->first_batch.as<int32_t>() + first, added, 0x7fffffff, ctx->stream);
+    CK(cudaMemsetAsync(ctx->constrained.as<uint8_t>() + first, 0, added, ctx->stream));
+    CK(cudaGetLastError());
+    if (ctx->accelerations_count == first && accelerations) {
+        CK(cudaMemcpyAsync(ctx->accelerations.as<char>() + (size_t)first * 32, accelerations, added * 32, cudaMemcpyHostToDevice, ctx->stream));
+        ctx->accelerations_count = (int)n;
+        bytes += (int64_t)added * 32;
+    }
+    if (ctx->shape_count == first && shapes) {
+        CK(cudaMemcpyAsync(ctx->body_shapes.as<char>() + (size_t)first * sizeof(BodyShape), shapes, added * sizeof(BodyShape), cudaMemcpyHostToDevice, ctx->stream));
+        ctx->shape_count = (int)n;
+        bytes += (int64_t)(added * sizeof(BodyShape));
+    }
+    ctx->h2d_accum += bytes;
+    ctx->body_count = (int)n;
+    refresh_body_buffers(ctx);
+    return upload_program(ctx);  // the final pose pass covers the new bodies
+}
+
+int32_t bepucuda_remove_bodies(bepucuda_ctx* ctx, int32_t count, const int32_t* body_indices) {
+    if (!ctx) return BEPUCUDA_ERR_INVALID_ARGUMENT;
+    TRY(check_body_change(ctx, "remove_bodies"));
+    const int old = ctx->body_count;
+    int32_t final_count = old;
+    std::vector<int32_t> moved_to;
+    std::string error;
+    if (replay_body_removes(old, count, body_indices, &final_count, &moved_to, &error) != BEPUCUDA_OK)
+        return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "remove_bodies: " + error);
+    if (count == 0) return BEPUCUDA_OK;
+    CK(cudaSetDevice(ctx->device));
+    CK(ctx->moved_to.reserve((size_t)count * 4));
+    CK(ctx->removed_marks.reserve((size_t)old));
+    ctx->upload_window.start_once(ctx->stream);
+    CK(cudaMemcpyAsync(ctx->moved_to.ptr, moved_to.data(), (size_t)count * 4, cudaMemcpyHostToDevice, ctx->stream));
+    ctx->h2d_accum += (int64_t)count * 4;
+    // Bodies.RemoveAt forbids orphans: no live constraint may reference a removed body. Checked before anything moves.
+    int32_t* flag = ctx->error_dev.as<int32_t>();
+    CK(cudaMemsetAsync(ctx->removed_marks.ptr, 0, (size_t)old, ctx->stream));
+    CK(cudaMemsetAsync(flag, 0, 4, ctx->stream));
+    launch_mark_removed_bodies(ctx->moved_to.as<int32_t>(), count, final_count, ctx->removed_marks.as<uint8_t>(), ctx->stream);
+    launch_check_removed_references(ctx->tb_table.as<DeviceTypeBatch>(), ctx->work_table.as<WorkItem>(), ctx->topo.all_work_count, ctx->removed_marks.as<uint8_t>(), old, flag,
+                                    ctx->stream);
+    CK(cudaGetLastError());
+    int32_t referenced = 0;
+    CK(cudaMemcpyAsync(&referenced, flag, 4, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    if (referenced) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "remove_bodies: a live constraint references a removed body; remove its constraints first");
+
+    std::vector<RefSpan> spans;
+    int64_t max_words = 0;
+    for (const SourceTypeBatch& s : ctx->sources) {
+        spans.push_back({s.raw_refs, (int64_t)(s.refs_bytes / 4)});
+        max_words = std::max(max_words, spans.back().words);
+    }
+    TRY(upload_table(ctx, "ref_spans", ctx->ref_spans, spans, 0));
+    // the device's rows of every constraint back into the sources, where the remap and the plan below read them
+    launch_transpose_out_all(ctx->tb_table.as<DeviceTypeBatch>(), ctx->tdesc_table.as<TransposeDesc>(), ctx->work_table.as<WorkItem>(), ctx->topo.all_work_count, ctx->W,
+                             kTransposePrestep | kTransposeImpulses, ctx->stream);
+    ctx->constraints_ready = false;  // from here on a failure leaves a context that needs a describe
+    const BodyRecords records{ctx->raw_bodies.as<float4>(), ctx->B, ctx->accelerations_count == old ? ctx->accelerations.as<float4>() : nullptr,
+                              ctx->shape_count == old ? ctx->body_shapes.as<float4>() : nullptr};
+    launch_move_bodies(records, ctx->moved_to.as<int32_t>(), count, final_count, ctx->stream);
+    launch_remap_body_references(ctx->ref_spans.as<RefSpan>(), (int)spans.size(), max_words, ctx->moved_to.as<int32_t>(), count, final_count, ctx->stream);
+    CK(cudaGetLastError());
+    // the same moves on the host's copies: fallback references (levelisation) and constrained kinematics (a removed one leaves the list)
+    auto new_index = [&](int32_t idx) { return idx < final_count || idx >= old ? idx : moved_to[(size_t)(idx - final_count)]; };
+    for (SourceTypeBatch& s : ctx->sources)
+        for (int32_t& r : s.host_refs)
+            if (r >= 0) {
+                const int32_t to = new_index((int32_t)((uint32_t)r & kRefIndexMask));
+                if (to >= 0) r = (int32_t)(((uint32_t)r & kRefKinematicBit) | (uint32_t)to);
+            }
+    std::vector<uint8_t> taken((size_t)final_count, 0);  // slots whose body was removed (a moved body took them)
+    for (const int32_t to : moved_to)
+        if (to >= 0) taken[(size_t)to] = 1;
+    std::vector<int32_t> kinematics;
+    for (const int32_t k : ctx->kinematics) {
+        const int32_t to = k < final_count ? (taken[(size_t)k] ? -1 : k) : new_index(k);
+        if (to >= 0) kinematics.push_back(to);
+    }
+    ctx->kinematics = std::move(kinematics);
+    if (ctx->accelerations_count == old) ctx->accelerations_count = final_count;
+    if (ctx->shape_count == old) ctx->shape_count = final_count;
+    ctx->body_count = final_count;
+    refresh_body_buffers(ctx);
+    return plan_device_rows(ctx);
 }
 
 int32_t bepucuda_get_timings(bepucuda_ctx* ctx, bepucuda_timings* out) {

@@ -3,7 +3,8 @@
 // owns (Bodies.ActiveSet.DynamicsState as 128-B AOS, Solver.ActiveSet.Batches[b].TypeBatches[t] as AOSOA-W) and feeds them
 // to libbepucuda through exactly the C ABI a C# CudaTimestepper would P/Invoke (include/bepucuda.h, INTEGRATION.md).
 //
-// Mirrored (names kept): Bodies.Add (Bodies.cs), Solver.Add -> TryAllocateInBatch -> AllocateInTypeBatch[ForFallback]
+// Mirrored (names kept): Bodies.Add and Bodies.RemoveAt with the handle pool and HandleToLocation (Bodies.cs:L183-260, BodySet.cs:L68-111),
+// Solver.UpdateForBodyMemoryMove (Solver.cs:L1444-1482), Solver.Add -> TryAllocateInBatch -> AllocateInTypeBatch[ForFallback]
 // (Solver.cs:L1093-1199, Constraints/TypeProcessor.cs:L314-334,L451-540), ConstrainedKinematicHandles (Solver.cs:L68),
 // SolveDescription (SolveDescription.cs:L16-137), ITimestepper.Timestep's Solve slot (DefaultTimestepper.cs:L28-43), Solver.Remove ->
 // RemoveFromBatch -> TypeProcessor.Remove, RemoveTypeBatchIfEmpty, RemoveBatchIfEmpty (Solver.cs:L1294-1405, TypeProcessor.cs:L634-720,
@@ -77,13 +78,19 @@ struct IndexSet {  // BepuUtilities/Collections/IndexSet.cs
 
 struct ConstraintLocation { int batch, type_id, index_in_type_batch; };  // batch -1: a removed handle
 
-// One Solver.Add / Solver.Remove since the last describe or bepuhost_cuda_change, for bepuhost_cuda_change: the location the call produced or
-// consumed, and for an add its handle and encoded body references.
+// One Solver.Add / Solver.Remove / Bodies.Add / Bodies.RemoveAt since the last describe or bepuhost_cuda_change, for bepuhost_cuda_change. A
+// constraint entry: the location the call produced or consumed, and for an add its handle and encoded body references. A body add: its handle, and
+// once that body is removed again its record as it was then. A body remove: the active-set index it removed. The last entry of a constraint run
+// that another kind of entry follows keeps the constrained kinematics (active-set indices) as they were right after the run (`kinematics`).
+enum ChangeKind { kConstraintAdd, kConstraintRemove, kBodyAdd, kBodyRemove };
 struct ChangeEntry {
-    bool remove;
+    ChangeKind kind;
     ConstraintLocation at;
     int handle;
     int32_t refs[4];
+    std::vector<float> record;
+    std::vector<int32_t> kinematics;
+    bool kinematics_kept = false;
 };
 
 struct Simulation {
@@ -93,13 +100,17 @@ struct Simulation {
     bepucuda_integrator_desc integrator{};
     AlignedBuffer<float> dynamics;             // Bodies.ActiveSet.DynamicsState: 32 floats per body
     int body_count = 0;
+    std::vector<int32_t> index_to_handle;      // Bodies.ActiveSet.IndexToHandle
+    std::vector<int32_t> handle_to_index;      // Bodies.HandleToLocation (active set only; -1: no body)
+    std::vector<int32_t> free_handles;         // Bodies.HandlePool's returned ids, taken last-in first-out (IdPool.Take)
     std::vector<ConstraintBatch*> batches;     // Solver.ActiveSet.Batches
-    std::vector<IndexSet> batch_referenced_handles;
+    std::vector<IndexSet> batch_referenced_handles;  // by body handle
     std::vector<int32_t> constrained_kinematic_handles;
     IndexSet constrained_kinematic_set;
     std::vector<ConstraintLocation> handle_to_constraint;
-    std::vector<int32_t> kinematic_constraint_count;  // per body: constraints referencing it as a kinematic (Bodies' constraint lists, kinematics only)
+    std::vector<int32_t> kinematic_constraint_count;  // per body handle: constraints referencing it as a kinematic (Bodies' constraint lists, kinematics only)
     std::vector<ChangeEntry> changes;
+    std::vector<int32_t> kinematic_indices;   // constrained_kinematic_handles as active-set indices (kinematic_indices())
     std::string error;
     ~Simulation() { for (auto b : batches) delete b; }
 };
@@ -108,6 +119,27 @@ bool is_kinematic(const float* body) {  // Bodies.cs:L339-353: all of local inve
     for (int i = 16; i < 23; ++i)
         if (body[i] != 0.0f) return false;
     return true;
+}
+
+// The constrained kinematics as active-set indices: what the device takes.
+const std::vector<int32_t>& kinematic_indices(Simulation& sim) {
+    sim.kinematic_indices.clear();
+    for (const int32_t h : sim.constrained_kinematic_handles) sim.kinematic_indices.push_back(sim.handle_to_index[(size_t)h]);
+    return sim.kinematic_indices;
+}
+
+// Appends an entry of `kind` to the change log; a constraint run that this entry ends keeps the constrained kinematics it left.
+ChangeEntry& log_change(Simulation& sim, ChangeKind kind) {
+    if (!sim.changes.empty()) {
+        ChangeEntry& last = sim.changes.back();
+        if (last.kind != kind && (last.kind == kConstraintAdd || last.kind == kConstraintRemove)) {
+            last.kinematics = kinematic_indices(sim);
+            last.kinematics_kept = true;
+        }
+    }
+    sim.changes.push_back({});
+    sim.changes.back().kind = kind;
+    return sim.changes.back();
 }
 
 TypeBatch* get_or_create_type_batch(Simulation& sim, ConstraintBatch& batch, int type_id) {
@@ -217,17 +249,18 @@ int allocate_in_type_batch_for_fallback(Simulation& sim, TypeBatch& t, int handl
     return index;
 }
 
-// GetBlockingBodyHandles (Solver.cs:L1058-1078): encodes the body references (kinematic flag in bit 30) and lists the dynamic handles, the only
-// ones that take part in batch membership.
+// GetBlockingBodyHandles (Solver.cs:L1058-1078): encodes the body references (active-set index, kinematic flag in bit 30) and lists the dynamic
+// handles, the only ones that take part in batch membership.
 int encode_references(Simulation& sim, int type_id, const int32_t* body_handles, int32_t* encoded, int32_t* blocking, int* blocking_count, int* body_count_out) {
     int32_t nb = 0;
     if (bepucuda_type_info(type_id, &nb, nullptr, nullptr) != BEPUCUDA_OK) { sim.error = "unsupported constraint type"; return -1; }
     *blocking_count = 0;
     for (int i = 0; i < nb; ++i) {
         const int h = body_handles[i];
-        if (h < 0 || h >= sim.body_count) { sim.error = "body handle out of range"; return -1; }
-        if (is_kinematic(sim.dynamics.data + (size_t)h * 32)) encoded[i] = h | (int32_t)kKinematicMask;
-        else { encoded[i] = h; blocking[(*blocking_count)++] = h; }
+        if (h < 0 || h >= (int)sim.handle_to_index.size() || sim.handle_to_index[(size_t)h] < 0) { sim.error = "body handle out of range"; return -1; }
+        const int index = sim.handle_to_index[(size_t)h];
+        if (is_kinematic(sim.dynamics.data + (size_t)index * 32)) encoded[i] = index | (int32_t)kKinematicMask;
+        else { encoded[i] = index; blocking[(*blocking_count)++] = h; }
     }
     *body_count_out = nb;
     return 0;
@@ -238,7 +271,7 @@ int allocate_in_batch(Simulation& sim, int target, int type_id, int nb, const in
     const int handle = (int)sim.handle_to_constraint.size();
     for (int i = 0; i < nb; ++i)
         if ((uint32_t)encoded[i] & kKinematicMask) {
-            const int h = encoded[i] & ~(int32_t)kKinematicMask;
+            const int h = sim.index_to_handle[(size_t)(encoded[i] & ~(int32_t)kKinematicMask)];
             if (!sim.constrained_kinematic_set.contains(h)) { sim.constrained_kinematic_set.set(h); sim.constrained_kinematic_handles.push_back(h); }
             if ((int)sim.kinematic_constraint_count.size() <= h) sim.kinematic_constraint_count.resize((size_t)h + 1, 0);
             ++sim.kinematic_constraint_count[(size_t)h];
@@ -249,9 +282,10 @@ int allocate_in_batch(Simulation& sim, int target, int type_id, int nb, const in
     write_lane(sim, *tb, index, encoded, prestep);
     for (int i = 0; i < blocking_count; ++i) sim.batch_referenced_handles[target].set(blocking[i]);
     sim.handle_to_constraint.push_back({target, type_id, index});
-    ChangeEntry e{false, {target, type_id, index}, handle, {-1, -1, -1, -1}};
-    for (int i = 0; i < nb; ++i) e.refs[i] = encoded[i];
-    sim.changes.push_back(e);
+    ChangeEntry& e = log_change(sim, kConstraintAdd);
+    e.at = {target, type_id, index};
+    e.handle = handle;
+    for (int i = 0; i < 4; ++i) e.refs[i] = i < nb ? encoded[i] : -1;
     return handle;
 }
 
@@ -276,7 +310,9 @@ void clear_lane_references(Simulation& sim, TypeBatch& t, int index) {  // Remov
 int solver_remove(Simulation& sim, int handle) {
     if (handle < 0 || handle >= (int)sim.handle_to_constraint.size() || sim.handle_to_constraint[(size_t)handle].batch < 0) { sim.error = "no such constraint handle"; return -1; }
     const ConstraintLocation at = sim.handle_to_constraint[(size_t)handle];
-    sim.changes.push_back({true, at, handle, {-1, -1, -1, -1}});
+    ChangeEntry& logged = log_change(sim, kConstraintRemove);
+    logged.at = at;
+    logged.handle = handle;
     ConstraintBatch& batch = *sim.batches[(size_t)at.batch];
     const int tb_index = batch.type_index_to_type_batch_index[at.type_id];
     TypeBatch& t = *batch.type_batches[(size_t)tb_index];
@@ -284,7 +320,7 @@ int solver_remove(Simulation& sim, int handle) {
     const int32_t* refs = t.body_references.data + (size_t)(index / W) * t.bodies * W + index % W;
     for (int b = 0; b < t.bodies; ++b) {
         const int32_t enc = refs[(size_t)b * W];
-        const int body = enc & ~(int32_t)kKinematicMask;
+        const int body = sim.index_to_handle[(size_t)(enc & ~(int32_t)kKinematicMask)];
         if ((uint32_t)enc & kKinematicMask) {
             // RemoveConstraintReferencesFromBodiesEnumerator: the last constraint of a kinematic takes it out of ConstrainedKinematicHandles (FastRemove)
             if (--sim.kinematic_constraint_count[(size_t)body] == 0) {
@@ -386,6 +422,72 @@ int solver_add_in_batch(Simulation& sim, int target, int type_id, const int32_t*
     return allocate_in_batch(sim, target, type_id, nb, encoded, blocking, blocking_count, prestep);
 }
 
+// Per active-set index: the handles of the live constraints that reference it.
+std::vector<std::vector<int>> constraints_by_body(const Simulation& sim) {
+    std::vector<std::vector<int>> out((size_t)sim.body_count);
+    for (size_t h = 0; h < sim.handle_to_constraint.size(); ++h) {
+        const ConstraintLocation& loc = sim.handle_to_constraint[h];
+        if (loc.batch < 0) continue;
+        const ConstraintBatch& batch = *sim.batches[(size_t)loc.batch];
+        const TypeBatch& t = *batch.type_batches[(size_t)batch.type_index_to_type_batch_index[loc.type_id]];
+        const int32_t* refs = t.body_references.data + (size_t)(loc.index_in_type_batch / sim.W) * t.bodies * sim.W + loc.index_in_type_batch % sim.W;
+        for (int b = 0; b < t.bodies; ++b) {
+            auto& list = out[(size_t)(refs[(size_t)b * sim.W] & ~(int32_t)kKinematicMask)];
+            if (list.empty() || list.back() != (int)h) list.push_back((int)h);
+        }
+    }
+    return out;
+}
+
+// Bodies.Remove (Bodies.cs:L244-260) of every listed body, in list order: first Solver.Remove of every constraint that references each body, the
+// last added first (the reference walks the body's constraint list from its end), then RemoveFromActiveSet (L214-239) of each body: BodySet.RemoveAt
+// moves the last body into the slot (BodySet.cs:L83-111) and Solver.UpdateForBodyMemoryMove points the moved body's constraint references at it,
+// the kinematic bit kept (TypeProcessor.UpdateForBodyMemoryMove, TypeProcessor.cs:L807-817); the handle goes back to the pool. This leaves the state
+// the reference's one Bodies.Remove per body leaves: a constraint remove moves lanes and a body move rewrites reference values, so the two commute.
+// Grouped, the change log holds one run of constraint removes and one of body removes.
+void bodies_remove(Simulation& sim, const std::vector<int32_t>& handles) {
+    const int W = sim.W;
+    std::vector<std::vector<int>> by_body = constraints_by_body(sim);
+    for (const int32_t handle : handles) {
+        const auto& attached = by_body[(size_t)sim.handle_to_index[(size_t)handle]];
+        for (auto it = attached.rbegin(); it != attached.rend(); ++it)
+            if (sim.handle_to_constraint[(size_t)*it].batch >= 0) solver_remove(sim, *it);
+    }
+    for (const int32_t handle : handles) {
+        const int index = sim.handle_to_index[(size_t)handle], last = sim.body_count - 1;
+        ChangeEntry& logged = log_change(sim, kBodyRemove);
+        logged.at = {-1, -1, index};
+        logged.handle = handle;
+        // a body added since the last forward and removed again: its add entry sends the record it had
+        for (auto it = sim.changes.rbegin(); it != sim.changes.rend(); ++it)
+            if (it->kind == kBodyAdd && it->handle == handle && it->record.empty()) {
+                it->record.assign(sim.dynamics.data + (size_t)index * 32, sim.dynamics.data + (size_t)index * 32 + 32);
+                break;
+            }
+        if (index < last) {
+            std::memcpy(sim.dynamics.data + (size_t)index * 32, sim.dynamics.data + (size_t)last * 32, 32 * sizeof(float));
+            const int moved_handle = sim.index_to_handle[(size_t)last];
+            sim.index_to_handle[(size_t)index] = moved_handle;
+            sim.handle_to_index[(size_t)moved_handle] = index;
+            for (const int h : by_body[(size_t)last]) {
+                const ConstraintLocation& loc = sim.handle_to_constraint[(size_t)h];
+                if (loc.batch < 0) continue;
+                ConstraintBatch& batch = *sim.batches[(size_t)loc.batch];
+                TypeBatch& t = *batch.type_batches[(size_t)batch.type_index_to_type_batch_index[loc.type_id]];
+                int32_t* refs = t.body_references.data + (size_t)(loc.index_in_type_batch / W) * t.bodies * W + loc.index_in_type_batch % W;
+                for (int b = 0; b < t.bodies; ++b)
+                    if ((refs[(size_t)b * W] & ~(int32_t)kKinematicMask) == last) refs[(size_t)b * W] = index | (refs[(size_t)b * W] & (int32_t)kKinematicMask);
+            }
+            by_body[(size_t)index] = std::move(by_body[(size_t)last]);
+        }
+        by_body.pop_back();
+        sim.index_to_handle.pop_back();
+        sim.handle_to_index[(size_t)handle] = -1;
+        sim.free_handles.push_back(handle);
+        --sim.body_count;
+    }
+}
+
 }  // namespace
 
 extern "C" {
@@ -425,17 +527,51 @@ int32_t bepuhost_set_integrator(void* simp, const bepucuda_integrator_desc* d) {
     return 0;
 }
 
-// Bodies.Add: appends `count` BodyDynamics records (32 floats each); returns the handle (== active-set index) of the first.
+// Bodies.Add: appends `count` BodyDynamics records (32 floats each) at the end of the active set; returns the handle of the first. Handles come
+// from the handle pool (IdPool.Take: the last returned handle first, else the next new one), so they equal active-set indices until a body is removed.
 int32_t bepuhost_add_bodies(void* simp, const float* dynamics, int32_t count) {
     Simulation& sim = *(Simulation*)simp;
     const int first = sim.body_count;
     sim.dynamics.ensure((size_t)(first + count) * 32, (size_t)first * 32);
     std::memcpy(sim.dynamics.data + (size_t)first * 32, dynamics, (size_t)count * 32 * sizeof(float));
+    int32_t first_handle = -1;
+    for (int i = 0; i < count; ++i) {
+        int handle = (int)sim.handle_to_index.size();
+        if (!sim.free_handles.empty()) {
+            handle = sim.free_handles.back();
+            sim.free_handles.pop_back();
+        } else {
+            sim.handle_to_index.push_back(-1);
+        }
+        sim.handle_to_index[(size_t)handle] = first + i;
+        sim.index_to_handle.push_back(handle);
+        log_change(sim, kBodyAdd).handle = handle;
+        if (i == 0) first_handle = handle;
+    }
     sim.body_count += count;
-    return first;
+    return first_handle;
+}
+// Bodies.Remove for `count` distinct body handles in order (bodies_remove). Returns 0, or -1 with nothing removed when a handle names no body or
+// is listed twice.
+int32_t bepuhost_remove_bodies(void* simp, int32_t count, const int32_t* handles) {
+    Simulation& sim = *(Simulation*)simp;
+    std::vector<int32_t> list(handles, handles + count);
+    IndexSet seen;
+    for (const int32_t h : list) {
+        if (h < 0 || h >= (int32_t)sim.handle_to_index.size() || sim.handle_to_index[(size_t)h] < 0 || seen.contains(h)) { sim.error = "no such body handle, or one listed twice"; return -1; }
+        seen.set(h);
+    }
+    bodies_remove(sim, list);
+    return 0;
 }
 float* bepuhost_body_dynamics(void* simp) { return ((Simulation*)simp)->dynamics.data; }
 int32_t bepuhost_body_count(void* simp) { return ((Simulation*)simp)->body_count; }
+// Bodies.ActiveSet.IndexToHandle (body_count entries) and HandleToLocation's active-set index of a handle (-1: no body).
+const int32_t* bepuhost_body_handles(void* simp) { return ((Simulation*)simp)->index_to_handle.data(); }
+int32_t bepuhost_body_index(void* simp, int32_t handle) {
+    const Simulation& sim = *(Simulation*)simp;
+    return handle >= 0 && handle < (int32_t)sim.handle_to_index.size() ? sim.handle_to_index[(size_t)handle] : -1;
+}
 
 // Solver.Add for `count` constraints of one type in order. body_handles: count x bodies; prestep: count x prestep floats in the type's
 // prestep row order (what IConstraintDescription.ApplyDescription writes). Returns the first constraint handle or -1.
@@ -514,7 +650,8 @@ int32_t bepuhost_get_type_batch(void* simp, int32_t batch, int32_t type_batch, b
     return 0;
 }
 int32_t bepuhost_constrained_kinematic_count(void* simp) { return (int32_t)((Simulation*)simp)->constrained_kinematic_handles.size(); }
-const int32_t* bepuhost_constrained_kinematics(void* simp) { return ((Simulation*)simp)->constrained_kinematic_handles.data(); }
+// Solver.ConstrainedKinematicHandles as active-set indices (valid until the next call).
+const int32_t* bepuhost_constrained_kinematics(void* simp) { return kinematic_indices(*(Simulation*)simp).data(); }
 int32_t bepuhost_bundle_width(void* simp) { return ((Simulation*)simp)->W; }
 int32_t bepuhost_fallback_batch_threshold(void* simp) { return ((Simulation*)simp)->fallback_batch_threshold; }
 int32_t bepuhost_substep_count(void* simp) { return (int32_t)((Simulation*)simp)->velocity_iterations.size(); }
@@ -539,31 +676,46 @@ int32_t bepuhost_cuda_describe(void* simp, bepucuda_ctx* ctx) {
             if ((rc = bepucuda_upload_type_batch(ctx, b, t, tb.type_id, tb.constraint_count, tb.body_references.data, tb.prestep.data, tb.impulses.data)) != 0) return rc;
         }
     }
-    if ((rc = bepucuda_set_constrained_kinematics(ctx, sim.constrained_kinematic_handles.data(), (int32_t)sim.constrained_kinematic_handles.size())) != 0) return rc;
+    const std::vector<int32_t>& kinematics = kinematic_indices(sim);
+    if ((rc = bepucuda_set_constrained_kinematics(ctx, kinematics.data(), (int32_t)kinematics.size())) != 0) return rc;
     sim.changes.clear();
     return bepucuda_end_constraints(ctx);
 }
 
-// The constraint adds and removes since the last describe or change on the resident rows: one bepucuda_add_constraints / bepucuda_remove_constraints
-// per run of adds or removes, in the order they were made, each with the constrained kinematics as they are now. An add's record is its lane as
-// the host holds it now (body references, impulses the host may have written since, prestep); a constraint added and removed again since sends its
-// body references and zero rows. add_feature_ids: 4 int32 per add in order, or NULL when no add is a contact. At a failing call the runs before it
-// leave the log and its code is returned; the failing run and those after it stay (add_feature_ids then starts at the first add still logged).
+// The body and constraint adds and removes since the last describe or change on the resident state: one bepucuda_add_bodies /
+// bepucuda_remove_bodies / bepucuda_add_constraints / bepucuda_remove_constraints per run of entries of one kind, in the order they were made. A
+// constraint run carries the constrained kinematics (active-set indices) as they were right after it. An add's record is its lane as the host holds
+// it now (body references as encoded when it was added, impulses the host may have written since, prestep); a constraint added and removed again
+// since sends its body references and zero rows. A body add sends the body's record as the host holds it now, or, for a body removed again since,
+// the record it had then; a body remove sends the active-set index it removed. add_feature_ids: 4 int32 per constraint add in order, or NULL when
+// no add is a contact. At a failing call the runs before it leave the log and its code is returned; the failing run and those after it stay
+// (add_feature_ids then starts at the first add still logged).
 int32_t bepuhost_cuda_change(void* simp, bepucuda_ctx* ctx, const int32_t* add_feature_ids) {
     Simulation& sim = *(Simulation*)simp;
     const int W = sim.W;
-    const int32_t* kin = sim.constrained_kinematic_handles.data();
-    const int32_t kin_count = (int32_t)sim.constrained_kinematic_handles.size();
     size_t adds = 0;
     for (size_t i = 0; i < sim.changes.size();) {
+        const ChangeKind kind = sim.changes[i].kind;
         size_t j = i;
-        while (j < sim.changes.size() && sim.changes[j].remove == sim.changes[i].remove) ++j;
+        while (j < sim.changes.size() && sim.changes[j].kind == kind) ++j;
+        const int32_t n = (int32_t)(j - i);
+        const std::vector<int32_t>& kin = sim.changes[j - 1].kinematics_kept ? sim.changes[j - 1].kinematics : kinematic_indices(sim);
         std::vector<bepucuda_constraint_location> locations;
-        std::vector<int32_t> records;
+        std::vector<int32_t> records, indices;
+        std::vector<float> bodies;
         for (size_t k = i; k < j; ++k) {
             const ChangeEntry& e = sim.changes[k];
+            if (kind == kBodyAdd) {
+                const float* r = e.record.empty() ? sim.dynamics.data + (size_t)sim.handle_to_index[(size_t)e.handle] * 32 : e.record.data();
+                bodies.insert(bodies.end(), r, r + 32);
+                continue;
+            }
+            if (kind == kBodyRemove) {
+                indices.push_back(e.at.index_in_type_batch);
+                continue;
+            }
             locations.push_back({0, e.at.batch, e.at.type_id, e.at.index_in_type_batch});
-            if (e.remove) continue;
+            if (kind == kConstraintRemove) continue;
             records.resize(records.size() + 64, 0);
             int32_t* r = records.data() + records.size() - 64;
             r[0] = e.at.type_id;
@@ -578,14 +730,20 @@ int32_t bepuhost_cuda_change(void* simp, bepucuda_ctx* ctx, const int32_t* add_f
             for (int q = 0; q < tb.impulse_rows; ++q) std::memcpy(r + 6 + q, tb.impulses.data + (bundle * tb.impulse_rows + q) * W + lane, 4);
             for (int q = 0; q < tb.prestep_rows; ++q) std::memcpy(r + 18 + q, tb.prestep.data + (bundle * tb.prestep_rows + q) * W + lane, 4);
         }
-        const int32_t n = (int32_t)(j - i);
-        const int32_t rc = sim.changes[i].remove ? bepucuda_remove_constraints(ctx, n, locations.data(), kin, kin_count)
-                                                 : bepucuda_add_constraints(ctx, n, locations.data(), records.data(), add_feature_ids ? add_feature_ids + adds * 4 : nullptr, kin, kin_count);
+        int32_t rc = 0;
+        switch (kind) {
+            case kBodyAdd: rc = bepucuda_add_bodies(ctx, bodies.data(), n, nullptr, nullptr); break;
+            case kBodyRemove: rc = bepucuda_remove_bodies(ctx, n, indices.data()); break;
+            case kConstraintRemove: rc = bepucuda_remove_constraints(ctx, n, locations.data(), kin.data(), (int32_t)kin.size()); break;
+            case kConstraintAdd:
+                rc = bepucuda_add_constraints(ctx, n, locations.data(), records.data(), add_feature_ids ? add_feature_ids + adds * 4 : nullptr, kin.data(), (int32_t)kin.size());
+                break;
+        }
         if (rc != 0) {
             sim.changes.erase(sim.changes.begin(), sim.changes.begin() + (std::ptrdiff_t)i);  // the runs before it went through: not forwarded again
             return rc;
         }
-        if (!sim.changes[i].remove) adds += (size_t)n;
+        if (kind == kConstraintAdd) adds += (size_t)n;
         i = j;
     }
     sim.changes.clear();

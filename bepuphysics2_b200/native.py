@@ -110,7 +110,8 @@ C_ABI_SYMBOLS = [
     "bepucuda_shard_set_fallback_rank",
     "bepucuda_color_constraints", "bepucuda_color_hash", "bepucuda_set_body_shapes", "bepucuda_predict_bounding_boxes",
     "bepucuda_set_body_accelerations", "bepucuda_set_point_gravity", "bepucuda_find_sleepable_islands", "bepucuda_read_constraints",
-    "bepucuda_write_constraints", "bepucuda_write_bodies", "bepucuda_add_constraints", "bepucuda_remove_constraints",
+    "bepucuda_write_constraints", "bepucuda_write_bodies", "bepucuda_add_constraints", "bepucuda_remove_constraints", "bepucuda_add_bodies",
+    "bepucuda_remove_bodies",
 ]
 
 
@@ -182,6 +183,8 @@ def load_libraries():
     cuda.bepucuda_write_constraints.argtypes = [vp, i32, vp, vp]
     cuda.bepucuda_add_constraints.argtypes = [vp, i32, vp, vp, vp, vp, i32]
     cuda.bepucuda_remove_constraints.argtypes = [vp, i32, vp, vp, i32]
+    cuda.bepucuda_add_bodies.argtypes = [vp, vp, i32, vp, vp]
+    cuda.bepucuda_remove_bodies.argtypes = [vp, i32, vp]
 
     host.bepuhost_create.restype = vp
     host.bepuhost_create.argtypes = [i32, i32]
@@ -195,6 +198,10 @@ def load_libraries():
     host.bepuhost_body_dynamics.argtypes = [vp]
     host.bepuhost_body_dynamics.restype = C.POINTER(C.c_float)
     host.bepuhost_body_count.argtypes = [vp]
+    host.bepuhost_remove_bodies.argtypes = [vp, i32, vp]
+    host.bepuhost_body_handles.argtypes = [vp]
+    host.bepuhost_body_handles.restype = C.POINTER(i32)
+    host.bepuhost_body_index.argtypes = [vp, i32]
     host.bepuhost_add_constraints.argtypes = [vp, i32, i32, vp, vp]
     host.bepuhost_add_constraints_in_batches.argtypes = [vp, i32, i32, vp, vp, vp]
     host.bepuhost_remove_constraints.argtypes = [vp, i32, vp]
@@ -281,8 +288,30 @@ class Simulation:
         self._host.bepuhost_set_integrator(self._sim, C.byref(integrator))
 
     def add_bodies(self, dynamics):
+        """Bodies.Add of each record in order, appended to the active set; returns the handle of the first (handles equal active-set indices until
+        a body is removed; then the pool hands out the last freed handle first)."""
         d = np.ascontiguousarray(dynamics, dtype=np.float32).reshape(-1, 32)
         return self._host.bepuhost_add_bodies(self._sim, d.ctypes.data, d.shape[0])
+
+    def remove_bodies(self, handles):
+        """Bodies.Remove for each body handle in order (Bodies.cs:L244-260): the constraints of every listed body are removed first (Solver.Remove),
+        then each body in turn: the last body of the active set moves into its slot and the moved body's constraint references follow it. Raises,
+        removing nothing, at a handle that names no body or is listed twice."""
+        h = np.ascontiguousarray(handles, dtype=np.int32).reshape(-1)
+        if self._host.bepuhost_remove_bodies(self._sim, h.shape[0], h.ctypes.data) != 0:
+            raise ValueError(self._host.bepuhost_last_error(self._sim).decode())
+
+    @property
+    def body_handles(self):
+        """Bodies.ActiveSet.IndexToHandle: the handle of every active-set index."""
+        n = self.body_count
+        if n == 0:
+            return np.zeros(0, dtype=np.int32)
+        return np.ctypeslib.as_array(self._host.bepuhost_body_handles(self._sim), shape=(n,)).copy()
+
+    def body_index(self, handle):
+        """Bodies.HandleToLocation: the active-set index of a body handle, -1 when it names no body."""
+        return self._host.bepuhost_body_index(self._sim, int(handle))
 
     @property
     def body_count(self):
@@ -515,9 +544,23 @@ class CudaTimestepper:
         k, kp = self._kinematics(kinematics)
         self._check(self._cuda.bepucuda_remove_constraints(self._ctx, loc.shape[0], loc.ctypes.data, kp, k.shape[0]))
 
+    def add_bodies(self, dynamics, shapes=None, accelerations=None):
+        """bepucuda_add_bodies: BodyDynamics records (n x 32 floats) appended to the device bodies, with BODY_SHAPE_DTYPE shapes and float32[n, 8]
+        accelerations appended to those arrays when given."""
+        d = np.ascontiguousarray(dynamics, dtype=np.float32).reshape(-1, 32)
+        sh = None if shapes is None else np.ascontiguousarray(shapes, dtype=BODY_SHAPE_DTYPE)
+        ac = None if accelerations is None else np.ascontiguousarray(accelerations, dtype=np.float32).reshape(-1, 8)
+        self._check(self._cuda.bepucuda_add_bodies(self._ctx, d.ctypes.data, d.shape[0], None if sh is None else sh.ctypes.data, None if ac is None else ac.ctypes.data))
+
+    def remove_bodies(self, indices):
+        """bepucuda_remove_bodies: BodySet.RemoveAt of each active-set index in order (the last body moves into the slot); the bodies' constraints
+        must be gone already."""
+        idx = np.ascontiguousarray(indices, dtype=np.int32).reshape(-1)
+        self._check(self._cuda.bepucuda_remove_bodies(self._ctx, idx.shape[0], idx.ctypes.data if idx.size else None))
+
     def change(self, add_feature_ids=None):
-        """bepuhost_cuda_change: every constraint add and remove of the simulation since the last describe or change, forwarded to the device rows
-        run by run. add_feature_ids: int32[adds, 4] in add order, or None when no add is a contact."""
+        """bepuhost_cuda_change: every body and constraint add and remove of the simulation since the last describe or change, forwarded to the
+        device run by run. add_feature_ids: int32[constraint adds, 4] in add order, or None when no add is a contact."""
         feat = None if add_feature_ids is None else np.ascontiguousarray(add_feature_ids, dtype=np.int32).reshape(-1, 4)
         self._check(self._host.bepuhost_cuda_change(self.sim._sim, self._ctx, None if feat is None else feat.ctypes.data))
 

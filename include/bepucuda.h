@@ -372,6 +372,32 @@ typedef struct bepucuda_body_activity {
 int32_t bepucuda_set_body_shapes(bepucuda_ctx* ctx, const bepucuda_body_shape* shapes, int32_t body_count);
 int32_t bepucuda_predict_bounding_boxes(bepucuda_ctx* ctx, float dt, bepucuda_body_activity* activities, float* bounds_out);
 
+/* Add and remove listed bodies of the device-resident body state: Bodies.Add (Bodies.cs:L183-212 -> BodySet.Add, BodySet.cs:L68-81) and the
+ * body half of Bodies.RemoveAt (Bodies.cs:L244-260 -> RemoveFromActiveSet L214-239, BodySet.RemoveAt BodySet.cs:L83-111,
+ * Solver.UpdateForBodyMemoryMove Solver.cs:L1444-1482, TypeProcessor.UpdateForBodyMemoryMove TypeProcessor.cs:L807-817,
+ * SequentialFallbackBatch.UpdateForDynamicBodyMemoryMove SequentialFallbackBatch.cs:L220-227) on the resident path, where a change in the body
+ * count would otherwise need bepucuda_download_impulses and a describe.
+ *   bepucuda_add_bodies appends count 128-B BodyDynamics records (what BodySet.Add wrote at [Count, Count + count)), inertia included, in order
+ *   at the current body count. No constraint references the new bodies: add their constraints afterwards with bepucuda_add_constraints.
+ *   bepucuda_remove_bodies applies body_indices in list order, each a BodySet.RemoveAt on the state the entries before it left: the body count
+ *   drops by one and, when the index is below the new count, the last body moves into that slot. Duplicates name whatever body sits at that index
+ *   at that point. Every constraint reference to a moved body takes its new index (the kinematic bit kept), and so do the constrained kinematic
+ *   indices of the context (a removed one leaves them). Remove the bodies' constraints first (bepucuda_remove_constraints), as RemoveAt does.
+ * Per-body arrays set for the current body count move with the bodies: bepucuda_set_body_accelerations and bepucuda_set_body_shapes. An add
+ * appends shapes[count] and accelerations[count * 8] to them; NULL for an array the context holds leaves that array at its old count, and then
+ * bepucuda_solve / bepucuda_predict_bounding_boxes return BEPUCUDA_ERR_BAD_STATE until it is set again or cleared.
+ * Afterwards every call takes the new indices and count: the body uploads, writes and downloads, bepucuda_read_constraints,
+ * bepucuda_find_sleepable_islands and the constraint change calls. The next solve re-captures the graph. Bus cost (bepucuda_timings h2d_bytes,
+ * inside upload_ms): an add 128 B per body plus 32 B per appended shape and acceleration record; a remove 4 B per index, its composed move table
+ * (the new index of each body at or above the new count). A remove re-plans the constraint rows as the constraint change calls do.
+ * BEPUCUDA_ERR_BAD_STATE before the first bepucuda_end_constraints, between begin and end, in peer mode, and while rows are pending (as for the
+ * constraint change calls). BEPUCUDA_ERR_INVALID_ARGUMENT for count < 0, a NULL body_dynamics / body_indices with count > 0, a body count past
+ * 2^28 - 1, an index outside [0, body count at that entry), and a removed body that a live constraint references. The index checks run on the
+ * host and the reference check on the device rows, both before any record, row, count or kinematic index changes: a failing call changes
+ * nothing. count == 0 is OK and changes nothing. */
+int32_t bepucuda_add_bodies(bepucuda_ctx* ctx, const void* body_dynamics, int32_t count, const bepucuda_body_shape* shapes, const float* accelerations);
+int32_t bepucuda_remove_bodies(bepucuda_ctx* ctx, int32_t count, const int32_t* body_indices);
+
 /* Device-side batch colouring (SURVEY.md §8 f3). Replaces, for a whole constraint set at once, the batch search Solver.Add runs per constraint
  * (Solver.cs:L1182-1199: the first batch whose referenced-handle set holds none of the constraint's dynamic bodies; kinematic references never
  * block, GetBlockingBodyHandles L1058-1078; index == fallback_batch_threshold is the fallback batch and accepts everything, TryAllocateInBatch

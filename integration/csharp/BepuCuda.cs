@@ -94,6 +94,8 @@ namespace BepuCuda
         [DllImport(Lib)] public static extern uint bepucuda_color_hash(uint constraintIndex);
         [DllImport(Lib)] public static extern int bepucuda_add_constraints(IntPtr ctx, int count, CudaConstraintLocation* locations, int* records, int* featureIds, int* constrainedKinematics, int kinematicCount);
         [DllImport(Lib)] public static extern int bepucuda_remove_constraints(IntPtr ctx, int count, CudaConstraintLocation* locations, int* constrainedKinematics, int kinematicCount);
+        [DllImport(Lib)] public static extern int bepucuda_add_bodies(IntPtr ctx, void* bodyDynamics, int count, BodyShape* shapes, float* accelerations);
+        [DllImport(Lib)] public static extern int bepucuda_remove_bodies(IntPtr ctx, int count, int* bodyIndices);
         /// <summary>Sleepable islands on the device: per body the smallest body index of its island, and the islands whose bodies are all sleep candidates (ascending, with body counts).
         /// Call after bepucuda_solve and before IncrementallyOptimizeDataStructures; see INTEGRATION.md.</summary>
         [DllImport(Lib)] public static extern int bepucuda_find_sleepable_islands(IntPtr ctx, BodyActivity* activities, int bodyCount, int* islandOfBodyOut, int* sleepableRootsOut, int* sleepableBodyCountsOut, int* sleepableCountOut, int* roundsOut);

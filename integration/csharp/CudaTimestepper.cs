@@ -180,6 +180,41 @@ public unsafe class CudaTimestepper<TCallbacks> : ITimestepper, IDisposable wher
             Check(Native.bepucuda_write_bodies(ctx, bodies.DynamicsState.Memory, handles.Length, p));
     }
 
+    /// <summary>Appends bodies the host just added with Bodies.Add to the device's body state (bepucuda_add_bodies): the handles, in the order
+    /// they were added, must name the last handles.Length bodies of the active set. Add their constraints afterwards (bepucuda_add_constraints).
+    /// shapes / accelerations extend the arrays set by bepucuda_set_body_shapes / bepucuda_set_body_accelerations (8 floats per body), or are
+    /// null.</summary>
+    public void AddBodies(Simulation simulation, ReadOnlySpan<BodyHandle> handles, BodyShape* shapes = null, float* accelerations = null)
+    {
+        ref var bodies = ref simulation.Bodies.ActiveSet;
+        int first = bodies.Count - handles.Length;
+        for (int i = 0; i < handles.Length; ++i)
+        {
+            ref var l = ref simulation.Bodies.HandleToLocation[handles[i].Value];                                      // Bodies.cs:L183-212
+            if (l.SetIndex != 0 || l.Index != first + i) throw new ArgumentException("AddBodies: the handles must be the last bodies of the active set, in order");
+        }
+        Check(Native.bepucuda_add_bodies(ctx, bodies.DynamicsState.Memory + first, handles.Length, shapes, accelerations));
+    }
+
+    /// <summary>Removes bodies from the simulation (Bodies.Remove) and from the device's body state (bepucuda_remove_bodies), in order: each
+    /// body's active-set index is read through HandleToLocation just before its removal, so the indices follow the reference's swap-removes. The
+    /// bodies' constraints must be removed first and forwarded (bepucuda_remove_constraints), as Bodies.RemoveAt removes them before the
+    /// body.</summary>
+    public void RemoveBodies(Simulation simulation, ReadOnlySpan<BodyHandle> handles)
+    {
+        var indices = new int[handles.Length];
+        for (int i = 0; i < handles.Length; ++i)
+        {
+            ref var l = ref simulation.Bodies.HandleToLocation[handles[i].Value];                                      // BodyMemoryLocation
+            if (l.SetIndex != 0) throw new ArgumentException("RemoveBodies: a sleeping body is not on the device");
+            if (simulation.Bodies.ActiveSet.Constraints[l.Index].Count != 0) throw new ArgumentException("RemoveBodies: remove the body's constraints first");
+            indices[i] = l.Index;
+            simulation.Bodies.Remove(handles[i]);                                                                     // Bodies.cs:L244-260
+        }
+        fixed (int* p = indices)
+            Check(Native.bepucuda_remove_bodies(ctx, handles.Length, p));
+    }
+
     // FNV-1a over everything bepucuda_end_constraints analyses: batch / type batch shape, every body reference, the constrained kinematics.
     // (~8 bytes per constraint body: a few hundred microseconds for 300 k contacts, against a graph re-capture per frame.)
     static ulong TopologySignature(Simulation simulation)
