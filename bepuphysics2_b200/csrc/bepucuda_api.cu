@@ -19,25 +19,73 @@ using namespace bepucuda;
 
 namespace bepucuda {
 
+// Raw rows of a source type batch on the device, in the reference's AOSOA-W layout: body references, prestep and impulses, and for the
+// device-side contact update (bepucuda_update_contacts) the feature ids of the resident impulses (old) and of the frame being uploaded (new).
+struct RawRows {
+    int32_t* refs = nullptr;
+    float* prestep = nullptr;
+    float* impulses = nullptr;
+    int32_t* features_old = nullptr;
+    int32_t* features_new = nullptr;
+};
+enum RowKind { kRowRefs, kRowPrestep, kRowImpulses, kRowFeatures };
+// Bytes of one kind of row for `count` constraints of type t: whole bundles of W for body references, prestep and impulses; exactly `count`
+// constraints for feature ids, which are [constraint][contact] and not bundled.
+static size_t row_bytes(const TypeInfo* t, RowKind k, int count, int W) {
+    const int per_constraint[4] = {t->bodies, t->prestep_rows, t->impulse_rows, t->contacts};
+    const size_t lanes = k == kRowFeatures ? (size_t)count : ((size_t)count + W - 1) / W * W;
+    return lanes * per_constraint[k] * 4;
+}
+
 struct SourceTypeBatch {
-    int batch_index, type_batch_index, type_id, count;
-    int capacity;          // constraints the raw arrays hold (whole bundles); bepucuda_add_constraints grows them
-    float* host_impulses;  // the host's AccumulatedImpulses (bepucuda_download_impulses); null after an add until the host passes it again
-    int32_t* raw_refs;     // device, reference AOSOA-W layout
-    float* raw_prestep;
-    float* raw_impulses;
-    size_t refs_bytes, prestep_bytes, impulse_bytes;
-    std::vector<int32_t> host_refs;  // retained only for fallback batches (levelisation)
-    // device-side contact update (bepucuda_update_contacts): feature ids of the resident impulses / of the frame being uploaded, `capacity`
-    // constraints each
-    int32_t* raw_features_old = nullptr;
-    int32_t* raw_features_new = nullptr;
-    size_t feature_bytes = 0;
+    ChangeSource host;     // the host's type batch: batch, type batch, type id, count, and body references retained only for fallback batches (levelisation)
+    int capacity = 0;      // constraints the rows hold (whole bundles); bepucuda_add_constraints grows them
+    RawRows rows;          // feature ids once bepucuda_set_contact_features set them or an add brought them
+    float* host_impulses = nullptr;  // the host's AccumulatedImpulses (bepucuda_download_impulses); null after an add until the host passes it again
     // rows uploaded since the last transposition (kTransposePrestep / kTransposeImpulses): refresh_device_rows transposes only these, so the rows
     // of every other type batch, the accumulated impulses in particular, stay as the last solve left them on the device
     int32_t pending = 0;
     bool redistribute = false;
+    const TypeInfo* type() const { return get_type_info(host.type_id); }
+    size_t bytes(RowKind k, int W) const { return row_bytes(type(), k, host.count, W); }
+    // the rows as the lane copies of bepucuda_add_constraints / bepucuda_remove_constraints and the reference remap of bepucuda_remove_bodies see them
+    SourceRows lane_rows() const {
+        const TypeInfo* t = type();
+        return {rows.refs, rows.prestep, rows.impulses, rows.features_old, t->bodies, t->prestep_rows, t->impulse_rows, t->contacts};
+    }
+    RefSpan ref_span(int W) const { return {rows.refs, (int64_t)(bytes(kRowRefs, W) / 4)}; }
 };
+
+// The per-body device arrays: the 128-B records that uploads and downloads pass through, and the arrays the kernels read through BodyBuffers.
+struct BodyArrays {
+    DeviceBuffer raw, pose, velocity, inertia_local, inertia_world, constrained, first_batch;
+    // Room for n bodies, contents dropped; constrained flags reallocated here start cleared. first_batch is sized and filled by the plan.
+    cudaError_t reserve(size_t n, cudaStream_t s) {
+        cudaError_t e = raw.reserve(n * 128);
+        for (DeviceBuffer* b : {&pose, &velocity, &inertia_local, &inertia_world})
+            if (e == cudaSuccess) e = b->reserve(n * 32);
+        const size_t old_constrained_capacity = constrained.capacity;
+        if (e == cudaSuccess) e = constrained.reserve(n + 1);
+        if (e == cudaSuccess && constrained.capacity != old_constrained_capacity) e = cudaMemsetAsync(constrained.ptr, 0, constrained.capacity, s);
+        return e;
+    }
+    // Room for n bodies, the records of the first `keep` kept. A failure leaves the arrays grown so far grown, records and all.
+    cudaError_t grow(size_t n, size_t keep, cudaStream_t s) {
+        cudaError_t e = raw.grow(n * 128, keep * 128, s);
+        for (DeviceBuffer* b : {&pose, &velocity, &inertia_local, &inertia_world})
+            if (e == cudaSuccess) e = b->grow(n * 32, keep * 32, s);
+        if (e == cudaSuccess) e = constrained.grow(n + 1, keep, s);
+        if (e == cudaSuccess) e = first_batch.grow(n * 4, keep * 4, s);
+        return e;
+    }
+    BodyBuffers view(int count) const {
+        return {pose.as<float4>(), velocity.as<float4>(), inertia_local.as<float4>(), inertia_world.as<float4>(), constrained.as<uint8_t>(), first_batch.as<int32_t>(), count};
+    }
+};
+inline bool operator==(const BodyBuffers& a, const BodyBuffers& b) {
+    return a.pose == b.pose && a.velocity == b.velocity && a.inertia_local == b.inertia_local && a.inertia_world == b.inertia_world && a.constrained == b.constrained &&
+           a.first_batch == b.first_batch && a.count == b.count;
+}
 
 // The stage sequence of the program captured as a graph (dropped when the program is replaced), and the body buffers and launch context its
 // launches bake in besides the program: matches() says whether a frame can replay it.
@@ -47,10 +95,7 @@ struct StageGraph {
     BodyBuffers bodies{};
     LaunchContext launch{};
     void reset() { exec.reset(); graph.reset(); }
-    bool matches(const BodyBuffers& b, const LaunchContext& lc) const {
-        return exec && bodies.pose == b.pose && bodies.velocity == b.velocity && bodies.inertia_local == b.inertia_local && bodies.inertia_world == b.inertia_world &&
-               bodies.constrained == b.constrained && bodies.first_batch == b.first_batch && bodies.count == b.count && same_launches(launch, lc);
-    }
+    bool matches(const BodyBuffers& b, const LaunchContext& lc) const { return exec && bodies == b && same_launches(launch, lc); }
 };
 
 }  // namespace bepucuda
@@ -80,8 +125,9 @@ struct bepucuda_ctx {
     // bodies
     int body_count = 0;
     bool bodies_uploaded = false;  // a bepucuda_upload_bodies has succeeded
-    DeviceBuffer raw_bodies, pose, velocity, inertia_local, inertia_world, constrained, first_batch, sync_refcount, sync_mask;
-    BodyBuffers B{};
+    BodyArrays bodies;
+    DeviceBuffer sync_refcount, sync_mask;
+    BodyBuffers B{};  // bodies.view(body_count), set by refresh_body_buffers
 
     // constraints
     int W = 8;
@@ -236,8 +282,73 @@ template <class T> int upload_table(bepucuda_ctx* ctx, const char* name, DeviceB
 
 SourceTypeBatch* find_source(bepucuda_ctx* ctx, int32_t batch_index, int32_t type_batch_index) {
     for (auto& s : ctx->sources)
-        if (s.batch_index == batch_index && s.type_batch_index == type_batch_index) return &s;
+        if (s.host.batch_index == batch_index && s.host.type_batch_index == type_batch_index) return &s;
     return nullptr;
+}
+
+// A block of `bytes` for source rows: a spare block of the arena between `bytes` and twice that, or a new one. Spare blocks are what grown and
+// removed sources left, so a run that stays on the change calls reuses them instead of growing the arena with every re-created type batch.
+void* take_rows(bepucuda_ctx* ctx, size_t bytes, cudaError_t* e) {
+    size_t best = ctx->spare_rows.size();
+    for (size_t i = 0; i < ctx->spare_rows.size(); ++i) {
+        const size_t have = ctx->spare_rows[i].second;
+        if (have >= bytes && have <= 2 * bytes && (best == ctx->spare_rows.size() || have < ctx->spare_rows[best].second)) best = i;
+    }
+    if (best == ctx->spare_rows.size()) return ctx->raw_arena.alloc(bytes, e);
+    void* p = ctx->spare_rows[best].first;
+    ctx->spare_rows[best] = ctx->spare_rows.back();
+    ctx->spare_rows.pop_back();
+    return p;
+}
+void give_rows(bepucuda_ctx* ctx, void* p, size_t bytes) {
+    if (p && bytes) ctx->spare_rows.push_back({p, bytes});
+}
+void give_source_rows(bepucuda_ctx* ctx, const TypeInfo* t, int capacity, const RawRows& r) {
+    auto give = [&](void* p, RowKind k) { give_rows(ctx, p, row_bytes(t, k, capacity, ctx->W)); };
+    give(r.refs, kRowRefs);
+    give(r.prestep, kRowPrestep);
+    give(r.impulses, kRowImpulses);
+    give(r.features_old, kRowFeatures);
+    give(r.features_new, kRowFeatures);
+}
+// The feature-id rows of `capacity` constraints into *r; on failure the block taken goes back and *r keeps none.
+cudaError_t take_feature_rows(bepucuda_ctx* ctx, const TypeInfo* t, int capacity, RawRows* r) {
+    cudaError_t e = cudaSuccess;
+    const size_t bytes = row_bytes(t, kRowFeatures, capacity, ctx->W);
+    r->features_old = (int32_t*)take_rows(ctx, bytes, &e);
+    if (r->features_old) r->features_new = (int32_t*)take_rows(ctx, bytes, &e);
+    if (r->features_new) return cudaSuccess;
+    give_rows(ctx, r->features_old, bytes);
+    r->features_old = nullptr;
+    return e == cudaSuccess ? cudaErrorMemoryAllocation : e;
+}
+// The rows of `capacity` constraints, with feature ids when `features` and t is a contact type; on failure every block taken goes back and the
+// error is returned. In a describe there are no spare blocks, so the rows are new arena blocks, taken in row order.
+cudaError_t take_source_rows(bepucuda_ctx* ctx, const TypeInfo* t, int capacity, bool features, RawRows* out) {
+    cudaError_t e = cudaSuccess;
+    auto take = [&](RowKind k) { return take_rows(ctx, row_bytes(t, k, capacity, ctx->W), &e); };
+    RawRows r;
+    r.refs = (int32_t*)take(kRowRefs);
+    if (r.refs) r.prestep = (float*)take(kRowPrestep);
+    if (r.prestep) r.impulses = (float*)take(kRowImpulses);
+    if (!r.impulses) e = e == cudaSuccess ? cudaErrorMemoryAllocation : e;
+    else if (features && t->contacts > 0) e = take_feature_rows(ctx, t, capacity, &r);
+    if (e != cudaSuccess) {
+        give_source_rows(ctx, t, capacity, r);
+        return e;
+    }
+    *out = r;
+    return cudaSuccess;
+}
+
+void refresh_body_buffers(bepucuda_ctx* ctx) { ctx->B = ctx->bodies.view(ctx->body_count); }
+
+// The device's AOSOA-32 rows of `what` (kTransposePrestep / kTransposeImpulses) back into the sources' raw rows.
+int transpose_out(bepucuda_ctx* ctx, int what) {
+    launch_transpose_out_all(ctx->tb_table.as<DeviceTypeBatch>(), ctx->tdesc_table.as<TransposeDesc>(), ctx->work_table.as<WorkItem>(), ctx->topo.all_work_count, ctx->W,
+                             what, ctx->stream);
+    CK(cudaGetLastError());
+    return BEPUCUDA_OK;
 }
 
 // The optional velocity terms that are set (bepucuda_set_body_accelerations / bepucuda_set_point_gravity): kIntegrateAccelerations |
@@ -436,10 +547,10 @@ int refresh_device_rows(bepucuda_ctx* ctx) {
         const SourceTypeBatch& s = ctx->sources[(size_t)ctx->topo.tbs[tb].source];
         TransposeDesc& d = ctx->tdescs[tb];
         const int32_t flags = s.pending | (s.redistribute ? kDescRedistribute : 0);
-        if (d.flags != flags || d.features_old != s.raw_features_old || d.features_new != s.raw_features_new) {
+        if (d.flags != flags || d.features_old != s.rows.features_old || d.features_new != s.rows.features_new) {
             d.flags = flags;
-            d.features_old = s.raw_features_old;
-            d.features_new = s.raw_features_new;
+            d.features_old = s.rows.features_old;
+            d.features_new = s.rows.features_new;
             descs_changed = true;
         }
         any_pending |= s.pending != 0;
@@ -465,7 +576,7 @@ int refresh_device_rows(bepucuda_ctx* ctx) {
         q.clear();
     }
     for (SourceTypeBatch& s : ctx->sources) {
-        if (s.redistribute) std::swap(s.raw_features_old, s.raw_features_new);  // the resident impulses now belong to the new ids
+        if (s.redistribute) std::swap(s.rows.features_old, s.rows.features_new);  // the resident impulses now belong to the new ids
         s.redistribute = false;
         s.pending = 0;
     }
@@ -637,22 +748,14 @@ int32_t bepucuda_upload_bodies(bepucuda_ctx* ctx, const void* body_dynamics, int
     const size_t n = (size_t)body_count;
     // constrained flags / ownership depend on the body count; force a rebuild of topology products.
     if (body_count != ctx->body_count) ctx->constraints_ready = false;
-    CK(ctx->raw_bodies.reserve(n * 128));
-    CK(ctx->pose.reserve(n * 32));
-    CK(ctx->velocity.reserve(n * 32));
-    CK(ctx->inertia_local.reserve(n * 32));
-    CK(ctx->inertia_world.reserve(n * 32));
-    const size_t old_constrained_cap = ctx->constrained.capacity;
-    CK(ctx->constrained.reserve(n + 1));
-    if (ctx->constrained.capacity != old_constrained_cap) CK(cudaMemsetAsync(ctx->constrained.ptr, 0, ctx->constrained.capacity, ctx->stream));
+    if (const cudaError_t e = ctx->bodies.reserve(n, ctx->stream)) return cuda_fail(ctx, e, "upload_bodies: body arrays");
     ctx->body_count = body_count;
     ctx->bodies_uploaded = true;
-    ctx->B = {ctx->pose.as<float4>(), ctx->velocity.as<float4>(), ctx->inertia_local.as<float4>(), ctx->inertia_world.as<float4>(), ctx->constrained.as<uint8_t>(),
-              ctx->first_batch.as<int32_t>(), body_count};
+    refresh_body_buffers(ctx);
     if (body_count > 0) {
-        CK(cudaMemcpyAsync(ctx->raw_bodies.ptr, body_dynamics, n * 128, cudaMemcpyHostToDevice, ctx->stream));
+        CK(cudaMemcpyAsync(ctx->bodies.raw.ptr, body_dynamics, n * 128, cudaMemcpyHostToDevice, ctx->stream));
         ctx->h2d_accum += (int64_t)n * 128;
-        launch_split_bodies(ctx->raw_bodies.ptr, body_count, ctx->B, ctx->stream);
+        launch_split_bodies(ctx->bodies.raw.ptr, body_count, ctx->B, ctx->stream);
         CK(cudaGetLastError());
     }
     return BEPUCUDA_OK;
@@ -688,22 +791,15 @@ int32_t bepucuda_upload_type_batch(bepucuda_ctx* ctx, int32_t batch_index, int32
     if (!body_references || !prestep || !accumulated_impulses) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "upload_type_batch: null buffer");
     CK(cudaSetDevice(ctx->device));
     const int W = ctx->W;
-    const size_t bundles = ((size_t)constraint_count + W - 1) / W;
-    SourceTypeBatch s{};
-    s.batch_index = batch_index; s.type_batch_index = type_batch_index; s.type_id = type_id; s.count = constraint_count; s.capacity = (int)bundles * W;
+    SourceTypeBatch s;
+    s.host = {batch_index, type_batch_index, type_id, constraint_count, {}};
+    s.capacity = (int)(((size_t)constraint_count + W - 1) / W) * W;
     s.host_impulses = accumulated_impulses;
-    s.refs_bytes = bundles * t->bodies * W * 4;
-    s.prestep_bytes = bundles * t->prestep_rows * W * 4;
-    s.impulse_bytes = bundles * t->impulse_rows * W * 4;
-    cudaError_t e = cudaSuccess;
-    s.raw_refs = (int32_t*)ctx->raw_arena.alloc(s.refs_bytes, &e);
-    s.raw_prestep = (float*)ctx->raw_arena.alloc(s.prestep_bytes, &e);
-    s.raw_impulses = (float*)ctx->raw_arena.alloc(s.impulse_bytes, &e);
-    if (!s.raw_refs || !s.raw_prestep || !s.raw_impulses) return cuda_fail(ctx, e, "raw arena");
-    TRY(copy_in(ctx, s.raw_refs, body_references, s.refs_bytes));
-    TRY(copy_in(ctx, s.raw_prestep, prestep, s.prestep_bytes));
-    TRY(copy_in(ctx, s.raw_impulses, accumulated_impulses, s.impulse_bytes));
-    if (batch_index >= ctx->fallback_threshold) s.host_refs.assign(body_references, body_references + s.refs_bytes / 4);
+    if (const cudaError_t e = take_source_rows(ctx, t, s.capacity, false, &s.rows)) return cuda_fail(ctx, e, "raw arena");
+    TRY(copy_in(ctx, s.rows.refs, body_references, s.bytes(kRowRefs, W)));
+    TRY(copy_in(ctx, s.rows.prestep, prestep, s.bytes(kRowPrestep, W)));
+    TRY(copy_in(ctx, s.rows.impulses, accumulated_impulses, s.bytes(kRowImpulses, W)));
+    if (batch_index >= ctx->fallback_threshold) s.host.refs.assign(body_references, body_references + s.bytes(kRowRefs, W) / 4);
     ctx->sources.push_back(std::move(s));
     return BEPUCUDA_OK;
 }
@@ -732,7 +828,7 @@ static int plan_device_rows(bepucuda_ctx* ctx) {
     const int W = ctx->W;
     {
         std::vector<SourceView> views;
-        for (const SourceTypeBatch& s : ctx->sources) views.push_back({s.batch_index, s.type_batch_index, s.type_id, s.count, s.host_refs.data()});
+        for (const SourceTypeBatch& s : ctx->sources) views.push_back({s.host.batch_index, s.host.type_batch_index, s.host.type_id, s.host.count, s.host.refs.data()});
         TopologyPlan plan;
         std::string error;
         const int rc = plan_topology(views, W, ctx->fallback_threshold, ctx->batch_count, ctx->body_count, ctx->peer_mode, &plan, &error, ctx->peers.rank, ctx->fallback_rank);
@@ -756,7 +852,7 @@ static int plan_device_rows(bepucuda_ctx* ctx) {
         const TypeInfo* t = get_type_info(p.type_id);
         tbs[i] = {p.type_id, p.bundle_count, p.device_batch, t->bodies, ctx->refs32.as<int32_t>() + p.refs_offset, ctx->prestep32.as<float>() + p.prestep_offset,
                   ctx->impulses32.as<float>() + p.impulse_offset};
-        ctx->tdescs[i] = {s.raw_refs, s.raw_prestep, s.raw_impulses, p.map_offset < 0 ? nullptr : ctx->map_table.as<int32_t>() + p.map_offset, s.count, t->bodies, t->prestep_rows,
+        ctx->tdescs[i] = {s.rows.refs, s.rows.prestep, s.rows.impulses, p.map_offset < 0 ? nullptr : ctx->map_table.as<int32_t>() + p.map_offset, s.host.count, t->bodies, t->prestep_rows,
                           t->impulse_rows, topo.source_bundle_base[(size_t)p.source], kTransposePrestep | kTransposeImpulses, t->contacts, nullptr, nullptr};
     }
     ctx->records = work_records(topo, ctx->refs32.as<int32_t>(), ctx->prestep32.as<float>(), ctx->impulses32.as<float>());
@@ -773,19 +869,19 @@ static int plan_device_rows(bepucuda_ctx* ctx) {
     launch_transpose_in_all(ctx->tb_table.as<DeviceTypeBatch>(), ctx->tdesc_table.as<TransposeDesc>(), ctx->work_table.as<WorkItem>(), topo.all_work_count, W,
                             kTransposeRefs | kTransposePrestep | kTransposeImpulses, ctx->stream);
     const size_t nb = (size_t)std::max(ctx->body_count, 1);
-    CK(ctx->first_batch.reserve(nb * 4));
+    CK(ctx->bodies.first_batch.reserve(nb * 4));
     CK(ctx->sync_refcount.reserve(nb * 4));
     CK(ctx->sync_mask.reserve(nb * 8));
-    ctx->B.first_batch = ctx->first_batch.as<int32_t>();
-    launch_fill_i32(ctx->first_batch.as<int32_t>(), nb, 0x7fffffff, ctx->stream);
+    refresh_body_buffers(ctx);
+    launch_fill_i32(ctx->bodies.first_batch.as<int32_t>(), nb, 0x7fffffff, ctx->stream);
     CK(cudaMemsetAsync(ctx->sync_refcount.ptr, 0, nb * 4, ctx->stream));
     CK(cudaMemsetAsync(ctx->sync_mask.ptr, 0, nb * 8, ctx->stream));
-    CK(cudaMemsetAsync(ctx->constrained.ptr, 0, nb, ctx->stream));
+    CK(cudaMemsetAsync(ctx->bodies.constrained.ptr, 0, nb, ctx->stream));
     CK(cudaMemsetAsync(ctx->error_dev.ptr, 0, 32, ctx->stream));
     CK(ctx->source_bundle_flags.reserve((size_t)std::max(topo.source_bundles, 1) * 16));
     CK(cudaMemsetAsync(ctx->source_bundle_flags.ptr, 0, (size_t)std::max(topo.source_bundles, 1) * 16, ctx->stream));
     launch_ownership_pass1(ctx->tb_table.as<DeviceTypeBatch>(), ctx->work_table.as<WorkItem>(), topo.all_work_count, topo.sync_batch_count,
-                           ctx->body_count, ctx->first_batch.as<int32_t>(), ctx->sync_refcount.as<int32_t>(), (unsigned long long*)ctx->sync_mask.ptr, ctx->error_dev.as<int32_t>(),
+                           ctx->body_count, ctx->bodies.first_batch.as<int32_t>(), ctx->sync_refcount.as<int32_t>(), (unsigned long long*)ctx->sync_mask.ptr, ctx->error_dev.as<int32_t>(),
                            ctx->stream);
     if (ctx->peer_mode && nb > 0) {
         // peer sharding: the integration owner of a body is the lowest batch referencing it on ANY rank (computed by the host over the whole graph);
@@ -793,15 +889,15 @@ static int plan_device_rows(bepucuda_ctx* ctx) {
         if ((int)ctx->global_first_batch.size() != ctx->body_count) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, "end_constraints: bepucuda_shard_set_global was not called for this body count");
         CK(ctx->global_first_batch_dev.reserve(nb * 4));
         CK(cudaMemcpyAsync(ctx->global_first_batch_dev.ptr, ctx->global_first_batch.data(), (size_t)ctx->body_count * 4, cudaMemcpyHostToDevice, ctx->stream));
-        launch_merge_first_batch(ctx->first_batch.as<int32_t>(), ctx->global_first_batch_dev.as<int32_t>(), ctx->body_count, ctx->fallback_threshold, ctx->stream);
+        launch_merge_first_batch(ctx->bodies.first_batch.as<int32_t>(), ctx->global_first_batch_dev.as<int32_t>(), ctx->body_count, ctx->fallback_threshold, ctx->stream);
     }
     launch_ownership_rest(ctx->tb_table.as<DeviceTypeBatch>(), ctx->work_table.as<WorkItem>(), topo.all_work_count, ctx->body_count,
-                          ctx->first_batch.as<int32_t>(), ctx->sync_refcount.as<int32_t>(), (const unsigned long long*)ctx->sync_mask.ptr, ctx->constrained.as<uint8_t>(),
+                          ctx->bodies.first_batch.as<int32_t>(), ctx->sync_refcount.as<int32_t>(), (const unsigned long long*)ctx->sync_mask.ptr, ctx->bodies.constrained.as<uint8_t>(),
                           ctx->kinematics_dev.as<int32_t>(), (int)ctx->kinematics.size(), ctx->error_dev.as<int32_t>(), ctx->tdesc_table.as<TransposeDesc>(), W,
                           ctx->source_bundle_flags.as<int32_t>(), ctx->stream);
     if (ctx->peer_mode) {
         // ... and a body is "constrained" (final pose pass) if any rank constrains it
-        CK(cudaMemcpyAsync(ctx->constrained.ptr, ctx->global_constrained.data(), (size_t)ctx->body_count, cudaMemcpyHostToDevice, ctx->stream));
+        CK(cudaMemcpyAsync(ctx->bodies.constrained.ptr, ctx->global_constrained.data(), (size_t)ctx->body_count, cudaMemcpyHostToDevice, ctx->stream));
         // per body reference, the other ranks that need what this rank's constraint writes
         CK(ctx->peer32.reserve(topo.refs_words * 4 + 1024));
         CK(ctx->body_masks_dev.reserve((size_t)ctx->body_count + 16));
@@ -846,23 +942,12 @@ int32_t bepucuda_update_type_batch(bepucuda_ctx* ctx, int32_t batch_index, int32
     if (!s) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "update_type_batch: unknown type batch");
     CK(cudaSetDevice(ctx->device));
     ctx->upload_window.start_once(ctx->stream);
-    TRY(copy_in(ctx, s->raw_prestep, prestep, s->prestep_bytes));
-    TRY(copy_in(ctx, s->raw_impulses, accumulated_impulses, s->impulse_bytes));
+    TRY(copy_in(ctx, s->rows.prestep, prestep, s->bytes(kRowPrestep, ctx->W)));
+    TRY(copy_in(ctx, s->rows.impulses, accumulated_impulses, s->bytes(kRowImpulses, ctx->W)));
     s->host_impulses = accumulated_impulses;
     s->pending = kTransposePrestep | kTransposeImpulses;
     s->redistribute = false;  // the host took the impulses back
     ctx->data_dirty = true;
-    return BEPUCUDA_OK;
-}
-
-static int ensure_feature_arrays(bepucuda_ctx* ctx, SourceTypeBatch& s) {
-    if (s.raw_features_old) return BEPUCUDA_OK;
-    const size_t contacts = (size_t)get_type_info(s.type_id)->contacts;
-    s.feature_bytes = (size_t)s.count * contacts * sizeof(int32_t);
-    cudaError_t e = cudaSuccess;
-    s.raw_features_old = (int32_t*)ctx->raw_arena.alloc((size_t)s.capacity * contacts * sizeof(int32_t), &e);
-    s.raw_features_new = (int32_t*)ctx->raw_arena.alloc((size_t)s.capacity * contacts * sizeof(int32_t), &e);
-    if (!s.raw_features_old || !s.raw_features_new) return cuda_fail(ctx, e, "raw arena (contact feature ids)");
     return BEPUCUDA_OK;
 }
 
@@ -871,12 +956,13 @@ int32_t bepucuda_set_contact_features(bepucuda_ctx* ctx, int32_t batch_index, in
     if (!ctx->constraints_open && !ctx->constraints_ready) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, "set_contact_features before the type batch was uploaded");
     SourceTypeBatch* s = find_source(ctx, batch_index, type_batch_index);
     if (!s) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "set_contact_features: unknown type batch");
-    if (get_type_info(s->type_id)->contacts == 0) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "set_contact_features: not a contact constraint type");
+    if (s->type()->contacts == 0) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "set_contact_features: not a contact constraint type");
     CK(cudaSetDevice(ctx->device));
-    TRY(ensure_feature_arrays(ctx, *s));
+    if (!s->rows.features_old)
+        if (const cudaError_t e = take_feature_rows(ctx, s->type(), s->capacity, &s->rows)) return cuda_fail(ctx, e, "raw arena (contact feature ids)");
     // from a mapped buffer the ids are only queued: the next solve copies them, before the host writes the next frame's ids into the same buffer
     if (ctx->constraints_ready) ctx->data_dirty = true;
-    return copy_in(ctx, s->raw_features_old, feature_ids, s->feature_bytes);
+    return copy_in(ctx, s->rows.features_old, feature_ids, s->bytes(kRowFeatures, ctx->W));
 }
 
 int32_t bepucuda_update_contacts(bepucuda_ctx* ctx, int32_t batch_index, int32_t type_batch_index, const float* prestep, const int32_t* new_feature_ids) {
@@ -884,13 +970,13 @@ int32_t bepucuda_update_contacts(bepucuda_ctx* ctx, int32_t batch_index, int32_t
     if (!ctx->constraints_ready) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, "update_contacts before end_constraints");
     SourceTypeBatch* s = find_source(ctx, batch_index, type_batch_index);
     if (!s) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "update_contacts: unknown type batch");
-    if (get_type_info(s->type_id)->contacts == 0) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "update_contacts: not a contact constraint type");
-    if (!s->raw_features_old) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, "update_contacts: bepucuda_set_contact_features was never called for this type batch");
+    if (s->type()->contacts == 0) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "update_contacts: not a contact constraint type");
+    if (!s->rows.features_old) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, "update_contacts: bepucuda_set_contact_features was never called for this type batch");
     if (s->redistribute) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, "update_contacts: called twice for the same type batch without a solve in between");
     CK(cudaSetDevice(ctx->device));
     ctx->upload_window.start_once(ctx->stream);
-    TRY(copy_in(ctx, s->raw_prestep, prestep, s->prestep_bytes));
-    TRY(copy_in(ctx, s->raw_features_new, new_feature_ids, s->feature_bytes));
+    TRY(copy_in(ctx, s->rows.prestep, prestep, s->bytes(kRowPrestep, ctx->W)));
+    TRY(copy_in(ctx, s->rows.features_new, new_feature_ids, s->bytes(kRowFeatures, ctx->W)));
     s->pending |= kTransposePrestep;  // the accumulated impulses stay resident
     s->redistribute = true;
     ctx->data_dirty = true;
@@ -906,8 +992,8 @@ int32_t bepucuda_upload_body_motion(bepucuda_ctx* ctx, const void* body_dynamics
     if (char* alias = map_host(ctx, body_dynamics, n * 128)) {
         launch_scatter_body_motion(alias, body_count, ctx->B, ctx->stream);  // 64 of every 128 bytes read straight from the mapped host buffer
     } else {
-        CK(cudaMemcpy2DAsync(ctx->raw_bodies.ptr, 128, body_dynamics, 128, 64, n, cudaMemcpyHostToDevice, ctx->stream));
-        launch_scatter_body_motion(ctx->raw_bodies.ptr, body_count, ctx->B, ctx->stream);
+        CK(cudaMemcpy2DAsync(ctx->bodies.raw.ptr, 128, body_dynamics, 128, 64, n, cudaMemcpyHostToDevice, ctx->stream));
+        launch_scatter_body_motion(ctx->bodies.raw.ptr, body_count, ctx->B, ctx->stream);
     }
     CK(cudaGetLastError());
     ctx->h2d_accum += (int64_t)n * 64;
@@ -947,8 +1033,8 @@ int32_t bepucuda_download_body_motion(bepucuda_ctx* ctx, void* out, int32_t body
     if (char* alias = map_host(ctx, out, n * 128)) {
         launch_gather_body_motion(alias, body_count, ctx->B, ctx->stream);
     } else {
-        launch_gather_body_motion(ctx->raw_bodies.ptr, body_count, ctx->B, ctx->stream);
-        CK(cudaMemcpy2DAsync(out, 128, ctx->raw_bodies.ptr, 128, 64, n, cudaMemcpyDeviceToHost, ctx->stream));
+        launch_gather_body_motion(ctx->bodies.raw.ptr, body_count, ctx->B, ctx->stream);
+        CK(cudaMemcpy2DAsync(out, 128, ctx->bodies.raw.ptr, 128, 64, n, cudaMemcpyDeviceToHost, ctx->stream));
     }
     CK(cudaGetLastError());
     CK(ctx->download_window.stop(ctx->stream));
@@ -1027,9 +1113,9 @@ int32_t bepucuda_download_bodies(bepucuda_ctx* ctx, void* out, int32_t body_coun
     if (!ctx || !out || body_count < 0 || body_count > ctx->body_count) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "download_bodies: bad arguments");
     CK(cudaSetDevice(ctx->device));
     CK(ctx->download_window.start(ctx->stream));
-    launch_merge_bodies(ctx->raw_bodies.ptr, body_count, ctx->B, ctx->stream);
+    launch_merge_bodies(ctx->bodies.raw.ptr, body_count, ctx->B, ctx->stream);
     CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(out, ctx->raw_bodies.ptr, (size_t)body_count * 128, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaMemcpyAsync(out, ctx->bodies.raw.ptr, (size_t)body_count * 128, cudaMemcpyDeviceToHost, ctx->stream));
     CK(ctx->download_window.stop(ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
     ctx->timings.d2h_bytes = (int64_t)body_count * 128;
@@ -1041,18 +1127,17 @@ int32_t bepucuda_download_impulses(bepucuda_ctx* ctx) {
     if (!ctx->constraints_ready) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, "download_impulses before end_constraints");
     for (const SourceTypeBatch& s : ctx->sources)
         if (!s.host_impulses)
-            return fail(ctx, BEPUCUDA_ERR_BAD_STATE, "download_impulses: type batch (" + std::to_string(s.batch_index) + ", " + std::to_string(s.type_batch_index) +
+            return fail(ctx, BEPUCUDA_ERR_BAD_STATE, "download_impulses: type batch (" + std::to_string(s.host.batch_index) + ", " + std::to_string(s.host.type_batch_index) +
                                                          ") took constraints through bepucuda_add_constraints; pass its buffers again (update_type_batch or a describe)");
     CK(cudaSetDevice(ctx->device));
-    launch_transpose_out_all(ctx->tb_table.as<DeviceTypeBatch>(), ctx->tdesc_table.as<TransposeDesc>(), ctx->work_table.as<WorkItem>(), ctx->topo.all_work_count, ctx->W,
-                             kTransposeImpulses, ctx->stream);
-    CK(cudaGetLastError());
+    TRY(transpose_out(ctx, kTransposeImpulses));
     int64_t bytes = 0;
     std::vector<CopyChunk> d2h;
     for (auto& s : ctx->sources) {
-        if (char* alias = map_host(ctx, s.host_impulses, s.impulse_bytes)) queue_chunks(d2h, alias, s.raw_impulses, s.impulse_bytes);
-        else CK(cudaMemcpyAsync(s.host_impulses, s.raw_impulses, s.impulse_bytes, cudaMemcpyDeviceToHost, ctx->stream));
-        bytes += (int64_t)s.impulse_bytes;
+        const size_t n = s.bytes(kRowImpulses, ctx->W);
+        if (char* alias = map_host(ctx, s.host_impulses, n)) queue_chunks(d2h, alias, s.rows.impulses, n);
+        else CK(cudaMemcpyAsync(s.host_impulses, s.rows.impulses, n, cudaMemcpyDeviceToHost, ctx->stream));
+        bytes += (int64_t)n;
     }
     TRY(flush_chunks(ctx, d2h));
     CK(cudaStreamSynchronize(ctx->stream));
@@ -1066,10 +1151,8 @@ int32_t bepucuda_download_prestep(bepucuda_ctx* ctx, int32_t batch_index, int32_
     const SourceTypeBatch* s = find_source(ctx, batch_index, type_batch_index);
     if (!s) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "download_prestep: unknown type batch");
     CK(cudaSetDevice(ctx->device));
-    launch_transpose_out_all(ctx->tb_table.as<DeviceTypeBatch>(), ctx->tdesc_table.as<TransposeDesc>(), ctx->work_table.as<WorkItem>(), ctx->topo.all_work_count, ctx->W,
-                             kTransposePrestep, ctx->stream);
-    CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(prestep_out, s->raw_prestep, s->prestep_bytes, cudaMemcpyDeviceToHost, ctx->stream));
+    TRY(transpose_out(ctx, kTransposePrestep));
+    CK(cudaMemcpyAsync(prestep_out, s->rows.prestep, s->bytes(kRowPrestep, ctx->W), cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
     return BEPUCUDA_OK;
 }
@@ -1113,68 +1196,31 @@ int32_t bepucuda_write_constraints(bepucuda_ctx* ctx, int32_t count, const bepuc
     return BEPUCUDA_OK;
 }
 
-// Raw rows of a source at `capacity` constraints: body references, prestep, impulses, and feature ids (old / new) when `contacts` > 0 and features
-// are kept.
-struct RawRows {
-    int32_t* refs = nullptr;
-    float* prestep = nullptr;
-    float* impulses = nullptr;
-    int32_t* features_old = nullptr;
-    int32_t* features_new = nullptr;
-};
-static size_t rows_bytes(const TypeInfo* t, int capacity, int k) {
-    const int per[5] = {t->bodies, t->prestep_rows, t->impulse_rows, t->contacts, t->contacts};
-    return (size_t)capacity * per[k] * 4;
+// ---- graph edits on the resident state: constraint and body adds and removes ----
+
+// The state rules of the four graph edits; `what` names what the call changes.
+static int check_graph_edit(bepucuda_ctx* ctx, const std::string& name, const char* what) {
+    if (ctx->peer_mode) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, name + " in peer mode");
+    if (ctx->constraints_open) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, name + " between begin_constraints and end_constraints");
+    if (!ctx->constraints_ready) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, name + " before end_constraints");
+    if (ctx->data_dirty)
+        return fail(ctx, BEPUCUDA_ERR_BAD_STATE, name + ": rows are pending (uploads or writes since the last solve); change the " + what + " before them");
+    return BEPUCUDA_OK;
 }
-// A block of `bytes` for source rows: a spare block of the arena between `bytes` and twice that, or a new one. Spare blocks are what grown and
-// removed sources left, so a run that stays on the change calls reuses them instead of growing the arena with every re-created type batch.
-static void* take_rows(bepucuda_ctx* ctx, size_t bytes, cudaError_t* e) {
-    size_t best = ctx->spare_rows.size();
-    for (size_t i = 0; i < ctx->spare_rows.size(); ++i) {
-        const size_t have = ctx->spare_rows[i].second;
-        if (have >= bytes && have <= 2 * bytes && (best == ctx->spare_rows.size() || have < ctx->spare_rows[best].second)) best = i;
-    }
-    if (best == ctx->spare_rows.size()) return ctx->raw_arena.alloc(bytes, e);
-    void* p = ctx->spare_rows[best].first;
-    ctx->spare_rows[best] = ctx->spare_rows.back();
-    ctx->spare_rows.pop_back();
-    return p;
-}
-static void give_rows(bepucuda_ctx* ctx, void* p, size_t bytes) {
-    if (p && bytes) ctx->spare_rows.push_back({p, bytes});
-}
-static void give_source_rows(bepucuda_ctx* ctx, const RawRows& r, const TypeInfo* t, int capacity) {
-    void* p[5] = {r.refs, r.prestep, r.impulses, r.features_old, r.features_new};
-    for (int k = 0; k < 5; ++k) give_rows(ctx, p[k], rows_bytes(t, capacity, k));
-}
-// The rows of `capacity` constraints, with feature arrays when `features`; on failure every block taken goes back and the error is returned.
-static cudaError_t take_source_rows(bepucuda_ctx* ctx, const TypeInfo* t, int capacity, bool features, RawRows* out) {
-    cudaError_t e = cudaSuccess;
-    RawRows r;
-    r.refs = (int32_t*)take_rows(ctx, rows_bytes(t, capacity, 0), &e);
-    if (r.refs) r.prestep = (float*)take_rows(ctx, rows_bytes(t, capacity, 1), &e);
-    if (r.prestep) r.impulses = (float*)take_rows(ctx, rows_bytes(t, capacity, 2), &e);
-    bool ok = r.impulses != nullptr;
-    if (ok && features && t->contacts > 0) {
-        r.features_old = (int32_t*)take_rows(ctx, rows_bytes(t, capacity, 3), &e);
-        if (r.features_old) r.features_new = (int32_t*)take_rows(ctx, rows_bytes(t, capacity, 4), &e);
-        ok = r.features_new != nullptr;
-    }
-    if (!ok) {
-        give_source_rows(ctx, r, t, capacity);
-        return e == cudaSuccess ? cudaErrorMemoryAllocation : e;
-    }
-    *out = r;
-    return cudaSuccess;
+
+// The device's rows of every constraint back into the sources, where a graph edit changes them and plan_device_rows reads them. From here on a
+// failure leaves a context that needs a describe.
+static int rows_to_sources(bepucuda_ctx* ctx) {
+    TRY(transpose_out(ctx, kTransposePrestep | kTransposeImpulses));
+    ctx->constraints_ready = false;
+    return BEPUCUDA_OK;
 }
 
 // bepucuda_add_constraints (remove = false) and bepucuda_remove_constraints: the dry run of the whole list on the host (replay_changes), then the
 // rows brought back to the sources, the lane copies, the new sources and counts, and the plan of the describe over the device rows.
 static int change_constraints(bepucuda_ctx* ctx, const std::string& name, bool remove, int32_t count, const bepucuda_constraint_location* locations, const int32_t* records,
                               const int32_t* feature_ids, const int32_t* kinematics, int32_t kinematic_count) {
-    if (ctx->peer_mode) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, name + " in peer mode");
-    if (!ctx->constraints_ready) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, name + " before end_constraints");
-    if (ctx->data_dirty) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, name + ": rows are pending (uploads or writes since the last solve); change the constraints before them");
+    TRY(check_graph_edit(ctx, name, "constraints"));
     if (count < 0 || (count > 0 && (!locations || (!remove && !records))) || kinematic_count < 0 || (kinematic_count > 0 && !kinematics))
         return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, name + ": bad arguments");
     for (int32_t i = 0; i < kinematic_count; ++i)
@@ -1185,7 +1231,7 @@ static int change_constraints(bepucuda_ctx* ctx, const std::string& name, bool r
     const int W = ctx->W;
     ChangeState next;
     next.batch_count = ctx->batch_count;
-    for (const SourceTypeBatch& s : ctx->sources) next.sources.push_back({s.batch_index, s.type_batch_index, s.type_id, s.count, s.host_refs});
+    for (const SourceTypeBatch& s : ctx->sources) next.sources.push_back(s.host);
     std::vector<LaneCopy> ops;
     std::string error;
     if (replay_changes(&next, remove, W, ctx->fallback_threshold, ctx->body_count, count, locations, records, &ops, &error) != BEPUCUDA_OK)
@@ -1205,68 +1251,37 @@ static int change_constraints(bepucuda_ctx* ctx, const std::string& name, bool r
         const int capacity = i < ctx->sources.size() ? ctx->sources[i].capacity : 0;
         const int needed = (n.count + W - 1) / W * W;
         if (needed <= capacity) continue;
-        const bool features = i < ctx->sources.size() ? ctx->sources[i].raw_features_old != nullptr : feature_ids != nullptr;
+        const bool features = i < ctx->sources.size() ? ctx->sources[i].rows.features_old != nullptr : feature_ids != nullptr;
         Growth g{i, std::max(needed, 2 * capacity), {}};
         if (const cudaError_t e = take_source_rows(ctx, get_type_info(n.type_id), g.capacity, features, &g.rows)) {
-            for (const Growth& h : growth) give_source_rows(ctx, h.rows, get_type_info(next.sources[h.source].type_id), h.capacity);
+            for (const Growth& h : growth) give_source_rows(ctx, get_type_info(next.sources[h.source].type_id), h.capacity, h.rows);
             return cuda_fail(ctx, e, (name + ": raw arena").c_str());
         }
         growth.push_back(g);
     }
     ctx->upload_window.start_once(ctx->stream);
-    // the device's rows of every constraint back into the sources, where the copies and the plan below read them
-    launch_transpose_out_all(ctx->tb_table.as<DeviceTypeBatch>(), ctx->tdesc_table.as<TransposeDesc>(), ctx->work_table.as<WorkItem>(), ctx->topo.all_work_count, W,
-                             kTransposePrestep | kTransposeImpulses, ctx->stream);
-    CK(cudaGetLastError());
-    ctx->constraints_ready = false;  // from here on a failure leaves a context that needs a describe
-    std::vector<SourceTypeBatch> old = std::move(ctx->sources);
-    std::vector<SourceTypeBatch> all(next.sources.size());
-    for (size_t i = 0; i < next.sources.size(); ++i) {
-        if (i < old.size()) all[i] = std::move(old[i]);
-        else all[i].type_id = next.sources[i].type_id;
-    }
+    TRY(rows_to_sources(ctx));
+    std::vector<SourceTypeBatch> all = std::move(ctx->sources);
+    for (size_t i = all.size(); i < next.sources.size(); ++i) all.emplace_back().host.type_id = next.sources[i].type_id;
     // grown sources: the rows of their old constraints (as transposed out above) into the new arrays; the old arrays become spare
     for (const Growth& g : growth) {
         SourceTypeBatch& s = all[g.source];
-        const TypeInfo* t = get_type_info(s.type_id);
-        const size_t kept = ((size_t)s.count + W - 1) / W * W;  // whole bundles of the old count (0 for a new source)
-        CK(cudaMemsetAsync(g.rows.refs, 0xff, rows_bytes(t, g.capacity, 0), ctx->stream));
-        if (g.rows.features_old) CK(cudaMemsetAsync(g.rows.features_old, 0, rows_bytes(t, g.capacity, 3), ctx->stream));
-        if (kept > 0) {
-            CK(cudaMemcpyAsync(g.rows.refs, s.raw_refs, kept * t->bodies * 4, cudaMemcpyDeviceToDevice, ctx->stream));
-            CK(cudaMemcpyAsync(g.rows.prestep, s.raw_prestep, kept * t->prestep_rows * 4, cudaMemcpyDeviceToDevice, ctx->stream));
-            CK(cudaMemcpyAsync(g.rows.impulses, s.raw_impulses, kept * t->impulse_rows * 4, cudaMemcpyDeviceToDevice, ctx->stream));
-            if (s.raw_features_old) CK(cudaMemcpyAsync(g.rows.features_old, s.raw_features_old, (size_t)s.count * t->contacts * 4, cudaMemcpyDeviceToDevice, ctx->stream));
+        const TypeInfo* t = s.type();
+        CK(cudaMemsetAsync(g.rows.refs, 0xff, row_bytes(t, kRowRefs, g.capacity, W), ctx->stream));
+        if (g.rows.features_old) CK(cudaMemsetAsync(g.rows.features_old, 0, row_bytes(t, kRowFeatures, g.capacity, W), ctx->stream));
+        if (s.host.count > 0) {  // the old count (0 for a new source)
+            CK(cudaMemcpyAsync(g.rows.refs, s.rows.refs, s.bytes(kRowRefs, W), cudaMemcpyDeviceToDevice, ctx->stream));
+            CK(cudaMemcpyAsync(g.rows.prestep, s.rows.prestep, s.bytes(kRowPrestep, W), cudaMemcpyDeviceToDevice, ctx->stream));
+            CK(cudaMemcpyAsync(g.rows.impulses, s.rows.impulses, s.bytes(kRowImpulses, W), cudaMemcpyDeviceToDevice, ctx->stream));
+            if (s.rows.features_old) CK(cudaMemcpyAsync(g.rows.features_old, s.rows.features_old, s.bytes(kRowFeatures, W), cudaMemcpyDeviceToDevice, ctx->stream));
         }
-        if (s.capacity > 0) give_source_rows(ctx, {s.raw_refs, s.raw_prestep, s.raw_impulses, s.raw_features_old, s.raw_features_new}, t, s.capacity);
-        s.raw_refs = g.rows.refs;
-        s.raw_prestep = g.rows.prestep;
-        s.raw_impulses = g.rows.impulses;
-        s.raw_features_old = g.rows.features_old;
-        s.raw_features_new = g.rows.features_new;
+        give_source_rows(ctx, t, s.capacity, s.rows);
+        s.rows = g.rows;
         s.capacity = g.capacity;
     }
-    for (size_t i = 0; i < next.sources.size(); ++i) {
-        const ChangeSource& n = next.sources[i];
-        SourceTypeBatch& s = all[i];
-        const TypeInfo* t = get_type_info(n.type_id);
-        s.batch_index = n.batch_index;
-        s.type_batch_index = n.type_batch_index;
-        s.count = n.count;
-        const size_t bundles = ((size_t)n.count + W - 1) / W;
-        s.refs_bytes = bundles * t->bodies * W * 4;
-        s.prestep_bytes = bundles * t->prestep_rows * W * 4;
-        s.impulse_bytes = bundles * t->impulse_rows * W * 4;
-        s.feature_bytes = (size_t)n.count * t->contacts * 4;
-        if (n.batch_index >= ctx->fallback_threshold) s.host_refs = n.refs;
-        if (took_add[i]) s.host_impulses = nullptr;
-    }
     if (!copies.empty()) {
-        std::vector<SourceRows> rows(all.size());
-        for (size_t i = 0; i < all.size(); ++i) {
-            const TypeInfo* t = get_type_info(all[i].type_id);
-            rows[i] = {all[i].raw_refs, all[i].raw_prestep, all[i].raw_impulses, all[i].raw_features_old, t->bodies, t->prestep_rows, t->impulse_rows, t->contacts};
-        }
+        std::vector<SourceRows> rows;
+        for (const SourceTypeBatch& s : all) rows.push_back(s.lane_rows());
         const size_t n = copies.size();
         TRY(upload_table(ctx, "change_sources", ctx->change_sources, rows, 0));
         TRY(upload_table(ctx, "change_copies", ctx->change_copies, copies, 0));
@@ -1294,10 +1309,13 @@ static int change_constraints(bepucuda_ctx* ctx, const std::string& name, bool r
         CK(cudaGetLastError());
         ctx->h2d_accum += bytes;
     }
+    // every source takes what the replay left it; an emptied one leaves, and stream order keeps this call's copies ahead of any reuse of its rows
     for (size_t i = 0; i < all.size(); ++i) {
-        if (next.sources[i].type_batch_index >= 0) ctx->sources.push_back(std::move(all[i]));
-        else give_source_rows(ctx, {all[i].raw_refs, all[i].raw_prestep, all[i].raw_impulses, all[i].raw_features_old, all[i].raw_features_new},
-                              get_type_info(all[i].type_id), all[i].capacity);  // stream order keeps this call's copies ahead of any reuse
+        SourceTypeBatch& s = all[i];
+        s.host = std::move(next.sources[i]);
+        if (took_add[i]) s.host_impulses = nullptr;
+        if (s.host.type_batch_index >= 0) ctx->sources.push_back(std::move(s));
+        else give_source_rows(ctx, s.type(), s.capacity, s.rows);
     }
     ctx->batch_count = next.batch_count;
     ctx->kinematics.assign(kinematics, kinematics + kinematic_count);
@@ -1317,55 +1335,31 @@ int32_t bepucuda_remove_constraints(bepucuda_ctx* ctx, int32_t count, const bepu
     return change_constraints(ctx, "remove_constraints", true, count, locations, nullptr, nullptr, constrained_kinematics, kinematic_count);
 }
 
-// ---- body adds and removes on the resident state ----
-static void refresh_body_buffers(bepucuda_ctx* ctx) {
-    ctx->B = {ctx->pose.as<float4>(), ctx->velocity.as<float4>(), ctx->inertia_local.as<float4>(), ctx->inertia_world.as<float4>(), ctx->constrained.as<uint8_t>(),
-              ctx->first_batch.as<int32_t>(), ctx->body_count};
-}
-
-// The state rules bepucuda_add_bodies / bepucuda_remove_bodies share with the constraint change calls.
-static int check_body_change(bepucuda_ctx* ctx, const std::string& name) {
-    if (ctx->peer_mode) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, name + " in peer mode");
-    if (ctx->constraints_open) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, name + " between begin_constraints and end_constraints");
-    if (!ctx->constraints_ready) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, name + " before end_constraints");
-    if (ctx->data_dirty) return fail(ctx, BEPUCUDA_ERR_BAD_STATE, name + ": rows are pending (uploads or writes since the last solve); change the bodies before them");
-    return BEPUCUDA_OK;
-}
-
-// Room for `n` bodies in every per-body array, the records of the first `keep` bodies kept. The per-body accelerations and shapes grow when they
-// are set for `keep` bodies. B is refreshed whether or not this succeeds: a failed growth leaves the arrays it grew, records and all.
-static cudaError_t grow_body_arrays(bepucuda_ctx* ctx, size_t n, size_t keep) {
-    cudaStream_t s = ctx->stream;
-    cudaError_t e = ctx->raw_bodies.grow(n * 128, keep * 128, s);
-    for (DeviceBuffer* b : {&ctx->pose, &ctx->velocity, &ctx->inertia_local, &ctx->inertia_world})
-        if (e == cudaSuccess) e = b->grow(n * 32, keep * 32, s);
-    if (e == cudaSuccess) e = ctx->constrained.grow(n + 1, keep, s);
-    if (e == cudaSuccess) e = ctx->first_batch.grow(n * 4, keep * 4, s);
-    if (e == cudaSuccess && ctx->accelerations_count == (int)keep) e = ctx->accelerations.grow(n * 32, keep * 32, s);
-    if (e == cudaSuccess && ctx->shape_count == (int)keep) e = ctx->body_shapes.grow(n * sizeof(BodyShape), keep * sizeof(BodyShape), s);
-    refresh_body_buffers(ctx);
-    return e;
-}
-
 int32_t bepucuda_add_bodies(bepucuda_ctx* ctx, const void* body_dynamics, int32_t count, const bepucuda_body_shape* shapes, const float* accelerations) {
     if (!ctx) return BEPUCUDA_ERR_INVALID_ARGUMENT;
-    TRY(check_body_change(ctx, "add_bodies"));
+    TRY(check_graph_edit(ctx, "add_bodies", "bodies"));
     if (count < 0 || (count > 0 && !body_dynamics)) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "add_bodies: bad arguments");
     if ((int64_t)ctx->body_count + count > (int64_t)kRefIndexMask) return fail(ctx, BEPUCUDA_ERR_INVALID_ARGUMENT, "add_bodies: too many bodies");
     if (count == 0) return BEPUCUDA_OK;
     CK(cudaSetDevice(ctx->device));
     const int first = ctx->body_count;
     const size_t n = (size_t)first + count, added = (size_t)count;
-    if (const cudaError_t e = grow_body_arrays(ctx, n, (size_t)first)) return cuda_fail(ctx, e, "add_bodies: body arrays");
+    // Room for n bodies in every per-body array, the accelerations and shapes included when they are set for the current count. B is refreshed
+    // whether or not this succeeds: a failed growth leaves the arrays it grew, records and all.
+    cudaError_t e = ctx->bodies.grow(n, (size_t)first, ctx->stream);
+    if (e == cudaSuccess && ctx->accelerations_count == first) e = ctx->accelerations.grow(n * 32, (size_t)first * 32, ctx->stream);
+    if (e == cudaSuccess && ctx->shape_count == first) e = ctx->body_shapes.grow(n * sizeof(BodyShape), (size_t)first * sizeof(BodyShape), ctx->stream);
+    refresh_body_buffers(ctx);
+    if (e != cudaSuccess) return cuda_fail(ctx, e, "add_bodies: body arrays");
     ctx->upload_window.start_once(ctx->stream);
     int64_t bytes = (int64_t)added * 128;
-    CK(cudaMemcpyAsync(ctx->raw_bodies.as<char>() + (size_t)first * 128, body_dynamics, added * 128, cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemcpyAsync(ctx->bodies.raw.as<char>() + (size_t)first * 128, body_dynamics, added * 128, cudaMemcpyHostToDevice, ctx->stream));
     // the appended range through the describe's split, and "unconstrained" until a plan says otherwise
     BodyBuffers appended = ctx->B;
     for (float4** p : {&appended.pose, &appended.velocity, &appended.inertia_local, &appended.inertia_world}) *p += (size_t)first * 2;
-    launch_split_bodies(ctx->raw_bodies.as<char>() + (size_t)first * 128, count, appended, ctx->stream);
-    launch_fill_i32(ctx->first_batch.as<int32_t>() + first, added, 0x7fffffff, ctx->stream);
-    CK(cudaMemsetAsync(ctx->constrained.as<uint8_t>() + first, 0, added, ctx->stream));
+    launch_split_bodies(ctx->bodies.raw.as<char>() + (size_t)first * 128, count, appended, ctx->stream);
+    launch_fill_i32(ctx->bodies.first_batch.as<int32_t>() + first, added, 0x7fffffff, ctx->stream);
+    CK(cudaMemsetAsync(ctx->bodies.constrained.as<uint8_t>() + first, 0, added, ctx->stream));
     CK(cudaGetLastError());
     if (ctx->accelerations_count == first && accelerations) {
         CK(cudaMemcpyAsync(ctx->accelerations.as<char>() + (size_t)first * 32, accelerations, added * 32, cudaMemcpyHostToDevice, ctx->stream));
@@ -1385,7 +1379,7 @@ int32_t bepucuda_add_bodies(bepucuda_ctx* ctx, const void* body_dynamics, int32_
 
 int32_t bepucuda_remove_bodies(bepucuda_ctx* ctx, int32_t count, const int32_t* body_indices) {
     if (!ctx) return BEPUCUDA_ERR_INVALID_ARGUMENT;
-    TRY(check_body_change(ctx, "remove_bodies"));
+    TRY(check_graph_edit(ctx, "remove_bodies", "bodies"));
     const int old = ctx->body_count;
     int32_t final_count = old;
     std::vector<int32_t> moved_to;
@@ -1415,15 +1409,12 @@ int32_t bepucuda_remove_bodies(bepucuda_ctx* ctx, int32_t count, const int32_t* 
     std::vector<RefSpan> spans;
     int64_t max_words = 0;
     for (const SourceTypeBatch& s : ctx->sources) {
-        spans.push_back({s.raw_refs, (int64_t)(s.refs_bytes / 4)});
+        spans.push_back(s.ref_span(ctx->W));
         max_words = std::max(max_words, spans.back().words);
     }
     TRY(upload_table(ctx, "ref_spans", ctx->ref_spans, spans, 0));
-    // the device's rows of every constraint back into the sources, where the remap and the plan below read them
-    launch_transpose_out_all(ctx->tb_table.as<DeviceTypeBatch>(), ctx->tdesc_table.as<TransposeDesc>(), ctx->work_table.as<WorkItem>(), ctx->topo.all_work_count, ctx->W,
-                             kTransposePrestep | kTransposeImpulses, ctx->stream);
-    ctx->constraints_ready = false;  // from here on a failure leaves a context that needs a describe
-    const BodyRecords records{ctx->raw_bodies.as<float4>(), ctx->B, ctx->accelerations_count == old ? ctx->accelerations.as<float4>() : nullptr,
+    TRY(rows_to_sources(ctx));
+    const BodyRecords records{ctx->bodies.raw.as<float4>(), ctx->B, ctx->accelerations_count == old ? ctx->accelerations.as<float4>() : nullptr,
                               ctx->shape_count == old ? ctx->body_shapes.as<float4>() : nullptr};
     launch_move_bodies(records, ctx->moved_to.as<int32_t>(), count, final_count, ctx->stream);
     launch_remap_body_references(ctx->ref_spans.as<RefSpan>(), (int)spans.size(), max_words, ctx->moved_to.as<int32_t>(), count, final_count, ctx->stream);
@@ -1431,7 +1422,7 @@ int32_t bepucuda_remove_bodies(bepucuda_ctx* ctx, int32_t count, const int32_t* 
     // the same moves on the host's copies: fallback references (levelisation) and constrained kinematics (a removed one leaves the list)
     auto new_index = [&](int32_t idx) { return idx < final_count || idx >= old ? idx : moved_to[(size_t)(idx - final_count)]; };
     for (SourceTypeBatch& s : ctx->sources)
-        for (int32_t& r : s.host_refs)
+        for (int32_t& r : s.host.refs)
             if (r >= 0) {
                 const int32_t to = new_index((int32_t)((uint32_t)r & kRefIndexMask));
                 if (to >= 0) r = (int32_t)(((uint32_t)r & kRefKinematicBit) | (uint32_t)to);
@@ -1610,7 +1601,7 @@ int32_t bepucuda_shard_export(bepucuda_ctx* ctx, bepucuda_ipc_handles* out) {
     CK(cudaSetDevice(ctx->device));
     CK(ctx->shard_flags.reserve(kShardFlagBlockWords * sizeof(unsigned long long)));  // barrier flags, arrival counters and targets (ShardStage)
     CK(cudaMemset(ctx->shard_flags.ptr, 0, kShardFlagBlockWords * sizeof(unsigned long long)));
-    void* ptrs[4] = {ctx->pose.ptr, ctx->velocity.ptr, ctx->inertia_world.ptr, ctx->shard_flags.ptr};
+    void* ptrs[4] = {ctx->bodies.pose.ptr, ctx->bodies.velocity.ptr, ctx->bodies.inertia_world.ptr, ctx->shard_flags.ptr};
     for (int i = 0; i < 4; ++i) {
         cudaIpcMemHandle_t h;
         CK(cudaIpcGetMemHandle(&h, ptrs[i]));
@@ -1637,7 +1628,7 @@ int32_t bepucuda_shard_import(bepucuda_ctx* ctx, int32_t rank, int32_t rank_coun
     p.rank = rank;
     p.rank_count = rank_count;
     for (int r = 0; r < rank_count; ++r) {
-        void* ptrs[4] = {ctx->pose.ptr, ctx->velocity.ptr, ctx->inertia_world.ptr, ctx->shard_flags.ptr};
+        void* ptrs[4] = {ctx->bodies.pose.ptr, ctx->bodies.velocity.ptr, ctx->bodies.inertia_world.ptr, ctx->shard_flags.ptr};
         if (r != rank)
             for (int i = 0; i < 4; ++i) {
                 cudaIpcMemHandle_t h;
@@ -1671,9 +1662,9 @@ int32_t bepucuda_shard_import_contexts(bepucuda_ctx* ctx, int32_t rank, int32_t 
             if (e != cudaSuccess && e != cudaErrorPeerAccessAlreadyEnabled) CK(e);
             (void)cudaGetLastError();
         }
-        p.pose[r] = o->pose.as<float4>();
-        p.velocity[r] = o->velocity.as<float4>();
-        p.inertia_world[r] = o->inertia_world.as<float4>();
+        p.pose[r] = o->bodies.pose.as<float4>();
+        p.velocity[r] = o->bodies.velocity.as<float4>();
+        p.inertia_world[r] = o->bodies.inertia_world.as<float4>();
         p.flags[r] = (unsigned long long*)o->shard_flags.ptr;
     }
     return enter_peer_mode(ctx, p);
