@@ -38,6 +38,7 @@ MUTATIONS = (
     "sleep_reads_integrated_velocity",  # sleep candidacy measured after the velocity callback (PoseIntegrator.cs:L334-341)
     "kinematic_test_bits",  # Bodies.IsKinematic as an integer comparison of the OR of the bits (Bodies.cs:L326-331 compares floats)
     "unmatched_zero_impulse",  # unmatched contacts start at zero instead of sharing the unmatched impulse (NarrowPhaseConstraintUpdate.cs:L110-131)
+    "prepare_previous_dt",  # the substeps' PrepareForIntegration given the previous frame's dt / substepCount (Solver_Solve.cs:L1417-1418)
 )
 
 _LIB = None
@@ -402,8 +403,9 @@ def _after_substepping(bodies, cb, constrained, dt, substep_count, W, mutation):
 
 
 # ---- Simulation.Solve: Solver.Solve single-threaded path (Solver_Solve.cs:L1415-1479), then IntegrateAfterSubstepping -------------------------------
-def solve(sim, dt, accelerations=None, center=None, strength=0.0, mutation=None):
-    """One frame of the reference's Solve on `sim`'s host buffers, in place (bodies, prestep, accumulated impulses)."""
+def solve(sim, dt, accelerations=None, center=None, strength=0.0, mutation=None, previous_dt=None):
+    """One frame of the reference's Solve on `sim`'s host buffers, in place (bodies, prestep, accumulated impulses). previous_dt: the dt of the frame
+    before, which only the mutation "prepare_previous_dt" reads (None on a first frame: it then reads dt)."""
     _check(mutation)
     assert library() is not None, "the transpiled reference is not built"
     W = sim.bundle_width
@@ -417,7 +419,10 @@ def solve(sim, dt, accelerations=None, center=None, strength=0.0, mutation=None)
     flags, constrained = integration_responsibilities(batches, sim.body_count, sim.fallback_batch_threshold, W, kinematics, mutation)
     substep_count = len(sim.velocity_iterations)
     substep_dt = f32(dt) / f32(substep_count)
-    cb.prepare(substep_dt)  # L1417-1418
+    if mutation == "prepare_previous_dt" and previous_dt is not None:
+        cb.prepare(f32(previous_dt) / f32(substep_count))
+    else:
+        cb.prepare(substep_dt)  # L1417-1418
     for substep in range(substep_count):
         if substep > 0:
             if mutation == "incremental_after_kinematic_pose":

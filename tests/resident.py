@@ -1,13 +1,98 @@
 """Frames of the resident device path (accumulated impulses kept on the device and redistributed there from the old to the new contact feature
-ids) next to the oracle's host path on a twin simulation, and the narrow-phase-like updates that drive them."""
+ids) next to the oracle's host path on a twin simulation, and the narrow-phase-like updates, body changes and per-frame descriptions that drive
+them."""
+import ctypes as C
+
 import numpy as np
 
 import bepuphysics2_b200 as bp
+from bepuphysics2_b200 import scenes
 from bepuphysics2_b200.native import EXEC_GRAPH, contact_count
 from oracle import binding as ob
 from tests import planner, util
 
 DT = 1.0 / 60.0
+REFERENCE_MASK = (1 << 30) - 1  # the body index bits of an encoded body reference
+
+
+def live_handles(sim):
+    _, batches = sim.constraint_references()
+    return np.flatnonzero(batches >= 0)
+
+
+def type_batch_at(sim, batch, type_id):
+    return next(tb for tb in sim.type_batches() if tb.batch_index == batch and tb.type_id == type_id)
+
+
+def lane_record(sim, handle):
+    """The 64-word record (bepucuda_read_constraints layout) of a constraint from the host's buffers."""
+    b, t, i = sim.constraint_location(handle)
+    tb = type_batch_at(sim, b, t)
+    W = sim.bundle_width
+    r = np.zeros(64, dtype=np.int32)
+    r[0], r[1] = t, 1
+    r[2:2 + tb.bodies] = tb.body_references[i // W, :, i % W]
+    r[2 + tb.bodies:6] = -1
+    r[6:6 + tb.impulse_rows] = tb.accumulated_impulses[i // W, :, i % W].view(np.int32)
+    r[18:18 + tb.prestep_rows] = tb.prestep[i // W, :, i % W].view(np.int32)
+    return r
+
+
+def projectile_prestep(rng, m):
+    return scenes.convex_prestep(rng.uniform(-0.2, 0.2, size=(m, 1, 3)), np.full((m, 1), 0.01), np.tile([0, 1, 0], (m, 1)), offset_b=rng.uniform(-0.2, 0.2, size=(m, 3)))
+
+
+def body_frame(sim, rng, spawn, removes, kinematic_mover=None):
+    """One frame of a game on the host: `removes` random bodies go (Bodies.Remove: their constraints first), then `spawn` projectiles are fired,
+    copies of random bodies 3 m higher with a velocity, each with a new contact to a random body. Returns the number of constraint adds."""
+    if removes:
+        pool = sim.body_handles
+        if kinematic_mover is not None:
+            pool = pool[pool != kinematic_mover]
+        sim.remove_bodies(rng.choice(pool, size=removes, replace=False))
+    if not spawn:
+        return 0
+    src = rng.integers(0, sim.body_count, size=spawn)
+    new = sim.bodies[src].copy()
+    new[:, 5] += 3
+    new[:, 8:11] = rng.normal(size=(spawn, 3))
+    new[:, 16:23] = np.where(new[:, 16:23].any(axis=1, keepdims=True), new[:, 16:23], [1, 0, 1, 0, 0, 1, 1])  # projectiles are dynamic
+    sim.add_bodies(new)
+    added = sim.body_handles[-spawn:]
+    partners = sim.body_handles[rng.integers(0, sim.body_count - spawn, size=spawn)]
+    sim.add_constraints(4, np.stack([added, partners], axis=1), projectile_prestep(rng, spawn))
+    return spawn
+
+
+def remove_a_ragdoll(sim, frame, extra):
+    """Removes every body joined to a random body by joints (one whole ragdoll)."""
+    refs, batches = sim.constraint_references()
+    joint = np.array([contact_count(sim.constraint_location(int(c))[1]) == 0 if batches[c] >= 0 else False for c in range(len(batches))])
+    rng = np.random.default_rng(frame)
+    seed_index = int(rng.integers(0, sim.body_count))
+    group, todo = {seed_index}, [seed_index]
+    while todo:
+        b = todo.pop()
+        for c in np.flatnonzero(joint & ((refs & REFERENCE_MASK) == b).any(axis=1) & (refs >= 0).any(axis=1)):
+            for r in refs[c]:
+                if r >= 0 and (r & REFERENCE_MASK) not in group:
+                    group.add(int(r & REFERENCE_MASK))
+                    todo.append(int(r & REFERENCE_MASK))
+    sim.remove_bodies([int(sim.body_handles[i]) for i in sorted(group)])
+
+
+def set_description(ts, sim):
+    """What a C# host sends at the start of every frame (integration/csharp/CudaTimestepper.cs): the simulation's solve description and
+    integrator, through the C ABI."""
+    its = (C.c_int32 * len(sim.velocity_iterations))(*sim.velocity_iterations)
+    ts._check(ts._cuda.bepucuda_set_solve_description(ts._ctx, len(sim.velocity_iterations), its, sim.fallback_batch_threshold))
+    ts._check(ts._cuda.bepucuda_set_integrator(ts._ctx, C.byref(sim.integrator)))
+
+
+def set_terms(ts, terms):
+    """The velocity terms of a frame's solve keywords (accelerations, center, strength) on the context: set, or cleared where they are absent."""
+    ts.set_body_accelerations(terms.get("accelerations"))
+    ts.set_point_gravity(terms.get("center"), terms.get("strength", 0.0))
 
 
 def initial_features(sim, rng):

@@ -12,7 +12,7 @@ from bepuphysics2_b200 import _build, scenes, sharding
 from bepuphysics2_b200.native import BODY_ACTIVITY_DTYPE, BODY_SHAPE_DTYPE, ERR_BAD_STATE, ERR_INVALID_ARGUMENT, EXEC_GRAPH, EXEC_STREAM, contact_count
 from oracle import binding as ob
 from tests import harness, util
-from tests.test_constraint_changes import lane_record, live_handles
+from tests.resident import body_frame, lane_record, live_handles, projectile_prestep, remove_a_ragdoll
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CSRC = os.path.join(ROOT, "bepuphysics2_b200", "csrc")
@@ -151,32 +151,6 @@ def test_the_mirror_keeps_references_and_kinematics_on_their_bodies(libs, case):
 
 
 # ---- GPU: the resident twin against the oracle's host twin ----------------------------------------------------------------------------------------
-def projectile_prestep(rng, m):
-    return scenes.convex_prestep(rng.uniform(-0.2, 0.2, size=(m, 1, 3)), np.full((m, 1), 0.01), np.tile([0, 1, 0], (m, 1)), offset_b=rng.uniform(-0.2, 0.2, size=(m, 3)))
-
-
-def body_frame(sim, rng, spawn, removes, kinematic_mover=None):
-    """One frame of a game on the host: `removes` random bodies go (Bodies.Remove: their constraints first), then `spawn` projectiles are fired,
-    copies of random bodies 3 m higher with a velocity, each with a new contact to a random body. Returns the number of constraint adds."""
-    if removes:
-        pool = sim.body_handles
-        if kinematic_mover is not None:
-            pool = pool[pool != kinematic_mover]
-        sim.remove_bodies(rng.choice(pool, size=removes, replace=False))
-    if not spawn:
-        return 0
-    src = rng.integers(0, sim.body_count, size=spawn)
-    new = sim.bodies[src].copy()
-    new[:, 5] += 3
-    new[:, 8:11] = rng.normal(size=(spawn, 3))
-    new[:, 16:23] = np.where(new[:, 16:23].any(axis=1, keepdims=True), new[:, 16:23], [1, 0, 1, 0, 0, 1, 1])  # projectiles are dynamic
-    sim.add_bodies(new)
-    added = sim.body_handles[-spawn:]
-    partners = sim.body_handles[rng.integers(0, sim.body_count - spawn, size=spawn)]
-    sim.add_constraints(4, np.stack([added, partners], axis=1), projectile_prestep(rng, spawn))
-    return spawn
-
-
 ZOO = lambda: scenes.merge(scenes.shape_pile(1200, seed=41, nonconvex_fraction=0.4), scenes.joint_zoo(500, per_type=16, seed=42), scenes.ragdolls(8, seed=43))
 GPU_SCENES = {
     "pile_w4": (lambda: scenes.shape_pile(2000, seed=33, nonconvex_fraction=0.3), dict(bundle_width=4)),
@@ -254,23 +228,6 @@ def test_the_resident_twin_stays_on_the_oracle_through_body_adds_and_removes(lib
         assert all(b - a == 1 for a, b in zip(captures, captures[1:]))
     if "fallback" in case:
         assert any(tb.batch_index >= 6 for tb in dev.type_batches())
-
-
-def remove_a_ragdoll(sim, frame, extra):
-    """Removes every body joined to a random body by joints (one whole ragdoll)."""
-    refs, batches = sim.constraint_references()
-    joint = np.array([contact_count(sim.constraint_location(int(c))[1]) == 0 if batches[c] >= 0 else False for c in range(len(batches))])
-    rng = np.random.default_rng(frame)
-    seed_index = int(rng.integers(0, sim.body_count))
-    group, todo = {seed_index}, [seed_index]
-    while todo:
-        b = todo.pop()
-        for c in np.flatnonzero(joint & ((refs & INDEX) == b).any(axis=1) & (refs >= 0).any(axis=1)):
-            for r in refs[c]:
-                if r >= 0 and (r & INDEX) not in group:
-                    group.add(int(r & INDEX))
-                    todo.append(int(r & INDEX))
-    sim.remove_bodies([int(sim.body_handles[i]) for i in sorted(group)])
 
 
 @pytest.mark.gpu

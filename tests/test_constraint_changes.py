@@ -12,6 +12,7 @@ from bepuphysics2_b200 import _build, scenes, sharding
 from bepuphysics2_b200.native import ERR_BAD_STATE, ERR_INVALID_ARGUMENT, EXEC_GRAPH, EXEC_STREAM, contact_count
 from oracle import binding as ob
 from tests import harness, planner, util
+from tests.resident import lane_record, live_handles, type_batch_at
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CSRC = os.path.join(ROOT, "bepuphysics2_b200", "csrc")
@@ -20,29 +21,6 @@ CLEAR, NEW = -1, -2  # kLaneClear / kLaneNew
 
 
 # ---- the mirror ---------------------------------------------------------------------------------------------------------------------------------
-def live_handles(sim):
-    _, batches = sim.constraint_references()
-    return np.flatnonzero(batches >= 0)
-
-
-def type_batch_at(sim, batch, type_id):
-    return next(tb for tb in sim.type_batches() if tb.batch_index == batch and tb.type_id == type_id)
-
-
-def lane_record(sim, handle):
-    """The 64-word record (bepucuda_read_constraints layout) of a constraint from the host's buffers."""
-    b, t, i = sim.constraint_location(handle)
-    tb = type_batch_at(sim, b, t)
-    W = sim.bundle_width
-    r = np.zeros(64, dtype=np.int32)
-    r[0], r[1] = t, 1
-    r[2:2 + tb.bodies] = tb.body_references[i // W, :, i % W]
-    r[2 + tb.bodies:6] = -1
-    r[6:6 + tb.impulse_rows] = tb.accumulated_impulses[i // W, :, i % W].view(np.int32)
-    r[18:18 + tb.prestep_rows] = tb.prestep[i // W, :, i % W].view(np.int32)
-    return r
-
-
 def write_impulses(sim, handle, record):
     b, t, i = sim.constraint_location(handle)
     tb = type_batch_at(sim, b, t)
